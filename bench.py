@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py — the QA-GNN message-passing hot path on B200 (BASELINE.json metric).
+"""bench.py — the QA-GNN message-passing hot path on H100 (BASELINE.json metric).
 
     python bench.py --gpus N --steps K --warmup W            # this repo's CUDA path
+    python bench.py ... --dump-outputs DIR                   # + the last timed step's results as DIR/<name>.npy
     python bench.py --impl reference --gpus N --steps K ...  # the reference algorithm on host cores
 
 One "step" = one QAGNN_Message_Passing.forward (k=5 GATConvE layers, modeling_qagnn.py:53-95) over one
@@ -38,6 +39,9 @@ def parse():
     ap.add_argument("--cpu-sample-graphs", type=int, default=64)
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-cuda-graph", action="store_true", help="launch the ~60 kernels of a step one by one")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step returned (logits, pool_attn, gnn_out) as float32 DIR/<name>.npy; "
+                         "inputs and weights are seeded, so two builds can be compared output for output")
     return ap.parse_args()
 
 
@@ -117,14 +121,15 @@ def gemm_roofline(N, D, H, avg_launch_ms, peaks):
     """Tensor roofline of the projection GEMM as the forward runs it since round 2: [N, D + D/2] x [D + D/2, 3*H*DP]
     ([x | score_emb] against the head-major padded Q|Kx|Mx weights; the type-embedding half of node_feature_extra is a
     per-type bias row), three bf16 passes (hi*hi, hi*lo, lo*hi) per launch."""
-    peak = peaks.get("bf16_tflops", 1590.0)
+    peak = peaks.get("bf16_tflops", 989.0)
     K = D + D // 2
     ncols = 3 * H * ((D // H + 3) // 4 * 4)
     flops = 3 * 2 * N * K * ncols
     achieved = flops / (avg_launch_ms * 1e-3) / 1e12 if avg_launch_ms > 0 else 0.0
     return {"kernel": "gemm_tc_kernel (projection Q|Kx|Mx, K = D + D/2)", "bound": "tensor", "achieved": achieved, "peak": peak,
             "unit": "TFLOP/s", "frac": achieved / peak, "avg_launch_ms": avg_launch_ms, "flops_per_launch": flops,
-            "peak_source": "MEASURED_PEAKS.json bf16_tflops (burst)" if "bf16_tflops" in peaks else "fallback 1590 TFLOP/s"}
+            "peak_source": "MEASURED_PEAKS.json bf16_tflops (burst)" if "bf16_tflops" in peaks else
+            "H100 SXM data sheet, dense BF16 at 700 W (not reached on a power-limited card)"}
 
 
 def run_reference_arm(args):
@@ -187,25 +192,6 @@ class ClockSampler:
                 "power_w_max": max(pw) if pw else None, "samples": len(sm), "reasons": reasons}
 
 
-# ------------------------------------------------------------------------------------------------
-# B200 arm
-# ------------------------------------------------------------------------------------------------
-def mp_traffic_from_profile(kernel_sha):
-    """dram bytes (read + write) of one mp_headtile launch from the committed ncu artefact that was captured with the SAME
-    kernel source (profiles/mp_traffic.json: {"mp_headtile_sha16": ..., "dram_bytes": ...}); None when the artefact is
-    missing or belongs to another version of the kernel — never a hard-coded literal."""
-    try:
-        art = json.load(open(os.path.join(ROOT, "profiles", "mp_traffic.json")))
-        return art["dram_bytes"] if art.get("mp_headtile_sha16") == kernel_sha else None
-    except Exception:  # noqa: BLE001
-        return None
-
-
-def mp_kernel_sha():
-    import hashlib
-    return hashlib.sha256(open(os.path.join(ROOT, "qagnn_b200", "csrc", "mp_headtile.cu"), "rb").read()).hexdigest()[:16]
-
-
 def build_decoder_tail(D, sent_dim, dev):
     """The pooling layer and answer MLP of the QAGNN decoder around the message passing (modeling_qagnn.py:121-125 with the
     scripts' defaults: 2 pooling heads, fc_layer_num 0 -> one Linear(2D+sent_dim -> 1); random init, seed 1)."""
@@ -232,7 +218,7 @@ def synth_step_inputs(rank):
 
 
 # ------------------------------------------------------------------------------------------------
-# B200 arm
+# GPU arm
 # ------------------------------------------------------------------------------------------------
 def run_b200_arm(args):
     import torch.distributed as dist
@@ -372,6 +358,8 @@ def run_b200_arm(args):
     if rank == 0:
         sampler.start()
     ms_total, _, _ = timed(step_resident, args.steps)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, step)
     ms_e2e = timed_e2e(runner, args.steps)
     ms_e2e_nodes = timed_e2e(runner_nodes, args.steps) if world == 1 else None
     # kernel-level pass: the same K steps launched kernel by kernel with the library's CUDA-event stage timers on the
@@ -391,8 +379,8 @@ def run_b200_arm(args):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak_gbs = peaks.get("hbm_gbs", 6650.0)
-    peak_src = "MEASURED_PEAKS.json hbm_gbs" if "hbm_gbs" in peaks else "fallback 6650 GB/s (B200_PROFILING.md)"
+    peak_gbs = peaks.get("hbm_gbs", 3350.0)
+    peak_src = "MEASURED_PEAKS.json hbm_gbs" if "hbm_gbs" in peaks else "H100 SXM data sheet, 3.35 TB/s HBM3"
     mp_ms, mp_cnt = prof["message_passing"]
     mp_avg_ms = mp_ms / max(mp_cnt, 1)
     balg = b_alg_per_layer(N, E, D)
@@ -404,7 +392,7 @@ def run_b200_arm(args):
 
     def finish():
         """Leaves the job without tearing NCCL down: the captured CUDA graphs hold NCCL kernels, and destroying the
-        communicator under them hung the 2-GPU run at exit (profiles/README.md).  Everybody meets at a last barrier, then
+        communicator under them hung a 2-GPU run at exit.  Everybody meets at a last barrier, then
         each process exits on its own."""
         sys.stdout.flush()
         if world > 1:
@@ -424,7 +412,7 @@ def run_b200_arm(args):
                    "shards; ONE NCCL all_gather_into_tensor of the pooled features [B, 2D+sent_dim] per step, inside the step's "
                    "CUDA graph, then the answer MLP on the whole job's batch)" if world > 1 else "single GPU",
                    "l2": f"no flush: a step streams the {lib.qagnn_forward_workspace_bytes(_lib.C.byref(mod._shape(N, E, n))) / 1e6:.0f} MB "
-                         "workspace + 51 MB inputs, > 126 MB L2", "step": "graph prep (packed batch: one launch) + 5 x (projection, message passing, "
+                         "workspace + 51 MB inputs, > 50 MB L2", "step": "graph prep (packed batch: one launch) + 5 x (projection, message passing, "
                    "node MLP) + Vh/Vx epilogue + attention pooling + (all-gather) + answer MLP, inputs resident in HBM",
                    "launch": launch_mode, "numa_node_bound": numa},
         "qa_pairs_per_s": world * B / (ms_step * 1e-3),
@@ -441,10 +429,8 @@ def run_b200_arm(args):
         "roofline": {"kernel": "mp_headtile_kernel (fused logits + per-source softmax + out-degree rescale + per-target sum), one GATConvE layer",
                      "bound": "hbm", "achieved": achieved, "peak": peak_gbs, "unit": "GB/s", "frac": achieved / peak_gbs,
                      "peak_source": peak_src, "algorithmic_bytes_per_launch": balg, "avg_launch_ms": mp_avg_ms,
-                     "launches_timed": int(mp_cnt),
-                     # dram__bytes_read.sum + dram__bytes_write.sum of one launch from the ncu capture of THIS kernel source
-                     "traffic": mp_traffic_from_profile(mp_kernel_sha()) if world == 1 else None},
-        # second-largest kernel: the tcgen05 projection GEMM, three bf16 passes (hi*hi, hi*lo, lo*hi)
+                     "launches_timed": int(mp_cnt)},
+        # second-largest kernel: the wgmma projection GEMM, three bf16 passes (hi*hi, hi*lo, lo*hi)
         "roofline_gemm": gemm_roofline(N, D, CFG["H"], prof["projection"][0] / max(prof["projection"][1], 1), peaks),
         "stages": stages,
         "parity_gate": {"checked": "graphs 0-3 and %d-%d of the timed batch vs the CPU oracle before timing" % (B - 4, B - 1),
@@ -462,6 +448,16 @@ def run_b200_arm(args):
         line["cpu_baseline"] = {k_: r[k_] for k_ in ("value", "unit", "cores", "kind", "sample", "full_batch")}
     print(json.dumps(line))
     finish()
+
+
+def dump_outputs(out_dir, step):
+    """The arrays a caller of DecoderStep.run receives, as left by the last timed step: logits [B_job, 1], pool_attn
+    [2B, n], gnn_out [B, n, D] — 52 MB in float32 at the benchmark's workload."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    torch.cuda.synchronize()
+    for name, t in zip(("logits", "pool_attn", "gnn_out"), (step.logits, step.pool_attn, step.gnn_out)):
+        np.save(os.path.join(out_dir, name + ".npy"), t.detach().float().cpu().numpy())
 
 
 def main():

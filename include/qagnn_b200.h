@@ -1,5 +1,5 @@
 /*
- * qagnn_b200 — C ABI of the B200-native QA-GNN message-passing path.
+ * qagnn_b200 — C ABI of the H100-native (sm_90a) QA-GNN message-passing path.
  *
  * The reference (michiyasunaga/qagnn) has no FFI layer: its operator API for this path is the
  * Python nn.Module surface in modeling/modeling_qagnn.py.  This header is the boundary a
@@ -205,7 +205,7 @@ int32_t qagnn_mp_core_backward(const qagnn_shape *shape, const void *prep, const
 
 /* A stand-alone dense layer on the same tensor-core path the forward uses (diagnostics / tests):
  *   C[M,N] (ldc) = act( [A1 | A2] @ W^T + bias ),  fp32 row-major operands, W [N, K1+K2] (ldw), act 0/1/2 = none/ReLU/GELU(tanh).
- * Splits the operands into bf16 hi/lo planes in `workspace` and runs the tcgen05 3-pass GEMM; returns
+ * Splits the operands into bf16 hi/lo planes in `workspace` and runs the wgmma 3-pass GEMM; returns
  * QAGNN_ERR_UNSUPPORTED when the tensor-core path cannot take the shape (K or ld not multiples of 8). */
 size_t qagnn_linear_workspace_bytes(int64_t M, int32_t N, int32_t K1, int32_t K2);
 int32_t qagnn_linear_bf16x3(const float *A1, int32_t lda1, int32_t K1, const float *A2, int32_t lda2, int32_t K2,

@@ -2,7 +2,7 @@
 
 Run in the build container only (needs /root/reference):
 
-    python -m oracle.make_goldens            # writes tests/golden/*.pt
+    python -m oracle.make_goldens            # writes tests/golden/*.pt and the stored reference data under tests/golden/ref/
     python -m oracle.make_goldens --check    # re-mints in memory, compares with the committed files, writes nothing
     python -m oracle.make_goldens --fuzz 24  # reference vs oracle on 24 random cases that are not committed as fixtures
 
@@ -22,6 +22,12 @@ from oracle import qagnn_oracle as O
 from oracle.ref_shim import load_reference
 
 GOLDEN_DIR = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests", "golden")
+# what the tests compare against the reference's own loader / batch generator and its fuzz cases, stored so that the
+# tests run without the reference tree (tests/test_loader_cpu.py, tests/test_oracle_golden.py)
+REF_DATA_DIR = os.path.join(GOLDEN_DIR, "ref")
+FUZZ_FILE = os.path.join(REF_DATA_DIR, "fuzz24.pt")
+LOADER_FILE = os.path.join(REF_DATA_DIR, "loader.pt")
+FUZZ_SAMPLES = 32  # values kept per compared tensor (a seeded sample: the full outputs would not be small)
 
 
 def fingerprint(*tensors):
@@ -325,31 +331,129 @@ def check(names=None):
     return out
 
 
+def fuzz_cases(count):
+    """The random small cases of --fuzz, deterministic: 1-4 graphs, 1-30 nodes, 0-80 edges, D 16-100, k 1-3, 6 / 17 / 38
+    edge types, both weight regimes."""
+    g = torch.Generator().manual_seed(12345)
+    ri = lambda lo, hi: int(torch.randint(lo, hi + 1, (1,), generator=g))  # noqa: E731
+    cases = []
+    for i in range(count):
+        n = ri(1, 30)
+        R = (38, 38, 6, 17)[ri(0, 3)]
+        case = dict(name=f"fuzz{i}", B=ri(1, 4), n=n, e=ri(0, 80), D=(16, 32, 64, 100)[ri(0, 3)], k=ri(1, 3),
+                    regime=("prod", "peaky")[ri(0, 1)], realistic=bool(ri(0, 1)) and n >= 8 and R >= 6, seed=100 + i)
+        cases.append(dict(case, n_etype=R))
+    return cases
+
+
+def fuzz_compared(out, extra, layers, keep):
+    """[(name, tensor)] that the fuzz comparison checks: output, node_feature_extra, x and attention of the layers `keep`."""
+    ts = [("out", out), ("extra", extra)]
+    for l in keep:
+        ts += [(f"x{l}", layers[l]["x"]), (f"alpha{l}", layers[l]["alpha"])]
+    return ts
+
+
+def oracle_fuzz_outputs(case):
+    inp = O.synth_graph_batch(case["B"], case["n"], case["e"], case["D"], case["n_etype"], case["seed"], case["realistic"])
+    sd = O.random_state_dict(case["k"], case["D"], 4, case["n_etype"], case["regime"], case["seed"])
+    return O.message_passing_forward(sd, inp["H"], inp["edge_index"], inp["edge_type"], inp["node_type"], inp["node_score"],
+                                     case["k"], 4, case["n_etype"], return_layers=True)
+
+
 def fuzz(count, tol_abs=2e-6, tol_rel=2e-5):
     """Random small cases that are NOT committed as fixtures: the reference's own QAGNN_Message_Passing against the oracle
     (output, node_feature_extra, first / last layer x and attention, edge_index').  Returns [(case, worst excess over the
     tolerance)]; excess <= 0 means inside `tol_abs + tol_rel*|ref|`."""
     torch.set_num_threads(8)
     ref = load_reference()
-    g = torch.Generator().manual_seed(12345)
-    ri = lambda lo, hi: int(torch.randint(lo, hi + 1, (1,), generator=g))  # noqa: E731
     results = []
-    for i in range(count):
-        n = ri(1, 30)
-        R = (38, 38, 6, 17)[ri(0, 3)]
-        case = dict(name=f"fuzz{i}", B=ri(1, 4), n=n, e=ri(0, 80), D=(16, 32, 64, 100)[ri(0, 3)], k=ri(1, 3),
-                    regime=("prod", "peaky")[ri(0, 1)], realistic=bool(ri(0, 1)) and n >= 8 and R >= 6, seed=100 + i)
-        fx = mint_mp_case(ref, case, 4, R)
-        inp = O.synth_graph_batch(case["B"], case["n"], case["e"], case["D"], R, case["seed"], case["realistic"])
-        sd = O.random_state_dict(case["k"], case["D"], 4, R, case["regime"], case["seed"])
-        out, extra, layers = O.message_passing_forward(sd, inp["H"], inp["edge_index"], inp["edge_type"], inp["node_type"],
-                                                       inp["node_score"], case["k"], 4, R, return_layers=True)
-        pairs = [(out, fx["out"]), (extra, fx["extra"])]
-        for l, want in fx["layers"].items():
-            pairs += [(layers[l]["x"], want["x"]), (layers[l]["alpha"], want["alpha"])]
+    for case in fuzz_cases(count):
+        fx = mint_mp_case(ref, case, 4, case["n_etype"])
+        out, extra, layers = oracle_fuzz_outputs(case)
+        keep = sorted(fx["layers"])
+        got = dict(fuzz_compared(out, extra, layers, keep))
+        pairs = [(got[name], want) for name, want in fuzz_compared(fx["out"], fx["extra"], fx["layers"], keep)]
         worst = max(float(((a - b).abs() - tol_abs - tol_rel * b.abs()).max()) if a.numel() else -tol_abs for a, b in pairs)
-        results.append((dict(case, n_etype=R), worst))
+        results.append((case, worst))
     return results
+
+
+def mint_fuzz_samples(ref, count=24):
+    """The reference's outputs on the fuzz cases: FUZZ_SAMPLES values of each compared tensor at seeded positions, all
+    concatenated into one index and one value tensor; `entries` says which slice belongs to which case and tensor."""
+    cases, entries, index, value = [], [], [], []
+    off = 0
+    for ci, case in enumerate(fuzz_cases(count)):
+        fx = mint_mp_case(ref, case, 4, case["n_etype"])
+        keep = sorted(fx["layers"])
+        cases.append(dict(case, keep=keep))
+        for name, t in fuzz_compared(fx["out"], fx["extra"], fx["layers"], keep):
+            idx = torch.randperm(t.numel(), generator=torch.Generator().manual_seed(case["seed"]))[:FUZZ_SAMPLES].sort().values
+            entries.append((ci, name, tuple(t.shape), off, idx.numel()))
+            index.append(idx.int())
+            value.append(t.reshape(-1)[idx])
+            off += idx.numel()
+    return {"kind": "fuzz", "cases": cases, "entries": entries, "index": torch.cat(index), "value": torch.cat(value)}
+
+
+def loader_fingerprint(obj):
+    """sha256 of a loader / batch-generator result: tensors by dtype, shape and bytes, lists and tuples element-wise."""
+    h = hashlib.sha256()
+
+    def walk(x):
+        if torch.is_tensor(x):
+            h.update(f"T{x.dtype}{tuple(x.shape)}".encode())
+            h.update(x.detach().contiguous().cpu().numpy().tobytes())
+        elif isinstance(x, (list, tuple)):
+            h.update(f"L{len(x)}".encode())
+            for y in x:
+                walk(y)
+        else:
+            h.update(repr(x).encode())
+    walk(obj)
+    return h.hexdigest()
+
+
+def loader_generator_case(ei, et, cids, ntypes, scores, lens):
+    """The batch-generator case of tests/test_loader_cpu.py: positional args and keywords (bs 4, eval order)."""
+    Q = cids.size(0)
+
+    class Args:
+        drop_partial_batch = False
+        fill_partial_batch = False
+    args = (Args(), "eval", "cpu", "cpu", 4, torch.randperm(Q, generator=torch.Generator().manual_seed(0)),
+            [f"q{i}" for i in range(Q)], torch.arange(Q) % 5)
+    kw = dict(tensors0=[torch.arange(Q * 5 * 7).view(Q, 5, 7)], tensors1=[cids, ntypes, scores, lens])
+    return args, kw
+
+
+def mint_loader_fingerprints():
+    """What the reference's own loader and batch generator return on the synthetic adjacency pickles of the loader tests."""
+    import tempfile
+    from oracle.ref_shim import REFERENCE_ROOT, _install_stubs
+    from qagnn_b200 import data as Dt
+    sys.path.insert(0, REFERENCE_ROOT)
+    try:
+        _install_stubs()
+        from utils import data_utils as RD
+        out = {"kind": "loader", "loader": {}}
+        with tempfile.TemporaryDirectory() as tmp:
+            path = os.path.join(tmp, "dev.graph.adj.pk")
+            Dt.synth_adj_pickle(path, 20, seed=4)
+            for max_node_num in (200, 30):
+                res = RD.load_sparse_adj_data_with_contextnode(path, max_node_num, 5, None)
+                os.remove(path + ".loaded_cache")
+                out["loader"][max_node_num] = loader_fingerprint(list(res[:4]) + [res[4][0], res[4][1]])
+            path = os.path.join(tmp, "s.graph.adj.pk")
+            Dt.synth_adj_pickle(path, 50, seed=2, max_nodes=60)
+            cids, ntypes, scores, lens, (ei, et) = Dt.load_sparse_adj_data_with_contextnode(path, 40, 5, None, use_cache=False,
+                                                                                            write_cache=False)
+            args, kw = loader_generator_case(ei, et, cids, ntypes, scores, lens)
+            out["generator"] = loader_fingerprint(list(RD.MultiGPUSparseAdjDataBatchGenerator(*args, adj_data=(ei, et), **kw)))
+    finally:
+        sys.path.remove(REFERENCE_ROOT)
+    return out
 
 
 def main():
@@ -373,6 +477,10 @@ def main():
         fx = mint(ref, case)
         torch.save(fx, os.path.join(GOLDEN_DIR, case["name"] + ".pt"))
         print("minted", case["name"], fx.get("kind"))
+    os.makedirs(REF_DATA_DIR, exist_ok=True)
+    torch.save(mint_fuzz_samples(ref), FUZZ_FILE)
+    torch.save(mint_loader_fingerprints(), LOADER_FILE)
+    print("minted", FUZZ_FILE, LOADER_FILE)
 
 
 if __name__ == "__main__":

@@ -1,4 +1,4 @@
-"""qagnn_b200 — B200-native implementation of QA-GNN's graph-attention message-passing path.
+"""qagnn_b200 — H100-native (sm_90a) implementation of QA-GNN's graph-attention message-passing path.
 
 Public surface mirrors the reference's modeling/modeling_qagnn.py:
     GATConvE, QAGNN_Message_Passing, QAGNN, LM_QAGNN, make_one_hot

@@ -1,4 +1,4 @@
-"""Builds libqagnn_b200.so (the C-ABI CUDA library) in-tree with nvcc for sm_100a."""
+"""Builds libqagnn_b200.so (the C-ABI CUDA library) in-tree with nvcc for sm_90a (H100)."""
 import glob
 import hashlib
 import os
@@ -10,8 +10,8 @@ CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 LIBNAME = "libqagnn_b200.so"
 
-NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+NVCC_FLAGS = ARCH + ["-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-v",
 ]
 
@@ -68,7 +68,7 @@ def build(force=False, verbose=False):
         log.append(f"== {os.path.basename(src)}\n{o}")
         if p.returncode != 0:
             raise RuntimeError(f"nvcc failed on {src}:\n{o}")
-    cmd = [_nvcc(), "-shared", "-o", out] + objs + ["-gencode", "arch=compute_100a,code=sm_100a"]
+    cmd = [_nvcc(), "-shared", "-o", out] + objs + ARCH
     r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode != 0:
         raise RuntimeError("link failed:\n" + r.stdout)

@@ -273,7 +273,7 @@ int32_t layer_forward(const qagnn_shape& s, const FoldLayout& L, const WorkLayou
   return QAGNN_OK;
 }
 
-// Dense-path selection: tcgen05 split-bf16 GEMMs when the driver exposes TMA descriptors and the row strides
+// Dense-path selection: wgmma split-bf16 GEMMs when the driver exposes TMA descriptors and the row strides
 // meet TMA's 16-byte rule (D % 8 == 0); else the exact-fp32 FFMA GEMM.  QAGNN_GEMM=ffma forces the latter.
 bool use_tc(const qagnn_shape& s) { return gemm_tc_available() && s.D % 8 == 0; }
 
@@ -301,8 +301,7 @@ int32_t layer_forward_tc(const qagnn_shape& s, const FoldLayout& L, const WorkLa
     TcOutput o{};
     if (tiled && type_bias_classes != nullptr) {
       // fast form (qagnn_mp_forward): x planes are [N, KS] rows of [x | score_emb] (K = D + D/2, ONE segment); the
-      // type-embedding half of node_feature_extra enters as a per-node-type bias row (T distinct rows).  One segment lets
-      // the GEMM keep its weight tile resident in shared memory (gemm_tc.cu, W-resident variant)
+      // type-embedding half of node_feature_extra enters as a per-node-type bias row (T distinct rows)
       const int DP = head_dim_padded(D / s.H), KS = round_up8(D + D / 2);
       TcOperand Ax{x.hi, x.lo, KS, D + D / 2}, none{nullptr, nullptr, 0, 0};
       TcOperand Wp{lb + L.wps_hi, lb + L.wps_lo, KS, D + D / 2};
@@ -374,7 +373,7 @@ int32_t extra_forward(const qagnn_shape& s, const FoldLayout& L, const WorkLayou
   }
   const int64_t n = s.N * Dh;
   int64_t g = (n + 255) / 256;
-  if (g > 148 * 32) g = 148 * 32;
+  if (g > kNumSMs * 32) g = kNumSMs * 32;
   node_feature_prologue_kernel<<<(unsigned)g, 256, 0, st>>>(s.N, D, s.T, node_type, node_score, folded + L.type_tab,
                                                             folded + L.basis, extra, ws + W.sinb);
   QAGNN_CHECK_LAUNCH();
@@ -501,7 +500,7 @@ extern "C" int32_t qagnn_mp_forward(const qagnn_shape* shape, const float* H_in,
     {
       ProfScope ps(QAGNN_PROF_PRO_EPILOGUE, st);
       int64_t g = (s.N * (Dh / 2) + 255) / 256;
-      if (g > 148 * 32) g = 148 * 32;
+      if (g > kNumSMs * 32) g = kNumSMs * 32;
       sin_basis_planes_kernel<<<(unsigned)g, 256, 0, st>>>(s.N, Dh, KSh, node_score, f + L.basis, (__nv_bfloat16*)(ws + W.sb_hi),
                                                            (__nv_bfloat16*)(ws + W.sb_lo));
       QAGNN_CHECK_LAUNCH();
@@ -514,7 +513,7 @@ extern "C" int32_t qagnn_mp_forward(const qagnn_shape* shape, const float* H_in,
       {
         const int w4 = Dh * 2 / 8, ld8 = KS * 2 / 8;  // Dh % 4 == 0 and KS % 8 == 0 (checked by `fast`)
         int64_t gc = (s.N * w4 + 255) / 256;
-        if (gc > 148 * 16) gc = 148 * 16;
+        if (gc > kNumSMs * 16) gc = kNumSMs * 16;
         const size_t off = (size_t)D * 2;
         copy_plane_columns_kernel<<<(unsigned)gc, 256, 0, st>>>(s.N, w4, ld8, (const uint2*)(xh[0] + off), (const uint2*)(xl[0] + off),
                                                               (uint2*)(xh[1] + off), (uint2*)(xl[1] + off), (uint2*)(xh[2] + off),

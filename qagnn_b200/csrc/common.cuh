@@ -1,4 +1,4 @@
-// Shared declarations for the qagnn_b200 CUDA sources (sm_100a only).
+// Shared declarations for the qagnn_b200 CUDA sources (sm_90a only).
 #pragma once
 
 #include <cuda_runtime.h>
@@ -10,6 +10,8 @@
 namespace qagnn {
 
 constexpr size_t kAlign = 256;
+// SM count of an H100 SXM: grid-stride kernels cap their grids at a multiple of it
+constexpr int kNumSMs = 132;
 __host__ __device__ inline size_t align_up(size_t x, size_t a = kAlign) { return (x + a - 1) / a * a; }
 
 // ---- launch bookkeeping -------------------------------------------------------------------------

@@ -3,11 +3,12 @@
 //
 //     C[M,N] = act( [A1 | A2] @ W^T + bias )          fp32 in, fp32 accumulate, fp32-faithful out
 //
-// Blackwell-native: tcgen05.mma (kind::f16, bf16 operands, fp32 accumulators in TMEM), operands
-// staged by TMA (cp.async.bulk.tensor, 128-byte swizzle) through an mbarrier ring, one elected
-// thread issuing the MMAs, tcgen05.ld epilogue, cp.async.bulk.tensor stores.  By default two CTAs of a cluster pair up
-// (cta_group::2, 256-row tiles, each CTA stages half of W).  Warp roles per CTA (320 threads):
-//     warps 0-7  epilogue      warp 8  TMA producer      warp 9  TMEM alloc + MMA issuer
+// Hopper-native: wgmma.mma_async (bf16 operands from shared memory, fp32 accumulators in registers), operands staged
+// by TMA (cp.async.bulk.tensor, 128-byte swizzle) through an mbarrier ring.  Warpgroup 0 is the producer (one thread
+// issues the TMA loads); warpgroups 1 and 2 each own 64 rows of the 128-row tile, issue its wgmma chain and run the
+// epilogue from their accumulator registers.  By default two CTAs of a cluster work on neighbouring row tiles of the
+// same n tile, and each loads HALF of the W tile with a TMA multicast into both CTAs' shared memory, which halves the
+// weight bytes each CTA pulls through L2.
 //
 // Precision: the reference runs these linears in fp32 and parity is 1e-4, which single-pass bf16
 // (2^-9) or tf32 (2^-11) cannot hold.  Operands are therefore stored as SPLIT-BF16 planes
@@ -27,34 +28,26 @@ namespace qagnn {
 
 namespace {
 
-constexpr int BM = 128;     // rows per CTA tile = UMMA M
-// k-block width in bf16: 64 (one 128-byte swizzle span per row)
-constexpr int kEpiWarps = 8;
-constexpr int kThreads = (kEpiWarps + 2) * 32;
-// warps 0-7: epilogue (TMEM lane quadrant = warp id % 4, two warps per quadrant alternate 32-column chunks: with one
-// warp per scheduler the epilogue was issue-latency bound, profiles/r1_gemm_tc.md); warp 8: TMA producer; warp 9: TMEM owner + MMA issuer.
-// The issuing warps get the highest warp ids: the SM's arbiter favours high warp ids (B300_MICROARCH.md), and a
-// late MMA/TMA issue stalls the whole pipeline while a late epilogue instruction does not.
-constexpr int kTmaWarp = kEpiWarps, kMmaWarp = kEpiWarps + 1;
+constexpr int BM = 128;      // rows per CTA tile: two consumer warpgroups x wgmma M = 64
+constexpr int BK = 64;       // k-block width in bf16: one 128-byte swizzle span per row
+constexpr int kThreads = 384;  // warpgroup 0: TMA producer; warpgroups 1-2: wgmma + epilogue
+constexpr size_t kSmemCap = 227 * 1024;  // opt-in shared memory per block on H100
+constexpr int kCtrlBytes = 1024;         // mbarriers after the operand ring
 
-struct alignas(64) TcParams {
+struct TcParams {
   CUtensorMap a_hi[2], a_lo[2], w_hi, w_lo;
-  CUtensorMap o_f32, o_hm, o_hi, o_lo;  // TMA-store maps of the requested outputs
   int nseg, kseg[2];
-  int umma_n, n_step, N, stages;
-  int nkb_total;  // k blocks of the (single) A segment: rows of the resident weight region (W-resident variant)
+  int n_step, N, stages;
   long long M;
   const float* bias;
   const int64_t* row_class;  // optional: bias row = clamp(row_class[r], 0, n_class-1) * class_stride
   int class_stride, n_class;
-  int act;
   float* c_f32;
   int ldc;
   float* c_hm;
   HeadMajorOut hm;
   __nv_bfloat16 *c_hi, *c_lo;
   int ldp;
-  unsigned tmem_cols;
 };
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -77,6 +70,12 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
         : "memory");
   } while (!done);
 }
+// arrive on the barrier at the same shared-memory offset in CTA `cta` of the cluster (this CTA included)
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
+  uint32_t remote;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(smem_u32(bar)), "r"(cta));
+  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
+}
 __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar) {
   asm volatile(
       "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(
@@ -84,42 +83,86 @@ __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, i
       "l"(map), "r"(c0), "r"(c1), "r"(smem_u32(bar))
       : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// K-major operand tile, 128-byte swizzle: rows of 128 B, 8-row groups 1024 B apart
-// (cute::UMMA::SmemDescriptor: start>>4 | LBO=1 | SBO=64 | version=1 | layout=SWIZZLE_128B)
-template <int BK>
-__device__ __forceinline__ uint64_t umma_desc(uint32_t saddr) {
-  // rows of BK*2 bytes; 8-row groups (SBO) 8*BK*2 bytes apart; layout type 2 = SWIZZLE_128B, 4 = SWIZZLE_64B
-  const uint32_t lo = ((saddr & 0x3FFFFu) >> 4) | (1u << 16);
-  const uint32_t hi = (uint32_t)(8 * BK * 2 / 16) | (1u << 14) | ((BK == 64 ? 2u : 4u) << 29);
-  return ((uint64_t)hi << 32) | lo;
-}
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t acc) {
+// the same box lands at the same offset in every CTA of `mask`, each completing its own barrier at `bar`'s offset
+__device__ __forceinline__ void tma_load_2d_multicast(void* dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar,
+                                                      uint16_t mask) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(da), "l"(db), "r"(idesc), "r"(acc)
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%2, %3}], "
+      "[%4], %5;" ::"r"(smem_u32(dst)),
+      "l"(map), "r"(c0), "r"(c1), "r"(smem_u32(bar)), "h"(mask)
       : "memory");
 }
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
 }
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float (&v)[32]) {
-  uint32_t r[32];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]),
-        "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]),
-        "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+__device__ __forceinline__ void cluster_sync_all() {
+  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
+  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+
+// K-major operand tile, 128-byte swizzle: rows of 128 B, 8-row groups 1024 B apart (wgmma matrix descriptor:
+// start >> 4 | LBO (unused for swizzled K-major) = 1 | SBO = 1024 >> 4 | layout type 1 = SWIZZLE_128B)
+__device__ __forceinline__ uint64_t wgmma_desc(uint32_t saddr) {
+  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 62);
+}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void fence_acc(float (&d)[N]) {  // keeps the compiler from moving accumulator accesses
 #pragma unroll
-  for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// D[64 x N] (+)= A[64 x 16] . B[16 x N], both operands K-major in shared memory; scale_d = 0 overwrites D
+template <int N>
+__device__ __forceinline__ void wgmma_bf16(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t scale_d);
+template <>
+__device__ __forceinline__ void wgmma_bf16<64>(float (&d)[32], uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "r"(scale_d));
+}
+template <>
+__device__ __forceinline__ void wgmma_bf16<128>(float (&d)[64], uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(scale_d));
+}
+template <>
+__device__ __forceinline__ void wgmma_bf16<208>(float (&d)[104], uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %106, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n208k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63,%64,%65,%66,%67,%68,%69,%70,%71,%72,%73,%74,%75,%76,%77,%78,%79,%80,%81,%82,%83,%84,%85,%86,%87,%88,%89,%90,%91,%92,%93,%94,%95,%96,%97,%98,%99,%100,%101,%102,%103}, %104, %105, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103])
+      : "l"(da), "l"(db), "r"(scale_d));
+}
+template <>
+__device__ __forceinline__ void wgmma_bf16<256>(float (&d)[128], uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63,%64,%65,%66,%67,%68,%69,%70,%71,%72,%73,%74,%75,%76,%77,%78,%79,%80,%81,%82,%83,%84,%85,%86,%87,%88,%89,%90,%91,%92,%93,%94,%95,%96,%97,%98,%99,%100,%101,%102,%103,%104,%105,%106,%107,%108,%109,%110,%111,%112,%113,%114,%115,%116,%117,%118,%119,%120,%121,%122,%123,%124,%125,%126,%127}, %128, %129, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(da), "l"(db), "r"(scale_d));
+}
+
+// the three split-bf16 passes (hi*hi, hi*lo, lo*hi) of the four k16-steps of one k block; A / W plane tiles at sa / sw
+template <int BN>
+__device__ __forceinline__ void mma_kblock(float (&acc)[BN / 2], uint32_t sa, uint32_t sw, uint32_t a_bytes, uint32_t w_bytes) {
+#pragma unroll
+  for (int k = 0; k < BK / 16; ++k) {
+    const uint64_t da_hi = wgmma_desc(sa + k * 32), da_lo = wgmma_desc(sa + a_bytes + k * 32);
+    const uint64_t dw_hi = wgmma_desc(sw + k * 32), dw_lo = wgmma_desc(sw + w_bytes + k * 32);
+    wgmma_bf16<BN>(acc, da_hi, dw_hi, 1u);
+    wgmma_bf16<BN>(acc, da_hi, dw_lo, 1u);
+    wgmma_bf16<BN>(acc, da_lo, dw_hi, 1u);
+  }
 }
 
 // tanh-approximation GELU (utils/layers.py:10-14) with tanh(u) = 1 - 2/(exp(2u)+1) on the fast exp/divide units:
@@ -130,87 +173,25 @@ __device__ __forceinline__ float gelu_tanh_fast(float x) {
   return 0.5f * x * (1.f + t);
 }
 
-// Per-warp epilogue staging tile: 32 rows x 128 B (fp32 x 32 columns, SWIZZLE_128B) or 2 x (32 rows x 64 B)
-// (bf16 hi / lo x 32 columns, SWIZZLE_64B) — written with conflict-free STS.128, drained by one TMA store.
-constexpr int kStageBytesPerWarp = 4096;
-
-__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, int c0, int c1, const void* src) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.tile.bulk_group [%0, {%1, %2}], [%3];" ::"l"(map), "r"(c0), "r"(c1),
-               "r"(smem_u32(src))
-               : "memory");
-}
-__device__ __forceinline__ void tma_store_3d(const CUtensorMap* map, int c0, int c1, int c2, const void* src) {
-  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.tile.bulk_group [%0, {%1, %2, %3}], [%4];" ::"l"(map), "r"(c0),
-               "r"(c1), "r"(c2), "r"(smem_u32(src))
-               : "memory");
-}
-__device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-__device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-__device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-
-// ---- 2-CTA (cta_group::2) variants: the CTA pair of a cluster computes a 256-row tile; each CTA stages its own 128 rows of
-// A and HALF of the W tile (the tensor core reads both halves), which cuts the W bytes through the operand ring in two.
-// Patterns follow cute/arch/copy_sm100_tma.hpp (SM100_TMA_2SM_LOAD), cutlass/arch/barrier.h (umma_arrive_multicast_2x1SM).
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;  // clears the CTA-rank bit of a shared::cluster address -> the even CTA of the pair
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tma_load_2d_2sm(void* dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(
-          smem_u32(dst)),
-      "l"(map), "r"(c0), "r"(c1), "r"(smem_u32(bar) & kPeerBitMask)
-      : "memory");
-}
-__device__ __forceinline__ void umma_bf16_2sm(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(da), "l"(db), "r"(idesc), "r"(acc)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit_2sm(uint64_t* bar) {  // arrives on the same barrier offset in BOTH CTAs
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(smem_u32(bar)),
-               "h"((uint16_t)3)
-               : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_leader(uint64_t* bar) {  // arrive on the even CTA's copy of `bar`
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(smem_u32(bar) & kPeerBitMask) : "memory");
+template <int ACT>
+__device__ __forceinline__ float act_fn(float v) {
+  if (ACT == ACT_RELU) return fmaxf(v, 0.f);
+  if (ACT == ACT_GELU) return gelu_tanh_fast(v);
+  return v;
 }
 
-// WRES = true ("W-resident"): one A segment, and a CTA pair works on ONE n tile for the whole launch, so its share of the
-// weight tile for ALL k blocks (umma_n/2 rows x K, hi + lo planes: 133 KB for the K = 300 projection, 115 KB for the K = 200
-// node MLP) is loaded once and stays in shared memory; the ring then carries only A (32 KB per stage instead of ~59 KB).
-// The streamed variant moved 607 MB through L2 -> SM per projection with the tensor pipe 38 % active and nothing
-// saturated (profiles/r2_gemm_ncu.md): the ring was latency bound, and most of its bytes were weights re-fetched per tile.
-template <int ACT, int BK, int CTAS, bool WRES>
+// Persistent CTAs (CTAS = 1) or CTA pairs (CTAS = 2, one cluster) walk the (row block, n tile) grid with n fastest.
+// Ring stage = [A hi | A lo | W hi | W lo], each a 1024-byte aligned K-major tile of 64 bf16 per row.
+template <int ACT, int BN, int CTAS>
 __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_constant__ TcParams p) {
   extern __shared__ __align__(1024) unsigned char smem[];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t a_bytes = BM * BK * 2;              // one A plane tile: 16 KB
-  const uint32_t wn = (uint32_t)p.umma_n / CTAS;     // W rows this CTA stages
-  const uint32_t w_bytes = wn * BK * 2;              // one W plane k-block
-  const uint32_t stage_bytes = WRES ? 2 * a_bytes : 2 * a_bytes + 2 * w_bytes;
+  constexpr uint32_t a_bytes = BM * BK * 2;  // one A plane tile: 16 KB
+  constexpr uint32_t w_bytes = BN * BK * 2;  // one W plane k block
+  constexpr uint32_t stage_bytes = 2 * a_bytes + 2 * w_bytes;
+  const int wg = threadIdx.x >> 7, tid = threadIdx.x & 127;
   const uint32_t rank = CTAS == 2 ? cluster_ctarank() : 0u;
-  const bool leader = rank == 0;
-  const unsigned cl_id = blockIdx.x / CTAS, n_cl = gridDim.x / CTAS;  // cluster index / count (tile scheduler)
-  // resident weights (WRES): [k block][hi | lo][wn rows x 128 B], after the ring
-  const uint32_t wres_bytes = WRES ? (uint32_t)p.nkb_total * 2u * w_bytes : 0u;
-  unsigned char* wres = smem + (size_t)p.stages * stage_bytes;
-  unsigned char* ctrl = wres + wres_bytes;
-  uint64_t* full = reinterpret_cast<uint64_t*>(ctrl);       // [stages]  TMA -> MMA
-  uint64_t* empty = full + p.stages;                        // [stages]  MMA -> TMA
-  uint64_t* acc_full = empty + p.stages;                    // [2]       MMA -> epilogue
-  uint64_t* acc_empty = acc_full + 2;                       // [2]       epilogue -> MMA
-  uint64_t* wfull = acc_empty + 2;                          // [1]       resident weights landed (WRES)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(wfull + 1);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + (size_t)p.stages * stage_bytes);  // [stages]  TMA -> MMA
+  uint64_t* empty = full + p.stages;                                                      // [stages]  MMA -> TMA
 
   // k-blocks across the (up to two) A segments
   int nkb_seg[2];
@@ -218,268 +199,137 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
   nkb_seg[1] = p.nseg > 1 ? (p.kseg[1] + BK - 1) / BK : 0;
   const int nkb = nkb_seg[0] + nkb_seg[1];
   const int n_tiles = (p.N + p.n_step - 1) / p.n_step;
-  const long long m_tiles = (p.M + BM * CTAS - 1) / (BM * CTAS);
-  const long long total_tiles = m_tiles * n_tiles;
-  // tile walk of this cluster.  Streamed: tile = cl_id, cl_id + n_cl, ... over (m, n) with n fastest.  W-resident: the
-  // cluster keeps n tile cl_id % n_tiles and walks the m tiles idx, idx + cnt, ... of the clusters that share it.
-  const int my_n = WRES ? (int)(cl_id % (unsigned)n_tiles) : 0;
-  const long long w_idx = cl_id / (unsigned)n_tiles;
-  const long long w_cnt = WRES ? ((long long)n_cl - my_n + n_tiles - 1) / n_tiles : 1;
-  const long long t_first = WRES ? w_idx * n_tiles + my_n : (long long)cl_id;
-  const long long t_step = WRES ? w_cnt * n_tiles : (long long)n_cl;
+  const long long total_tiles = (p.M + BM * CTAS - 1) / (BM * CTAS) * n_tiles;
+  const long long cl_id = blockIdx.x / CTAS, n_cl = gridDim.x / CTAS;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 1);
+      mbar_init(&empty[s], 8 * CTAS);  // one arrival per consumer warp of every CTA whose W half lands here
     }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&acc_full[a], 1);
-      mbar_init(&acc_empty[a], kEpiWarps * CTAS);  // one arrival per epilogue warp (of both CTAs: only the leader's copy is used)
-    }
-    mbar_init(wfull, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == kMmaWarp) {  // TMEM allocation is warp-collective; the same warp frees it
-    if (CTAS == 1) {
-      asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512u) : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    } else {  // both CTAs of the pair, same warp id, same destination offset
-      asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512u) : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    }
-  }
-  tc_fence_before();
   __syncthreads();
-  if (CTAS == 2) cluster_sync_all();  // the peer's barriers are initialised before any remote arrive / multicast commit
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  if (CTAS == 2) cluster_sync_all();  // the peer's barriers are initialised before any multicast or remote arrive
 
-  if (warp == kTmaWarp) {
+  if (wg == 0) {
     // ===================================== TMA producer =====================================
-    if (lane == 0) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (tid == 0) {
       long long it = 0;  // k-block counter across tiles
-      if (WRES && t_first < total_tiles) {  // this CTA's rows of the n tile, every k block, once
-        const int n0 = my_n * p.n_step + (int)(rank * wn);
-        if (CTAS == 1) mbar_expect_tx(wfull, wres_bytes);
-        else if (leader) mbar_expect_tx(wfull, 2 * wres_bytes);
-        for (int kb = 0; kb < nkb; ++kb) {
-          unsigned char* dst = wres + (size_t)kb * 2 * w_bytes;
-          if (CTAS == 1) {
-            tma_load_2d(dst, &p.w_hi, kb * BK, n0, wfull);
-            tma_load_2d(dst + w_bytes, &p.w_lo, kb * BK, n0, wfull);
-          } else {
-            tma_load_2d_2sm(dst, &p.w_hi, kb * BK, n0, wfull);
-            tma_load_2d_2sm(dst + w_bytes, &p.w_lo, kb * BK, n0, wfull);
-          }
-        }
-      }
-      for (long long tile = t_first; tile < total_tiles; tile += t_step) {
-        const int n0 = (int)(tile % n_tiles) * p.n_step + (int)(rank * wn);
+      for (long long tile = cl_id; tile < total_tiles; tile += n_cl) {
+        const int n0 = (int)(tile % n_tiles) * p.n_step;
         const int m0 = (int)((tile / n_tiles) * BM * CTAS + rank * BM);
         for (int kb = 0; kb < nkb; ++kb, ++it) {
           const int s = (int)(it % p.stages);
+          // the stage is free once the consumers of BOTH CTAs have read it (the W half of this CTA lands in both)
           if (it >= p.stages) mbar_wait(&empty[s], (uint32_t)((it / p.stages) - 1) & 1u);
           const int seg = kb < nkb_seg[0] ? 0 : 1;
           const int k_in_seg = (seg == 0 ? kb : kb - nkb_seg[0]) * BK;
           const int k_glob = (seg == 0 ? 0 : p.kseg[0]) + k_in_seg;
           unsigned char* st = smem + (size_t)s * stage_bytes;
-          if (WRES) {
-            if (CTAS == 1) {
-              mbar_expect_tx(&full[s], stage_bytes);
-              tma_load_2d(st, &p.a_hi[0], k_in_seg, m0, &full[s]);
-              tma_load_2d(st + a_bytes, &p.a_lo[0], k_in_seg, m0, &full[s]);
-            } else {
-              if (leader) mbar_expect_tx(&full[s], 2 * stage_bytes);
-              tma_load_2d_2sm(st, &p.a_hi[0], k_in_seg, m0, &full[s]);
-              tma_load_2d_2sm(st + a_bytes, &p.a_lo[0], k_in_seg, m0, &full[s]);
-            }
-          } else if (CTAS == 1) {
-            mbar_expect_tx(&full[s], stage_bytes);
-            tma_load_2d(st, &p.a_hi[seg], k_in_seg, m0, &full[s]);
-            tma_load_2d(st + a_bytes, &p.a_lo[seg], k_in_seg, m0, &full[s]);
+          mbar_expect_tx(&full[s], stage_bytes);
+          tma_load_2d(st, &p.a_hi[seg], k_in_seg, m0, &full[s]);
+          tma_load_2d(st + a_bytes, &p.a_lo[seg], k_in_seg, m0, &full[s]);
+          if (CTAS == 1) {
             tma_load_2d(st + 2 * a_bytes, &p.w_hi, k_glob, n0, &full[s]);
             tma_load_2d(st + 2 * a_bytes + w_bytes, &p.w_lo, k_glob, n0, &full[s]);
-          } else {  // both CTAs' bytes complete on the LEADER's barrier, which expects the pair's total
-            if (leader) mbar_expect_tx(&full[s], 2 * stage_bytes);
-            tma_load_2d_2sm(st, &p.a_hi[seg], k_in_seg, m0, &full[s]);
-            tma_load_2d_2sm(st + a_bytes, &p.a_lo[seg], k_in_seg, m0, &full[s]);
-            tma_load_2d_2sm(st + 2 * a_bytes, &p.w_hi, k_glob, n0, &full[s]);
-            tma_load_2d_2sm(st + 2 * a_bytes + w_bytes, &p.w_lo, k_glob, n0, &full[s]);
+          } else {
+            const uint32_t half = w_bytes / 2;
+            tma_load_2d_multicast(st + 2 * a_bytes + rank * half, &p.w_hi, k_glob, n0 + (int)rank * (BN / 2), &full[s], 3);
+            tma_load_2d_multicast(st + 2 * a_bytes + w_bytes + rank * half, &p.w_lo, k_glob, n0 + (int)rank * (BN / 2), &full[s], 3);
           }
         }
-      }
-    }
-  } else if (warp == kMmaWarp) {
-    // ===================================== MMA issuer =====================================
-    if (lane == 0 && leader) {  // cta_group::2: the even CTA issues for the pair
-      // cute::UMMA::InstrDescriptor: D=f32 (bit 4), A=B=bf16 (bits 7, 10), K-major both, N>>3 @17, M>>4 @24
-      const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(p.umma_n >> 3) << 17) | ((uint32_t)((BM * CTAS) >> 4) << 24);
-      long long it = 0;
-      int ti = 0;
-      if (WRES && t_first < total_tiles) {
-        mbar_wait(wfull, 0);
-        tc_fence_after();
-      }
-      for (long long tile = t_first; tile < total_tiles; tile += t_step, ++ti) {
-        const int acc = ti & 1;
-        if (ti >= 2) {  // the epilogue must have drained this accumulator
-          mbar_wait(&acc_empty[acc], (uint32_t)((ti >> 1) - 1) & 1u);
-          tc_fence_after();
-        }
-        const uint32_t tmem_d = tmem_base + (uint32_t)acc * 256u;
-        for (int kb = 0; kb < nkb; ++kb, ++it) {
-          const int s = (int)(it % p.stages);
-          mbar_wait(&full[s], (uint32_t)(it / p.stages) & 1u);
-          tc_fence_after();
-          const int seg = kb < nkb_seg[0] ? 0 : 1;
-          const int k_in_seg = (seg == 0 ? kb : kb - nkb_seg[0]) * BK;
-          const int krem = p.kseg[seg] - k_in_seg;
-          const int nsteps = krem >= BK ? BK / 16 : (krem + 15) / 16;  // skip k-steps that are pure zero fill
-          const uint32_t sa = smem_u32(smem + (size_t)s * stage_bytes);
-          for (int k = 0; k < nsteps; ++k) {
-            const uint64_t da_hi = umma_desc<BK>(sa + k * 32), da_lo = umma_desc<BK>(sa + a_bytes + k * 32);
-            const uint32_t sw = WRES ? smem_u32(wres + (size_t)kb * 2 * w_bytes) : sa + 2 * a_bytes;
-            const uint64_t dw_hi = umma_desc<BK>(sw + k * 32), dw_lo = umma_desc<BK>(sw + w_bytes + k * 32);
-            if (CTAS == 1) {
-              umma_bf16(tmem_d, da_hi, dw_hi, idesc, (kb | k) != 0);
-              umma_bf16(tmem_d, da_hi, dw_lo, idesc, 1u);
-              umma_bf16(tmem_d, da_lo, dw_hi, idesc, 1u);
-            } else {
-              umma_bf16_2sm(tmem_d, da_hi, dw_hi, idesc, (kb | k) != 0);
-              umma_bf16_2sm(tmem_d, da_hi, dw_lo, idesc, 1u);
-              umma_bf16_2sm(tmem_d, da_lo, dw_hi, idesc, 1u);
-            }
-          }
-          if (CTAS == 1) umma_commit(&empty[s]);  // implies tcgen05.fence::before_thread_sync
-          else umma_commit_2sm(&empty[s]);        // frees the stage in both CTAs
-        }
-        if (CTAS == 1) umma_commit(&acc_full[acc]);
-        else umma_commit_2sm(&acc_full[acc]);
       }
     }
   } else {
-    // ===================================== epilogue (warps 0..7) =====================================
-    // TMEM -> registers (thread = row, 32 columns) -> bias/activation -> swizzled per-warp staging tile (STS.128) ->
-    // one cp.async.bulk.tensor store per 32x32 block.  TMA clips rows >= M and columns past the tensor, so there are
-    // no bound checks; the store drains asynchronously while the warp loads the next block from TMEM.
-    const int quad = warp & 3;  // TMEM lane quadrant this warp may read (warp id % 4)
-    unsigned char* stg = ctrl + 1024 + (size_t)warp * kStageBytesPerWarp;
-    const bool hm_mode = p.c_hm != nullptr;
-    const int DP = hm_mode ? p.hm.DP : 0;
-    const int per_head = hm_mode ? (DP + 31) / 32 : 0;                      // 32-column blocks per head slab
-    const int nblk = hm_mode ? p.hm.H * per_head : (p.n_step + 31) / 32;    // blocks per tile
-    int ti = 0;
-    for (long long tile = t_first; tile < total_tiles; tile += t_step, ++ti) {
-      const int acc = ti & 1;
+    // ===================================== consumers (warpgroups 1, 2) =====================================
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+    const int wc = wg - 1;  // rows wc*64 .. wc*64+63 of the tile
+    const int warp = tid >> 5, lane = tid & 31;
+    float acc[BN / 2];
+    long long it = 0;
+    for (long long tile = cl_id; tile < total_tiles; tile += n_cl) {
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+      for (int kb = 0; kb < nkb; ++kb, ++it) {
+        const int s = (int)(it % p.stages);
+        mbar_wait(&full[s], (uint32_t)(it / p.stages) & 1u);
+        const uint32_t sbase = smem_u32(smem + (size_t)s * stage_bytes);
+        const uint32_t sa = sbase + (uint32_t)wc * 64 * 128, sw = sbase + 2 * a_bytes;
+        fence_acc<BN / 2>(acc);
+        wgmma_fence();
+        // always all four k16-steps: the tensor map zero-fills A past its K, and a run-time step count makes ptxas fence
+        // every wgmma of the chain
+        mma_kblock<BN>(acc, sa, sw, a_bytes, w_bytes);
+        wgmma_commit();
+        wgmma_wait_all();
+        fence_acc<BN / 2>(acc);
+        __syncwarp();
+        if (lane == 0) {
+          if (CTAS == 1) mbar_arrive_cluster(&empty[s], 0);
+          else { mbar_arrive_cluster(&empty[s], 0); mbar_arrive_cluster(&empty[s], 1); }
+        }
+      }
+      // ---- epilogue straight from the accumulator fragment: thread holds rows g, g + 8 and column pairs 8j + 2q
       const int n_tile = (int)(tile % n_tiles);
       const int n0 = n_tile * p.n_step;
-      const int row0 = (int)((tile / n_tiles) * BM * CTAS + rank * BM) + quad * 32;  // first row of this warp
-      const float* bias_row = p.bias;  // per-row bias table (node-type classes): this thread's row is row0 + lane
-      if (p.row_class != nullptr) {
-        const long long r = (long long)row0 + lane;
-        long long c = r < p.M ? p.row_class[r] : 0;
-        c = c < 0 ? 0 : (c >= p.n_class ? p.n_class - 1 : c);
-        bias_row = p.bias + (size_t)c * p.class_stride;
-      }
-      mbar_wait(&acc_full[acc], (uint32_t)(ti >> 1) & 1u);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + (uint32_t)acc * 256u + ((uint32_t)(quad * 32) << 16);
-      for (int blk = warp >> 2; blk < nblk; blk += kEpiWarps / 4) {
-        // accumulator column of the block, and where it lands in the output
-        int tcol, oc0, oslab = 0;
-        if (hm_mode) {
-          const int hh = blk / per_head, q = blk % per_head;
-          tcol = hh * DP + 32 * q;
-          oc0 = 32 * q;
-          oslab = n_tile * p.hm.H + hh;  // one `which` (Q / Kx / Mx) per n tile
-        } else {
-          tcol = 32 * blk;
-          oc0 = n0 + tcol;
-          if (oc0 >= p.N) break;
+      const long long row_g = (tile / n_tiles) * BM * CTAS + rank * BM + wc * 64 + warp * 16 + (lane >> 2);
+      const bool hm_mode = p.c_hm != nullptr;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const long long r = row_g + 8 * h;
+        if (r >= p.M) continue;
+        const float* bias_row = p.bias;  // per-row bias table (node-type classes)
+        if (p.bias != nullptr && p.row_class != nullptr) {
+          long long c = p.row_class[r];
+          c = c < 0 ? 0 : (c >= p.n_class ? p.n_class - 1 : c);
+          bias_row = p.bias + (size_t)c * p.class_stride;
         }
-        float v[32];
-        tmem_ld32(taddr + (uint32_t)tcol, v);
-        if (p.bias != nullptr) {  // bias is indexed by GEMM column (padded like the weight rows)
-          if (n0 + tcol + 32 <= p.N) {
-            const float4* b4 = reinterpret_cast<const float4*>(bias_row + n0 + tcol);
 #pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              const float4 b = __ldg(b4 + i);
-              v[4 * i] += b.x; v[4 * i + 1] += b.y; v[4 * i + 2] += b.z; v[4 * i + 3] += b.w;
-            }
-          } else {
-#pragma unroll
-            for (int i = 0; i < 32; ++i)
-              if (n0 + tcol + i < p.N) v[i] += __ldg(bias_row + n0 + tcol + i);
+        for (int j = 0; j < BN / 8; ++j) {
+          const int c = 8 * j + 2 * (lane & 3);  // tile column (even); n_step is even, so c + 1 < n_step too
+          const int gc = n0 + c;
+          if (c >= p.n_step || gc >= p.N) continue;
+          const bool two = gc + 1 < p.N;
+          float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+          if (p.bias != nullptr) {  // bias is indexed by GEMM column (padded like the weight rows)
+            v0 += __ldg(bias_row + gc);
+            if (two) v1 += __ldg(bias_row + gc + 1);
           }
-        }
-#pragma unroll
-        for (int i = 0; i < 32; ++i) {
-          if (ACT == ACT_RELU) v[i] = fmaxf(v[i], 0.f);
-          if (ACT == ACT_GELU) v[i] = gelu_tanh_fast(v[i]);
-        }
-        if (p.c_f32 != nullptr || hm_mode) {
-          tma_store_wait_read();  // the previous store has finished reading the staging tile
-          __syncwarp();
-#pragma unroll
-          for (int c = 0; c < 8; ++c)  // row = lane, 16-byte chunk c -> chunk c ^ (row & 7)  (SWIZZLE_128B)
-            *reinterpret_cast<float4*>(stg + lane * 128 + ((c ^ (lane & 7)) << 4)) = make_float4(v[4 * c], v[4 * c + 1], v[4 * c + 2], v[4 * c + 3]);
-          asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-          __syncwarp();
-          if (lane == 0) {
-            if (hm_mode) tma_store_3d(&p.o_hm, oc0, row0, oslab, stg);
-            else tma_store_2d(&p.o_f32, oc0, row0, stg);
-            tma_store_commit();
+          v0 = act_fn<ACT>(v0);
+          v1 = act_fn<ACT>(v1);
+          if (hm_mode) {  // tile = one `which` (Q / Kx / Mx): column c is element c % DP of head c / DP
+            const int hh = c / p.hm.DP, jj = c - hh * p.hm.DP;
+            float* o = p.c_hm + ((size_t)(n_tile * p.hm.H + hh) * p.M + r) * p.hm.DP + jj;
+            *reinterpret_cast<float2*>(o) = make_float2(v0, v1);
+          } else if (p.c_f32 != nullptr) {
+            float* o = p.c_f32 + (size_t)r * p.ldc + gc;
+            if (two) *reinterpret_cast<float2*>(o) = make_float2(v0, v1);
+            else o[0] = v0;
           }
-        }
-        if (p.c_hi != nullptr) {
-          tma_store_wait_read();
-          __syncwarp();
-          uint32_t hi[16], lo[16];
-#pragma unroll
-          for (int i = 0; i < 16; ++i) {
+          if (p.c_hi != nullptr) {
             __nv_bfloat162 h2, l2;
-            h2.x = __float2bfloat16_rn(v[2 * i]);
-            h2.y = __float2bfloat16_rn(v[2 * i + 1]);
-            l2.x = __float2bfloat16_rn(v[2 * i] - __bfloat162float(h2.x));
-            l2.y = __float2bfloat16_rn(v[2 * i + 1] - __bfloat162float(h2.y));
-            hi[i] = *reinterpret_cast<uint32_t*>(&h2);
-            lo[i] = *reinterpret_cast<uint32_t*>(&l2);
-          }
-#pragma unroll
-          for (int c = 0; c < 4; ++c) {  // rows of 64 B: chunk c -> c ^ ((row >> 1) & 3)  (SWIZZLE_64B)
-            const int off = lane * 64 + ((c ^ ((lane >> 1) & 3)) << 4);
-            *reinterpret_cast<uint4*>(stg + off) = make_uint4(hi[4 * c], hi[4 * c + 1], hi[4 * c + 2], hi[4 * c + 3]);
-            *reinterpret_cast<uint4*>(stg + 2048 + off) = make_uint4(lo[4 * c], lo[4 * c + 1], lo[4 * c + 2], lo[4 * c + 3]);
-          }
-          asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-          __syncwarp();
-          if (lane == 0) {
-            tma_store_2d(&p.o_hi, oc0, row0, stg);
-            tma_store_2d(&p.o_lo, oc0, row0, stg + 2048);
-            tma_store_commit();
+            h2.x = __float2bfloat16_rn(v0);
+            h2.y = __float2bfloat16_rn(v1);
+            l2.x = __float2bfloat16_rn(v0 - __bfloat162float(h2.x));
+            l2.y = __float2bfloat16_rn(v1 - __bfloat162float(h2.y));
+            __nv_bfloat16* oh = p.c_hi + (size_t)r * p.ldp + gc;
+            __nv_bfloat16* ol = p.c_lo + (size_t)r * p.ldp + gc;
+            if (two) {
+              *reinterpret_cast<__nv_bfloat162*>(oh) = h2;
+              *reinterpret_cast<__nv_bfloat162*>(ol) = l2;
+            } else {
+              oh[0] = h2.x;
+              ol[0] = l2.x;
+            }
           }
         }
-      }
-      // accumulator drained: hand it back to the MMA issuer
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if (CTAS == 1) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&acc_empty[acc])) : "memory");
-        else mbar_arrive_leader(&acc_empty[acc]);
       }
     }
-    tma_store_wait_all();  // global writes of this warp's stores are complete before the CTA exits
   }
-  tc_fence_before();
   __syncthreads();
-  if (CTAS == 2) cluster_sync_all();  // the leader's MMAs read the peer's shared memory: nobody leaves early
-  if (warp == kMmaWarp) {
-    tc_fence_after();
-    if (CTAS == 1) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512u) : "memory");
-    else asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512u) : "memory");
-  }
+  if (CTAS == 2) cluster_sync_all();  // the peer's multicasts and remote arrivals target this CTA: nobody leaves early
 }
 
 __global__ void split_bf16_kernel(const float* __restrict__ a, int lda, long long M, int K, __nv_bfloat16* __restrict__ hi,
@@ -515,8 +365,9 @@ EncodeTiledFn encode_fn() {
   return fn;
 }
 
-// [rows, K] bf16 row-major (ld elements) -> 2-D tensor map with a {64, box_rows} box, 128-byte swizzle
-bool make_map(CUtensorMap* m, const void* base, long long rows, int K, int ld, int box_rows, int BK) {
+// [rows, K] bf16 row-major (ld elements) -> 2-D tensor map with a {64, box_rows} box, 128-byte swizzle; out-of-range
+// rows and columns of a box are zero-filled
+bool make_map(CUtensorMap* m, const void* base, long long rows, int K, int ld, int box_rows) {
   EncodeTiledFn enc = encode_fn();
   if (!enc) return false;
   cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)rows};
@@ -524,24 +375,32 @@ bool make_map(CUtensorMap* m, const void* base, long long rows, int K, int ld, i
   cuuint32_t box[2] = {(cuuint32_t)BK, (cuuint32_t)box_rows};
   cuuint32_t estr[2] = {1, 1};
   return enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
-             CU_TENSOR_MAP_INTERLEAVE_NONE, BK == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
-             CU_TENSOR_MAP_L2_PROMOTION_L2_128B,  // 256-byte promotion measured: no gain (1.566 vs 1.552 ms/step)
+             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-// output tensor: dims {cols, rows[, slabs]}, box {32, 32[, 1]}; fp32 -> SWIZZLE_128B, bf16 -> SWIZZLE_64B
-bool make_out_map(CUtensorMap* m, void* base, int elem_bytes, long long cols, long long rows, long long slabs,
-                  size_t row_stride_bytes, size_t slab_stride_bytes) {
-  EncodeTiledFn enc = encode_fn();
-  if (!enc) return false;
-  cuuint64_t dims[3] = {(cuuint64_t)cols, (cuuint64_t)rows, (cuuint64_t)(slabs > 0 ? slabs : 1)};
-  cuuint64_t strides[2] = {(cuuint64_t)row_stride_bytes, (cuuint64_t)slab_stride_bytes};
-  cuuint32_t box[3] = {32, 32, 1};
-  cuuint32_t estr[3] = {1, 1, 1};
-  const int rank = slabs > 0 ? 3 : 2;
-  return enc(m, elem_bytes == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, rank, base, dims, strides,
-             box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, elem_bytes == 4 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
-             CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+template <int ACT, int BN, int CTAS>
+int32_t launch(const cudaLaunchConfig_t& cfg, const TcParams& p) {
+  static bool attr_set[kMaxDevices] = {false};  // the attribute is per device
+  const int dev = current_device();
+  if (!attr_set[dev]) {
+    QAGNN_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<ACT, BN, CTAS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemCap));
+    attr_set[dev] = true;
+  }
+  QAGNN_CHECK_CUDA(cudaLaunchKernelEx(&cfg, gemm_tc_kernel<ACT, BN, CTAS>, p));
+  return QAGNN_OK;
+}
+
+template <int BN, int CTAS>
+int32_t launch_act(Act act, const cudaLaunchConfig_t& cfg, const TcParams& p) {
+  if (act == ACT_NONE) return launch<ACT_NONE, BN, CTAS>(cfg, p);
+  if (act == ACT_RELU) return launch<ACT_RELU, BN, CTAS>(cfg, p);
+  return launch<ACT_GELU, BN, CTAS>(cfg, p);
+}
+
+template <int BN>
+int32_t launch_bn(int ctas, Act act, const cudaLaunchConfig_t& cfg, const TcParams& p) {
+  return ctas == 2 ? launch_act<BN, 2>(act, cfg, p) : launch_act<BN, 1>(act, cfg, p);
 }
 
 }  // namespace
@@ -562,7 +421,7 @@ int32_t split_bf16(const float* a, int lda, long long M, int K, void* hi, void* 
   if (M <= 0 || K <= 0) return QAGNN_OK;
   if (K % 2 != 0 || lda % 2 != 0) return QAGNN_ERR_UNSUPPORTED;
   long long g = (M * (K / 2) + 255) / 256;
-  if (g > 148 * 32) g = 148 * 32;
+  if (g > kNumSMs * 32) g = kNumSMs * 32;
   split_bf16_kernel<<<(unsigned)g, 256, 0, st>>>(a, lda, M, K, (__nv_bfloat16*)hi, (__nv_bfloat16*)lo, ldp);
   QAGNN_CHECK_LAUNCH();
   return QAGNN_OK;
@@ -576,73 +435,40 @@ int32_t gemm_tc(const TcOperand& A1, const TcOperand& A2, const TcOperand& W, co
   if (!gemm_tc_shape_ok(K1, K2, A1.ld, A2.ld, W.ld, N)) return QAGNN_ERR_UNSUPPORTED;
   TcParams p;
   memset(&p, 0, sizeof(p));
-  int n_tiles = (N + 223) / 224;  // UMMA_N <= 224 leaves room for two stages + the epilogue staging buffers
+  int n_tiles = (N + 255) / 256;  // wgmma N <= 256
   p.n_step = (N + n_tiles - 1) / n_tiles;
-  p.n_step = (p.n_step + 31) / 32 * 32;  // whole 32-column store blocks: neighbouring tiles never overlap
+  p.n_step = (p.n_step + 15) / 16 * 16;  // even columns per thread pair; half tiles of whole 8-row swizzle groups
   if (out.hm_buf != nullptr) {  // one `which` (Q / Kx / Mx) per tile: H*DP padded columns
     p.n_step = out.hm.H * out.hm.DP;
     if (p.n_step > 256 || p.n_step % 16 != 0 || N % p.n_step != 0) return QAGNN_ERR_UNSUPPORTED;
     n_tiles = N / p.n_step;
   }
-  p.umma_n = (p.n_step + 15) / 16 * 16;
+  // wgmma tile width: the smallest compiled one that covers n_step (208 = the H*DP and D of the QA-GNN shapes)
+  const int bn = p.n_step <= 64 ? 64 : p.n_step <= 128 ? 128 : p.n_step <= 208 ? 208 : 256;
   p.N = N;
   p.M = M;
   p.nseg = K2 > 0 ? 2 : 1;
   p.kseg[0] = K1;
   p.kseg[1] = K2;
-  p.tmem_cols = 512;
-  // default: cta_group::2 tiles (cluster of 2 CTAs, 256 rows, half of W per CTA); QAGNN_TC_2CTA=0 -> 1-CTA tiles.
+  // default: CTA pairs (cluster of 2, W tile multicast, half loaded by each); QAGNN_TC_2CTA=0 -> single CTAs.
   // Read at every call so that a test can cover both in one process.
   const char* e2 = getenv("QAGNN_TC_2CTA");
   const int CTAS = (e2 && atoi(e2) == 0) ? 1 : 2;
-  constexpr int BK = 64;
-  const size_t smem_cap = 227 * 1024, epi_bytes = kEpiWarps * (size_t)kStageBytesPerWarp;
-  const size_t w_blk = (size_t)(p.umma_n / CTAS) * BK * 2;  // one plane, one k block, this CTA's rows
-  // W-resident variant: single A segment, 2-CTA tiles, enough pairs for every n tile, and the CTA's share of the weight
-  // tile for all k blocks must leave room for at least two A stages.  QAGNN_TC_WRES=0 keeps the streamed variant.
-  const int nkb1 = (K1 + BK - 1) / BK;
-  // Measured at cfg2 (profiles/r2_gemm_ncu.md): 85 vs 80 us for the K = 300 projection, 74 vs 71 us per node MLP — with the
-  // weights resident only two A stages fit, and the ring is bound by its depth, not by its bytes.  Opt-in: QAGNN_TC_WRES=1.
-  const char* ewr = getenv("QAGNN_TC_WRES");
-  bool wres = K2 == 0 && CTAS == 2 && (ewr && atoi(ewr) == 1);
-  size_t stage_bytes = 2 * (size_t)BM * BK * 2 + 2 * w_blk;
-  size_t wres_bytes = 0;
-  int stages = 0;
-  if (wres) {
-    wres_bytes = (size_t)nkb1 * 2 * w_blk;
-    const size_t a_stage = 2 * (size_t)BM * BK * 2;
-    if (wres_bytes + 2 * a_stage + 1024 + epi_bytes > smem_cap) { wres = false; wres_bytes = 0; }
-    else {
-      stage_bytes = a_stage;
-      stages = (int)((smem_cap - 1024 - epi_bytes - wres_bytes) / a_stage);
-    }
-  }
-  if (!wres) stages = (int)((226 * 1024 - 1024 - epi_bytes) / stage_bytes);
+  const size_t stage_bytes = 2 * (size_t)BM * BK * 2 + 2 * (size_t)bn * BK * 2;
+  int stages = (int)((kSmemCap - kCtrlBytes) / stage_bytes);
   if (stages > 6) stages = 6;
   if (stages < 2) return QAGNN_ERR_UNSUPPORTED;
   p.stages = stages;
-  p.nkb_total = nkb1;
-  // operand ring | resident weights (W-resident variant) | 1 KB of barriers | per-warp transpose buffers
-  const size_t smem_bytes = stages * stage_bytes + wres_bytes + 1024 + epi_bytes;
-  bool ok = make_map(&p.a_hi[0], A1.hi, M, K1, A1.ld, BM, BK) && make_map(&p.a_lo[0], A1.lo, M, K1, A1.ld, BM, BK);
-  if (K2 > 0) ok = ok && make_map(&p.a_hi[1], A2.hi, M, K2, A2.ld, BM, BK) && make_map(&p.a_lo[1], A2.lo, M, K2, A2.ld, BM, BK);
-  ok = ok && make_map(&p.w_hi, W.hi, N, K1 + K2, W.ld, p.umma_n / CTAS, BK) &&
-       make_map(&p.w_lo, W.lo, N, K1 + K2, W.ld, p.umma_n / CTAS, BK);
-  // output maps (TMA stores): fp32 boxes of 32 columns x 32 rows (128-byte swizzle), bf16 boxes 32 x 32 (64-byte swizzle)
-  if (out.f32 != nullptr) ok = ok && make_out_map(&p.o_f32, out.f32, 4, N, M, 0, (size_t)out.ldc * 4, 0);
-  if (out.hm_buf != nullptr)
-    ok = ok && make_out_map(&p.o_hm, out.hm_buf, 4, out.hm.DP, M, N / p.n_step * out.hm.H, (size_t)out.hm.DP * 4,
-                            (size_t)M * out.hm.DP * 4);
-  if (out.hi != nullptr)
-    ok = ok && make_out_map(&p.o_hi, out.hi, 2, N, M, 0, (size_t)out.ldp * 2, 0) &&
-         make_out_map(&p.o_lo, out.lo, 2, N, M, 0, (size_t)out.ldp * 2, 0);
+  const size_t smem_bytes = stages * stage_bytes + kCtrlBytes;
+  bool ok = make_map(&p.a_hi[0], A1.hi, M, K1, A1.ld, BM) && make_map(&p.a_lo[0], A1.lo, M, K1, A1.ld, BM);
+  if (K2 > 0) ok = ok && make_map(&p.a_hi[1], A2.hi, M, K2, A2.ld, BM) && make_map(&p.a_lo[1], A2.lo, M, K2, A2.ld, BM);
+  ok = ok && make_map(&p.w_hi, W.hi, N, K1 + K2, W.ld, bn / CTAS) && make_map(&p.w_lo, W.lo, N, K1 + K2, W.ld, bn / CTAS);
   if (!ok) return QAGNN_ERR_CUDA;
   if ((out.f32 && (out.ldc % 4 != 0)) || (out.hi && (out.ldp % 8 != 0))) return QAGNN_ERR_UNSUPPORTED;
   p.bias = bias;
   p.row_class = bias != nullptr ? out.row_class : nullptr;
   p.class_stride = out.class_stride;
   p.n_class = out.n_class > 0 ? out.n_class : 1;
-  p.act = (int)act;
   p.c_f32 = out.f32;
   p.ldc = out.ldc;
   p.c_hm = out.hm_buf;
@@ -650,27 +476,12 @@ int32_t gemm_tc(const TcOperand& A1, const TcOperand& A2, const TcOperand& W, co
   p.c_hi = (__nv_bfloat16*)out.hi;
   p.c_lo = (__nv_bfloat16*)out.lo;
   p.ldp = out.ldp;
-  static size_t attr_c[kMaxDevices] = {0};  // the attribute is per device
-  const int dev_i = current_device();
-  size_t& attr = attr_c[dev_i];
-  if (attr == 0) {
-#define QAGNN_SET_ATTR(A, B, Cn) \
-  QAGNN_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<A, B, Cn, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(226 * 1024)))
-    QAGNN_SET_ATTR(ACT_NONE, 64, 1); QAGNN_SET_ATTR(ACT_RELU, 64, 1); QAGNN_SET_ATTR(ACT_GELU, 64, 1);
-    QAGNN_SET_ATTR(ACT_NONE, 64, 2); QAGNN_SET_ATTR(ACT_RELU, 64, 2); QAGNN_SET_ATTR(ACT_GELU, 64, 2);
-#undef QAGNN_SET_ATTR
-#define QAGNN_SET_ATTR_W(A) \
-  QAGNN_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<A, 64, 2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_cap))
-    QAGNN_SET_ATTR_W(ACT_NONE); QAGNN_SET_ATTR_W(ACT_RELU); QAGNN_SET_ATTR_W(ACT_GELU);
-#undef QAGNN_SET_ATTR_W
-    attr = smem_bytes;
-  }
   static int sms_c[kMaxDevices] = {0};
+  const int dev_i = current_device();
   if (sms_c[dev_i] == 0) QAGNN_CHECK_CUDA(cudaDeviceGetAttribute(&sms_c[dev_i], cudaDevAttrMultiProcessorCount, dev_i));
   const int sms = sms_c[dev_i];
   const long long total_tiles = (long long)n_tiles * ((M + (long long)BM * CTAS - 1) / ((long long)BM * CTAS));
-  long long units = total_tiles < sms / CTAS ? total_tiles : sms / CTAS;  // CTAs (or CTA pairs) to launch
-  if (wres && units < n_tiles) units = n_tiles;  // every n tile needs a pair that keeps its weights
+  const long long units = total_tiles < sms / CTAS ? total_tiles : sms / CTAS;  // CTAs (or CTA pairs) to launch
   const unsigned grid = (unsigned)(units * CTAS);
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
@@ -685,17 +496,13 @@ int32_t gemm_tc(const TcOperand& A1, const TcOperand& A2, const TcOperand& W, co
   lattr[0].val.clusterDim.z = 1;
   cfg.attrs = lattr;
   cfg.numAttrs = CTAS == 2 ? 1 : 0;
-  if (getenv("QAGNN_DEBUG")) fprintf(stderr, "gemm_tc: M=%lld N=%d K1=%d K2=%d act=%d wres=%d CTAS=%d stages=%d smem=%zu grid=%u umma_n=%d n_tiles=%d\n", M, N, K1, K2, (int)act, (int)wres, CTAS, stages, smem_bytes, grid, p.umma_n, n_tiles);
-#define QAGNN_LAUNCH(A)                                                                          \
-  do {                                                                                           \
-    if (wres) QAGNN_CHECK_CUDA(cudaLaunchKernelEx(&cfg, gemm_tc_kernel<A, 64, 2, true>, p));               \
-    else if (CTAS == 2) QAGNN_CHECK_CUDA(cudaLaunchKernelEx(&cfg, gemm_tc_kernel<A, 64, 2, false>, p));    \
-    else QAGNN_CHECK_CUDA(cudaLaunchKernelEx(&cfg, gemm_tc_kernel<A, 64, 1, false>, p));                   \
-  } while (0)
-  if (act == ACT_NONE) QAGNN_LAUNCH(ACT_NONE);
-  else if (act == ACT_RELU) QAGNN_LAUNCH(ACT_RELU);
-  else QAGNN_LAUNCH(ACT_GELU);
-#undef QAGNN_LAUNCH
+  if (getenv("QAGNN_DEBUG")) fprintf(stderr, "gemm_tc: M=%lld N=%d K1=%d K2=%d act=%d CTAS=%d stages=%d smem=%zu grid=%u bn=%d n_step=%d n_tiles=%d\n", M, N, K1, K2, (int)act, CTAS, stages, smem_bytes, grid, bn, p.n_step, n_tiles);
+  int32_t rc;
+  if (bn == 64) rc = launch_bn<64>(CTAS, act, cfg, p);
+  else if (bn == 128) rc = launch_bn<128>(CTAS, act, cfg, p);
+  else if (bn == 208) rc = launch_bn<208>(CTAS, act, cfg, p);
+  else rc = launch_bn<256>(CTAS, act, cfg, p);
+  QAGNN_RETURN_IF(rc);
   QAGNN_CHECK_LAUNCH();
   return QAGNN_OK;
 }

@@ -497,7 +497,7 @@ __global__ void __launch_bounds__(kPackedThreads) prep_packed_graph_kernel(const
   }
 }
 
-inline int grid_for(int64_t n, int block, int cap = 148 * 16) {
+inline int grid_for(int64_t n, int block, int cap = kNumSMs * 16) {
   int64_t g = (n + block - 1) / block;
   if (g < 1) g = 1;
   return (int)(g < cap ? g : cap);
@@ -588,12 +588,12 @@ extern "C" int32_t qagnn_graph_prep(const int64_t* edge_index, const int64_t* ed
                                                       scr + sc.cnt_src, scr + sc.cnt_tgt, scr + sc.tmp_src,
                                                       scr + sc.tmp_tgt);
   QAGNN_CHECK_LAUNCH();
-  prep_sort_segments_kernel<<<grid_for(2 * N * 32, 256, 148 * 32), 256, 0, st>>>(
+  prep_sort_segments_kernel<<<grid_for(2 * N * 32, 256, kNumSMs * 32), 256, 0, st>>>(
       N, I(pl.rowptr_src), I(pl.rowptr_tgt), scr + sc.tmp_src, scr + sc.tmp_tgt, I(pl.perm_src), I(pl.perm_tgt),
       scr + sc.big_list, I(pl.status) + 1);
   QAGNN_CHECK_LAUNCH();
   // hub nodes (more than 32 edges in a segment): one CTA per listed segment; exits at once when the list is empty
-  prep_sort_big_segments_kernel<<<148, kBigThreads, 0, st>>>(N, I(pl.rowptr_src), I(pl.rowptr_tgt), scr + sc.tmp_src,
+  prep_sort_big_segments_kernel<<<kNumSMs, kBigThreads, 0, st>>>(N, I(pl.rowptr_src), I(pl.rowptr_tgt), scr + sc.tmp_src,
                                                              scr + sc.tmp_tgt, I(pl.perm_src), I(pl.perm_tgt),
                                                              scr + sc.big_list, I(pl.status) + 1);
   QAGNN_CHECK_LAUNCH();

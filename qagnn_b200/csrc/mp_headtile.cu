@@ -21,7 +21,7 @@
 //     its time there and 16 % in the od->rowptr->degree set-up chain, profiles/r1_mp_stall_breakdown.md);
 //   * consumers: 8 lanes per node (quarter-warp), each lane owning float4 chunks l, l+8 of the padded
 //     head row: a quarter-warp LDS.128 covers 128 contiguous bytes = one conflict-free wavefront;
-//     packed FP32x2 math (FADD2/FFMA2, sm_100a); the 8 lane-partials of 8 edges are reduced by a 7-shuffle
+//     fp32 math on float2 pairs; the 8 lane-partials of 8 edges are reduced by a 7-shuffle
 //     transposing tree (lane j ends up with the logit of edge j); the softmax runs lane-parallel.
 // a' is written and read back by ordinary (generic-proxy) accesses of the same CTA, ordered by a CTA fence and
 // the phase-switch mbarrier: no async-proxy fence per graph (5 % in round 1).
@@ -96,6 +96,11 @@ __device__ __forceinline__ float4 lds128(uint32_t addr) {
 }
 __device__ __forceinline__ float2 lo2(const float4& v) { return make_float2(v.x, v.y); }
 __device__ __forceinline__ float2 hi2(const float4& v) { return make_float2(v.z, v.w); }
+// element-wise fp32x2 add / fused multiply-add, each lane rounded once (the same bits as a packed FP32x2 unit gives)
+__device__ __forceinline__ float2 fadd2(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
+  return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
+}
 
 // shared-memory carve-up (bytes from the start of dynamic smem)
 struct SmemMap {
@@ -305,8 +310,8 @@ __global__ void __launch_bounds__((WMAX + 1) * 32, 1) mp_headtile_kernel(const H
 #pragma unroll
           for (int k = 0; k < CPL; ++k) {
             const float4 x0 = lds128(tile_addr(ktc[k], w0)), y0 = lds128(table_addr(tabu[k], w0));
-            a0 = __ffma2_rn(__fadd2_rn(lo2(x0), lo2(y0)), lo2(qc[k]), a0);
-            a0 = __ffma2_rn(__fadd2_rn(hi2(x0), hi2(y0)), hi2(qc[k]), a0);
+            a0 = ffma2(fadd2(lo2(x0), lo2(y0)), lo2(qc[k]), a0);
+            a0 = ffma2(fadd2(hi2(x0), hi2(y0)), hi2(qc[k]), a0);
           }
           return a0.x + a0.y;
         };
@@ -319,10 +324,10 @@ __global__ void __launch_bounds__((WMAX + 1) * 32, 1) mp_headtile_kernel(const H
             for (int k = 0; k < CPL; ++k) {
               const float4 x0 = lds128(tile_addr(ktc[k], w0)), y0 = lds128(table_addr(tabu[k], w0));
               const float4 x1 = lds128(tile_addr(ktc[k], w1)), y1 = lds128(table_addr(tabu[k], w1));
-              a0 = __ffma2_rn(__fadd2_rn(lo2(x0), lo2(y0)), lo2(qc[k]), a0);
-              a0 = __ffma2_rn(__fadd2_rn(hi2(x0), hi2(y0)), hi2(qc[k]), a0);
-              a1 = __ffma2_rn(__fadd2_rn(lo2(x1), lo2(y1)), lo2(qc[k]), a1);
-              a1 = __ffma2_rn(__fadd2_rn(hi2(x1), hi2(y1)), hi2(qc[k]), a1);
+              a0 = ffma2(fadd2(lo2(x0), lo2(y0)), lo2(qc[k]), a0);
+              a0 = ffma2(fadd2(hi2(x0), hi2(y0)), hi2(qc[k]), a0);
+              a1 = ffma2(fadd2(lo2(x1), lo2(y1)), lo2(qc[k]), a1);
+              a1 = ffma2(fadd2(hi2(x1), hi2(y1)), hi2(qc[k]), a1);
             }
             v[j] = a0.x + a0.y;
             v[j + 1] = a1.x + a1.y;
@@ -458,10 +463,10 @@ __global__ void __launch_bounds__((WMAX + 1) * 32, 1) mp_headtile_kernel(const H
             for (int k = 0; k < CPL; ++k) {
               const float4 x0 = lds128(tile_addr(mtc[k], w0)), y0 = lds128(table_addr(tabu[k], w0));
               const float4 x1 = lds128(tile_addr(mtc[k], w1)), y1 = lds128(table_addr(tabu[k], w1));
-              acc[k][0] = __ffma2_rn(__fadd2_rn(lo2(x0), lo2(y0)), aa0, acc[k][0]);
-              acc[k][1] = __ffma2_rn(__fadd2_rn(hi2(x0), hi2(y0)), aa0, acc[k][1]);
-              acc[k][0] = __ffma2_rn(__fadd2_rn(lo2(x1), lo2(y1)), aa1, acc[k][0]);
-              acc[k][1] = __ffma2_rn(__fadd2_rn(hi2(x1), hi2(y1)), aa1, acc[k][1]);
+              acc[k][0] = ffma2(fadd2(lo2(x0), lo2(y0)), aa0, acc[k][0]);
+              acc[k][1] = ffma2(fadd2(hi2(x0), hi2(y0)), aa0, acc[k][1]);
+              acc[k][0] = ffma2(fadd2(lo2(x1), lo2(y1)), aa1, acc[k][0]);
+              acc[k][1] = ffma2(fadd2(hi2(x1), hi2(y1)), aa1, acc[k][1]);
             }
           } else if (j < lim) {  // odd tail: one edge
             const uint32_t w0 = __shfl_sync(0xffffffffu, pko, qbase + j);
@@ -470,8 +475,8 @@ __global__ void __launch_bounds__((WMAX + 1) * 32, 1) mp_headtile_kernel(const H
 #pragma unroll
             for (int k = 0; k < CPL; ++k) {
               const float4 x0 = lds128(tile_addr(mtc[k], w0)), y0 = lds128(table_addr(tabu[k], w0));
-              acc[k][0] = __ffma2_rn(__fadd2_rn(lo2(x0), lo2(y0)), aa0, acc[k][0]);
-              acc[k][1] = __ffma2_rn(__fadd2_rn(hi2(x0), hi2(y0)), aa0, acc[k][1]);
+              acc[k][0] = ffma2(fadd2(lo2(x0), lo2(y0)), aa0, acc[k][0]);
+              acc[k][1] = ffma2(fadd2(hi2(x0), hi2(y0)), aa0, acc[k][1]);
             }
           }
         }
@@ -602,7 +607,7 @@ int32_t zero_head_pads(const qagnn_shape& s, float* qkmh, cudaStream_t st) {
   if (DP == d) return QAGNN_OK;
   const int64_t rows = (int64_t)3 * s.H * s.N;
   int64_t g = (rows * (DP - d) + 255) / 256;
-  if (g > 148 * 16) g = 148 * 16;
+  if (g > kNumSMs * 16) g = kNumSMs * 16;
   zero_head_pads_kernel<<<(unsigned)g, 256, 0, st>>>(rows, d, DP, qkmh);
   QAGNN_CHECK_LAUNCH();
   return QAGNN_OK;

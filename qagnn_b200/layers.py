@@ -168,7 +168,7 @@ class CustomizedEmbedding(nn.Module):
         lin = self.cpt_transform
         if (e.is_cuda and not self.training and not torch.is_grad_enabled() and e.dtype == torch.float32
                 and lin.in_features % 8 == 0 and lin.out_features >= 8):
-            # GELU(cpt_transform(e)) on the tcgen05 split-bf16 GEMM with the activation fused in the epilogue: the
+            # GELU(cpt_transform(e)) on the wgmma split-bf16 GEMM with the activation fused in the epilogue: the
             # [B*(n-1), concept_in_dim] x [concept_in_dim, concept_dim] product is the largest dense op outside the GNN
             from . import ops
             try:

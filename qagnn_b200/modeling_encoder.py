@@ -1,6 +1,6 @@
 """Text-encoder wrapper on the caller side of the hot path (reference: modeling/modeling_encoder.py:89-143).
 
-Out of scope for the B200 kernels ("drops in behind the existing RoBERTa encoder"): this is a thin
+Out of scope for the CUDA kernels ("drops in behind the existing RoBERTa encoder"): this is a thin
 HuggingFace wrapper with the reference's interface — `TextEncoder(model_name, **kwargs)`, `.sent_dim`,
 `forward(input_ids, attention_mask, token_type_ids, output_mask, layer_id=-1) -> (sent_vecs, all_hidden_states)`
 — for the BERT/RoBERTa family the QA-GNN configs use.  Offline environments pass

@@ -2,7 +2,7 @@
 
 Same class names, constructor arguments, forward signatures, return values and state_dict key
 names as the reference (SURVEY.md §8b), but `GATConvE.forward` and
-`QAGNN_Message_Passing.forward` run entirely in the hand-written sm_100a kernels of
+`QAGNN_Message_Passing.forward` run entirely in the hand-written sm_90a kernels of
 libqagnn_b200.so, reached through the C ABI in include/qagnn_b200.h.  The nn.Modules below only
 own parameters and device buffers (PyTorch = memory + streams).
 

@@ -5,7 +5,7 @@ from . import _lib
 
 
 def linear_bf16x3(a1, weight, bias=None, a2=None, act="none"):
-    """act([a1 | a2] @ weight^T + bias) through the tcgen05 split-bf16 (3-pass) GEMM.  fp32 CUDA tensors."""
+    """act([a1 | a2] @ weight^T + bias) through the wgmma split-bf16 (3-pass) GEMM.  fp32 CUDA tensors."""
     lib = _lib.load()
     a1 = _lib.f32c(a1, "a1")
     w = _lib.f32c(weight, "weight")

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Times the tcgen05 split-bf16 GEMM on the hot-path shapes and checks it against an fp64 matmul."""
+"""Times the wgmma split-bf16 GEMM on the hot-path shapes and checks it against an fp64 matmul."""
 import os
 import sys
 import torch

@@ -1,7 +1,7 @@
-// Micro-benchmarks that size the message-passing design on the actual B200:
+// Micro-benchmarks that size the message-passing design on the actual GPU:
 //   hbm_read / l2_read (streaming float4), table_gather (random 800-B rows from a 1 MB table = the
 //   Ke/Me access pattern), smem_read (LDS.128 from a resident tile).
-// build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o gpurun_out/microbench tools/microbench.cu
+// build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/bin/microbench tools/microbench.cu
 #include <cstdio>
 #include <cstdlib>
 #include <cuda_runtime.h>

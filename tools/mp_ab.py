@@ -1,4 +1,4 @@
-"""In-process A/B of the tiled message-passing kernel's launch-time switches on a B200 (the library reads them at every
+"""In-process A/B of the tiled message-passing kernel's launch-time switches on the GPU (the library reads them at every
 launch): bit-equality of the outputs across settings and the message-passing stage time of each.
 
     python tools/mp_ab.py QAGNN_MP_WARPS=24 QAGNN_MP_WARPS=28 QAGNN_MP_WARPS=31      # -> gpurun_out/mp_ab.txt
