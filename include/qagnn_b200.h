@@ -173,6 +173,13 @@ int32_t qagnn_gatconve_forward(const qagnn_shape *shape, int32_t layer, const fl
                                const void *prep, const void *folded, float *out, float *alpha_out,
                                float *aggr_out, void *workspace, size_t workspace_bytes, void *stream);
 
+/* Which message-passing kernels qagnn_gatconve_forward / qagnn_mp_forward run for `shape` on the current device, under the
+ * current QAGNN_MP_PATH: the shared-memory-tiled per-graph kernel, the column-sliced kernels, or the basic CSR kernels
+ * (head counts 1, 2, 4, 8, 16 and D % 4 == 0, D <= 1024; other shapes are refused there with QAGNN_ERR_UNSUPPORTED).
+ * Read-only; a negative status for an invalid shape. */
+enum { QAGNN_MP_PATH_TILED = 0, QAGNN_MP_PATH_SLICE = 1, QAGNN_MP_PATH_BASIC = 2 };
+int32_t qagnn_mp_path(const qagnn_shape *shape);
+
 /* node_feature_extra[N,D] = [GELU(emb_node_type(onehot(type))) ‖ GELU(emb_score(sin(basis*score)))] */
 int32_t qagnn_node_feature_extra(const qagnn_shape *shape, const int64_t *node_type, const float *node_score,
                                  const void *folded, float *extra_out, void *workspace, size_t workspace_bytes,

@@ -58,6 +58,7 @@ EXPORTS = {
                                        C.POINTER(MPParams), _P, C.c_size_t, _P]),
     "qagnn_forward_workspace_bytes": (C.c_size_t, [C.POINTER(Shape)]),
     "qagnn_gatconve_forward": (C.c_int32, [C.POINTER(Shape), C.c_int32, _P, _P, _P, _P, _P, _P, _P, _P, C.c_size_t, _P]),
+    "qagnn_mp_path": (C.c_int32, [C.POINTER(Shape)]),
     "qagnn_node_feature_extra": (C.c_int32, [C.POINTER(Shape), _P, _P, _P, _P, _P, C.c_size_t, _P]),
     "qagnn_mp_forward": (C.c_int32, [C.POINTER(Shape), _P, _P, _P, _P, _P, _P, _P, _P, C.c_size_t, _P]),
     "qagnn_mp_core_forward": (C.c_int32, [C.POINTER(Shape), _P, _P, _P, _P, _P, _P, _P, _P, _P]),

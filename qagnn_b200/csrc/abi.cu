@@ -460,6 +460,12 @@ extern "C" int32_t qagnn_gatconve_forward(const qagnn_shape* shape, int32_t laye
                        ACT_NONE, tiled, st);
 }
 
+extern "C" int32_t qagnn_mp_path(const qagnn_shape* shape) {
+  QAGNN_RETURN_IF(check_shape_fwd(shape));
+  if (use_headtile(*shape)) return QAGNN_MP_PATH_TILED;
+  return use_slice(*shape) ? QAGNN_MP_PATH_SLICE : QAGNN_MP_PATH_BASIC;
+}
+
 extern "C" int32_t qagnn_node_feature_extra(const qagnn_shape* shape, const int64_t* node_type, const float* node_score,
                                             const void* folded, float* extra_out, void* workspace,
                                             size_t workspace_bytes, void* stream) {

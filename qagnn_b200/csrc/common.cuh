@@ -152,6 +152,9 @@ struct TcOutput {
 };
 bool gemm_tc_available();
 bool gemm_tc_shape_ok(int K1, int K2, int lda1, int lda2, int ldw, int N);
+// Columns per n tile of the head-major output: hpt * DP for the largest divisor hpt of H with hpt * DP <= 256 (the widest
+// wgmma), so a tile holds whole heads of one `which`.  0 when no head fits (DP > 256) or DP is odd.
+int hm_n_step(const HeadMajorOut& hm);
 int32_t split_bf16(const float* a, int lda, long long M, int K, void* hi, void* lo, int ldp, cudaStream_t st);
 int32_t gemm_tc(const TcOperand& A1, const TcOperand& A2, const TcOperand& W, const float* bias, long long M, int N,
                 Act act, const TcOutput& out, cudaStream_t st);

@@ -276,6 +276,8 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
       const int n0 = n_tile * p.n_step;
       const long long row_g = (tile / n_tiles) * BM * CTAS + rank * BM + wc * 64 + warp * 16 + (lane >> 2);
       const bool hm_mode = p.c_hm != nullptr;
+      // head-major output: the tile's first column starts plane n0 / DP (= which * H + head) of [3][H][N][DP]
+      const int hm_plane0 = hm_mode ? n0 / p.hm.DP : 0;
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const long long r = row_g + 8 * h;
@@ -299,9 +301,9 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
           }
           v0 = act_fn<ACT>(v0);
           v1 = act_fn<ACT>(v1);
-          if (hm_mode) {  // tile = one `which` (Q / Kx / Mx): column c is element c % DP of head c / DP
+          if (hm_mode) {  // tile = whole heads of one `which`: column c is element c % DP of plane hm_plane0 + c / DP
             const int hh = c / p.hm.DP, jj = c - hh * p.hm.DP;
-            float* o = p.c_hm + ((size_t)(n_tile * p.hm.H + hh) * p.M + r) * p.hm.DP + jj;
+            float* o = p.c_hm + ((size_t)(hm_plane0 + hh) * p.M + r) * p.hm.DP + jj;
             *reinterpret_cast<float2*>(o) = make_float2(v0, v1);
           } else if (p.c_f32 != nullptr) {
             float* o = p.c_f32 + (size_t)r * p.ldc + gc;
@@ -417,6 +419,14 @@ bool gemm_tc_shape_ok(int K1, int K2, int lda1, int lda2, int ldw, int N) {
   return K1 > 0 && K1 % 2 == 0 && K2 >= 0 && lda1 % 8 == 0 && (K2 == 0 || lda2 % 8 == 0) && ldw % 8 == 0 && N >= 8;
 }
 
+int hm_n_step(const HeadMajorOut& hm) {
+  // the epilogue stores column pairs, so a tile must start on an even column: DP even keeps every tile start even
+  if (hm.DP <= 0 || hm.DP % 2 != 0 || hm.H <= 0) return 0;
+  for (int hpt = hm.H; hpt >= 1; --hpt)
+    if (hm.H % hpt == 0 && hpt * hm.DP <= 256) return hpt * hm.DP;
+  return 0;
+}
+
 int32_t split_bf16(const float* a, int lda, long long M, int K, void* hi, void* lo, int ldp, cudaStream_t st) {
   if (M <= 0 || K <= 0) return QAGNN_OK;
   if (K % 2 != 0 || lda % 2 != 0) return QAGNN_ERR_UNSUPPORTED;
@@ -438,9 +448,9 @@ int32_t gemm_tc(const TcOperand& A1, const TcOperand& A2, const TcOperand& W, co
   int n_tiles = (N + 255) / 256;  // wgmma N <= 256
   p.n_step = (N + n_tiles - 1) / n_tiles;
   p.n_step = (p.n_step + 15) / 16 * 16;  // even columns per thread pair; half tiles of whole 8-row swizzle groups
-  if (out.hm_buf != nullptr) {  // one `which` (Q / Kx / Mx) per tile: H*DP padded columns
-    p.n_step = out.hm.H * out.hm.DP;
-    if (p.n_step > 256 || p.n_step % 16 != 0 || N % p.n_step != 0) return QAGNN_ERR_UNSUPPORTED;
+  if (out.hm_buf != nullptr) {  // n tiles of whole heads: hpt heads (hpt | H) of DP padded columns each
+    p.n_step = hm_n_step(out.hm);
+    if (p.n_step == 0 || N % p.n_step != 0) return QAGNN_ERR_UNSUPPORTED;
     n_tiles = N / p.n_step;
   }
   // wgmma tile width: the smallest compiled one that covers n_step (208 = the H*DP and D of the QA-GNN shapes)

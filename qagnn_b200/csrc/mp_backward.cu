@@ -320,6 +320,7 @@ int32_t launch_message_passing_backward(const qagnn_shape& s, const int32_t* pre
     case 2: return launch_bwd_h<2>(s, prep_base, pl, combo_order, qkm, ke, me, alpha_s, d_aggr, ds, d_qkm, d_ke, d_me, st);
     case 4: return launch_bwd_h<4>(s, prep_base, pl, combo_order, qkm, ke, me, alpha_s, d_aggr, ds, d_qkm, d_ke, d_me, st);
     case 8: return launch_bwd_h<8>(s, prep_base, pl, combo_order, qkm, ke, me, alpha_s, d_aggr, ds, d_qkm, d_ke, d_me, st);
+    case 16: return launch_bwd_h<16>(s, prep_base, pl, combo_order, qkm, ke, me, alpha_s, d_aggr, ds, d_qkm, d_ke, d_me, st);
     default: return QAGNN_ERR_UNSUPPORTED;
   }
 }

@@ -553,6 +553,8 @@ HeadTilePlan make_plan(const qagnn_shape& s) {
   pl.DP = head_dim_padded(d);
   pl.C = s.R * s.T * s.T + s.T;
   if (pl.DP > 64) return pl;
+  // the projection writes the head-major [3][H][N][DP] input of this kernel; its tensor-core GEMM must take the shape too
+  if (hm_n_step(HeadMajorOut{1, s.D, d, pl.DP, s.H}) == 0) return pl;
   // the 16|16-bit offsets words: tile rows in 16-byte units below 2^15, table rows in 2-byte units below 2^16
   const long nch = pl.DP / 4;
   if ((long)(s.n_per_graph - 1) * nch > 32767 || (long)(pl.C - 1) * nch * 8 > 65535) return pl;

@@ -24,6 +24,8 @@ import torch.nn as nn
 from . import _lib
 from .layers import GELU, MLP, CustomizedEmbedding, MultiheadAttPoolLayer
 
+# head counts GATConvE accepts: every message-passing path (tiled, column-sliced, basic CSR, training backward) runs them
+SUPPORTED_HEAD_COUNTS = (1, 2, 4, 8, 16)
 
 def make_one_hot(labels, C_):
     """int64 [M] -> float32 one-hot [M, C] on labels.device (modeling_qagnn.py:352-367)."""
@@ -210,6 +212,10 @@ class GATConvE(nn.Module):
         super().__init__()
         if aggr != "add":
             raise ValueError("GATConvE only supports aggr='add' (the only mode the reference uses)")
+        if head_count not in SUPPORTED_HEAD_COUNTS:
+            # the general-graph and training kernels are instantiated per head count; the tiled kernel alone would take
+            # any, so another value would work or fail depending on the batch layout
+            raise ValueError(f"head_count must be one of {SUPPORTED_HEAD_COUNTS} (got {head_count})")
         if emb_dim % 2 != 0 or emb_dim % head_count != 0:
             raise ValueError("emb_dim must be even and divisible by head_count")
         self.args = args

@@ -50,7 +50,9 @@ def _worker(rank, world, port, case, out_q):
         logits, _ = D.decoder_forward_sharded(dec, sent_vecs[lo:hi], concept_ids[lo:hi], inp["node_type"][lo:hi],
                                               inp["node_score"][lo:hi], inp["adj_lengths"][lo:hi],
                                               (ei, inp["edge_type"][sel]), world)
-    out_q.put((rank, logits))
+    # by value: a tensor would travel as a file descriptor served by this process, which may have exited by the time the
+    # parent unpickles it
+    out_q.put((rank, logits.numpy()))
     dist.barrier()
     dist.destroy_process_group()
 
@@ -62,7 +64,7 @@ def test_two_rank_shard_and_all_gather_matches_reference_logits():
     q = ctx.Queue()
     procs = [ctx.Process(target=_worker, args=(r, 2, port, case, q)) for r in range(2)]
     [p.start() for p in procs]
-    got = dict(q.get(timeout=120) for _ in range(2))
+    got = {r: torch.from_numpy(a) for r, a in (q.get(timeout=120) for _ in range(2))}
     [p.join(timeout=60) for p in procs]
     assert all(p.exitcode == 0 for p in procs)
     fx = torch.load(os.path.join(os.path.dirname(__file__), "golden", case + ".pt"), weights_only=False)
