@@ -152,11 +152,12 @@ __device__ __forceinline__ void wgmma_bf16<256>(float (&d)[128], uint64_t da, ui
       : "l"(da), "l"(db), "r"(scale_d));
 }
 
-// the three split-bf16 passes (hi*hi, hi*lo, lo*hi) of the four k16-steps of one k block; A / W plane tiles at sa / sw
-template <int BN>
+// the three split-bf16 passes (hi*hi, hi*lo, lo*hi) of the first STEPS k16-steps of one k block; A / W plane tiles at
+// sa / sw.  STEPS is a compile-time count: a run-time one makes ptxas fence every wgmma of the chain.
+template <int BN, int STEPS>
 __device__ __forceinline__ void mma_kblock(float (&acc)[BN / 2], uint32_t sa, uint32_t sw, uint32_t a_bytes, uint32_t w_bytes) {
 #pragma unroll
-  for (int k = 0; k < BK / 16; ++k) {
+  for (int k = 0; k < STEPS; ++k) {
     const uint64_t da_hi = wgmma_desc(sa + k * 32), da_lo = wgmma_desc(sa + a_bytes + k * 32);
     const uint64_t dw_hi = wgmma_desc(sw + k * 32), dw_lo = wgmma_desc(sw + w_bytes + k * 32);
     wgmma_bf16<BN>(acc, da_hi, dw_hi, 1u);
@@ -198,6 +199,9 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
   nkb_seg[0] = (p.kseg[0] + BK - 1) / BK;
   nkb_seg[1] = p.nseg > 1 ? (p.kseg[1] + BK - 1) / BK : 0;
   const int nkb = nkb_seg[0] + nkb_seg[1];
+  // k16 steps of the last k block of each segment: only those that reach its K (the rest would multiply TMA's zero fill)
+  const int tail_steps0 = (p.kseg[0] - 1) % BK / 16 + 1;
+  const int tail_steps1 = nkb_seg[1] > 0 ? (p.kseg[1] - 1) % BK / 16 + 1 : BK / 16;
   const int n_tiles = (p.N + p.n_step - 1) / p.n_step;
   const long long total_tiles = (p.M + BM * CTAS - 1) / (BM * CTAS) * n_tiles;
   const long long cl_id = blockIdx.x / CTAS, n_cl = gridDim.x / CTAS;
@@ -247,6 +251,12 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
     asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
     const int wc = wg - 1;  // rows wc*64 .. wc*64+63 of the tile
     const int warp = tid >> 5, lane = tid & 31;
+    // head-major epilogue: column c = 8j + 2(lane & 3) of a tile is element jj of head hh (c = hh * DP + jj).  The divisions
+    // happen once here; the column loop carries (hh, jj) along.
+    const bool hm_mode = p.c_hm != nullptr;
+    const int DP = hm_mode ? p.hm.DP : 8;
+    const int hh0 = 2 * (lane & 3) / DP, jj0 = 2 * (lane & 3) - hh0 * DP;
+    const int q8 = 8 / DP, r8 = 8 - q8 * DP;
     float acc[BN / 2];
     long long it = 0;
     for (long long tile = cl_id; tile < total_tiles; tile += n_cl) {
@@ -257,12 +267,16 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
         mbar_wait(&full[s], (uint32_t)(it / p.stages) & 1u);
         const uint32_t sbase = smem_u32(smem + (size_t)s * stage_bytes);
         const uint32_t sa = sbase + (uint32_t)wc * 64 * 128, sw = sbase + 2 * a_bytes;
+        const int steps = kb == nkb_seg[0] - 1 ? tail_steps0 : kb == nkb - 1 ? tail_steps1 : BK / 16;
         fence_acc<BN / 2>(acc);
         wgmma_fence();
-        // always all four k16-steps: the tensor map zero-fills A past its K, and a run-time step count makes ptxas fence
-        // every wgmma of the chain
-        mma_kblock<BN>(acc, sa, sw, a_bytes, w_bytes);
-        wgmma_commit();
+        // one compile-time chain per step count, each committing its own group
+        switch (steps) {
+          case 1: mma_kblock<BN, 1>(acc, sa, sw, a_bytes, w_bytes); wgmma_commit(); break;
+          case 2: mma_kblock<BN, 2>(acc, sa, sw, a_bytes, w_bytes); wgmma_commit(); break;
+          case 3: mma_kblock<BN, 3>(acc, sa, sw, a_bytes, w_bytes); wgmma_commit(); break;
+          default: mma_kblock<BN, 4>(acc, sa, sw, a_bytes, w_bytes); wgmma_commit(); break;
+        }
         wgmma_wait_all();
         fence_acc<BN / 2>(acc);
         __syncwarp();
@@ -275,9 +289,8 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
       const int n_tile = (int)(tile % n_tiles);
       const int n0 = n_tile * p.n_step;
       const long long row_g = (tile / n_tiles) * BM * CTAS + rank * BM + wc * 64 + warp * 16 + (lane >> 2);
-      const bool hm_mode = p.c_hm != nullptr;
       // head-major output: the tile's first column starts plane n0 / DP (= which * H + head) of [3][H][N][DP]
-      const int hm_plane0 = hm_mode ? n0 / p.hm.DP : 0;
+      const int hm_plane0 = hm_mode ? n0 / DP : 0;
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const long long r = row_g + 8 * h;
@@ -288,8 +301,14 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
           c = c < 0 ? 0 : (c >= p.n_class ? p.n_class - 1 : c);
           bias_row = p.bias + (size_t)c * p.class_stride;
         }
+        int hh = hh0, jj = jj0;
 #pragma unroll
         for (int j = 0; j < BN / 8; ++j) {
+          if (hm_mode && j > 0) {  // c += 8 = q8 heads + r8 columns, r8 < DP
+            jj += r8;
+            hh += q8;
+            if (jj >= DP) { jj -= DP; ++hh; }
+          }
           const int c = 8 * j + 2 * (lane & 3);  // tile column (even); n_step is even, so c + 1 < n_step too
           const int gc = n0 + c;
           if (c >= p.n_step || gc >= p.N) continue;
@@ -301,9 +320,8 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
           }
           v0 = act_fn<ACT>(v0);
           v1 = act_fn<ACT>(v1);
-          if (hm_mode) {  // tile = whole heads of one `which`: column c is element c % DP of plane hm_plane0 + c / DP
-            const int hh = c / p.hm.DP, jj = c - hh * p.hm.DP;
-            float* o = p.c_hm + ((size_t)(hm_plane0 + hh) * p.M + r) * p.hm.DP + jj;
+          if (hm_mode) {  // tile = whole heads of one `which`: column c is element jj of plane hm_plane0 + hh
+            float* o = p.c_hm + ((size_t)(hm_plane0 + hh) * p.M + r) * DP + jj;
             *reinterpret_cast<float2*>(o) = make_float2(v0, v1);
           } else if (p.c_f32 != nullptr) {
             float* o = p.c_f32 + (size_t)r * p.ldc + gc;
@@ -382,12 +400,25 @@ bool make_map(CUtensorMap* m, const void* base, long long rows, int K, int ld, i
 }
 
 template <int ACT, int BN, int CTAS>
-int32_t launch(const cudaLaunchConfig_t& cfg, const TcParams& p) {
+int32_t launch(cudaLaunchConfig_t cfg, const TcParams& p) {
   static bool attr_set[kMaxDevices] = {false};  // the attribute is per device
+  static int max_clusters[kMaxDevices] = {0};
   const int dev = current_device();
   if (!attr_set[dev]) {
     QAGNN_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<ACT, BN, CTAS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemCap));
     attr_set[dev] = true;
+  }
+  if (CTAS > 1) {
+    // a CTA pair must sit in one GPC, so fewer than #SM / 2 pairs may fit at once; the tiles are walked persistently, and
+    // pairs beyond what is resident would only start as a second wave.  Launch at most the resident count.
+    if (max_clusters[dev] == 0) {
+      cudaLaunchConfig_t q = cfg;
+      int n = 0;
+      QAGNN_CHECK_CUDA(cudaOccupancyMaxActiveClusters(&n, gemm_tc_kernel<ACT, BN, CTAS>, &q));
+      max_clusters[dev] = n > 0 ? n : 1;
+      if (getenv("QAGNN_DEBUG")) fprintf(stderr, "gemm_tc: %d CTA pairs resident at %zu B of shared memory\n", n, cfg.dynamicSmemBytes);
+    }
+    if (cfg.gridDim.x > (unsigned)(max_clusters[dev] * CTAS)) cfg.gridDim.x = (unsigned)(max_clusters[dev] * CTAS);
   }
   QAGNN_CHECK_CUDA(cudaLaunchKernelEx(&cfg, gemm_tc_kernel<ACT, BN, CTAS>, p));
   return QAGNN_OK;

@@ -1,0 +1,172 @@
+#!/usr/bin/env python
+"""Kernel time of every split-bf16 GEMM (`gemm_tc_kernel`) of one cfg2 step, beside its bounds.
+
+    python tools/profile_gemm.py --out DIR [--steps 5]
+
+Runs the benchmark's step (bench.py: cfg2, 320 graphs x 200 nodes x 1000 edges, D = 200, H = 4, k = 5) eagerly under
+torch.profiler with CUDA activities, writes the trace to DIR/gemm_trace.json and prints, per GEMM call of a step:
+the median kernel time over the profiled steps, the data-sheet tensor and HBM bounds computed from the shapes, and the time
+of three cuBLAS BF16 `torch.mm` calls at the same M, N, K (the card's practical tensor ceiling for the three passes).
+The calls are told apart by the template arguments <ACT, BN, CTAS> and, for mlp.3 and Vh/Vx (both <2, 208, CTAS>), by
+launch order.  One JSON line with everything follows the table.
+"""
+import argparse
+import json
+import os
+import re
+import subprocess
+import sys
+
+import torch
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+PEAK_BF16 = 989e12  # H100 SXM data sheet, dense BF16 (700 W card)
+PEAK_HBM = 3.35e12  # H100 SXM data sheet, HBM3
+
+# (M, N, K, output bytes per element) per call of the cfg2 step; K is the GEMM's K (both A segments for Vh/Vx)
+N_NODES, D, H, DP = 64000, 200, 4, 52
+SHAPES = {
+    "emb_score": (N_NODES, D // 2, D // 2, 4),       # bf16 hi + lo planes out
+    "projection": (N_NODES, 3 * H * DP, D + D // 2, 4),  # fp32 head-major [3][H][N][DP] out
+    "mlp.0": (N_NODES, D, D, 4),                     # bf16 hi + lo planes out
+    "mlp.3": (N_NODES, D, D, 4),                     # bf16 hi + lo planes out
+    "Vh/Vx": (N_NODES, D, 2 * D, 4),                 # fp32 out
+}
+ORDER = ["emb_score", "projection", "mlp.0", "mlp.3", "Vh/Vx"]
+
+
+def card():
+    info = {"name": torch.cuda.get_device_name(0)}
+    try:
+        r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                           capture_output=True, text=True, timeout=60)
+        info["nvidia_smi"] = r.stdout.strip().splitlines()[0] if r.stdout.strip() else r.stderr.strip()
+    except (OSError, subprocess.SubprocessError) as exc:
+        info["nvidia_smi"] = f"unavailable: {exc}"
+    return info
+
+
+def label_calls(kernels):
+    """kernels: [(template args, µs)] of one step in launch order -> [(label, µs)]."""
+    out, prev = [], None
+    for (act, bn, _ctas), us in kernels:
+        if act == 0:
+            lab = "projection"
+        elif act == 1:
+            lab = "mlp.0"
+        elif bn == 208 and prev == "mlp.0":
+            lab = "mlp.3"
+        elif bn == 208:
+            lab = "Vh/Vx"
+        else:
+            lab = "emb_score"
+        out.append((lab, us))
+        prev = lab
+    return out
+
+
+def cublas_ceiling_us(M, N, K, reps=20):
+    a = torch.randn(M, K, device="cuda", dtype=torch.bfloat16)
+    b = torch.randn(K, N, device="cuda", dtype=torch.bfloat16)
+    c = torch.empty(M, N, device="cuda", dtype=torch.bfloat16)
+    for _ in range(3):
+        torch.mm(a, b, out=c)
+    torch.cuda.synchronize()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(reps):
+        for _ in range(3):
+            torch.mm(a, b, out=c)
+    e1.record()
+    torch.cuda.synchronize()
+    return e0.elapsed_time(e1) * 1e3 / reps
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--out", required=True, help="directory for the trace")
+    ap.add_argument("--steps", type=int, default=5, help="profiled eager steps")
+    args = ap.parse_args()
+    if not torch.cuda.is_available():
+        raise SystemExit("profile_gemm.py: needs a CUDA device")
+    os.makedirs(args.out, exist_ok=True)
+
+    import bench
+    import qagnn_b200
+    from qagnn_b200.pipeline import DecoderStep
+    from oracle import qagnn_oracle as O
+
+    dev = torch.device("cuda", 0)
+    torch.cuda.set_device(dev)
+    C = bench.CFG
+    inp = bench.synth_step_inputs(0)
+    sd = O.random_state_dict(C["k"], C["D"], C["T"], C["R"], "prod", seed=0)
+    mod = qagnn_b200.QAGNN_Message_Passing(None, C["k"], C["T"], C["R"], C["D"], C["D"], C["D"]).eval()
+    mod.load_state_dict(sd)
+    mod = mod.to(dev)
+    pooler, fc = bench.build_decoder_tail(C["D"], bench.SENT_DIM, dev)
+    d = {k: inp[k].to(dev) for k in DecoderStep.PACKED_FIELDS}
+    max_edges = int((inp["graph_ptr"][1:] - inp["graph_ptr"][:-1]).max())
+    step = DecoderStep(mod, pooler, fc, d, 1, None, use_cuda_graph=False, max_edges=max_edges)
+    for _ in range(3):
+        step.run()
+    torch.cuda.synchronize()
+
+    from torch.profiler import ProfilerActivity, profile
+    with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
+        for _ in range(args.steps):
+            step.run()
+        torch.cuda.synchronize()
+    trace = os.path.join(args.out, "gemm_trace.json")
+    prof.export_chrome_trace(trace)
+
+    pat = re.compile(r"gemm_tc_kernel<(\d+), *(\d+), *(\d+)>")
+    kern = []
+    for e in prof.events():
+        if e.device_type != torch.autograd.DeviceType.CUDA:
+            continue
+        m = pat.search(e.name)
+        if m:
+            kern.append((e.time_range.start, tuple(int(x) for x in m.groups()), e.time_range.elapsed_us()))
+    kern.sort()
+    per_step = len(kern) // args.steps
+    if per_step == 0 or len(kern) % args.steps:
+        raise SystemExit(f"profile_gemm.py: {len(kern)} gemm_tc_kernel launches over {args.steps} steps")
+    times, templ = {}, {}
+    for s in range(args.steps):
+        one = kern[s * per_step:(s + 1) * per_step]
+        for (lab, us), (_, t, _) in zip(label_calls([(t, us) for _, t, us in one]), one):
+            times.setdefault(lab, []).append(us)
+            templ[lab] = t
+
+    rows = []
+    info = card()
+    print(f"card: {info['name']} | nvidia-smi name, power limit, max SM clock: {info['nvidia_smi']}")
+    print(f"{'call':<11} {'<ACT,BN,CTAS>':<14} {'calls/step':>10} {'median µs':>10} {'tensor µs':>10} {'HBM µs':>8} "
+          f"{'cuBLAS 3x µs':>12} {'TFLOP/s-eq':>10}")
+    for lab in ORDER:
+        if lab not in times:
+            continue
+        M, N, K, ob = SHAPES[lab]
+        ts = sorted(times[lab])
+        med = ts[len(ts) // 2]
+        flops = 3 * 2 * M * N * K
+        hbm = M * K * 4 + M * N * ob
+        cub = cublas_ceiling_us(M, N, K)
+        row = dict(call=lab, template=list(templ[lab]), calls_per_step=len(ts) // args.steps, median_us=med,
+                   min_us=ts[0], max_us=ts[-1], M=M, N=N, K=K, flop_equiv=flops, hbm_bytes=hbm,
+                   tensor_bound_us=flops / PEAK_BF16 * 1e6, hbm_bound_us=hbm / PEAK_HBM * 1e6, cublas_3x_us=cub,
+                   tflops_equiv=flops / med / 1e6)
+        rows.append(row)
+        print(f"{lab:<11} {str(tuple(templ[lab])):<14} {row['calls_per_step']:>10} {med:>10.1f} {row['tensor_bound_us']:>10.1f} "
+              f"{row['hbm_bound_us']:>8.1f} {cub:>12.1f} {row['tflops_equiv']:>10.1f}")
+    total = sum(sum(v) for v in times.values()) / args.steps
+    print(f"all gemm_tc_kernel launches: {total:.1f} µs per step ({per_step} launches)")
+    print(json.dumps({"card": info, "gemm_us_per_step": total, "launches_per_step": per_step, "calls": rows,
+                      "trace": trace}))
+
+
+if __name__ == "__main__":
+    main()
