@@ -277,6 +277,14 @@ int32_t layer_forward(const qagnn_shape& s, const FoldLayout& L, const WorkLayou
 // meet TMA's 16-byte rule (D % 8 == 0); else the exact-fp32 FFMA GEMM.  QAGNN_GEMM=ffma forces the latter.
 bool use_tc(const qagnn_shape& s) { return gemm_tc_available() && s.D % 8 == 0; }
 
+// Node MLP on the tensor-core path: the fused one-launch kernel when it takes the width (D <= 208), else mlp.0 and mlp.3 as
+// two GEMMs with the hidden planes in the workspace.  QAGNN_MLP_FUSED=0 forces the two launches (read at every call: tests
+// and A/B runs cover both in one process).
+bool use_mlp_fused(int D) {
+  const char* e = getenv("QAGNN_MLP_FUSED");
+  return !(e && atoi(e) == 0) && mlp_tc_shape_ok(D);
+}
+
 struct Planes {
   const void* hi;
   const void* lo;
@@ -341,6 +349,11 @@ int32_t layer_forward_tc(const qagnn_shape& s, const FoldLayout& L, const WorkLa
     if (!fused_split) QAGNN_RETURN_IF(split_bf16(aggr, D, s.N, D, ws + W.ap_hi, ws + W.ap_lo, D, st));
     TcOperand A{ws + W.ap_hi, ws + W.ap_lo, D, D}, none{nullptr, nullptr, 0, 0};
     TcOperand W1{lb + L.w1_hi, lb + L.w1_lo, D, D}, W2{lb + L.w2_hi, lb + L.w2_lo, D, D};
+    if (use_mlp_fused(D)) {  // one launch, the hidden layer never leaves registers
+      TcOutput o{};
+      o.f32 = out_f32; o.ldc = D; o.hi = out_hi; o.lo = out_lo; o.ldp = out_ldp;
+      return mlp_tc(A, W1, lb + L.b1, W2, lb + L.b2, s.N, final_act, o, st);
+    }
     TcOutput o1{};
     o1.hi = ws + W.mp_hi; o1.lo = ws + W.mp_lo; o1.ldp = D;
     QAGNN_RETURN_IF(gemm_tc(A, none, W1, lb + L.b1, s.N, D, ACT_RELU, o1, st));

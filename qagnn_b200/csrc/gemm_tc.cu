@@ -166,6 +166,19 @@ __device__ __forceinline__ void mma_kblock(float (&acc)[BN / 2], uint32_t sa, ui
   }
 }
 
+// D[64 x N] += A[64 x 16] . B[16 x N], A from registers (the m64nNk16 A fragment: four bf16x2 words), B K-major in shared
+// memory: the second GEMM of the fused MLP (mlp_tc_kernel)
+template <int N>
+__device__ __forceinline__ void wgmma_bf16_rs(float (&d)[N / 2], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint64_t db);
+template <>
+__device__ __forceinline__ void wgmma_bf16_rs<72>(float (&d)[36], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint64_t db) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %41, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n72k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35}, {%36,%37,%38,%39}, %40, p, 1, 1, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35])
+      : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "l"(db), "r"(1u));
+}
+
 // tanh-approximation GELU (utils/layers.py:10-14) with tanh(u) = 1 - 2/(exp(2u)+1) on the fast exp/divide units:
 // ~1e-6 absolute, far inside the parity bar, and ~6 instructions instead of tanhf's ~30
 __device__ __forceinline__ float gelu_tanh_fast(float x) {
@@ -352,6 +365,250 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
   if (CTAS == 2) cluster_sync_all();  // the peer's multicasts and remote arrivals target this CTA: nobody leaves early
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// Fused node MLP:  out = act2( W2 . ReLU(W1 . aggr + b1) + b2 ),  D <= 208, every operand a split-bf16 plane pair.
+//
+// The first GEMM is gemm_tc_kernel's mainloop at BN = 208 (aggr and W1 k blocks through the same ring).  Its accumulator
+// fragment is turned into the hidden layer in place: + b1, ReLU, hi = bf16(v), lo = bf16(v - hi) - the rounding of
+// gemm_tc_kernel's plane epilogue.  The f32 accumulator fragment of m64nNk16 has the layout of the register A fragment of
+// the next m64nNk16, so fragment groups 2t and 2t+1 (columns 16t .. 16t+15) are the four A words of k16 step t.  The second
+// GEMM takes A from those registers and streams W2 through the ring in N chunks of 72 rows (all of K in one ring stage), so
+// only one 36-register accumulator is live beside the 104 hidden words.  Each output element sees the same k16 steps, in
+// the same order and with the same three passes, as the two-launch path (mlp.0 writing the hidden planes, mlp.3 reading them).
+constexpr int kMlpMaxD = 208;                      // hidden width held in registers: 13 k16 steps
+constexpr int kMlpChunk = 72;                      // W2 rows (output columns) per chunk
+// Two warpgroups and no producer warpgroup: 256 threads may hold 255 registers each.  With a third warpgroup (or even one
+// extra warp: registers are split per SM sub-partition) every thread is held to 168 - ptxas allocates against that bound
+// whatever setmaxnreg hands out at run time - and the 104 hidden words, a chunk accumulator and the epilogue spill there.
+// One consumer thread issues the TMA fills instead, `stages` fills ahead of the consumers.
+constexpr int kMlpThreads = 256;
+constexpr uint32_t kW2Sub = kMlpChunk * BK * 2;    // one W2 plane k block of a chunk: 9216 B (a multiple of 1024)
+
+struct MlpParams {
+  CUtensorMap a_hi, a_lo, w1_hi, w1_lo, w2_hi, w2_lo;
+  int D, stages;
+  long long M;
+  const float *b1, *b2;
+  float* c_f32;
+  int ldc;
+  __nv_bfloat16 *c_hi, *c_lo;
+  int ldp;
+};
+
+// hi = bf16(v), lo = bf16(v - hi) of a column pair, packed low column first (the order of a bf16x2 fragment word)
+__device__ __forceinline__ void split_pair(float v0, float v1, uint32_t& hi, uint32_t& lo) {
+  __nv_bfloat162 h2, l2;
+  h2.x = __float2bfloat16_rn(v0);
+  h2.y = __float2bfloat16_rn(v1);
+  l2.x = __float2bfloat16_rn(v0 - __bfloat162float(h2.x));
+  l2.y = __float2bfloat16_rn(v1 - __bfloat162float(h2.y));
+  hi = *reinterpret_cast<uint32_t*>(&h2);
+  lo = *reinterpret_cast<uint32_t*>(&l2);
+}
+
+// the three split-bf16 passes of the first STEPS k16 steps of the hidden layer against one W2 chunk (hi planes at sw, lo
+// planes lo_off further; k block kb of a plane at kb * kW2Sub)
+template <int STEPS>
+__device__ __forceinline__ void mma_chunk(float (&acc)[kMlpChunk / 2], const uint32_t (&hh)[kMlpMaxD / 4],
+                                          const uint32_t (&hl)[kMlpMaxD / 4], uint32_t sw, uint32_t lo_off) {
+#pragma unroll
+  for (int t = 0; t < STEPS; ++t) {
+    const uint32_t off = (uint32_t)(t >> 2) * kW2Sub + (uint32_t)(t & 3) * 32;
+    const uint64_t dw_hi = wgmma_desc(sw + off), dw_lo = wgmma_desc(sw + lo_off + off);
+    wgmma_bf16_rs<kMlpChunk>(acc, hh[4 * t], hh[4 * t + 1], hh[4 * t + 2], hh[4 * t + 3], dw_hi);
+    wgmma_bf16_rs<kMlpChunk>(acc, hh[4 * t], hh[4 * t + 1], hh[4 * t + 2], hh[4 * t + 3], dw_lo);
+    wgmma_bf16_rs<kMlpChunk>(acc, hl[4 * t], hl[4 * t + 1], hl[4 * t + 2], hl[4 * t + 3], dw_hi);
+  }
+}
+
+// Ring fills per 128-row tile: the k blocks of GEMM1 ([aggr hi | aggr lo | W1 hi | W1 lo], as gemm_tc_kernel at BN = 208),
+// then one fill per W2 chunk ([W2 hi kb 0..nkb-1 | W2 lo kb 0..nkb-1], 72 rows each).  Thread 0 issues them.  With CTA
+// pairs each CTA loads half of W1's rows and every other W2 k block, multicast into both.
+template <int ACT, int CTAS>
+__global__ void __launch_bounds__(kMlpThreads, 1) mlp_tc_kernel(const __grid_constant__ MlpParams p) {
+  extern __shared__ __align__(1024) unsigned char smem[];
+  constexpr int BN = kMlpMaxD;
+  constexpr uint32_t a_bytes = BM * BK * 2;
+  constexpr uint32_t w_bytes = BN * BK * 2;
+  constexpr uint32_t stage_bytes = 2 * a_bytes + 2 * w_bytes;
+  static_assert(2 * 4 * kW2Sub <= stage_bytes, "a W2 chunk fills one ring stage");
+  const int wg = threadIdx.x >> 7, tid = threadIdx.x & 127;
+  const uint32_t rank = CTAS == 2 ? cluster_ctarank() : 0u;
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + (size_t)p.stages * stage_bytes);
+  uint64_t* empty = full + p.stages;
+
+  const int D = p.D;
+  const int nkb = (D + BK - 1) / BK;          // k blocks of both GEMMs (K = D)
+  const int tail_steps = (D - 1) % BK / 16 + 1;
+  const int ksteps = (D + 15) / 16;           // k16 steps of GEMM2 = hidden fragment groups in use
+  const int nch = (D + kMlpChunk - 1) / kMlpChunk;
+  const uint32_t chunk_bytes = 2u * (uint32_t)nkb * kW2Sub;
+  const long long total_tiles = (p.M + BM * CTAS - 1) / (BM * CTAS);
+  const long long cl_id = blockIdx.x / CTAS, n_cl = gridDim.x / CTAS;
+
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < p.stages; ++s) {
+      mbar_init(&full[s], 1);
+      mbar_init(&empty[s], 8 * CTAS);
+    }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+  if (CTAS == 2) cluster_sync_all();
+
+  // ---- ring fills: this cluster's tiles, each nkb GEMM1 k blocks then nch W2 chunks; fill f goes to stage f % stages
+  const int fills_per_tile = nkb + nch;
+  const long long n_fills = (cl_id < total_tiles ? (total_tiles - 1 - cl_id) / n_cl + 1 : 0) * fills_per_tile;
+  auto issue = [&](long long f) {
+    const long long tile = cl_id + f / fills_per_tile * n_cl;
+    const int sub = (int)(f % fills_per_tile);
+    unsigned char* st = smem + (size_t)(f % p.stages) * stage_bytes;
+    uint64_t* bar = &full[f % p.stages];
+    if (sub < nkb) {  // GEMM1 k block: [aggr hi | aggr lo | W1 hi | W1 lo]
+      const int kb = sub, m0 = (int)(tile * BM * CTAS + rank * BM);
+      mbar_expect_tx(bar, stage_bytes);
+      tma_load_2d(st, &p.a_hi, kb * BK, m0, bar);
+      tma_load_2d(st + a_bytes, &p.a_lo, kb * BK, m0, bar);
+      if (CTAS == 1) {
+        tma_load_2d(st + 2 * a_bytes, &p.w1_hi, kb * BK, 0, bar);
+        tma_load_2d(st + 2 * a_bytes + w_bytes, &p.w1_lo, kb * BK, 0, bar);
+      } else {
+        const uint32_t half = w_bytes / 2;
+        tma_load_2d_multicast(st + 2 * a_bytes + rank * half, &p.w1_hi, kb * BK, (int)rank * (BN / 2), bar, 3);
+        tma_load_2d_multicast(st + 2 * a_bytes + w_bytes + rank * half, &p.w1_lo, kb * BK, (int)rank * (BN / 2), bar, 3);
+      }
+    } else {  // W2 chunk: [W2 hi kb 0 .. nkb-1 | W2 lo kb 0 .. nkb-1]
+      const int ch = sub - nkb;
+      mbar_expect_tx(bar, chunk_bytes);
+      for (int kb = (int)rank; kb < nkb; kb += CTAS) {
+        unsigned char* hi = st + (size_t)kb * kW2Sub;
+        unsigned char* lo = st + (size_t)(nkb + kb) * kW2Sub;
+        if (CTAS == 1) {
+          tma_load_2d(hi, &p.w2_hi, kb * BK, ch * kMlpChunk, bar);
+          tma_load_2d(lo, &p.w2_lo, kb * BK, ch * kMlpChunk, bar);
+        } else {
+          tma_load_2d_multicast(hi, &p.w2_hi, kb * BK, ch * kMlpChunk, bar, 3);
+          tma_load_2d_multicast(lo, &p.w2_lo, kb * BK, ch * kMlpChunk, bar, 3);
+        }
+      }
+    }
+  };
+  const bool producer = threadIdx.x == 0;
+  if (producer)
+    for (long long f = 0; f < p.stages && f < n_fills; ++f) issue(f);
+  {  // both warpgroups consume: warpgroup wc owns rows wc*64 .. wc*64+63 of the tile
+    const int wc = wg;
+    const int warp = tid >> 5, lane = tid & 31;
+    const int q2 = 2 * (lane & 3);  // fragment column pair 8j + q2
+    long long it = 0;
+    // fill `it` (stage s) is consumed: release it to both CTAs; once every consumer warp of both has, the producer thread
+    // refills the stage with fill it + stages
+    auto release = [&](int s) {
+      __syncwarp();
+      if (lane == 0) {
+        if (CTAS == 1) mbar_arrive_cluster(&empty[s], 0);
+        else { mbar_arrive_cluster(&empty[s], 0); mbar_arrive_cluster(&empty[s], 1); }
+      }
+      if (producer && it + p.stages < n_fills) {
+        mbar_wait(&empty[s], (uint32_t)(it / p.stages) & 1u);
+        issue(it + p.stages);
+      }
+      __syncwarp();
+    };
+    for (long long tile = cl_id; tile < total_tiles; tile += n_cl) {
+      // ---- GEMM1: acc1 = aggr . W1^T over all 208 (zero-padded) hidden columns
+      float acc1[BN / 2];
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc1[i] = 0.f;
+      for (int kb = 0; kb < nkb; ++kb, ++it) {
+        const int s = (int)(it % p.stages);
+        mbar_wait(&full[s], (uint32_t)(it / p.stages) & 1u);
+        const uint32_t sbase = smem_u32(smem + (size_t)s * stage_bytes);
+        const uint32_t sa = sbase + (uint32_t)wc * 64 * 128, sw = sbase + 2 * a_bytes;
+        const int steps = kb == nkb - 1 ? tail_steps : BK / 16;
+        fence_acc<BN / 2>(acc1);
+        wgmma_fence();
+        switch (steps) {
+          case 1: mma_kblock<BN, 1>(acc1, sa, sw, a_bytes, w_bytes); wgmma_commit(); break;
+          case 2: mma_kblock<BN, 2>(acc1, sa, sw, a_bytes, w_bytes); wgmma_commit(); break;
+          case 3: mma_kblock<BN, 3>(acc1, sa, sw, a_bytes, w_bytes); wgmma_commit(); break;
+          default: mma_kblock<BN, 4>(acc1, sa, sw, a_bytes, w_bytes); wgmma_commit(); break;
+        }
+        wgmma_wait_all();
+        fence_acc<BN / 2>(acc1);
+        release(s);
+      }
+      // ---- hidden layer in registers: fragment group j (columns 8j + q2, +1; rows g and g + 8) -> words 2j, 2j + 1
+      uint32_t hh[BN / 4], hl[BN / 4];
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int c = 8 * j + q2;
+        const bool in = c < D;  // columns D .. 207 are exact zeros (D even: c + 1 < D too)
+        const float bb0 = in ? __ldg(p.b1 + c) : 0.f, bb1 = in ? __ldg(p.b1 + c + 1) : 0.f;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          float v0 = acc1[4 * j + 2 * h] + bb0, v1 = acc1[4 * j + 2 * h + 1] + bb1;
+          v0 = in ? act_fn<ACT_RELU>(v0) : 0.f;
+          v1 = in ? act_fn<ACT_RELU>(v1) : 0.f;
+          split_pair(v0, v1, hh[2 * j + h], hl[2 * j + h]);
+        }
+      }
+      // ---- GEMM2 in N chunks, each followed by its epilogue
+      const long long row_g = tile * BM * CTAS + rank * BM + wc * 64 + warp * 16 + (lane >> 2);
+      for (int ch = 0; ch < nch; ++ch, ++it) {
+        const int s = (int)(it % p.stages);
+        float acc2[kMlpChunk / 2];
+#pragma unroll
+        for (int i = 0; i < kMlpChunk / 2; ++i) acc2[i] = 0.f;
+        mbar_wait(&full[s], (uint32_t)(it / p.stages) & 1u);
+        const uint32_t sw = smem_u32(smem + (size_t)s * stage_bytes), lo_off = (uint32_t)nkb * kW2Sub;
+        fence_acc<kMlpChunk / 2>(acc2);
+        wgmma_fence();
+        switch (ksteps) {  // compile-time chains: the hidden words are registers, indexed by the step
+          case 1: mma_chunk<1>(acc2, hh, hl, sw, lo_off); break;
+          case 2: mma_chunk<2>(acc2, hh, hl, sw, lo_off); break;
+          case 3: mma_chunk<3>(acc2, hh, hl, sw, lo_off); break;
+          case 4: mma_chunk<4>(acc2, hh, hl, sw, lo_off); break;
+          case 5: mma_chunk<5>(acc2, hh, hl, sw, lo_off); break;
+          case 6: mma_chunk<6>(acc2, hh, hl, sw, lo_off); break;
+          case 7: mma_chunk<7>(acc2, hh, hl, sw, lo_off); break;
+          case 8: mma_chunk<8>(acc2, hh, hl, sw, lo_off); break;
+          case 9: mma_chunk<9>(acc2, hh, hl, sw, lo_off); break;
+          case 10: mma_chunk<10>(acc2, hh, hl, sw, lo_off); break;
+          case 11: mma_chunk<11>(acc2, hh, hl, sw, lo_off); break;
+          case 12: mma_chunk<12>(acc2, hh, hl, sw, lo_off); break;
+          default: mma_chunk<13>(acc2, hh, hl, sw, lo_off); break;
+        }
+        wgmma_commit();
+        wgmma_wait_all();
+        fence_acc<kMlpChunk / 2>(acc2);
+        release(s);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const long long r = row_g + 8 * h;
+          if (r >= p.M) continue;
+#pragma unroll
+          for (int j = 0; j < kMlpChunk / 8; ++j) {
+            const int gc = ch * kMlpChunk + 8 * j + q2;
+            if (gc >= D) continue;
+            const float v0 = act_fn<ACT>(acc2[4 * j + 2 * h] + __ldg(p.b2 + gc));
+            const float v1 = act_fn<ACT>(acc2[4 * j + 2 * h + 1] + __ldg(p.b2 + gc + 1));
+            if (p.c_f32 != nullptr) *reinterpret_cast<float2*>(p.c_f32 + (size_t)r * p.ldc + gc) = make_float2(v0, v1);
+            if (p.c_hi != nullptr) {
+              uint32_t hi, lo;
+              split_pair(v0, v1, hi, lo);
+              *reinterpret_cast<uint32_t*>(p.c_hi + (size_t)r * p.ldp + gc) = hi;
+              *reinterpret_cast<uint32_t*>(p.c_lo + (size_t)r * p.ldp + gc) = lo;
+            }
+          }
+        }
+      }
+    }
+  }
+  __syncthreads();
+  if (CTAS == 2) cluster_sync_all();
+}
+
 __global__ void split_bf16_kernel(const float* __restrict__ a, int lda, long long M, int K, __nv_bfloat16* __restrict__ hi,
                                   __nv_bfloat16* __restrict__ lo, int ldp) {
   const long long total = M * (long long)(K / 2);
@@ -399,29 +656,43 @@ bool make_map(CUtensorMap* m, const void* base, long long rows, int K, int ld, i
              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-template <int ACT, int BN, int CTAS>
-int32_t launch(cudaLaunchConfig_t cfg, const TcParams& p) {
-  static bool attr_set[kMaxDevices] = {false};  // the attribute is per device
-  static int max_clusters[kMaxDevices] = {0};
+// Launches one persistent instantiation; attr_set / max_clusters are that instantiation's per-device caches.
+template <typename Params>
+int32_t launch_persistent(void (*kernel)(Params), int ctas, cudaLaunchConfig_t cfg, const Params& p, bool* attr_set,
+                          int* max_clusters) {
   const int dev = current_device();
-  if (!attr_set[dev]) {
-    QAGNN_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<ACT, BN, CTAS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemCap));
+  if (!attr_set[dev]) {  // the attribute is per device
+    QAGNN_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemCap));
     attr_set[dev] = true;
   }
-  if (CTAS > 1) {
+  if (ctas > 1) {
     // a CTA pair must sit in one GPC, so fewer than #SM / 2 pairs may fit at once; the tiles are walked persistently, and
     // pairs beyond what is resident would only start as a second wave.  Launch at most the resident count.
     if (max_clusters[dev] == 0) {
       cudaLaunchConfig_t q = cfg;
       int n = 0;
-      QAGNN_CHECK_CUDA(cudaOccupancyMaxActiveClusters(&n, gemm_tc_kernel<ACT, BN, CTAS>, &q));
+      QAGNN_CHECK_CUDA(cudaOccupancyMaxActiveClusters(&n, kernel, &q));
       max_clusters[dev] = n > 0 ? n : 1;
       if (getenv("QAGNN_DEBUG")) fprintf(stderr, "gemm_tc: %d CTA pairs resident at %zu B of shared memory\n", n, cfg.dynamicSmemBytes);
     }
-    if (cfg.gridDim.x > (unsigned)(max_clusters[dev] * CTAS)) cfg.gridDim.x = (unsigned)(max_clusters[dev] * CTAS);
+    if (cfg.gridDim.x > (unsigned)(max_clusters[dev] * ctas)) cfg.gridDim.x = (unsigned)(max_clusters[dev] * ctas);
   }
-  QAGNN_CHECK_CUDA(cudaLaunchKernelEx(&cfg, gemm_tc_kernel<ACT, BN, CTAS>, p));
+  QAGNN_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kernel, p));
   return QAGNN_OK;
+}
+
+template <int ACT, int BN, int CTAS>
+int32_t launch(cudaLaunchConfig_t cfg, const TcParams& p) {
+  static bool attr_set[kMaxDevices] = {false};
+  static int max_clusters[kMaxDevices] = {0};
+  return launch_persistent(gemm_tc_kernel<ACT, BN, CTAS>, CTAS, cfg, p, attr_set, max_clusters);
+}
+
+template <int ACT, int CTAS>
+int32_t launch_mlp(cudaLaunchConfig_t cfg, const MlpParams& p) {
+  static bool attr_set[kMaxDevices] = {false};
+  static int max_clusters[kMaxDevices] = {0};
+  return launch_persistent(mlp_tc_kernel<ACT, CTAS>, CTAS, cfg, p, attr_set, max_clusters);
 }
 
 template <int BN, int CTAS>
@@ -434,6 +705,21 @@ int32_t launch_act(Act act, const cudaLaunchConfig_t& cfg, const TcParams& p) {
 template <int BN>
 int32_t launch_bn(int ctas, Act act, const cudaLaunchConfig_t& cfg, const TcParams& p) {
   return ctas == 2 ? launch_act<BN, 2>(act, cfg, p) : launch_act<BN, 1>(act, cfg, p);
+}
+
+// default: CTA pairs (cluster of 2, W tile multicast, half loaded by each); QAGNN_TC_2CTA=0 -> single CTAs.
+// Read at every call so that a test can cover both in one process.
+int tc_ctas() {
+  const char* e = getenv("QAGNN_TC_2CTA");
+  return (e && atoi(e) == 0) ? 1 : 2;
+}
+
+int32_t sm_count(int* sms) {
+  static int sms_c[kMaxDevices] = {0};
+  const int dev = current_device();
+  if (sms_c[dev] == 0) QAGNN_CHECK_CUDA(cudaDeviceGetAttribute(&sms_c[dev], cudaDevAttrMultiProcessorCount, dev));
+  *sms = sms_c[dev];
+  return QAGNN_OK;
 }
 
 }  // namespace
@@ -491,10 +777,7 @@ int32_t gemm_tc(const TcOperand& A1, const TcOperand& A2, const TcOperand& W, co
   p.nseg = K2 > 0 ? 2 : 1;
   p.kseg[0] = K1;
   p.kseg[1] = K2;
-  // default: CTA pairs (cluster of 2, W tile multicast, half loaded by each); QAGNN_TC_2CTA=0 -> single CTAs.
-  // Read at every call so that a test can cover both in one process.
-  const char* e2 = getenv("QAGNN_TC_2CTA");
-  const int CTAS = (e2 && atoi(e2) == 0) ? 1 : 2;
+  const int CTAS = tc_ctas();
   const size_t stage_bytes = 2 * (size_t)BM * BK * 2 + 2 * (size_t)bn * BK * 2;
   int stages = (int)((kSmemCap - kCtrlBytes) / stage_bytes);
   if (stages > 6) stages = 6;
@@ -517,10 +800,8 @@ int32_t gemm_tc(const TcOperand& A1, const TcOperand& A2, const TcOperand& W, co
   p.c_hi = (__nv_bfloat16*)out.hi;
   p.c_lo = (__nv_bfloat16*)out.lo;
   p.ldp = out.ldp;
-  static int sms_c[kMaxDevices] = {0};
-  const int dev_i = current_device();
-  if (sms_c[dev_i] == 0) QAGNN_CHECK_CUDA(cudaDeviceGetAttribute(&sms_c[dev_i], cudaDevAttrMultiProcessorCount, dev_i));
-  const int sms = sms_c[dev_i];
+  int sms = 0;
+  QAGNN_RETURN_IF(sm_count(&sms));
   const long long total_tiles = (long long)n_tiles * ((M + (long long)BM * CTAS - 1) / ((long long)BM * CTAS));
   const long long units = total_tiles < sms / CTAS ? total_tiles : sms / CTAS;  // CTAs (or CTA pairs) to launch
   const unsigned grid = (unsigned)(units * CTAS);
@@ -543,6 +824,65 @@ int32_t gemm_tc(const TcOperand& A1, const TcOperand& A2, const TcOperand& W, co
   else if (bn == 128) rc = launch_bn<128>(CTAS, act, cfg, p);
   else if (bn == 208) rc = launch_bn<208>(CTAS, act, cfg, p);
   else rc = launch_bn<256>(CTAS, act, cfg, p);
+  QAGNN_RETURN_IF(rc);
+  QAGNN_CHECK_LAUNCH();
+  return QAGNN_OK;
+}
+
+bool mlp_tc_shape_ok(int D) { return D >= 8 && D % 8 == 0 && D <= kMlpMaxD; }
+
+int32_t mlp_tc(const TcOperand& A, const TcOperand& W1, const float* b1, const TcOperand& W2, const float* b2, long long M,
+               Act act2, const TcOutput& out, cudaStream_t st) {
+  if (M <= 0) return QAGNN_OK;
+  if (!gemm_tc_available()) return QAGNN_ERR_UNSUPPORTED;
+  const int D = A.K;
+  if (!mlp_tc_shape_ok(D) || W1.K != D || W2.K != D || b1 == nullptr || b2 == nullptr) return QAGNN_ERR_UNSUPPORTED;
+  if (A.ld % 8 != 0 || W1.ld % 8 != 0 || W2.ld % 8 != 0) return QAGNN_ERR_UNSUPPORTED;
+  if (out.hm_buf != nullptr || out.row_class != nullptr) return QAGNN_ERR_UNSUPPORTED;
+  if ((out.f32 && (out.ldc % 4 != 0)) || (out.hi && (out.ldp % 8 != 0))) return QAGNN_ERR_UNSUPPORTED;
+  const int CTAS = tc_ctas();
+  MlpParams p;
+  memset(&p, 0, sizeof(p));
+  const size_t stage_bytes = 2 * (size_t)BM * BK * 2 + 2 * (size_t)kMlpMaxD * BK * 2;
+  int stages = (int)((kSmemCap - kCtrlBytes) / stage_bytes);
+  if (stages > 6) stages = 6;
+  if (stages < 2) return QAGNN_ERR_UNSUPPORTED;
+  const size_t smem_bytes = stages * stage_bytes + kCtrlBytes;
+  bool ok = make_map(&p.a_hi, A.hi, M, D, A.ld, BM) && make_map(&p.a_lo, A.lo, M, D, A.ld, BM);
+  ok = ok && make_map(&p.w1_hi, W1.hi, D, D, W1.ld, kMlpMaxD / CTAS) && make_map(&p.w1_lo, W1.lo, D, D, W1.ld, kMlpMaxD / CTAS);
+  ok = ok && make_map(&p.w2_hi, W2.hi, D, D, W2.ld, kMlpChunk) && make_map(&p.w2_lo, W2.lo, D, D, W2.ld, kMlpChunk);
+  if (!ok) return QAGNN_ERR_CUDA;
+  p.D = D;
+  p.stages = stages;
+  p.M = M;
+  p.b1 = b1;
+  p.b2 = b2;
+  p.c_f32 = out.f32;
+  p.ldc = out.ldc;
+  p.c_hi = (__nv_bfloat16*)out.hi;
+  p.c_lo = (__nv_bfloat16*)out.lo;
+  p.ldp = out.ldp;
+  int sms = 0;
+  QAGNN_RETURN_IF(sm_count(&sms));
+  const long long total_tiles = (M + (long long)BM * CTAS - 1) / ((long long)BM * CTAS);
+  const long long units = total_tiles < sms / CTAS ? total_tiles : sms / CTAS;
+  cudaLaunchConfig_t cfg;
+  memset(&cfg, 0, sizeof(cfg));
+  cfg.gridDim = dim3((unsigned)(units * CTAS));
+  cfg.blockDim = dim3(kMlpThreads);
+  cfg.dynamicSmemBytes = smem_bytes;
+  cfg.stream = st;
+  cudaLaunchAttribute lattr[1];
+  lattr[0].id = cudaLaunchAttributeClusterDimension;
+  lattr[0].val.clusterDim.x = CTAS;
+  lattr[0].val.clusterDim.y = 1;
+  lattr[0].val.clusterDim.z = 1;
+  cfg.attrs = lattr;
+  cfg.numAttrs = CTAS == 2 ? 1 : 0;
+  if (getenv("QAGNN_DEBUG")) fprintf(stderr, "mlp_tc: M=%lld D=%d act2=%d CTAS=%d stages=%d smem=%zu grid=%u\n", M, D, (int)act2, CTAS, stages, smem_bytes, cfg.gridDim.x);
+  int32_t rc;
+  if (CTAS == 2) rc = act2 == ACT_NONE ? launch_mlp<ACT_NONE, 2>(cfg, p) : act2 == ACT_RELU ? launch_mlp<ACT_RELU, 2>(cfg, p) : launch_mlp<ACT_GELU, 2>(cfg, p);
+  else rc = act2 == ACT_NONE ? launch_mlp<ACT_NONE, 1>(cfg, p) : act2 == ACT_RELU ? launch_mlp<ACT_RELU, 1>(cfg, p) : launch_mlp<ACT_GELU, 1>(cfg, p);
   QAGNN_RETURN_IF(rc);
   QAGNN_CHECK_LAUNCH();
   return QAGNN_OK;

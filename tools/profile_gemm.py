@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Kernel time of every split-bf16 GEMM (`gemm_tc_kernel`) of one cfg2 step, beside its bounds.
+"""Kernel time of every split-bf16 GEMM (`gemm_tc_kernel`, `mlp_tc_kernel`) of one cfg2 step, beside its bounds.
 
     python tools/profile_gemm.py --out DIR [--steps 5]
 
@@ -8,7 +8,10 @@ torch.profiler with CUDA activities, writes the trace to DIR/gemm_trace.json and
 the median kernel time over the profiled steps, the data-sheet tensor and HBM bounds computed from the shapes, and the time
 of three cuBLAS BF16 `torch.mm` calls at the same M, N, K (the card's practical tensor ceiling for the three passes).
 The calls are told apart by the template arguments <ACT, BN, CTAS> and, for mlp.3 and Vh/Vx (both <2, 208, CTAS>), by
-launch order.  One JSON line with everything follows the table.
+launch order.  The step is profiled twice: with the fused node MLP (`mlp_tc_kernel`, one launch per layer) and with
+QAGNN_MLP_FUSED=0 (mlp.0 + mlp.3), so the fused kernel is timed beside the pair at the same shape; the "mlp.0+mlp.3" row
+sums the pair's medians and bounds (the pair also writes and reads back the hidden planes).  One JSON line with everything
+follows the table.
 """
 import argparse
 import json
@@ -34,7 +37,7 @@ SHAPES = {
     "mlp.3": (N_NODES, D, D, 4),                     # bf16 hi + lo planes out
     "Vh/Vx": (N_NODES, D, 2 * D, 4),                 # fp32 out
 }
-ORDER = ["emb_score", "projection", "mlp.0", "mlp.3", "Vh/Vx"]
+ORDER = ["emb_score", "projection", "mlp.0", "mlp.3", "mlp.0+mlp.3", "mlp fused", "Vh/Vx"]
 
 
 def card():
@@ -52,7 +55,9 @@ def label_calls(kernels):
     """kernels: [(template args, µs)] of one step in launch order -> [(label, µs)]."""
     out, prev = [], None
     for (act, bn, _ctas), us in kernels:
-        if act == 0:
+        if bn is None:
+            lab = "mlp fused"
+        elif act == 0:
             lab = "projection"
         elif act == 1:
             lab = "mlp.0"
@@ -110,36 +115,47 @@ def main():
     d = {k: inp[k].to(dev) for k in DecoderStep.PACKED_FIELDS}
     max_edges = int((inp["graph_ptr"][1:] - inp["graph_ptr"][:-1]).max())
     step = DecoderStep(mod, pooler, fc, d, 1, None, use_cuda_graph=False, max_edges=max_edges)
-    for _ in range(3):
-        step.run()
-    torch.cuda.synchronize()
-
     from torch.profiler import ProfilerActivity, profile
-    with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
-        for _ in range(args.steps):
+    pat = re.compile(r"gemm_tc_kernel<(\d+), *(\d+), *(\d+)>")
+    pat_mlp = re.compile(r"mlp_tc_kernel<(\d+), *(\d+)>")
+    times, templ, per_step = {}, {}, {}
+    for fused in ("1", "0"):
+        os.environ["QAGNN_MLP_FUSED"] = fused
+        for _ in range(3):
             step.run()
         torch.cuda.synchronize()
-    trace = os.path.join(args.out, "gemm_trace.json")
-    prof.export_chrome_trace(trace)
-
-    pat = re.compile(r"gemm_tc_kernel<(\d+), *(\d+), *(\d+)>")
-    kern = []
-    for e in prof.events():
-        if e.device_type != torch.autograd.DeviceType.CUDA:
-            continue
-        m = pat.search(e.name)
-        if m:
-            kern.append((e.time_range.start, tuple(int(x) for x in m.groups()), e.time_range.elapsed_us()))
-    kern.sort()
-    per_step = len(kern) // args.steps
-    if per_step == 0 or len(kern) % args.steps:
-        raise SystemExit(f"profile_gemm.py: {len(kern)} gemm_tc_kernel launches over {args.steps} steps")
-    times, templ = {}, {}
-    for s in range(args.steps):
-        one = kern[s * per_step:(s + 1) * per_step]
-        for (lab, us), (_, t, _) in zip(label_calls([(t, us) for _, t, us in one]), one):
-            times.setdefault(lab, []).append(us)
-            templ[lab] = t
+        with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
+            for _ in range(args.steps):
+                step.run()
+            torch.cuda.synchronize()
+        trace = os.path.join(args.out, f"gemm_trace_fused{fused}.json")
+        prof.export_chrome_trace(trace)
+        kern = []
+        for e in prof.events():
+            if e.device_type != torch.autograd.DeviceType.CUDA:
+                continue
+            m, mm = pat.search(e.name), pat_mlp.search(e.name)
+            if m:
+                kern.append((e.time_range.start, tuple(int(x) for x in m.groups()), e.time_range.elapsed_us()))
+            elif mm:
+                act, ctas = (int(x) for x in mm.groups())
+                kern.append((e.time_range.start, (act, None, ctas), e.time_range.elapsed_us()))
+        kern.sort()
+        n = len(kern) // args.steps
+        if n == 0 or len(kern) % args.steps:
+            raise SystemExit(f"profile_gemm.py: {len(kern)} GEMM launches over {args.steps} steps")
+        per_step[fused] = n
+        for s in range(args.steps):
+            one = kern[s * n:(s + 1) * n]
+            for (lab, us), (_, t, _) in zip(label_calls([(t, us) for _, t, us in one]), one):
+                if fused == "0" and lab not in ("mlp.0", "mlp.3"):
+                    continue  # the other calls are the same kernels in both runs: keep the default run's times
+                times.setdefault(lab, []).append(us)
+                templ[lab] = t
+    os.environ.pop("QAGNN_MLP_FUSED", None)
+    if "mlp.0" in times and "mlp.3" in times:  # the pair, call by call
+        times["mlp.0+mlp.3"] = [a + b for a, b in zip(times["mlp.0"], times["mlp.3"])]
+        templ["mlp.0+mlp.3"] = templ["mlp.0"]
 
     rows = []
     info = card()
@@ -149,12 +165,19 @@ def main():
     for lab in ORDER:
         if lab not in times:
             continue
-        M, N, K, ob = SHAPES[lab]
         ts = sorted(times[lab])
         med = ts[len(ts) // 2]
-        flops = 3 * 2 * M * N * K
-        hbm = M * K * 4 + M * N * ob
-        cub = cublas_ceiling_us(M, N, K)
+        if lab in ("mlp.0+mlp.3", "mlp fused"):
+            M, N, K, ob = SHAPES["mlp.0"]
+            flops = 2 * 3 * 2 * M * N * K
+            # the pair moves the hidden planes out and back in; the fused kernel reads aggr and writes x only
+            hbm = 2 * (M * K * 4 + M * N * ob) if lab == "mlp.0+mlp.3" else M * K * 4 + M * N * ob
+            cub = 2 * cublas_ceiling_us(M, N, K)
+        else:
+            M, N, K, ob = SHAPES[lab]
+            flops = 3 * 2 * M * N * K
+            hbm = M * K * 4 + M * N * ob
+            cub = cublas_ceiling_us(M, N, K)
         row = dict(call=lab, template=list(templ[lab]), calls_per_step=len(ts) // args.steps, median_us=med,
                    min_us=ts[0], max_us=ts[-1], M=M, N=N, K=K, flop_equiv=flops, hbm_bytes=hbm,
                    tensor_bound_us=flops / PEAK_BF16 * 1e6, hbm_bound_us=hbm / PEAK_HBM * 1e6, cublas_3x_us=cub,
@@ -162,10 +185,11 @@ def main():
         rows.append(row)
         print(f"{lab:<11} {str(tuple(templ[lab])):<14} {row['calls_per_step']:>10} {med:>10.1f} {row['tensor_bound_us']:>10.1f} "
               f"{row['hbm_bound_us']:>8.1f} {cub:>12.1f} {row['tflops_equiv']:>10.1f}")
-    total = sum(sum(v) for v in times.values()) / args.steps
-    print(f"all gemm_tc_kernel launches: {total:.1f} µs per step ({per_step} launches)")
+    total = sum(sum(times[k]) for k in ORDER if k in times and k not in ("mlp.0", "mlp.3", "mlp.0+mlp.3")) / args.steps
+    print(f"all GEMM launches of the default (fused) step: {total:.1f} µs per step ({per_step['1']} launches; "
+          f"{per_step['0']} with QAGNN_MLP_FUSED=0)")
     print(json.dumps({"card": info, "gemm_us_per_step": total, "launches_per_step": per_step, "calls": rows,
-                      "trace": trace}))
+                      "trace_dir": args.out}))
 
 
 if __name__ == "__main__":
