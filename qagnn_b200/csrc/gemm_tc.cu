@@ -70,11 +70,26 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
         : "memory");
   } while (!done);
 }
-// arrive on the barrier at the same shared-memory offset in CTA `cta` of the cluster (this CTA included)
+// Stage release: arrive on the `empty` barrier at the same shared-memory offset in CTA `cta` of the cluster (CTAS = 1: this
+// CTA's own).  Default (.release.cta) semantics on purpose: the only accesses a release orders are the wgmma reads of the
+// stage, which are complete once wgmma.wait_group has returned, and the refill it unblocks is a TMA write in the async proxy.
+// The .release.cluster form compiles to MEMBAR.ALL.GPU in front of the arrive, which waits for every global store the thread
+// has in flight (the previous tile's epilogue) - on the critical path of every k block.
+template <int CTAS>
 __device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
-  uint32_t remote;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(smem_u32(bar)), "r"(cta));
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
+  if (CTAS == 1) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+  } else {
+    uint32_t remote;
+    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(smem_u32(bar)), "r"(cta));
+    asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
+  }
+}
+// one arrival per warp on `empty` in every CTA of the pair: lane c arrives on CTA c, so both arrivals issue at once
+template <int CTAS>
+__device__ __forceinline__ void release_stage(uint64_t* empty, int lane) {
+  __syncwarp();
+  if (lane < CTAS) mbar_arrive_cluster<CTAS>(empty, (uint32_t)lane);
 }
 __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar) {
   asm volatile(
@@ -292,11 +307,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
         }
         wgmma_wait_all();
         fence_acc<BN / 2>(acc);
-        __syncwarp();
-        if (lane == 0) {
-          if (CTAS == 1) mbar_arrive_cluster(&empty[s], 0);
-          else { mbar_arrive_cluster(&empty[s], 0); mbar_arrive_cluster(&empty[s], 1); }
-        }
+        release_stage<CTAS>(&empty[s], lane);
       }
       // ---- epilogue straight from the accumulator fragment: thread holds rows g, g + 8 and column pairs 8j + 2q
       const int n_tile = (int)(tile % n_tiles);
@@ -504,11 +515,7 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_tc_kernel(const __grid_con
     // fill `it` (stage s) is consumed: release it to both CTAs; once every consumer warp of both has, the producer thread
     // refills the stage with fill it + stages
     auto release = [&](int s) {
-      __syncwarp();
-      if (lane == 0) {
-        if (CTAS == 1) mbar_arrive_cluster(&empty[s], 0);
-        else { mbar_arrive_cluster(&empty[s], 0); mbar_arrive_cluster(&empty[s], 1); }
-      }
+      release_stage<CTAS>(&empty[s], lane);
       if (producer && it + p.stages < n_fills) {
         mbar_wait(&empty[s], (uint32_t)(it / p.stages) & 1u);
         issue(it + p.stages);
