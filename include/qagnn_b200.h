@@ -146,7 +146,16 @@ int32_t qagnn_graph_prep(const int64_t *edge_index, const int64_t *edge_type, co
  * LM_QAGNN.batch_graph, modeling_qagnn.py:244-251, and qagnn_b200.data.pack_adj produce; graph_ptr int64 [N/n_per_graph + 1] on the
  * DEVICE) and max_edges_per_graph bounds their length (host value).  One CTA builds everything for one sub-graph in shared memory:
  * one launch instead of twelve, bit-identical arrays.  QAGNN_ERR_UNSUPPORTED when a sub-graph does not fit one CTA's shared
- * memory (use qagnn_graph_prep); an edge outside its sub-graph's node range sets the same status bit as qagnn_graph_prep. */
+ * memory (use qagnn_graph_prep); an edge outside its sub-graph's node range sets the same status bit as qagnn_graph_prep.
+ *
+ * Edge capacity: shape->E may exceed the batch's edge count.  The real count is graph_ptr[N/n_per_graph], read on the device, so
+ * one set of buffer shapes (and one captured CUDA graph) serves batches with different edge counts.  With E' = graph_ptr[B] + N:
+ *   - columns [graph_ptr[B], E) of edge_index / edge_type are never read;
+ *   - src / tgt / combo hold -1 at those ids; self loops keep the ids E + v, behind every real edge;
+ *   - rowptr_src[N] = rowptr_tgt[N] = E', and every CSR-ordered array is defined at positions below E' only;
+ *   - graph_ptr[B] > E sets a status bit (QAGNN_ERR_INDEX_RANGE with validate) and nothing past E is read.
+ * The forward / training calls take the same shape and touch no entry of the unused ids; alpha_out rows of those ids are 0.
+ * When graph_ptr[B] == E every array is what it was without the capacity rule. */
 int32_t qagnn_graph_prep_packed(const int64_t *edge_index, const int64_t *edge_type, const int64_t *node_type,
                                 const int64_t *graph_ptr, int32_t max_edges_per_graph, const qagnn_shape *shape, void *prep,
                                 size_t prep_bytes, int32_t validate, void *stream);
@@ -204,8 +213,8 @@ int32_t qagnn_mp_core_forward(const qagnn_shape *shape, const void *prep, const 
                               float *aggr, float *alpha_scaled, float *alpha_out, float *scratch, void *stream);
 
 /* Gradient of qagnn_mp_core_forward: given d_aggr [N, D] writes d_qkm [N, 3D], d_ke / d_me [C, D] (zeroed here first).
- * combo_order int32 [E+N]: the by-source edge positions stably sorted by qagnn_prep_layout.csr_src_combo (the caller
- * builds it once per batch).  `scratch` = [E+N, H] floats.  Only dKe / dMe use atomics (a few thousand vector adds). */
+ * combo_order int32 [E']: the by-source edge positions below E' = rowptr_src[N] stably sorted by
+ * qagnn_prep_layout.csr_src_combo (the caller builds it once per batch; E' < E + N under an edge capacity).  `scratch` = [E+N, H] floats.  Only dKe / dMe use atomics (a few thousand vector adds). */
 int32_t qagnn_mp_core_backward(const qagnn_shape *shape, const void *prep, const int32_t *combo_order, const float *qkm,
                                const float *ke, const float *me, const float *alpha_scaled, const float *d_aggr,
                                float *d_qkm, float *d_ke, float *d_me, float *scratch, void *stream);

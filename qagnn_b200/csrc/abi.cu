@@ -214,6 +214,26 @@ __global__ void __launch_bounds__(256) node_feature_fused_kernel(int64_t N, int 
   }
 }
 
+// alpha_out rows of the edge ids [rowptr_src[N] - N, E) are 0: the unused columns of an edge capacity
+// (qagnn_graph_prep_packed).  No row is written when the batch fills E, as every batch the general prep takes does.
+__global__ void zero_alpha_holes_kernel(int64_t N, int64_t E, int H, const int32_t* __restrict__ rowptr_src,
+                                        float* __restrict__ alpha_out) {
+  const int64_t e0 = min(max((int64_t)rowptr_src[N] - N, (int64_t)0), E);
+  for (int64_t i = e0 * H + blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < E * H; i += (int64_t)gridDim.x * blockDim.x)
+    alpha_out[i] = 0.f;
+}
+
+int32_t zero_alpha_holes(const qagnn_shape& s, const void* prep, const qagnn_prep_layout& pl, float* alpha_out,
+                         cudaStream_t st) {
+  if (alpha_out == nullptr || s.E == 0) return QAGNN_OK;
+  int64_t g = (s.E * s.H + 255) / 256;
+  if (g > kNumSMs * 4) g = kNumSMs * 4;
+  zero_alpha_holes_kernel<<<(unsigned)g, 256, 0, st>>>(s.N, s.E, s.H, (const int32_t*)((const char*)prep + pl.rowptr_src),
+                                                        alpha_out);
+  QAGNN_CHECK_LAUNCH();
+  return QAGNN_OK;
+}
+
 int32_t check_shape_fwd(const qagnn_shape* s) {
   if (!s) return QAGNN_ERR_INVALID_ARGUMENT;
   if (s->N <= 0 || s->E < 0 || s->D <= 0 || s->H <= 0 || s->T <= 0 || s->R <= 0 || s->k < 0)
@@ -254,6 +274,7 @@ int32_t layer_forward(const qagnn_shape& s, const FoldLayout& L, const WorkLayou
   }
   {  // logits -> per-source softmax -> out-degree rescale -> per-target sum   (:442, :469-484)
     ProfScope ps(QAGNN_PROF_MESSAGE_PASSING, st);
+    QAGNN_RETURN_IF(zero_alpha_holes(s, prep, pl, alpha_out, st));
     if (tiled) {
       QAGNN_RETURN_IF(launch_message_passing_headtile(s, (const int32_t*)prep, pl, qkm, lb + L.keh, lb + L.meh,
                                                       ws + W.score, ws + W.alpha2, aggr, alpha_out, nullptr, nullptr, st));
@@ -332,6 +353,7 @@ int32_t layer_forward_tc(const qagnn_shape& s, const FoldLayout& L, const WorkLa
   }
   {  // logits -> per-source softmax -> out-degree rescale -> per-target sum   (:442, :469-484)
     ProfScope ps(QAGNN_PROF_MESSAGE_PASSING, st);
+    QAGNN_RETURN_IF(zero_alpha_holes(s, prep, pl, alpha_out, st));
     if (tiled) {
       QAGNN_RETURN_IF(launch_message_passing_headtile(s, (const int32_t*)prep, pl, qkm, lb + L.keh, lb + L.meh,
                                                       ws + W.score, ws + W.alpha2, aggr, alpha_out,
@@ -610,6 +632,7 @@ extern "C" int32_t qagnn_mp_core_forward(const qagnn_shape* shape, const void* p
   QAGNN_RETURN_IF(qagnn_graph_prep_layout(shape->N, shape->E, &pl));
   cudaStream_t st = (cudaStream_t)stream;
   ProfScope ps(QAGNN_PROF_MESSAGE_PASSING, st);
+  QAGNN_RETURN_IF(zero_alpha_holes(*shape, prep, pl, alpha_out, st));
   return launch_message_passing(*shape, (const int32_t*)prep, pl, qkm, ke, me, scratch, alpha_scaled, aggr, alpha_out, st);
 }
 

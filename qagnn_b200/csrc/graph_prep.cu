@@ -329,6 +329,8 @@ __global__ void __launch_bounds__(256) prep_degree_order_kernel(int npg, const i
 // to a sub-graph: ~1200 edges and 200 nodes at cfg2.  One launch instead of twelve; the result is bit-identical to the
 // general pipeline (tests/test_gpu_parity.py) because every array is a function of the stable edge-id order only.
 // Local edge index i: real edges i < e_g (edge id gp[g] + i), then the self loop of local node i - e_g (edge id E + g*n + ...).
+// E may be an edge capacity larger than the batch (see qagnn_graph_prep_packed in include/qagnn_b200.h): every CSR-ordered
+// array then ends at E' = graph_ptr[G] + N, and the positions a sub-graph writes do not depend on E at all.
 struct PackedPrepArgs {
   const int64_t *edge_index, *edge_type, *node_type, *graph_ptr;
   int64_t N, E;
@@ -359,7 +361,15 @@ __global__ void __launch_bounds__(kPackedThreads) prep_packed_graph_kernel(const
   int32_t* inv_t = inv_s + cap;       // [cap]
   __shared__ int hist[256], hbase[256];
 
-  const int64_t g = blockIdx.x;
+  const int64_t g = blockIdx.x, G = gridDim.x;
+  // a.E is the edge CAPACITY of edge_index / edge_type; the batch's edges are the first graph_ptr[G] columns (clamped: a
+  // graph_ptr past the capacity sets bit 16 in the CTA of the last sub-graph below).  The ids of the unused columns keep
+  // src / tgt / combo = -1; the self loops stay at ids E + v, behind every real edge.
+  const int64_t e_real = min(max(a.graph_ptr[G], (int64_t)0), a.E);
+  if (g == G - 1 && tid == 0) { a.rowptr_src[a.N] = (int32_t)(e_real + a.N); a.rowptr_tgt[a.N] = (int32_t)(e_real + a.N); }
+  for (int64_t e = e_real + g * kPackedThreads + tid; e < a.E; e += G * kPackedThreads) {
+    a.src[e] = -1; a.tgt[e] = -1; a.combo[e] = -1;
+  }
   const int64_t e0 = a.graph_ptr[g], e1 = a.graph_ptr[g + 1];
   const int eg = (int)(e1 - e0), ep = eg + n;  // real edges, edges incl. self loops (ep <= cap, checked on the host)
   const int64_t v0 = g * n;
@@ -426,7 +436,6 @@ __global__ void __launch_bounds__(kPackedThreads) prep_packed_graph_kernel(const
     a.rowptr_src[v0 + i] = (int32_t)(base + cnt_s[i]);
     a.rowptr_tgt[v0 + i] = (int32_t)(base + cnt_t[i]);
   }
-  if (g == gridDim.x - 1 && tid == 0) { a.rowptr_src[a.N] = (int32_t)(a.E + a.N); a.rowptr_tgt[a.N] = (int32_t)(a.E + a.N); }
   // unordered fill, then ascending edge order inside every segment (== stable sort by node)
   for (int i = tid; i < ep; i += kPackedThreads) {
     tmp_s[cnt_s[lsrc[i]] + atomicAdd(&cur_s[lsrc[i]], 1)] = i;

@@ -207,7 +207,8 @@ __device__ __forceinline__ void atomic_add4(float* p, const float4& v) {
 }
 
 template <int H, int CH>
-__global__ void __launch_bounds__(256) mp_bwd_table_kernel(int64_t Ep, int D, const int32_t* __restrict__ combo_order,
+__global__ void __launch_bounds__(256) mp_bwd_table_kernel(int64_t N, int D, const int32_t* __restrict__ rowptr_src,
+                                                           const int32_t* __restrict__ combo_order,
                                                            const int32_t* __restrict__ csr_src_tgt,
                                                            const int32_t* __restrict__ csr_src_combo,
                                                            const int32_t* __restrict__ perm_src,
@@ -218,6 +219,8 @@ __global__ void __launch_bounds__(256) mp_bwd_table_kernel(int64_t Ep, int D, co
   const int lane = threadIdx.x & 31;
   const int64_t w = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
   const int64_t i0 = w * kTableRun;
+  // the real E' of the batch: the grid covers E + N, which may be an edge capacity (qagnn_graph_prep_packed)
+  const int64_t Ep = rowptr_src[N];
   if (i0 >= Ep) return;
   const int64_t i1 = min(i0 + (int64_t)kTableRun, Ep);
   const int d = D / H, ld = 3 * D;
@@ -290,7 +293,7 @@ int32_t launch_bwd_hc(const qagnn_shape& s, const int32_t* base, const qagnn_pre
   QAGNN_CHECK_LAUNCH();
   const int64_t runs = (Ep + kTableRun - 1) / kTableRun;
   mp_bwd_table_kernel<H, CH><<<(unsigned)((runs * 32 + block - 1) / block), block, 0, st>>>(
-      Ep, s.D, combo_order, I(pl.csr_src_tgt), I(pl.csr_src_combo), I(pl.perm_src), I(pl.src), qkm, alpha_s, ds, d_aggr, d_ke,
+      s.N, s.D, I(pl.rowptr_src), combo_order, I(pl.csr_src_tgt), I(pl.csr_src_combo), I(pl.perm_src), I(pl.src), qkm, alpha_s, ds, d_aggr, d_ke,
       d_me);
   QAGNN_CHECK_LAUNCH();
   return QAGNN_OK;

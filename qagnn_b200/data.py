@@ -18,7 +18,11 @@ import torch
 class PackedAdj:
     """edge_index int64 [2, total_E] with per-graph node offsets already applied, edge_type int64 [total_E],
     graph_ptr int64 [n_graphs + 1] = first edge of each graph.  When built by FlatAdjCache.pack the two tensors are views
-    of ONE [3, total_E] buffer (`buf`), so the whole adjacency of a batch moves to the device in a single copy."""
+    of ONE [3, total_E] buffer (`buf`), so the whole adjacency of a batch moves to the device in a single copy.
+
+    Packed with an edge capacity K, edge_index / edge_type are [2, K] / [K]: the batch's `n_edges` = graph_ptr[-1] edges
+    fill the first columns and the rest is zero.  Every batch of a split then has the same shapes, and the one-launch
+    graph prep reads the real edge count from graph_ptr on the device (include/qagnn_b200.h, qagnn_graph_prep_packed)."""
     edge_index: torch.Tensor
     edge_type: torch.Tensor
     graph_ptr: torch.Tensor
@@ -27,6 +31,8 @@ class PackedAdj:
 
     graph_ptr_dev: torch.Tensor = None   # graph_ptr on the device of edge_index (packed graph prep, one launch per batch)
     max_edges: int = -1                  # max edges of one sub-graph (host value; -1 = derive from graph_ptr)
+    n_edges: int = -1                    # edges of the batch = graph_ptr[-1] (host value; -1 = unknown)
+    edge_capacity: int = -1              # width of edge_index (host value; -1 = unknown)
 
     def to(self, device, non_blocking=True):
         gp = self.graph_ptr
@@ -36,9 +42,10 @@ class PackedAdj:
         me = self.max_edges if self.max_edges >= 0 else (int((self.graph_ptr[1:] - self.graph_ptr[:-1]).max()) if self.graph_ptr.numel() > 1 else 0)
         if self.buf is not None:
             b = self.buf.to(device, non_blocking=non_blocking)
-            return PackedAdj(b[:2], b[2], self.graph_ptr, self.n_nodes, b, gpd, me)
+            return PackedAdj(b[:2], b[2], self.graph_ptr, self.n_nodes, b, gpd, me, self.n_edges, self.edge_capacity)
         return PackedAdj(self.edge_index.to(device, non_blocking=non_blocking),
-                         self.edge_type.to(device, non_blocking=non_blocking), self.graph_ptr, self.n_nodes, None, gpd, me)
+                         self.edge_type.to(device, non_blocking=non_blocking), self.graph_ptr, self.n_nodes, None, gpd, me,
+                         self.n_edges, self.edge_capacity)
 
     # LM_QAGNN.forward slices inputs positionally and calls .size() only on tensors before the last two; everywhere an
     # (edge_index, edge_type) pair is expected a PackedAdj unpacks / indexes as that pair
@@ -52,22 +59,39 @@ class PackedAdj:
         return 2
 
 
-def pack_adj(edge_index_nested, edge_type_nested, n_nodes, pin=True):
+def _capacity(total, edge_capacity):
+    """Width of a packed batch's edge buffer; raises before anything is copied when the batch does not fit."""
+    if edge_capacity is None:
+        return total
+    if int(edge_capacity) < total:
+        raise ValueError(f"batch has {total} edges, more than the edge capacity {int(edge_capacity)}")
+    return int(edge_capacity)
+
+
+def pack_adj(edge_index_nested, edge_type_nested, n_nodes, pin=True, edge_capacity=None):
     """[batch][num_choice] nested lists (load_sparse_adj_data_with_contextnode format,
-    utils/data_utils.py:189-190) -> PackedAdj, equal to LM_QAGNN.batch_graph's output."""
+    utils/data_utils.py:189-190) -> PackedAdj, equal to LM_QAGNN.batch_graph's output.  With `edge_capacity` K the edges
+    go into one pinned [3, K] buffer with a zero tail (ValueError if the batch has more than K edges)."""
     flat_ei = [e for row in edge_index_nested for e in row] if isinstance(edge_index_nested[0], (list, tuple)) else list(edge_index_nested)
     flat_et = [e for row in edge_type_nested for e in row] if isinstance(edge_type_nested[0], (list, tuple)) else list(edge_type_nested)
     counts = torch.tensor([e.size(1) for e in flat_ei], dtype=torch.long)
     graph_ptr = torch.zeros(len(flat_ei) + 1, dtype=torch.long)
     graph_ptr[1:] = torch.cumsum(counts, 0)
     total = int(graph_ptr[-1])
+    if edge_capacity is not None:
+        K = _capacity(total, edge_capacity)
+        buf = torch.zeros(3, K, dtype=torch.long, pin_memory=pin and torch.cuda.is_available())
+        if total:
+            buf[:2, :total] = torch.cat(flat_ei, dim=1) + torch.repeat_interleave(torch.arange(len(flat_ei)) * n_nodes, counts)
+            buf[2, :total] = torch.cat(flat_et, dim=0)
+        return PackedAdj(buf[:2], buf[2], graph_ptr, n_nodes, buf, n_edges=total, edge_capacity=K)
     edge_index = torch.empty(2, total, dtype=torch.long, pin_memory=pin and torch.cuda.is_available())
     edge_type = torch.empty(total, dtype=torch.long, pin_memory=pin and torch.cuda.is_available())
     if total:
         torch.cat(flat_ei, dim=1, out=edge_index)
         torch.cat(flat_et, dim=0, out=edge_type)
         edge_index += torch.repeat_interleave(torch.arange(len(flat_ei)) * n_nodes, counts).unsqueeze(0)
-    return PackedAdj(edge_index, edge_type, graph_ptr, n_nodes)
+    return PackedAdj(edge_index, edge_type, graph_ptr, n_nodes, n_edges=total, edge_capacity=total)
 
 
 def load_sparse_adj_data_with_contextnode(adj_pk_path, max_node_num, num_choice, args=None, use_cache=True,
@@ -226,6 +250,17 @@ class FlatAdjCache:
     def n_questions(self):
         return self.n_graphs() // self.num_choice
 
+    def max_graph_edges(self):
+        """Edges of the largest sub-graph: a `max_edges` of the packed graph prep that holds for every batch of the split."""
+        return int(np.diff(self.graph_ptr).max()) if self.n_graphs() else 0
+
+    def max_batch_edges(self, batch_size):
+        """Edges of the `batch_size * num_choice` largest sub-graphs together: an edge capacity that holds for every batch
+        of `batch_size` questions, however the split is shuffled."""
+        counts = np.diff(self.graph_ptr)
+        m = min(int(batch_size) * self.num_choice, len(counts))
+        return int(np.sort(counts)[len(counts) - m:].sum()) if m > 0 else 0
+
     def __getitem__(self, i):
         """What LM_QAGNN_DataLoader does with `adj_data` besides handing it to the batch generator
         (modeling_qagnn.py:281-287,307-308): `len(adj_data[0])` must be the number of questions, and `adj_data[:n]` is taken
@@ -243,9 +278,10 @@ class FlatAdjCache:
             return range(self.n_questions())
         raise IndexError("FlatAdjCache stands in for the (edge_index, edge_type) pair: index 0 or 1")
 
-    def pack(self, question_indexes, pin=True):
+    def pack(self, question_indexes, pin=True, edge_capacity=None):
         """PackedAdj of the questions `question_indexes` (all their choices, in order) — equal to
-        LM_QAGNN.batch_graph applied to the corresponding nested-list slice (modeling_qagnn.py:244-251)."""
+        LM_QAGNN.batch_graph applied to the corresponding nested-list slice (modeling_qagnn.py:244-251).  With
+        `edge_capacity` K the buffer is [3, K] with a zero tail (ValueError if the batch has more than K edges)."""
         q = np.asarray(question_indexes, dtype=np.int64).reshape(-1)
         gids = (q[:, None] * self.num_choice + np.arange(self.num_choice)[None, :]).reshape(-1)
         beg, end = self.graph_ptr[gids], self.graph_ptr[gids + 1]
@@ -253,15 +289,17 @@ class FlatAdjCache:
         ptr = np.zeros(len(gids) + 1, dtype=np.int64)
         ptr[1:] = np.cumsum(counts)
         total = int(ptr[-1])
+        K = _capacity(total, edge_capacity)
         # flat positions of every edge of the batch: beg[g] + (0 .. counts[g]-1)
         pos = np.repeat(beg - ptr[:-1], counts) + np.arange(total, dtype=np.int64)
         off = np.repeat(np.arange(len(gids), dtype=np.int64) * self.n_nodes, counts)
-        buf = torch.empty(3, total, dtype=torch.long, pin_memory=pin and torch.cuda.is_available())
+        buf = torch.empty(3, K, dtype=torch.long, pin_memory=pin and torch.cuda.is_available())
         b = buf.numpy()
-        np.add(self.src[pos], off, out=b[0], casting="unsafe")
-        np.add(self.tgt[pos], off, out=b[1], casting="unsafe")
-        b[2] = self.etype[pos]
-        return PackedAdj(buf[:2], buf[2], torch.from_numpy(ptr), self.n_nodes, buf)
+        np.add(self.src[pos], off, out=b[0, :total], casting="unsafe")
+        np.add(self.tgt[pos], off, out=b[1, :total], casting="unsafe")
+        b[2, :total] = self.etype[pos]
+        b[:, total:] = 0
+        return PackedAdj(buf[:2], buf[2], torch.from_numpy(ptr), self.n_nodes, buf, n_edges=total, edge_capacity=K)
 
 
 def load_flat_adj_cache(adj_pk_path, max_node_num, num_choice, args=None):
@@ -287,16 +325,23 @@ class PackedAdjBatchGenerator:
     well, so every copy of a batch is asynchronous.  With nested-list `adj_data` it behaves exactly like the reference."""
 
     def __init__(self, args, mode, device0, device1, batch_size, indexes, qids, labels, tensors0=[], lists0=[], tensors1=[],
-                 lists1=[], adj_data=None, prefetch=0):
+                 lists1=[], adj_data=None, prefetch=0, edge_capacity=None):
         """`prefetch` > 0 (not in the reference): a worker thread slices / packs / pins up to that many batches ahead on the
         host while the consumer trains on the current one; the device copies are still issued by the consuming thread (on
-        ITS current stream), in order, so the batches and their order are exactly those of prefetch=0."""
+        ITS current stream), in order, so the batches and their order are exactly those of prefetch=0.
+
+        `edge_capacity` K (not in the reference; needs a FlatAdjCache): every batch's adjacency is packed into a [3, K]
+        buffer (see PackedAdj), so all full batches have the same shapes and can be written into the buffers of one captured
+        step.  `adj_data.max_batch_edges(batch_size)` is a K that holds for every batch of the split."""
+        if edge_capacity is not None and not isinstance(adj_data, FlatAdjCache):
+            raise ValueError("edge_capacity needs adj_data to be a FlatAdjCache")
         self.args, self.mode = args, mode
         self.device0, self.device1 = device0, device1
         self.batch_size, self.indexes, self.qids, self.labels = batch_size, indexes, qids, labels
         self.tensors0, self.lists0, self.tensors1, self.lists1 = tensors0, lists0, tensors1, lists1
         self.adj_data = adj_data
         self.prefetch = int(prefetch)
+        self.edge_capacity = edge_capacity
 
     def __len__(self):
         return (self.indexes.size(0) - 1) // self.batch_size + 1
@@ -329,7 +374,7 @@ class PackedAdjBatchGenerator:
         lists0 = [self._pin([x[i] for i in batch_indexes], d0) for x in self.lists0]
         lists1 = [self._pin([x[i] for i in batch_indexes], d1) for x in self.lists1]
         if isinstance(self.adj_data, FlatAdjCache):
-            adj = self.adj_data.pack(batch_indexes.numpy())
+            adj = self.adj_data.pack(batch_indexes.numpy(), edge_capacity=self.edge_capacity)
         else:
             edge_index_all, edge_type_all = self.adj_data
             adj = (self._pin([edge_index_all[i] for i in batch_indexes], d1),

@@ -70,9 +70,11 @@ class GraphPrep:
     """Owns the opaque graph-prep workspace of one batched graph (qagnn_graph_prep)."""
 
     def __init__(self, edge_index, edge_type, node_type, n_ntype, n_etype, n_per_graph=0, validate=True,
-                 allow_general_fallback=False, graph_ptr=None, max_edges=-1):
+                 allow_general_fallback=False, graph_ptr=None, max_edges=-1, n_edges=-1):
         """graph_ptr (device int64 [n_graphs + 1]) + max_edges (host int): the batch is PACKED graph by graph — the whole
-        prep is then one kernel launch (qagnn_graph_prep_packed) instead of twelve."""
+        prep is then one kernel launch (qagnn_graph_prep_packed) instead of twelve.  edge_index may then be an edge
+        capacity wider than the batch: the real count graph_ptr[-1] is read on the device.  `n_edges` (host int, -1 =
+        unknown) is that count when the caller knows it; only a fallback to the general prep needs it on the host."""
         lib = _lib.load()
         ei = _lib.i64c(edge_index, "edge_index")
         et = _lib.i64c(edge_type, "edge_type")
@@ -86,14 +88,17 @@ class GraphPrep:
         _lib.check(lib.qagnn_graph_prep_layout(self.N, self.E, C.byref(self.layout)), "qagnn_graph_prep_layout")
         self.buf = torch.empty(self.layout.total_bytes, dtype=torch.uint8, device=self.device)
         self._combo_order = None
+        self.packed = False  # built by qagnn_graph_prep_packed: the edge columns past graph_ptr[-1] are unused
 
         packed = graph_ptr is not None and max_edges >= 0 and self.n_per_graph > 0
+        on_graph_ptr = packed  # the general prep below then reads only the graph_ptr[-1] real columns
         if packed:
             gp = _lib.i64c(graph_ptr, "graph_ptr")
             if gp.numel() != self.N // max(self.n_per_graph, 1) + 1:
                 raise ValueError("graph_ptr must have one entry per sub-graph plus one")
 
         def run():
+            nonlocal ei, et
             shape = _lib.Shape(self.N, self.E, 4, 1, n_ntype, n_etype, 0, self.n_per_graph)
             with torch.cuda.device(self.device):
                 if packed and self.n_per_graph > 0:
@@ -101,7 +106,19 @@ class GraphPrep:
                                                       _lib.ptr(gp), int(max_edges), C.byref(shape), _lib.ptr(self.buf), self.buf.numel(),
                                                       int(bool(validate)), _lib.stream_ptr(self.device))
                     if st_ != -5:  # QAGNN_ERR_UNSUPPORTED: sub-graphs too large for one CTA -> the general pipeline below
+                        self.packed = True
                         return st_
+                if on_graph_ptr:  # the general prep takes every column as an edge: drop the unused tail of an edge capacity
+                    ne = n_edges if n_edges >= 0 else (self.E if torch.cuda.is_current_stream_capturing() else int(gp[-1]))
+                    if not 0 <= ne <= self.E:
+                        raise IndexError(f"graph_ptr[-1] = {ne} is outside the {self.E} columns of edge_index")
+                    if ne < self.E:
+                        ei, et = ei[:, :ne].contiguous(), et[:ne]
+                        self.E = ne
+                        self.layout = _lib.PrepLayout()
+                        _lib.check(lib.qagnn_graph_prep_layout(self.N, self.E, C.byref(self.layout)), "qagnn_graph_prep_layout")
+                        shape.E = ne
+                self.packed = False
                 return lib.qagnn_graph_prep(_lib.ptr(ei) if self.E else None, _lib.ptr(et) if self.E else None, _lib.ptr(nt),
                                             C.byref(shape), _lib.ptr(self.buf), self.buf.numel(), int(bool(validate)),
                                             _lib.stream_ptr(self.device))
@@ -115,15 +132,29 @@ class GraphPrep:
         _lib.check(st, "qagnn_graph_prep")
         self._keep = (ei, et, nt, graph_ptr)
 
+    def real_edges(self):
+        """Edges of the batch (self loops excluded).  Below E only for a packed prep on an edge capacity; read from the
+        device then (synchronising), because graph_ptr lives there."""
+        if not self.packed:
+            return self.E
+        return int(self.array("rowptr_src")[self.N].item()) - self.N
+
+    def compact_edges(self, t):
+        """Rows of an [E+N, ...] edge-id-ordered array without the unused ids [real_edges(), E) of an edge capacity: the
+        [E'+N, ...] array the same batch packed without spare columns gives."""
+        e = self.real_edges()
+        return t if e == self.E else torch.cat([t[:e], t[self.E:]])
+
     def combo_order(self):
-        """int32 [E+N]: by-source edge positions stably sorted by combo (for the backward's edge-table gradient)."""
+        """int32 [E']: by-source edge positions stably sorted by combo (for the backward's edge-table gradient)."""
         if self._combo_order is None:
-            self._combo_order = torch.argsort(self.array("csr_src_combo"), stable=True).to(torch.int32)
+            Ep = self.real_edges() + self.N
+            self._combo_order = torch.argsort(self.array("csr_src_combo")[:Ep], stable=True).to(torch.int32)
         return self._combo_order
 
     def combo_count(self):
         """int64 [C]: number of edges (self loops included) per combo index."""
-        return torch.bincount(self.array("combo").long(), minlength=self.R * self.T * self.T + self.T)
+        return torch.bincount(self.compact_edges(self.array("combo")).long(), minlength=self.R * self.T * self.T + self.T)
 
     def status_word(self):
         """Device-side error bits of the last qagnn_graph_prep on this buffer (0 = all indices in range)."""
@@ -137,8 +168,10 @@ class GraphPrep:
         return self.buf[off:off + 4 * n].view(torch.int32)
 
     def edge_index_prime(self):
-        """edge_index' = [edge_index | self loops] as int64 [2, E+N] (modeling_qagnn.py:436-438)."""
-        return torch.stack([self.array("src"), self.array("tgt")]).long()
+        """edge_index' = [edge_index | self loops] as int64 [2, E+N] (modeling_qagnn.py:436-438); E = real_edges()."""
+        ei = torch.stack([self.array("src"), self.array("tgt")]).long()
+        e = self.real_edges()
+        return ei if e == self.E else torch.cat([ei[:, :e], ei[:, self.E:]], 1)
 
 
 def _edge_encoder_params(enc):
@@ -236,6 +269,13 @@ class GATConvE(nn.Module):
         self._prep_cache = (None, None)
 
     def _prep(self, edge_index, edge_type, node_type):
+        if getattr(edge_index, "graph_ptr_dev", None) is not None:  # a qagnn_b200.data.PackedAdj: one-launch packed prep
+            A = edge_index
+            key = _version_key([A.edge_index, A.edge_type, node_type, A.graph_ptr_dev])
+            if self._prep_cache[0] != key:
+                prep = _packed_graph_prep(A, node_type.reshape(-1), A.n_nodes, self.n_ntype, self.n_etype, self.check_indices)
+                self._prep_cache = (key, prep)
+            return self._prep_cache[1]
         key = _version_key([edge_index, edge_type, node_type])
         if self._prep_cache[0] != key:
             prep = GraphPrep(edge_index, edge_type, node_type, self.n_ntype, self.n_etype, 0, self.check_indices)
@@ -246,7 +286,9 @@ class GATConvE(nn.Module):
                 prep=None, return_aggr=False):
         """x [N, emb_dim]; edge_index [2, E]; edge_type [E]; node_type [N]; node_feature_extra [N, emb_dim].
         Returns out [N, emb_dim], or (out, (edge_index' [2,E+N], alpha [E+N, heads])) with
-        return_attention_weights=True (alpha = softmax before the out-degree rescale, :473)."""
+        return_attention_weights=True (alpha = softmax before the out-degree rescale, :473).  edge_index may be a
+        qagnn_b200.data.PackedAdj (edge_type is then ignored), also one packed at an edge capacity: E is then its real
+        edge count."""
         if self.training:  # dropout-free layer, BatchNorm batch statistics, autograd through the CUDA message passing
             from . import training as TR
             if prep is None:
@@ -281,7 +323,7 @@ class GATConvE(nn.Module):
         self._alpha = None
         res = out
         if return_attention_weights:
-            res = (out, (prep.edge_index_prime(), alpha))
+            res = (out, (prep.edge_index_prime(), prep.compact_edges(alpha)))
         if return_aggr:
             return res, aggr
         return res
@@ -361,7 +403,8 @@ class QAGNN_Message_Passing(nn.Module):
         """Validates the indices of a batch once (synchronising); raises IndexError like forward() with check_indices."""
         n = node_type.size(1) if node_type.dim() == 2 else 0
         GraphPrep(A[0], A[1], node_type.reshape(-1), self.n_ntype, self.n_etype, n, True, allow_general_fallback=True,
-                  graph_ptr=getattr(A, "graph_ptr_dev", None), max_edges=getattr(A, "max_edges", -1))
+                  graph_ptr=getattr(A, "graph_ptr_dev", None), max_edges=getattr(A, "max_edges", -1),
+                  n_edges=getattr(A, "n_edges", -1))
 
     def prepare_graph(self, edge_index, edge_type, node_type):
         """Builds the layer-invariant graph workspace; pass it back via forward(..., prep=) to amortise
@@ -402,7 +445,10 @@ class QAGNN_Message_Passing(nn.Module):
         if self.training:  # dropout, BatchNorm batch statistics, autograd through the CUDA message passing (training.py)
             from . import training as TR
             if prep is None:
-                prep = GraphPrep(A[0], A[1], node_type.reshape(-1), self.n_ntype, self.n_etype, 0, self.check_indices)
+                if getattr(A, "graph_ptr_dev", None) is not None:  # PackedAdj, possibly at an edge capacity
+                    prep = _packed_graph_prep(A, node_type.reshape(-1), H.size(1), self.n_ntype, self.n_etype, self.check_indices)
+                else:
+                    prep = GraphPrep(A[0], A[1], node_type.reshape(-1), self.n_ntype, self.n_etype, 0, self.check_indices)
             return TR.mp_forward_train(self, H, A, node_type, node_score, prep)
         _warn_if_grad_wanted("QAGNN_Message_Passing", H, node_score)
         if self.use_cuda_graph and prep is None and not return_layers:
@@ -419,11 +465,7 @@ class QAGNN_Message_Passing(nn.Module):
             raise ValueError("node_type / node_score must be [batch, n_node(, 1)]")
         edge_index, edge_type = A  # a (edge_index, edge_type) pair, or a qagnn_b200.data.PackedAdj (iterates as that pair)
         if prep is None:
-            gp, me = getattr(A, "graph_ptr_dev", None), getattr(A, "max_edges", -1)
-            if gp is not None and getattr(A, "n_nodes", n) != n:
-                gp = None  # packed for another node count: its graph_ptr still holds, its offsets do not -> general prep
-            prep = GraphPrep(edge_index, edge_type, nt, self.n_ntype, self.n_etype, n, self.check_indices,
-                             allow_general_fallback=True, graph_ptr=gp, max_edges=me)
+            prep = _packed_graph_prep(A, nt, n, self.n_ntype, self.n_etype, self.check_indices)
         self._last_prep = prep
         if prep.N != B * n:
             raise ValueError("graph workspace was built for a different number of nodes")
@@ -440,6 +482,22 @@ class QAGNN_Message_Passing(nn.Module):
         if return_layers:
             return out, layers
         return out
+
+
+def _packed_graph_prep(A, node_type, n, n_ntype, n_etype, validate):
+    """GraphPrep of a batch with n-node sub-graphs: one launch when A is a qagnn_b200.data.PackedAdj packed for n-node
+    sub-graphs, else (or when the packed prep refuses) the general pipeline on the batch's real edge columns."""
+    gp, me = getattr(A, "graph_ptr_dev", None), getattr(A, "max_edges", -1)
+    ne = getattr(A, "n_edges", -1)
+    if gp is not None and getattr(A, "n_nodes", n) != n:
+        # packed for another node count: its graph_ptr still holds, its offsets do not -> general prep on the real columns
+        if ne < 0:
+            ne = int(gp[-1]) if not torch.cuda.is_current_stream_capturing() else A[0].size(1)
+        gp, ei, et = None, A[0][:, :ne], A[1][:ne]
+    else:
+        ei, et = A[0], A[1]
+    return GraphPrep(ei, et, node_type, n_ntype, n_etype, n, validate, allow_general_fallback=True, graph_ptr=gp,
+                     max_edges=me, n_edges=ne)
 
 
 def _mp_forward_graphed(self, H, A, node_type, node_score):

@@ -30,7 +30,11 @@ class DecoderStep:
 
     def __init__(self, gnn, pooler, fc, inputs, world_size=1, group=None, use_cuda_graph=True, max_edges=-1):
         """`inputs` may carry "graph_ptr" (device int64 [B + 1]) with `max_edges` = an upper bound of the edges of one sub-graph
-        for every batch that will be written into these buffers: graph prep is then ONE launch (qagnn_graph_prep_packed)."""
+        for every batch that will be written into these buffers: graph prep is then ONE launch (qagnn_graph_prep_packed).
+        edge_index / edge_type may then be an edge capacity K wider than any batch (qagnn_b200.data.PackedAdj): the real
+        edge count is read from graph_ptr on the device, so one capture serves every batch of a split that fits K and
+        `max_edges`.  A capture raises ValueError if the packed prep refuses the shape, since the general prep would freeze
+        the edge count of the batch it was captured on."""
         self.gnn, self.pooler, self.fc = gnn, pooler, fc
         self.inp = {k: inputs[k] for k in self.FIELDS}
         self.adj = (self.inp["edge_index"], self.inp["edge_type"])
@@ -38,13 +42,15 @@ class DecoderStep:
             from .data import PackedAdj
             self.inp["graph_ptr"] = inputs["graph_ptr"]
             self.adj = PackedAdj(self.inp["edge_index"], self.inp["edge_type"], None, self.inp["H"].size(1), None,
-                                 self.inp["graph_ptr"], int(max_edges))
+                                 self.inp["graph_ptr"], int(max_edges), -1, self.inp["edge_index"].size(1))
         self.world, self.group = world_size, group
         dev = self.inp["H"].device
         B, n, D = self.inp["H"].shape
         S = self.inp["sent_vecs"].size(1)
         self.full = torch.empty(world_size * B, 2 * D + S, device=dev) if world_size > 1 else None
         self.graph = None
+        self._status = None  # (device accumulator, pinned host copy) of graph prep's status word over the replays
+        self._pending = None  # event after the last replay's copy of it
         self.logits = self.pool_attn = self.gnn_out = None
         self.mode = "eager"
         if use_cuda_graph:
@@ -84,22 +90,65 @@ class DecoderStep:
                     self._eager()
             torch.cuda.current_stream(dev).wait_stream(side)
             torch.cuda.synchronize(dev)
+            if "graph_ptr" in self.inp and not self.gnn._last_prep.packed:
+                raise ValueError("DecoderStep: the packed graph prep refuses these sub-graphs (too large for one CTA); a "
+                                 "captured general prep would keep the edge count of this batch for every later one")
+            # batches written into the buffers later are validated without a sync: every replay ORs graph prep's status
+            # word into a device accumulator and copies it to pinned memory, which run() looks at once it has landed
+            status = (torch.zeros(1, dtype=torch.int32, device=dev), torch.zeros(1, dtype=torch.int32).pin_memory())
             graph = torch.cuda.CUDAGraph()
             with torch.cuda.graph(graph):
                 self.logits, self.pool_attn, self.gnn_out = self._eager()
+                if check:
+                    status[0].bitwise_or_(self.gnn._last_prep.status_word())
+                    status[1].copy_(status[0], non_blocking=True)
             self.graph = graph
+            if check:
+                self._status = status
             self._keep = (self.gnn._ws.buf, self.gnn._folded.blob, self.gnn._last_prep)  # addresses baked into the graph
             self.mode = "one CUDA graph (prep + k layers + pooling" + (" + all-gather" if self.world > 1 else "") + " + fc)"
         finally:
             self.gnn.use_cuda_graph, self.gnn.check_indices = saved, check
 
     def run(self):
-        """Enqueues one step on the current stream; returns (logits, pool_attn, gnn_out)."""
+        """Enqueues one step on the current stream; returns (logits, pool_attn, gnn_out).  A replay whose batch had an
+        index out of range (or an edge crossing its sub-graph) raises IndexError at a later call, once the copy of the
+        status word has landed; its results were computed from clamped indices."""
         if self.graph is not None:
+            self._raise_status()
             self.graph.replay()
+            if self._status is not None:
+                self._pending = torch.cuda.Event()
+                self._pending.record()
         else:
             self.logits, self.pool_attn, self.gnn_out = self._eager()
         return self.logits, self.pool_attn, self.gnn_out
+
+    def _raise_status(self):
+        if self._pending is None or not self._pending.query():  # never blocks: the accumulated word is looked at later
+            return
+        self._pending = None
+        accum, host = self._status
+        if int(host.item()) != 0:
+            bits = int(host.item())
+            accum.zero_()
+            host.zero_()
+            raise IndexError("qagnn_b200: a DecoderStep replay saw edge_index / edge_type / node_type values out of range or "
+                             f"crossing a sub-graph boundary (status bits {bits}); its results were computed from clamped indices")
+
+
+def packed_host_batch(adj, H, node_type, node_score, sent_vecs, adj_lengths):
+    """The host-batch dict StreamedRunner(fields=DecoderStep.PACKED_FIELDS) uploads, from one batch of
+    qagnn_b200.data.PackedAdjBatchGenerator (with device "cpu"): `adj` its PackedAdj, packed at an edge capacity so that
+    every batch has the same shapes; node_type / node_score / adj_lengths its [bs, nc, ...] decoder tensors; H [bs*nc, n, D]
+    and sent_vecs [bs*nc, S] the node features and sentence vectors of the same graphs.  Every tensor is pinned."""
+    def pin(t):
+        t = t.contiguous()
+        return t if t.is_pinned() else t.pin_memory()
+    n = H.size(1)
+    return {"H": pin(H), "edge_index": pin(adj.edge_index), "edge_type": pin(adj.edge_type),
+            "node_type": pin(node_type.reshape(-1, n)), "node_score": pin(node_score.reshape(-1, n, 1)),
+            "sent_vecs": pin(sent_vecs), "adj_lengths": pin(adj_lengths.reshape(-1)), "graph_ptr": pin(adj.graph_ptr)}
 
 
 class StreamedRunner:

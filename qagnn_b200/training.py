@@ -129,7 +129,7 @@ def gatconve_train(layer, x, extra, node_type, prep, tab, return_attention_weigh
                                 return_attention_weights)
     out = layer.mlp(aggr)                                                    # :443 (BatchNorm batch statistics)
     if return_attention_weights:
-        return out, (prep.edge_index_prime(), alpha)
+        return out, (prep.edge_index_prime(), prep.compact_edges(alpha))
     return out
 
 
