@@ -219,6 +219,17 @@ int32_t qagnn_mp_core_backward(const qagnn_shape *shape, const void *prep, const
                                const float *ke, const float *me, const float *alpha_scaled, const float *d_aggr,
                                float *d_qkm, float *d_ke, float *d_me, float *scratch, void *stream);
 
+/* What the training path needs per batch besides the prep, without a host synchronisation: a stable counting sort of the
+ * by-source positions [0, E') by qagnn_prep_layout.csr_src_combo, with E' = rowptr_src[N] read on the device (shape->N and
+ * shape->E are those the prep was built with; E may be an edge capacity, see qagnn_graph_prep_packed).
+ *   combo_count_out int64 [C]    number of positions per combo (self loops included), C = R*T*T + T;
+ *   combo_order_out int32 [E+N]  the combo_order of qagnn_mp_core_backward in its first E' entries; the rest is not written.
+ * Positions with equal combo keep ascending order, so both arrays are unique and the same on every run.  `scratch` is
+ * qagnn_combo_sort_bytes(shape) bytes; that query returns 0 for an invalid shape or C > 6144 (QAGNN_ERR_UNSUPPORTED). */
+size_t qagnn_combo_sort_bytes(const qagnn_shape *shape);
+int32_t qagnn_combo_sort(const qagnn_shape *shape, const void *prep, int64_t *combo_count_out, int32_t *combo_order_out,
+                         void *scratch, size_t scratch_bytes, void *stream);
+
 /* A stand-alone dense layer on the same tensor-core path the forward uses (diagnostics / tests):
  *   C[M,N] (ldc) = act( [A1 | A2] @ W^T + bias ),  fp32 row-major operands, W [N, K1+K2] (ldw), act 0/1/2 = none/ReLU/GELU(tanh).
  * Splits the operands into bf16 hi/lo planes in `workspace` and runs the wgmma 3-pass GEMM; returns

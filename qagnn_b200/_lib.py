@@ -63,6 +63,8 @@ EXPORTS = {
     "qagnn_mp_forward": (C.c_int32, [C.POINTER(Shape), _P, _P, _P, _P, _P, _P, _P, _P, C.c_size_t, _P]),
     "qagnn_mp_core_forward": (C.c_int32, [C.POINTER(Shape), _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "qagnn_mp_core_backward": (C.c_int32, [C.POINTER(Shape), _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
+    "qagnn_combo_sort_bytes": (C.c_size_t, [C.POINTER(Shape)]),
+    "qagnn_combo_sort": (C.c_int32, [C.POINTER(Shape), _P, _P, _P, _P, C.c_size_t, _P]),
     "qagnn_linear_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int32, C.c_int32, C.c_int32]),
     "qagnn_linear_bf16x3": (C.c_int32, [_P, C.c_int32, C.c_int32, _P, C.c_int32, C.c_int32, _P, C.c_int32, _P, _P, C.c_int32,
                                         C.c_int64, C.c_int32, C.c_int32, _P, C.c_size_t, _P]),

@@ -190,6 +190,34 @@ int32_t launch_message_passing_backward(const qagnn_shape& s, const int32_t* pre
                                         const float* alpha_s, const float* d_aggr, float* ds, float* d_qkm, float* d_ke,
                                         float* d_me, cudaStream_t st);
 
+// Exclusive scan of one int per thread over a 1024-thread block; *total = the block's sum.  Every thread must call it.
+__device__ __forceinline__ int block_exclusive_scan_1024(int v, int* total) {
+  __shared__ int warp_sums[32];
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  int x = v;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    int y = __shfl_up_sync(0xffffffffu, x, o);
+    if (lane >= o) x += y;
+  }
+  if (lane == 31) warp_sums[wid] = x;
+  __syncthreads();
+  if (wid == 0) {
+    int w = warp_sums[lane];
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      int y = __shfl_up_sync(0xffffffffu, w, o);
+      if (lane >= o) w += y;
+    }
+    warp_sums[lane] = w;
+  }
+  __syncthreads();
+  const int base = wid ? warp_sums[wid - 1] : 0;
+  *total = warp_sums[31];
+  __syncthreads();
+  return base + x - v;
+}
+
 __device__ __forceinline__ float gelu_tanh(float x) {
   // utils/layers.py:10-14
   const float k0 = 0.7978845608028654f;  // sqrt(2/pi)

@@ -80,33 +80,6 @@ __global__ void prep_edges_kernel(const int64_t* __restrict__ edge_index, const 
 }
 
 // ---- 3-phase exclusive scan of two length-N count arrays (blockIdx.y selects the array) ----
-__device__ __forceinline__ int block_exclusive_scan_1024(int v, int* total) {
-  __shared__ int warp_sums[32];
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  int x = v;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    int y = __shfl_up_sync(0xffffffffu, x, o);
-    if (lane >= o) x += y;
-  }
-  if (lane == 31) warp_sums[wid] = x;
-  __syncthreads();
-  if (wid == 0) {
-    int w = warp_sums[lane];
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      int y = __shfl_up_sync(0xffffffffu, w, o);
-      if (lane >= o) w += y;
-    }
-    warp_sums[lane] = w;
-  }
-  __syncthreads();
-  const int base = wid ? warp_sums[wid - 1] : 0;
-  *total = warp_sums[31];
-  __syncthreads();
-  return base + x - v;
-}
-
 __global__ void __launch_bounds__(kScanChunk) scan_block_sums_kernel(const int32_t* __restrict__ cnt_a,
                                                                        const int32_t* __restrict__ cnt_b, int64_t N,
                                                                        int32_t* __restrict__ bsum, int nb) {

@@ -87,7 +87,7 @@ class GraphPrep:
         self.layout = _lib.PrepLayout()
         _lib.check(lib.qagnn_graph_prep_layout(self.N, self.E, C.byref(self.layout)), "qagnn_graph_prep_layout")
         self.buf = torch.empty(self.layout.total_bytes, dtype=torch.uint8, device=self.device)
-        self._combo_order = None
+        self._combo = None
         self.packed = False  # built by qagnn_graph_prep_packed: the edge columns past graph_ptr[-1] are unused
 
         packed = graph_ptr is not None and max_edges >= 0 and self.n_per_graph > 0
@@ -145,16 +145,34 @@ class GraphPrep:
         e = self.real_edges()
         return t if e == self.E else torch.cat([t[:e], t[self.E:]])
 
+    def combo_sort(self):
+        """(combo_count int64 [C], combo_order int32 [E+N]) from qagnn_combo_sort, computed once per prep and without a host
+        synchronisation: E' = rowptr_src[N] is read on the device, and only the first E' entries of combo_order are
+        written.  This is what the training forward and backward use."""
+        if self._combo is None:
+            lib = _lib.load()
+            shape = _lib.Shape(self.N, self.E, 4, 1, self.T, self.R, 0, self.n_per_graph)
+            nbytes = lib.qagnn_combo_sort_bytes(C.byref(shape))
+            if nbytes == 0:
+                raise _lib.QagnnError(f"qagnn_combo_sort_bytes: unsupported shape (T={self.T}, R={self.R})")
+            count = torch.empty(self.R * self.T * self.T + self.T, dtype=torch.int64, device=self.device)
+            order = torch.empty(self.N + self.E, dtype=torch.int32, device=self.device)
+            scratch = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+            with torch.cuda.device(self.device):
+                st = lib.qagnn_combo_sort(C.byref(shape), _lib.ptr(self.buf), _lib.ptr(count), _lib.ptr(order), _lib.ptr(scratch),
+                                          nbytes, _lib.stream_ptr(self.device))
+            _lib.check(st, "qagnn_combo_sort")
+            self._combo = (count, order)
+        return self._combo
+
     def combo_order(self):
-        """int32 [E']: by-source edge positions stably sorted by combo (for the backward's edge-table gradient)."""
-        if self._combo_order is None:
-            Ep = self.real_edges() + self.N
-            self._combo_order = torch.argsort(self.array("csr_src_combo")[:Ep], stable=True).to(torch.int32)
-        return self._combo_order
+        """int32 [E']: by-source edge positions stably sorted by combo (for the backward's edge-table gradient).  Cutting it
+        to E' reads E' from the device for a packed prep (see real_edges); combo_sort() gives the uncut array without that."""
+        return self.combo_sort()[1][:self.real_edges() + self.N]
 
     def combo_count(self):
         """int64 [C]: number of edges (self loops included) per combo index."""
-        return torch.bincount(self.compact_edges(self.array("combo")).long(), minlength=self.R * self.T * self.T + self.T)
+        return self.combo_sort()[0]
 
     def status_word(self):
         """Device-side error bits of the last qagnn_graph_prep on this buffer (0 = all indices in range)."""
@@ -449,6 +467,7 @@ class QAGNN_Message_Passing(nn.Module):
                     prep = _packed_graph_prep(A, node_type.reshape(-1), H.size(1), self.n_ntype, self.n_etype, self.check_indices)
                 else:
                     prep = GraphPrep(A[0], A[1], node_type.reshape(-1), self.n_ntype, self.n_etype, 0, self.check_indices)
+            self._last_prep = prep
             return TR.mp_forward_train(self, H, A, node_type, node_score, prep)
         _warn_if_grad_wanted("QAGNN_Message_Passing", H, node_score)
         if self.use_cuda_graph and prep is None and not return_layers:

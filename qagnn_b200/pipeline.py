@@ -12,10 +12,46 @@ are all graph nodes; inputs and outputs are static device buffers).  With world_
 `QAGNN_Message_Passing`) with the copies on their own CUDA streams: while batch i computes, batch i+1 is uploaded and
 the result of batch i-1 is downloaded (PCIe is full duplex), each batch in one of `depth` device buffer sets.  Every
 batch still pays its own H2D and D2H; they just stop serialising with the kernels.
+
+`TrainStep` is the training counterpart of DecoderStep: QAGNN.forward in .train() and its backward as two CUDA graphs,
+behind one autograd node, for the micro-steps of qagnn.py:252-278.
 """
+import contextlib
+
 import torch
 
 from . import distributed as _dist
+
+
+class StatusWord:
+    """Graph prep's index checks across CUDA-graph replays, without blocking the host.  A replay cannot synchronise to
+    validate a batch, so inside the capture `record(word)` ORs graph prep's status word into a device word and copies that
+    to pinned memory.  `replayed()` marks the end of a replay, and `check()` raises IndexError once the copy of a replay
+    has landed with a bit set: at a later call, never by waiting for the GPU."""
+
+    def __init__(self, device):
+        self.accum = torch.zeros(1, dtype=torch.int32, device=device)
+        self.host = torch.zeros(1, dtype=torch.int32).pin_memory()
+        self.pending = None  # event after the last replay's copy
+
+    def record(self, word):
+        self.accum.bitwise_or_(word)
+        self.host.copy_(self.accum, non_blocking=True)
+
+    def replayed(self):
+        self.pending = torch.cuda.Event()
+        self.pending.record()
+
+    def check(self, what):
+        if self.pending is None or not self.pending.query():  # the accumulated word is looked at again later
+            return
+        self.pending = None
+        bits = int(self.host.item())
+        if bits != 0:
+            self.accum.zero_()
+            self.host.zero_()
+            raise IndexError(f"qagnn_b200: a {what} replay saw edge_index / edge_type / node_type values out of range or "
+                             f"crossing a sub-graph boundary (status bits {bits}); its results were computed from clamped indices")
 
 
 class DecoderStep:
@@ -49,8 +85,7 @@ class DecoderStep:
         S = self.inp["sent_vecs"].size(1)
         self.full = torch.empty(world_size * B, 2 * D + S, device=dev) if world_size > 1 else None
         self.graph = None
-        self._status = None  # (device accumulator, pinned host copy) of graph prep's status word over the replays
-        self._pending = None  # event after the last replay's copy of it
+        self._status = None  # StatusWord of the captured graph prep (None: eager, or check_indices off)
         self.logits = self.pool_attn = self.gnn_out = None
         self.mode = "eager"
         if use_cuda_graph:
@@ -93,15 +128,13 @@ class DecoderStep:
             if "graph_ptr" in self.inp and not self.gnn._last_prep.packed:
                 raise ValueError("DecoderStep: the packed graph prep refuses these sub-graphs (too large for one CTA); a "
                                  "captured general prep would keep the edge count of this batch for every later one")
-            # batches written into the buffers later are validated without a sync: every replay ORs graph prep's status
-            # word into a device accumulator and copies it to pinned memory, which run() looks at once it has landed
-            status = (torch.zeros(1, dtype=torch.int32, device=dev), torch.zeros(1, dtype=torch.int32).pin_memory())
+            # batches written into the buffers later are validated without a sync (StatusWord)
+            status = StatusWord(dev)
             graph = torch.cuda.CUDAGraph()
             with torch.cuda.graph(graph):
                 self.logits, self.pool_attn, self.gnn_out = self._eager()
                 if check:
-                    status[0].bitwise_or_(self.gnn._last_prep.status_word())
-                    status[1].copy_(status[0], non_blocking=True)
+                    status.record(self.gnn._last_prep.status_word())
             self.graph = graph
             if check:
                 self._status = status
@@ -115,26 +148,208 @@ class DecoderStep:
         index out of range (or an edge crossing its sub-graph) raises IndexError at a later call, once the copy of the
         status word has landed; its results were computed from clamped indices."""
         if self.graph is not None:
-            self._raise_status()
+            if self._status is not None:
+                self._status.check("DecoderStep")
             self.graph.replay()
             if self._status is not None:
-                self._pending = torch.cuda.Event()
-                self._pending.record()
+                self._status.replayed()
         else:
             self.logits, self.pool_attn, self.gnn_out = self._eager()
         return self.logits, self.pool_attn, self.gnn_out
 
-    def _raise_status(self):
-        if self._pending is None or not self._pending.query():  # never blocks: the accumulated word is looked at later
-            return
-        self._pending = None
-        accum, host = self._status
-        if int(host.item()) != 0:
-            bits = int(host.item())
-            accum.zero_()
-            host.zero_()
-            raise IndexError("qagnn_b200: a DecoderStep replay saw edge_index / edge_type / node_type values out of range or "
-                             f"crossing a sub-graph boundary (status bits {bits}); its results were computed from clamped indices")
+
+class _TrainReplay(torch.autograd.Function):
+    """The captured forward and backward of a TrainStep as one autograd node.  Gradient accumulation into `.grad` stays in
+    autograd, outside the graphs.  The backward hands out the static gradient buffers themselves: autograd then copies
+    them into a `.grad` that is still None instead of adopting them, which the next replay would overwrite."""
+
+    @staticmethod
+    def forward(ctx, step, sent_vecs, node_scores, *params):
+        for static, given in ((step._sv, sent_vecs), (step._ns, node_scores)):
+            if static.data_ptr() != given.data_ptr():
+                static.copy_(given)
+        step._fwd.replay()
+        ctx.step = step
+        logits, pool_attn = step._logits.detach(), step._pool_attn.detach()
+        ctx.mark_non_differentiable(pool_attn)
+        return logits, pool_attn
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, d_logits, _d_pool_attn):
+        step = ctx.step
+        step._g_logits.copy_(d_logits)
+        step._bwd.replay()
+        return (None,) + tuple(g if need else None for g, need in zip(step._grads, ctx.needs_input_grad[1:]))
+
+
+class TrainStep:
+    """QAGNN.forward in .train() and its backward, each replayed as one CUDA graph: the training counterpart of DecoderStep
+    for the loop body of qagnn.py:252-278, on packed batches at a fixed edge capacity K
+    (qagnn_b200.data.PackedAdjBatchGenerator(..., edge_capacity=K)):
+
+        sent_vecs, _ = model.encoder(*lm_inputs)                                    # eager
+        logits, pool_attn = step(sent_vecs, concept_ids, node_type_ids, node_scores, adj_lengths, packed_adj)
+        loss = compute_loss(logits.view(bs, nc), labels)
+        scaler.scale(loss).backward()     # replays the backward graph; dL/dsent_vecs flows on into the encoder
+
+    Every call copies its batch into static buffers, so a batch with any edge count up to K and sub-graphs of at most
+    `max_edges` edges replays the same two graphs; a larger batch raises ValueError before anything is copied.  Parameter
+    gradients accumulate into `.grad` as in eager mode; dL/dsent_vecs reaches `sent_vecs`, and dL/dnode_scores reaches
+    `node_scores` when it requires grad.  `pool_attn` is returned without a gradient.  Both outputs are static buffers that
+    the next call overwrites.  Dropout draws a new mask on every replay and BatchNorm running statistics advance on every
+    replay, as in eager mode.  `autocast_dtype` (None or torch.float16) runs capture and calls under
+    torch.autocast(cache_enabled=False); the message passing keeps fp32 inside.  Construction runs two warm-up iterations
+    and restores the buffers, `.grad` and the CUDA RNG state it found.
+
+    Out-of-range indices in a later batch raise IndexError at a later call, as with DecoderStep, without blocking the host;
+    that batch's results were computed from clamped indices.  The graphs hold the addresses of the parameters and buffers:
+    in-place optimiser steps and load_state_dict keep them, `.to()` / `.cuda()` / `.half()` do not, and a call after one
+    raises RuntimeError (build a new TrainStep).  `use_cuda_graph=False` runs the same code eagerly."""
+
+    def __init__(self, decoder, sent_vecs, concept_ids, node_type_ids, node_scores, adj_lengths, packed_adj, *, max_edges,
+                 edge_capacity=None, autocast_dtype=None, use_cuda_graph=True):
+        """The example batch (device tensors with the shapes of every later batch, valid indices, `packed_adj` a PackedAdj)
+        sizes the static buffers and is what warm-up and capture run on.  `edge_capacity` K defaults to the width of
+        packed_adj's edge buffer; `max_edges` bounds the edges of one sub-graph over the whole split
+        (FlatAdjCache.max_graph_edges())."""
+        if autocast_dtype not in (None, torch.float16):
+            raise ValueError("autocast_dtype must be None or torch.float16")
+        if not decoder.training:
+            raise ValueError("TrainStep captures the training forward: call decoder.train() first")
+        self.decoder, self.autocast_dtype = decoder, autocast_dtype
+        dev = node_type_ids.device
+        B, n = node_type_ids.shape
+        K = int(edge_capacity) if edge_capacity is not None else packed_adj.edge_index.size(1)
+        self.edge_capacity, self.max_edges = K, int(max_edges)
+        self._sv = sent_vecs.detach().clone().requires_grad_(True)
+        self._ns = node_scores.detach().clone().requires_grad_(True)
+        self._cid, self._nt, self._al = concept_ids.clone(), node_type_ids.clone(), adj_lengths.clone()
+        self._edges = torch.zeros(3, K, dtype=torch.int64, device=dev)
+        self._gp = torch.zeros(B + 1, dtype=torch.int64, device=dev)
+        from .data import PackedAdj
+        self._adj = PackedAdj(self._edges[:2], self._edges[2], None, n, self._edges, self._gp, self.max_edges, -1, K)
+        self._copy_batch(sent_vecs, concept_ids, node_type_ids, node_scores, adj_lengths, packed_adj)
+        self._fwd = self._status = None
+        self.mode = "eager"
+        if use_cuda_graph:
+            self._capture()
+
+    def _autocast(self):
+        if self.autocast_dtype is None:
+            return contextlib.nullcontext()
+        return torch.autocast("cuda", dtype=self.autocast_dtype, cache_enabled=False)
+
+    def _copy_batch(self, sent_vecs, concept_ids, node_type_ids, node_scores, adj_lengths, adj):
+        for name, t, static in (("sent_vecs", sent_vecs, self._sv), ("concept_ids", concept_ids, self._cid),
+                                ("node_type_ids", node_type_ids, self._nt), ("node_scores", node_scores, self._ns),
+                                ("adj_lengths", adj_lengths, self._al)):
+            if t.shape != static.shape or t.dtype != static.dtype:
+                raise ValueError(f"TrainStep: {name} is {tuple(t.shape)} {t.dtype}, the step was built for "
+                                 f"{tuple(static.shape)} {static.dtype}")
+        gp = adj.graph_ptr if adj.graph_ptr is not None else adj.graph_ptr_dev
+        gp = gp.cpu() if gp.is_cuda else gp  # PackedAdj keeps graph_ptr on the host: no synchronisation
+        if gp.numel() != self._gp.numel():
+            raise ValueError(f"TrainStep: graph_ptr has {gp.numel()} entries, the step was built for {self._gp.numel()}")
+        ne = adj.n_edges if adj.n_edges >= 0 else int(gp[-1])
+        if ne > self.edge_capacity:
+            raise ValueError(f"TrainStep: batch has {ne} edges, more than the edge capacity {self.edge_capacity}")
+        me = int((gp[1:] - gp[:-1]).max()) if gp.numel() > 1 else 0
+        if me > self.max_edges:
+            raise ValueError(f"TrainStep: a sub-graph has {me} edges, more than max_edges = {self.max_edges}")
+        for static, t in ((self._cid, concept_ids), (self._nt, node_type_ids), (self._al, adj_lengths)):
+            static.copy_(t, non_blocking=True)
+        if adj.buf is not None and adj.buf.shape == self._edges.shape:
+            self._edges.copy_(adj.buf, non_blocking=True)
+        elif ne > 0:
+            self._edges[:2, :ne].copy_(adj.edge_index[:, :ne], non_blocking=True)
+            self._edges[2, :ne].copy_(adj.edge_type[:ne], non_blocking=True)
+        self._gp.copy_(adj.graph_ptr_dev if adj.graph_ptr_dev is not None else gp, non_blocking=True)
+
+    def _forward(self, sent_vecs, node_scores):
+        logits, pool_attn = self.decoder(sent_vecs, self._cid, self._nt, node_scores, self._al, self._adj)
+        if self._status is not None:
+            self._status.record(self.decoder.gnn._last_prep.status_word())
+        return logits, pool_attn
+
+    def _addresses(self):
+        return tuple(t.data_ptr() for t in self._params + self._buffers)
+
+    def _capture(self):
+        dec, gnn = self.decoder, self.decoder.gnn
+        dev = self._nt.device
+        self._params = [p for p in dec.parameters() if p.requires_grad]
+        self._buffers = list(dec.buffers())
+        inputs = [self._sv, self._ns] + self._params
+        check = gnn.check_indices
+        if check:  # validate once, eagerly (a synchronising call), before trusting the capture
+            gnn.check_batch(self._adj, self._nt)
+        # the warm-up iterations really run: BatchNorm statistics, RNG offsets and .grad are put back afterwards
+        buffers = [b.detach().clone() for b in self._buffers]
+        grads = [None if p.grad is None else p.grad.detach().clone() for p in self._params]
+        rng = torch.cuda.get_rng_state(dev)
+        gnn.check_indices = False
+        status = StatusWord(dev) if check else None
+        try:
+            cur = torch.cuda.current_stream(dev)
+            side = torch.cuda.Stream(device=dev)
+            side.wait_stream(cur)
+            with torch.cuda.stream(side):
+                for _ in range(2):  # sizes the allocations, loads the kernels, builds the cached tables
+                    with self._autocast():
+                        logits, _ = self._forward(self._sv, self._ns)
+                    torch.autograd.grad(logits, inputs, torch.ones_like(logits), allow_unused=True)
+            cur.wait_stream(side)
+            if not gnn._last_prep.packed:
+                raise ValueError("TrainStep: the packed graph prep refuses these sub-graphs (too large for one CTA); a "
+                                 "captured general prep would keep the edge count of this batch for every later one")
+            self._status = status
+            pool = torch.cuda.graph_pool_handle()
+            fwd, bwd = torch.cuda.CUDAGraph(), torch.cuda.CUDAGraph()
+            with torch.cuda.graph(fwd, pool=pool):
+                with self._autocast():
+                    logits, pool_attn = self._forward(self._sv, self._ns)
+            self._g_logits = torch.empty_like(logits)
+            with torch.cuda.graph(bwd, pool=pool):
+                self._grads = torch.autograd.grad(logits, inputs, self._g_logits, allow_unused=True)
+            self._logits, self._pool_attn = logits.detach(), pool_attn.detach()
+            self._fwd, self._bwd = fwd, bwd
+            self._bn_buffers = [b for m in dec.modules() if isinstance(m, torch.nn.modules.batchnorm._BatchNorm)
+                                for b in (m.running_mean, m.running_var, m.num_batches_tracked) if b is not None]
+            self._ptrs = self._addresses()
+            self.mode = "two CUDA graphs (forward + backward)"
+        except BaseException:
+            self._status = None
+            raise
+        finally:
+            gnn.check_indices = check
+            with torch.no_grad():
+                for b, s in zip(self._buffers, buffers):
+                    b.copy_(s)
+            for p, g in zip(self._params, grads):
+                p.grad = g
+            torch.cuda.set_rng_state(rng, dev)
+
+    def __call__(self, sent_vecs, concept_ids, node_type_ids, node_scores, adj_lengths, packed_adj):
+        """Returns (logits [B, 1], pool_attn) of one micro-batch; `.backward()` through logits replays the backward graph."""
+        if self._fwd is not None:
+            if not self.decoder.training:
+                raise RuntimeError("TrainStep replays the training forward: call decoder.train() first")
+            if self._addresses() != self._ptrs:
+                raise RuntimeError("TrainStep: the decoder's parameters or buffers moved since capture (.to() / .cuda() / "
+                                   ".half()?); the graphs would read the old addresses. Build a new TrainStep.")
+            if self._status is not None:
+                self._status.check("TrainStep")
+        self._copy_batch(sent_vecs, concept_ids, node_type_ids, node_scores, adj_lengths, packed_adj)
+        with self._autocast():
+            if self._fwd is None:
+                return self._forward(sent_vecs, node_scores)
+            out = _TrainReplay.apply(self, sent_vecs, node_scores, *self._params)
+        if self._status is not None:
+            self._status.replayed()
+        # the replay changed the running statistics behind autograd's back: the eval path's folded weights key on versions
+        torch.autograd.graph.increment_version(self._bn_buffers)
+        return out
 
 
 def packed_host_batch(adj, H, node_type, node_score, sent_vecs, adj_lengths):

@@ -18,6 +18,7 @@ edge's combo, so the batch mean / variance are the combo-histogram-weighted mome
 statistics receive the k momentum updates the reference's k calls of the shared module apply.
 """
 import ctypes as C
+import functools
 
 import torch
 import torch.nn.functional as F
@@ -25,9 +26,11 @@ import torch.nn.functional as F
 from . import _lib
 
 
+@functools.lru_cache(maxsize=None)
 def combo_onehot_table(n_ntype, n_etype, device):
     """[C, R+1+2T] one-hot edge-feature rows, one per combo index used by graph prep
-    (c = (etype*T + type_src)*T + type_tgt for real edges, R*T*T + type for the self loop; modeling_qagnn.py:419-432)."""
+    (c = (etype*T + type_src)*T + type_tgt for real edges, R*T*T + type for the self loop; modeling_qagnn.py:419-432).
+    A constant: built once per (T, R, device) and shared, so a training step does not rebuild it (callers only read it)."""
     T, R = n_ntype, n_etype
     Cn = R * T * T + T
     c = torch.arange(Cn, device=device)
@@ -56,7 +59,7 @@ def edge_table_train(enc, onehot_tab, combo_count, k_calls):
         if bn.track_running_stats and bn.running_mean is not None:
             m = bn.momentum if bn.momentum is not None else 0.1
             keep = (1.0 - m) ** k_calls
-            unbiased = var * (n / (n - 1.0)) if float(n) > 1 else var
+            unbiased = torch.where(n > 1, var * (n / (n - 1.0)), var)  # tensor ops: no host synchronisation
             bn.running_mean.mul_(keep).add_(mean * (1.0 - keep))
             bn.running_var.mul_(keep).add_(unbiased * (1.0 - keep))
             bn.num_batches_tracked += k_calls
@@ -104,7 +107,7 @@ class _MPCore(torch.autograd.Function):
         d_qkm = torch.empty_like(qkm)
         d_ke, d_me = torch.empty_like(ke), torch.empty_like(me)
         scratch = torch.empty(N + E, H, dtype=torch.float32, device=dev)
-        order = ctx.prep.combo_order()
+        order = ctx.prep.combo_sort()[1]  # device-side E': valid under an edge capacity without a host read
         with torch.cuda.device(dev):
             st = lib.qagnn_mp_core_backward(C.byref(shape), _lib.ptr(ctx.prep.buf), _lib.ptr(order), _lib.ptr(qkm), _lib.ptr(ke),
                                             _lib.ptr(me), _lib.ptr(alpha_s), _lib.ptr(g), _lib.ptr(d_qkm), _lib.ptr(d_ke),
