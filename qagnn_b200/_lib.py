@@ -134,7 +134,11 @@ def profile_read():
 
 
 class QagnnError(RuntimeError):
-    pass
+    """A library call failed; `status` is its return code (a key of STATUS) when there is one."""
+
+    def __init__(self, msg, status=None):
+        super().__init__(msg)
+        self.status = status
 
 
 def check(status, what):
@@ -145,7 +149,7 @@ def check(status, what):
             msg += ": " + lib.qagnn_last_cuda_error().decode()
         if status == -3:
             raise IndexError(f"{what}: {msg}")
-        raise QagnnError(f"{what}: {msg} (status {status})")
+        raise QagnnError(f"{what}: {msg} (status {status})", status)
 
 
 def ptr(t):

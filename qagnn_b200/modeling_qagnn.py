@@ -66,15 +66,28 @@ class _DeviceBlob:
         return self.buf
 
 
+CROSS_GRAPH = 8  # graph prep status bit: an edge crosses a sub-graph boundary
+
+
+class GraphPrepIndexError(IndexError):
+    """Indices a validating graph prep found out of range.  `bits` is its status word: 1 edge_index, 2 edge_type,
+    4 node_type, CROSS_GRAPH, 16 graph_ptr disagreeing with the edges or with max_edges."""
+
+    def __init__(self, bits):
+        super().__init__(f"qagnn_graph_prep: index out of range (status bits {bits})")
+        self.bits = bits
+
+
 class GraphPrep:
     """Owns the opaque graph-prep workspace of one batched graph (qagnn_graph_prep)."""
 
-    def __init__(self, edge_index, edge_type, node_type, n_ntype, n_etype, n_per_graph=0, validate=True,
-                 allow_general_fallback=False, graph_ptr=None, max_edges=-1, n_edges=-1):
+    def __init__(self, edge_index, edge_type, node_type, n_ntype, n_etype, n_per_graph=0, validate=True, graph_ptr=None,
+                 max_edges=-1):
         """graph_ptr (device int64 [n_graphs + 1]) + max_edges (host int): the batch is PACKED graph by graph — the whole
         prep is then one kernel launch (qagnn_graph_prep_packed) instead of twelve.  edge_index may then be an edge
-        capacity wider than the batch: the real count graph_ptr[-1] is read on the device.  `n_edges` (host int, -1 =
-        unknown) is that count when the caller knows it; only a fallback to the general prep needs it on the host."""
+        capacity wider than the batch: the real count graph_ptr[-1] is read on the device.  That prep raises QagnnError
+        with status -5 when it refuses the shape (sub-graphs too large for one CTA).  Without graph_ptr every column of
+        edge_index is an edge.  A validating prep raises GraphPrepIndexError.  graph_prep() picks which prep a batch gets."""
         lib = _lib.load()
         ei = _lib.i64c(edge_index, "edge_index")
         et = _lib.i64c(edge_type, "edge_type")
@@ -88,48 +101,24 @@ class GraphPrep:
         _lib.check(lib.qagnn_graph_prep_layout(self.N, self.E, C.byref(self.layout)), "qagnn_graph_prep_layout")
         self.buf = torch.empty(self.layout.total_bytes, dtype=torch.uint8, device=self.device)
         self._combo = None
-        self.packed = False  # built by qagnn_graph_prep_packed: the edge columns past graph_ptr[-1] are unused
-
-        packed = graph_ptr is not None and max_edges >= 0 and self.n_per_graph > 0
-        on_graph_ptr = packed  # the general prep below then reads only the graph_ptr[-1] real columns
-        if packed:
-            gp = _lib.i64c(graph_ptr, "graph_ptr")
-            if gp.numel() != self.N // max(self.n_per_graph, 1) + 1:
-                raise ValueError("graph_ptr must have one entry per sub-graph plus one")
-
-        def run():
-            nonlocal ei, et
-            shape = _lib.Shape(self.N, self.E, 4, 1, n_ntype, n_etype, 0, self.n_per_graph)
-            with torch.cuda.device(self.device):
-                if packed and self.n_per_graph > 0:
-                    st_ = lib.qagnn_graph_prep_packed(_lib.ptr(ei) if self.E else None, _lib.ptr(et) if self.E else None, _lib.ptr(nt),
-                                                      _lib.ptr(gp), int(max_edges), C.byref(shape), _lib.ptr(self.buf), self.buf.numel(),
-                                                      int(bool(validate)), _lib.stream_ptr(self.device))
-                    if st_ != -5:  # QAGNN_ERR_UNSUPPORTED: sub-graphs too large for one CTA -> the general pipeline below
-                        self.packed = True
-                        return st_
-                if on_graph_ptr:  # the general prep takes every column as an edge: drop the unused tail of an edge capacity
-                    ne = n_edges if n_edges >= 0 else (self.E if torch.cuda.is_current_stream_capturing() else int(gp[-1]))
-                    if not 0 <= ne <= self.E:
-                        raise IndexError(f"graph_ptr[-1] = {ne} is outside the {self.E} columns of edge_index")
-                    if ne < self.E:
-                        ei, et = ei[:, :ne].contiguous(), et[:ne]
-                        self.E = ne
-                        self.layout = _lib.PrepLayout()
-                        _lib.check(lib.qagnn_graph_prep_layout(self.N, self.E, C.byref(self.layout)), "qagnn_graph_prep_layout")
-                        shape.E = ne
-                self.packed = False
-                return lib.qagnn_graph_prep(_lib.ptr(ei) if self.E else None, _lib.ptr(et) if self.E else None, _lib.ptr(nt),
-                                            C.byref(shape), _lib.ptr(self.buf), self.buf.numel(), int(bool(validate)),
-                                            _lib.stream_ptr(self.device))
-        st = run()
-        if st == -3 and self.n_per_graph > 0 and allow_general_fallback and int(self.array("status")[0].item()) == 8:
-            packed = False
-            # the only complaint is an edge that crosses a sub-graph boundary: n_per_graph is a layout HINT for the
-            # shared-memory-tiled kernels, the reference accepts any batched edge_index -> use the general CSR kernels
-            self.n_per_graph = 0
-            st = run()
-        _lib.check(st, "qagnn_graph_prep")
+        # built by qagnn_graph_prep_packed: the edge columns past graph_ptr[-1] are unused
+        self.packed = graph_ptr is not None and max_edges >= 0 and self.n_per_graph > 0
+        shape = _lib.Shape(self.N, self.E, 4, 1, n_ntype, n_etype, 0, self.n_per_graph)
+        eptr, tptr = (_lib.ptr(ei), _lib.ptr(et)) if self.E else (None, None)
+        with torch.cuda.device(self.device):
+            if self.packed:
+                gp = _lib.i64c(graph_ptr, "graph_ptr")
+                if gp.numel() != self.N // self.n_per_graph + 1:
+                    raise ValueError("graph_ptr must have one entry per sub-graph plus one")
+                st = lib.qagnn_graph_prep_packed(eptr, tptr, _lib.ptr(nt), _lib.ptr(gp), int(max_edges), C.byref(shape),
+                                                 _lib.ptr(self.buf), self.buf.numel(), int(bool(validate)),
+                                                 _lib.stream_ptr(self.device))
+            else:
+                st = lib.qagnn_graph_prep(eptr, tptr, _lib.ptr(nt), C.byref(shape), _lib.ptr(self.buf), self.buf.numel(),
+                                          int(bool(validate)), _lib.stream_ptr(self.device))
+        if st == -3:  # the validating prep has synchronised: its status word says which check failed
+            raise GraphPrepIndexError(int(self.status_word().item()))
+        _lib.check(st, "qagnn_graph_prep_packed" if self.packed else "qagnn_graph_prep")
         self._keep = (ei, et, nt, graph_ptr)
 
     def real_edges(self):
@@ -190,6 +179,39 @@ class GraphPrep:
         ei = torch.stack([self.array("src"), self.array("tgt")]).long()
         e = self.real_edges()
         return ei if e == self.E else torch.cat([ei[:, :e], ei[:, self.E:]], 1)
+
+
+def graph_prep(A, node_type, n, n_ntype, n_etype, validate):
+    """The GraphPrep of batch A, an (edge_index, edge_type) pair or a qagnn_b200.data.PackedAdj, with `n` nodes per
+    sub-graph as a layout hint (0: none).  Every prep the modules build is chosen here:
+      * a PackedAdj packed for n-node sub-graphs gets the one-launch packed prep;
+      * when that prep refuses the shape, or the PackedAdj was packed for another node count, the general prep runs on
+        the batch's real edge columns (graph_ptr[-1] of them, read on the host when A.n_edges is unknown);
+      * an edge that crosses a sub-graph boundary (validate only) is legal, as in the reference: n is then dropped and
+        the batch goes to the general CSR kernels."""
+    ei, et, nt = A[0], A[1], node_type.reshape(-1)
+    gp = getattr(A, "graph_ptr_dev", None)
+    if gp is not None:
+        if n > 0 and A.n_nodes == n and A.max_edges >= 0:
+            try:
+                return GraphPrep(ei, et, nt, n_ntype, n_etype, n, validate, graph_ptr=gp, max_edges=A.max_edges)
+            except GraphPrepIndexError as e:
+                if e.bits != CROSS_GRAPH:
+                    raise
+                n = 0
+            except _lib.QagnnError as e:
+                if e.status != -5:  # QAGNN_ERR_UNSUPPORTED
+                    raise
+        ne = A.n_edges if A.n_edges >= 0 else int(gp[-1])
+        if not 0 <= ne <= ei.size(1):
+            raise IndexError(f"graph_ptr[-1] = {ne} is outside the {ei.size(1)} columns of edge_index")
+        ei, et = ei[:, :ne], et[:ne]
+    try:
+        return GraphPrep(ei, et, nt, n_ntype, n_etype, n, validate)
+    except GraphPrepIndexError as e:
+        if n == 0 or e.bits != CROSS_GRAPH:
+            raise
+    return GraphPrep(ei, et, nt, n_ntype, n_etype, 0, validate)
 
 
 def _edge_encoder_params(enc):
@@ -287,17 +309,14 @@ class GATConvE(nn.Module):
         self._prep_cache = (None, None)
 
     def _prep(self, edge_index, edge_type, node_type):
-        if getattr(edge_index, "graph_ptr_dev", None) is not None:  # a qagnn_b200.data.PackedAdj: one-launch packed prep
-            A = edge_index
-            key = _version_key([A.edge_index, A.edge_type, node_type, A.graph_ptr_dev])
-            if self._prep_cache[0] != key:
-                prep = _packed_graph_prep(A, node_type.reshape(-1), A.n_nodes, self.n_ntype, self.n_etype, self.check_indices)
-                self._prep_cache = (key, prep)
-            return self._prep_cache[1]
-        key = _version_key([edge_index, edge_type, node_type])
+        gp = getattr(edge_index, "graph_ptr_dev", None)
+        if gp is not None:  # a qagnn_b200.data.PackedAdj: one-launch packed prep
+            A, n, srcs = edge_index, edge_index.n_nodes, [edge_index.edge_index, edge_index.edge_type, node_type, gp]
+        else:
+            A, n, srcs = (edge_index, edge_type), 0, [edge_index, edge_type, node_type]
+        key = _version_key(srcs)
         if self._prep_cache[0] != key:
-            prep = GraphPrep(edge_index, edge_type, node_type, self.n_ntype, self.n_etype, 0, self.check_indices)
-            self._prep_cache = (key, prep)
+            self._prep_cache = (key, graph_prep(A, node_type, n, self.n_ntype, self.n_etype, self.check_indices))
         return self._prep_cache[1]
 
     def forward(self, x, edge_index, edge_type, node_type, node_feature_extra, return_attention_weights=False,
@@ -373,13 +392,13 @@ class QAGNN_Message_Passing(nn.Module):
         self.check_indices = True
         # use_cuda_graph: capture graph prep + the whole k-layer launch sequence (~60 kernels) into one CUDA graph per
         # (input buffers, weights) and replay it; the returned tensor is then a static buffer that the next replay
-        # overwrites.  Index validation needs a stream sync, so it is skipped inside the captured region.
+        # overwrites.  A replay cannot synchronise to validate indices: see _graphed_forward.
         self.use_cuda_graph = False
         self._graphs = {}
+        self._replayed = []  # pipeline.StatusWord of every replay whose status word has not been looked at yet
         self._folded = _FoldedWeights()
         # a captured graph bakes in the workspace / folded-blob addresses: drop the graphs before either is replaced
         self._ws = _DeviceBlob(on_replace=self._graphs.clear)
-        self._deferred_status = None
         self.register_load_state_dict_post_hook(lambda module, incompatible: module.invalidate())
 
     def invalidate(self):
@@ -402,33 +421,15 @@ class QAGNN_Message_Passing(nn.Module):
         return [self.emb_node_type.weight, self.emb_node_type.bias, self.emb_score.weight, self.emb_score.bias,
                 self.Vh.weight, self.Vh.bias, self.Vx.weight, self.Vx.bias, self._score_basis]
 
-    def _raise_deferred_status(self):
-        """CUDA-graph replays cannot synchronise to validate indices: every replay ORs graph prep's status word into a
-        device accumulator, which is copied to pinned memory asynchronously and inspected here once that copy has landed."""
-        if self._deferred_status is None:
-            return
-        host, ev, accum = self._deferred_status
-        if not ev.query():  # never block the host on the GPU here: the OR-accumulated word is looked at again later
-            return
-        self._deferred_status = None
-        if int(host.item()) != 0:
-            accum.zero_()
-            raise IndexError("qagnn_b200: the previous CUDA-graph replay saw edge_index / edge_type / node_type values out "
-                             f"of range or crossing a sub-graph boundary (status bits {int(host.item())}); its output was "
-                             "computed from clamped indices")
-
     def check_batch(self, A, node_type):
         """Validates the indices of a batch once (synchronising); raises IndexError like forward() with check_indices."""
-        n = node_type.size(1) if node_type.dim() == 2 else 0
-        GraphPrep(A[0], A[1], node_type.reshape(-1), self.n_ntype, self.n_etype, n, True, allow_general_fallback=True,
-                  graph_ptr=getattr(A, "graph_ptr_dev", None), max_edges=getattr(A, "max_edges", -1),
-                  n_edges=getattr(A, "n_edges", -1))
+        graph_prep(A, node_type, node_type.size(1) if node_type.dim() == 2 else 0, self.n_ntype, self.n_etype, True)
 
     def prepare_graph(self, edge_index, edge_type, node_type):
         """Builds the layer-invariant graph workspace; pass it back via forward(..., prep=) to amortise
         it over repeated forwards on the same batch."""
-        n_per_graph = node_type.size(1) if node_type.dim() == 2 else 0
-        return GraphPrep(edge_index, edge_type, node_type, self.n_ntype, self.n_etype, n_per_graph, self.check_indices)
+        n = node_type.size(1) if node_type.dim() == 2 else 0
+        return graph_prep((edge_index, edge_type), node_type, n, self.n_ntype, self.n_etype, self.check_indices)
 
     def mp_helper(self, _X, edge_index, edge_type, _node_type, _node_feature_extra):
         for layer in self.gnn_layers:
@@ -459,19 +460,19 @@ class QAGNN_Message_Passing(nn.Module):
         node_score: tensor (batch_size, n_node, 1)
         returns (batch_size, n_node, d_node)
         """
-        self._raise_deferred_status()
+        for status in self._replayed:  # never waits for the GPU: a replay whose copy has not landed is looked at later
+            status.check("QAGNN_Message_Passing")
+        self._replayed = [s for s in self._replayed if s.pending is not None]
         if self.training:  # dropout, BatchNorm batch statistics, autograd through the CUDA message passing (training.py)
             from . import training as TR
-            if prep is None:
-                if getattr(A, "graph_ptr_dev", None) is not None:  # PackedAdj, possibly at an edge capacity
-                    prep = _packed_graph_prep(A, node_type.reshape(-1), H.size(1), self.n_ntype, self.n_etype, self.check_indices)
-                else:
-                    prep = GraphPrep(A[0], A[1], node_type.reshape(-1), self.n_ntype, self.n_etype, 0, self.check_indices)
+            if prep is None:  # a PackedAdj (possibly at an edge capacity) gets the packed prep, a plain pair the general one
+                n = H.size(1) if getattr(A, "graph_ptr_dev", None) is not None else 0
+                prep = graph_prep(A, node_type, n, self.n_ntype, self.n_etype, self.check_indices)
             self._last_prep = prep
             return TR.mp_forward_train(self, H, A, node_type, node_score, prep)
         _warn_if_grad_wanted("QAGNN_Message_Passing", H, node_score)
         if self.use_cuda_graph and prep is None and not return_layers:
-            return self._forward_graphed(H, A, node_type, node_score)
+            return self._graphed_forward(H, A, node_type, node_score)
         lib = _lib.load()
         Hc = _lib.f32c(H, "H")
         if Hc.dim() != 3 or Hc.size(2) != self.hidden_size:
@@ -484,7 +485,7 @@ class QAGNN_Message_Passing(nn.Module):
             raise ValueError("node_type / node_score must be [batch, n_node(, 1)]")
         edge_index, edge_type = A  # a (edge_index, edge_type) pair, or a qagnn_b200.data.PackedAdj (iterates as that pair)
         if prep is None:
-            prep = _packed_graph_prep(A, nt, n, self.n_ntype, self.n_etype, self.check_indices)
+            prep = graph_prep(A, nt, n, self.n_ntype, self.n_etype, self.check_indices)
         self._last_prep = prep
         if prep.N != B * n:
             raise ValueError("graph workspace was built for a different number of nodes")
@@ -502,65 +503,31 @@ class QAGNN_Message_Passing(nn.Module):
             return out, layers
         return out
 
-
-def _packed_graph_prep(A, node_type, n, n_ntype, n_etype, validate):
-    """GraphPrep of a batch with n-node sub-graphs: one launch when A is a qagnn_b200.data.PackedAdj packed for n-node
-    sub-graphs, else (or when the packed prep refuses) the general pipeline on the batch's real edge columns."""
-    gp, me = getattr(A, "graph_ptr_dev", None), getattr(A, "max_edges", -1)
-    ne = getattr(A, "n_edges", -1)
-    if gp is not None and getattr(A, "n_nodes", n) != n:
-        # packed for another node count: its graph_ptr still holds, its offsets do not -> general prep on the real columns
-        if ne < 0:
-            ne = int(gp[-1]) if not torch.cuda.is_current_stream_capturing() else A[0].size(1)
-        gp, ei, et = None, A[0][:, :ne], A[1][:ne]
-    else:
-        ei, et = A[0], A[1]
-    return GraphPrep(ei, et, node_type, n_ntype, n_etype, n, validate, allow_general_fallback=True, graph_ptr=gp,
-                     max_edges=me, n_edges=ne)
-
-
-def _mp_forward_graphed(self, H, A, node_type, node_score):
-    """CUDA-graph replay of forward() for inputs that live in the same device buffers as when it was captured."""
-    tensors = [H, A[0], A[1], node_type, node_score]
-    if getattr(A, "graph_ptr_dev", None) is not None:
-        tensors.append(A.graph_ptr_dev)
-    key = (tuple((t.data_ptr(), tuple(t.shape), t.dtype) for t in tensors),
-           _version_key(list(self.parameters()) + list(self.buffers())))
-    entry = self._graphs.get(key)
-    if entry is None:
-        saved, self.use_cuda_graph = self.use_cuda_graph, False
-        check, self.check_indices = self.check_indices, False
-        try:
-            if check:  # validate once, eagerly, before trusting the capture
-                self.check_batch(A, node_type)
-            side = torch.cuda.Stream(device=H.device)
-            side.wait_stream(torch.cuda.current_stream(H.device))
-            with torch.cuda.stream(side):
-                for _ in range(2):  # warm-up: folds the weights, sizes the workspaces, sets kernel attributes
-                    self.forward(H, A, node_type, node_score)
-            torch.cuda.current_stream(H.device).wait_stream(side)
-            accum = torch.zeros(1, dtype=torch.int32, device=H.device)
-            graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(graph):
-                out = self.forward(H, A, node_type, node_score)
-                accum.bitwise_or_(self._last_prep.status_word())
+    def _graphed_forward(self, H, A, node_type, node_score):
+        """CUDA-graph replay of forward() for inputs that live in the same device buffers as when it was captured.  With
+        check_indices on at capture, each replay's index checks reach the host through its graph's StatusWord: forward()
+        raises IndexError once the copy of a bad replay has landed, also after the graph was evicted or invalidated."""
+        tensors = [H, A[0], A[1], node_type, node_score]
+        if getattr(A, "graph_ptr_dev", None) is not None:
+            tensors.append(A.graph_ptr_dev)
+        key = (tuple((t.data_ptr(), tuple(t.shape), t.dtype) for t in tensors),
+               _version_key(list(self.parameters()) + list(self.buffers())))
+        entry = self._graphs.get(key)
+        if entry is None:
+            from .pipeline import capture
+            graph, out, status = capture(self, A, node_type, "QAGNN_Message_Passing",
+                                         lambda: self.forward(H, A, node_type, node_score))
             if len(self._graphs) >= 8:
                 self._graphs.pop(next(iter(self._graphs)))
             # the entry keeps alive everything whose address the graph baked in: inputs, workspace, folded blob, prep
-            entry = self._graphs[key] = (graph, out, tensors, self._ws.buf, self._folded.blob, self._last_prep, accum,
-                                         torch.zeros(1, dtype=torch.int32).pin_memory())
-        finally:
-            self.use_cuda_graph, self.check_indices = saved, check
-    entry[0].replay()
-    if self.check_indices:  # later batches written into the same buffers: checked at the next call, without a sync here
-        entry[7].copy_(entry[6], non_blocking=True)
-        ev = torch.cuda.Event()
-        ev.record(torch.cuda.current_stream(H.device))
-        self._deferred_status = (entry[7], ev, entry[6])
-    return entry[1]
-
-
-QAGNN_Message_Passing._forward_graphed = _mp_forward_graphed
+            entry = self._graphs[key] = (graph, out, status, tensors, self._ws.buf, self._folded.blob, self._last_prep)
+        graph, out, status = entry[:3]
+        graph.replay()
+        if status is not None:
+            status.replayed()
+            if status not in self._replayed:
+                self._replayed.append(status)
+        return out
 
 
 class QAGNN(nn.Module):

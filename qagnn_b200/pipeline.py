@@ -54,6 +54,49 @@ class StatusWord:
                              f"crossing a sub-graph boundary (status bits {bits}); its results were computed from clamped indices")
 
 
+@contextlib.contextmanager
+def capture_guard(gnn, adj, node_type, what, warmup):
+    """Prepares the capture of CUDA graphs that run QAGNN_Message_Passing `gnn` on the batch (adj, node_type) and yields the
+    StatusWord the capture records graph prep's status word into (None with gnn.check_indices off).  Before it yields, it
+    validates the batch once, eagerly, and runs `warmup` twice on a side stream: that folds the weights, sizes the
+    workspaces and loads the kernels.  Inside, gnn.use_cuda_graph and gnn.check_indices are off: the module's kernels
+    become nodes of the caller's graph, and a replay cannot synchronise.  Both are restored on exit.
+
+    An adjacency that carries graph_ptr must get the packed prep, else ValueError: the general prep would keep the edge
+    count of the batch it was captured on for every later batch written into the same buffers."""
+    saved = gnn.use_cuda_graph, gnn.check_indices
+    gnn.use_cuda_graph = False
+    try:
+        if saved[1]:
+            gnn.check_batch(adj, node_type)
+        gnn.check_indices = False
+        dev = node_type.device
+        side = torch.cuda.Stream(device=dev)
+        side.wait_stream(torch.cuda.current_stream(dev))
+        with torch.cuda.stream(side):
+            for _ in range(2):
+                warmup()
+        torch.cuda.current_stream(dev).wait_stream(side)
+        if getattr(adj, "graph_ptr_dev", None) is not None and not gnn._last_prep.packed:
+            raise ValueError(f"{what}: the packed graph prep refuses these sub-graphs (too large for one CTA); a captured "
+                             "general prep would keep the edge count of this batch for every later one")
+        yield StatusWord(dev) if saved[1] else None
+    finally:
+        gnn.use_cuda_graph, gnn.check_indices = saved
+
+
+def capture(gnn, adj, node_type, what, fn):
+    """`fn()` captured as one CUDA graph under capture_guard, with graph prep's status word recorded at its end.  Returns
+    (graph, what fn returned, StatusWord or None)."""
+    with capture_guard(gnn, adj, node_type, what, fn) as status:
+        graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(graph):
+            out = fn()
+            if status is not None:
+                status.record(gnn._last_prep.status_word())
+    return graph, out, status
+
+
 class DecoderStep:
     """MP forward + pooling + (all-gather) + answer MLP on static device buffers, replayed as one CUDA graph.
 
@@ -109,39 +152,11 @@ class DecoderStep:
         return self.fc(full), pool_attn, out                                                # :188
 
     def _capture(self):
-        dev = self.inp["H"].device
-        saved = self.gnn.use_cuda_graph
-        self.gnn.use_cuda_graph = False  # its kernels become nodes of THIS graph
-        check, self.gnn.check_indices = self.gnn.check_indices, False
-        try:
-            if check:  # validate once, eagerly (a synchronising call), before trusting the capture
-                self.gnn.check_indices = True
-                self.gnn.check_batch(self.adj, self.inp["node_type"])
-                self.gnn.check_indices = False
-            side = torch.cuda.Stream(device=dev)
-            side.wait_stream(torch.cuda.current_stream(dev))
-            with torch.cuda.stream(side):
-                for _ in range(2):  # warm-up: folds the weights, sizes the workspaces, opens the NCCL channels
-                    self._eager()
-            torch.cuda.current_stream(dev).wait_stream(side)
-            torch.cuda.synchronize(dev)
-            if "graph_ptr" in self.inp and not self.gnn._last_prep.packed:
-                raise ValueError("DecoderStep: the packed graph prep refuses these sub-graphs (too large for one CTA); a "
-                                 "captured general prep would keep the edge count of this batch for every later one")
-            # batches written into the buffers later are validated without a sync (StatusWord)
-            status = StatusWord(dev)
-            graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(graph):
-                self.logits, self.pool_attn, self.gnn_out = self._eager()
-                if check:
-                    status.record(self.gnn._last_prep.status_word())
-            self.graph = graph
-            if check:
-                self._status = status
-            self._keep = (self.gnn._ws.buf, self.gnn._folded.blob, self.gnn._last_prep)  # addresses baked into the graph
-            self.mode = "one CUDA graph (prep + k layers + pooling" + (" + all-gather" if self.world > 1 else "") + " + fc)"
-        finally:
-            self.gnn.use_cuda_graph, self.gnn.check_indices = saved, check
+        # the warm-up also opens the NCCL channels of the all-gather
+        self.graph, (self.logits, self.pool_attn, self.gnn_out), self._status = capture(
+            self.gnn, self.adj, self.inp["node_type"], "DecoderStep", self._eager)
+        self._keep = (self.gnn._ws.buf, self.gnn._folded.blob, self.gnn._last_prep)  # addresses baked into the graph
+        self.mode = "one CUDA graph (prep + k layers + pooling" + (" + all-gather" if self.world > 1 else "") + " + fc)"
 
     def run(self):
         """Enqueues one step on the current stream; returns (logits, pool_attn, gnn_out).  A replay whose batch had an
@@ -281,37 +296,27 @@ class TrainStep:
         self._params = [p for p in dec.parameters() if p.requires_grad]
         self._buffers = list(dec.buffers())
         inputs = [self._sv, self._ns] + self._params
-        check = gnn.check_indices
-        if check:  # validate once, eagerly (a synchronising call), before trusting the capture
-            gnn.check_batch(self._adj, self._nt)
+
+        def warmup():  # also builds the cached tables of the training path
+            with self._autocast():
+                logits, _ = self._forward(self._sv, self._ns)
+            torch.autograd.grad(logits, inputs, torch.ones_like(logits), allow_unused=True)
+
         # the warm-up iterations really run: BatchNorm statistics, RNG offsets and .grad are put back afterwards
         buffers = [b.detach().clone() for b in self._buffers]
         grads = [None if p.grad is None else p.grad.detach().clone() for p in self._params]
         rng = torch.cuda.get_rng_state(dev)
-        gnn.check_indices = False
-        status = StatusWord(dev) if check else None
         try:
-            cur = torch.cuda.current_stream(dev)
-            side = torch.cuda.Stream(device=dev)
-            side.wait_stream(cur)
-            with torch.cuda.stream(side):
-                for _ in range(2):  # sizes the allocations, loads the kernels, builds the cached tables
+            with capture_guard(gnn, self._adj, self._nt, "TrainStep", warmup) as status:
+                self._status = status  # _forward records graph prep's status word into it
+                pool = torch.cuda.graph_pool_handle()
+                fwd, bwd = torch.cuda.CUDAGraph(), torch.cuda.CUDAGraph()
+                with torch.cuda.graph(fwd, pool=pool):
                     with self._autocast():
-                        logits, _ = self._forward(self._sv, self._ns)
-                    torch.autograd.grad(logits, inputs, torch.ones_like(logits), allow_unused=True)
-            cur.wait_stream(side)
-            if not gnn._last_prep.packed:
-                raise ValueError("TrainStep: the packed graph prep refuses these sub-graphs (too large for one CTA); a "
-                                 "captured general prep would keep the edge count of this batch for every later one")
-            self._status = status
-            pool = torch.cuda.graph_pool_handle()
-            fwd, bwd = torch.cuda.CUDAGraph(), torch.cuda.CUDAGraph()
-            with torch.cuda.graph(fwd, pool=pool):
-                with self._autocast():
-                    logits, pool_attn = self._forward(self._sv, self._ns)
-            self._g_logits = torch.empty_like(logits)
-            with torch.cuda.graph(bwd, pool=pool):
-                self._grads = torch.autograd.grad(logits, inputs, self._g_logits, allow_unused=True)
+                        logits, pool_attn = self._forward(self._sv, self._ns)
+                self._g_logits = torch.empty_like(logits)
+                with torch.cuda.graph(bwd, pool=pool):
+                    self._grads = torch.autograd.grad(logits, inputs, self._g_logits, allow_unused=True)
             self._logits, self._pool_attn = logits.detach(), pool_attn.detach()
             self._fwd, self._bwd = fwd, bwd
             self._bn_buffers = [b for m in dec.modules() if isinstance(m, torch.nn.modules.batchnorm._BatchNorm)
@@ -322,7 +327,6 @@ class TrainStep:
             self._status = None
             raise
         finally:
-            gnn.check_indices = check
             with torch.no_grad():
                 for b, s in zip(self._buffers, buffers):
                     b.copy_(s)
