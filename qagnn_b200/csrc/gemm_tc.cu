@@ -34,6 +34,19 @@ constexpr int kThreads = 384;  // warpgroup 0: TMA producer; warpgroups 1-2: wgm
 constexpr size_t kSmemCap = 227 * 1024;  // opt-in shared memory per block on H100
 constexpr int kCtrlBytes = 1024;         // mbarriers after the operand ring
 
+// Epilogue staging (after the mbarriers): each consumer warpgroup writes a column chunk of its 64 rows here and one of its
+// threads stores it with TMA, so the warpgroup is back at the next tile's MMAs while the copy drains.  13 KB = 64 rows x 52
+// fp32 columns, one head of the QA-GNN projection at D = 200.  Two buffers per warpgroup where the ring keeps its stage count
+// with them (bn = 208: 2 stages of 86 KB leave 58 KB), else one (bn = 64 / 128 keep 4 / 3 stages, bn = 256 its 2).
+constexpr uint32_t kStBytes = 13312;
+__host__ __device__ constexpr int st_bufs(int bn) { return bn == 208 ? 2 : 1; }
+__host__ __device__ constexpr size_t ring_stage_bytes(int bn) { return 2 * (size_t)BM * BK * 2 + 2 * (size_t)bn * BK * 2; }
+__host__ __device__ constexpr int ring_stages(int bn) {
+  return (kSmemCap - kCtrlBytes - 2 * st_bufs(bn) * kStBytes) / ring_stage_bytes(bn) > 6
+             ? 6
+             : (int)((kSmemCap - kCtrlBytes - 2 * st_bufs(bn) * kStBytes) / ring_stage_bytes(bn));
+}
+
 struct TcParams {
   CUtensorMap a_hi[2], a_lo[2], w_hi, w_lo;
   int nseg, kseg[2];
@@ -48,6 +61,10 @@ struct TcParams {
   HeadMajorOut hm;
   __nv_bfloat16 *c_hi, *c_lo;
   int ldp;
+  // TMA-store epilogue when st_w > 0: st_chunks chunks of st_w tile columns; boxes of st_w columns x 64 rows over the fp32
+  // output ([3H][M][DP] head-major or [1][M][N] row-major) and the bf16 planes ([1][M][N]), clipped to M and N
+  CUtensorMap st_f32, st_hi, st_lo;
+  int st_w, st_chunks;
 };
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -116,6 +133,25 @@ __device__ __forceinline__ void cluster_sync_all() {
   asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
   asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
+// epilogue staging: the warpgroup's generic-proxy writes are made visible to the TMA engine (async proxy) by each writer's
+// proxy fence and a warpgroup barrier; a buffer is rewritten only once the store that read it has finished reading
+__device__ __forceinline__ void wg_bar(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
+__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+__device__ __forceinline__ void tma_store_3d(const CUtensorMap* map, const void* src, int c0, int c1, int c2) {
+  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(map),
+               "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2)
+               : "memory");
+}
+__device__ __forceinline__ void st_shared_f2(uint32_t a, float x, float y) {
+  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a), "f"(x), "f"(y) : "memory");
+}
+__device__ __forceinline__ void st_shared_u32(uint32_t a, uint32_t v) { asm volatile("st.shared.u32 [%0], %1;" ::"r"(a), "r"(v) : "memory"); }
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() {  // at most N committed stores still reading shared memory
+  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
+}
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
 // K-major operand tile, 128-byte swizzle: rows of 128 B, 8-row groups 1024 B apart (wgmma matrix descriptor:
 // start >> 4 | LBO (unused for swizzled K-major) = 1 | SBO = 1024 >> 4 | layout type 1 = SWIZZLE_128B)
@@ -209,6 +245,17 @@ __device__ __forceinline__ float act_fn(float v) {
   return v;
 }
 
+// hi = bf16(v), lo = bf16(v - hi) of a column pair, packed low column first (the order of a bf16x2 fragment word)
+__device__ __forceinline__ void split_pair(float v0, float v1, uint32_t& hi, uint32_t& lo) {
+  __nv_bfloat162 h2, l2;
+  h2.x = __float2bfloat16_rn(v0);
+  h2.y = __float2bfloat16_rn(v1);
+  l2.x = __float2bfloat16_rn(v0 - __bfloat162float(h2.x));
+  l2.y = __float2bfloat16_rn(v1 - __bfloat162float(h2.y));
+  hi = *reinterpret_cast<uint32_t*>(&h2);
+  lo = *reinterpret_cast<uint32_t*>(&l2);
+}
+
 // Persistent CTAs (CTAS = 1) or CTA pairs (CTAS = 2, one cluster) walk the (row block, n tile) grid with n fastest.
 // Ring stage = [A hi | A lo | W hi | W lo], each a 1024-byte aligned K-major tile of 64 bf16 per row.
 template <int ACT, int BN, int CTAS>
@@ -217,10 +264,13 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
   constexpr uint32_t a_bytes = BM * BK * 2;  // one A plane tile: 16 KB
   constexpr uint32_t w_bytes = BN * BK * 2;  // one W plane k block
   constexpr uint32_t stage_bytes = 2 * a_bytes + 2 * w_bytes;
+  constexpr int kBufs = st_bufs(BN);
+  static_assert(ring_stages(BN) >= 2, "the epilogue staging leaves room for two ring stages");
   const int wg = threadIdx.x >> 7, tid = threadIdx.x & 127;
   const uint32_t rank = CTAS == 2 ? cluster_ctarank() : 0u;
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + (size_t)p.stages * stage_bytes);  // [stages]  TMA -> MMA
   uint64_t* empty = full + p.stages;                                                      // [stages]  MMA -> TMA
+  unsigned char* staging = smem + (size_t)p.stages * stage_bytes + kCtrlBytes;           // [2 warpgroups][kBufs]
 
   // k-blocks across the (up to two) A segments
   int nkb_seg[2];
@@ -287,6 +337,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
     const int q8 = 8 / DP, r8 = 8 - q8 * DP;
     float acc[BN / 2];
     long long it = 0;
+    int st_it = 0;  // staged chunks so far: buffer st_it % kBufs
     for (long long tile = cl_id; tile < total_tiles; tile += n_cl) {
 #pragma unroll
       for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
@@ -309,12 +360,90 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
         fence_acc<BN / 2>(acc);
         release_stage<CTAS>(&empty[s], lane);
       }
-      // ---- epilogue straight from the accumulator fragment: thread holds rows g, g + 8 and column pairs 8j + 2q
+      // ---- epilogue: thread holds rows g, g + 8 and column pairs 8j + 2q of the accumulator fragment
       const int n_tile = (int)(tile % n_tiles);
       const int n0 = n_tile * p.n_step;
       const long long row_g = (tile / n_tiles) * BM * CTAS + rank * BM + wc * 64 + warp * 16 + (lane >> 2);
       // head-major output: the tile's first column starts plane n0 / DP (= which * H + head) of [3][H][N][DP]
       const int hm_plane0 = hm_mode ? n0 / DP : 0;
+      if (p.st_w > 0) {
+        // through shared memory in chunks of W tile columns (W >= 8 divides n_step and, head-major, DP): the fragment is
+        // walked in column order, as below, so each accumulator dies once written.  A chunk opens (its buffer free) in the
+        // group that holds its first column and closes in the one that holds its last: thread 0 of the warpgroup then
+        // stores its [64][W] fp32 / bf16 hi / bf16 lo boxes with TMA.  A group straddles two chunks only with two buffers.
+        const int W = p.st_w;
+        const int rl = warp * 16 + (lane >> 2);  // fragment rows rl, rl + 8 of the warpgroup's 64
+        const int r0 = (int)(row_g - rl);
+        int boff[2] = {0, 0};  // per-row bias table offsets
+        if (p.bias != nullptr && p.row_class != nullptr) {
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            long long c = row_g + 8 * h < p.M ? p.row_class[row_g + 8 * h] : 0;
+            c = c < 0 ? 0 : (c >= p.n_class ? p.n_class - 1 : c);
+            boff[h] = (int)c * p.class_stride;
+          }
+        }
+        const bool f32_out = hm_mode || p.c_f32 != nullptr, pl_out = p.c_hi != nullptr;
+        const uint32_t f32_bytes = f32_out ? 64u * W * 4 : 0u, pl_bytes = 64u * W * 2;
+        const uint32_t st0 = smem_u32(staging) + (uint32_t)wc * kBufs * kStBytes;
+        int open_end = 0;  // columns [0, open_end) are in chunks opened so far
+        int close_end = W;  // the oldest open chunk is [close_end - W, close_end)
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          if (8 * j >= p.n_step) break;
+          if (open_end < 8 * j + 8) {  // a chunk starts here: wait until the store that read its buffer last is done
+            if (tid == 0) {
+              if (kBufs == 2 && open_end == close_end) bulk_wait_read<0>();  // the chunk before is still open
+              else bulk_wait_read<kBufs - 1>();
+            }
+            wg_bar(1 + wc);
+            open_end += W;
+          }
+          const int c = 8 * j + 2 * (lane & 3), gc = n0 + c;
+          const bool second = c >= close_end;
+          const uint32_t buf = st0 + (uint32_t)((st_it + (second ? 1 : 0)) % kBufs) * kStBytes;
+          const int cc = c - (second ? close_end : close_end - W);
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+            if (p.bias != nullptr) {  // columns from N on are clipped by the store
+              if (gc < p.N) v0 += __ldg(p.bias + boff[h] + gc);
+              if (gc + 1 < p.N) v1 += __ldg(p.bias + boff[h] + gc + 1);
+            }
+            v0 = act_fn<ACT>(v0);
+            v1 = act_fn<ACT>(v1);
+            const uint32_t e = (uint32_t)((rl + 8 * h) * W + cc);
+            if (f32_out) st_shared_f2(buf + 4 * e, v0, v1);
+            if (pl_out) {
+              uint32_t hi, lo;
+              split_pair(v0, v1, hi, lo);
+              st_shared_u32(buf + f32_bytes + 2 * e, hi);
+              st_shared_u32(buf + f32_bytes + pl_bytes + 2 * e, lo);
+            }
+          }
+          if (close_end <= 8 * j + 8) {  // the oldest open chunk is complete
+            fence_proxy_async();
+            wg_bar(1 + wc);
+            if (tid == 0) {
+              const int cb = close_end - W;
+              const unsigned char* b = staging + (size_t)(wc * kBufs + st_it % kBufs) * kStBytes;
+              if (f32_out) {
+                if (hm_mode) tma_store_3d(&p.st_f32, b, cb % DP, r0, hm_plane0 + cb / DP);
+                else tma_store_3d(&p.st_f32, b, n0 + cb, r0, 0);
+              }
+              if (pl_out) {
+                tma_store_3d(&p.st_hi, b + f32_bytes, n0 + cb, r0, 0);
+                tma_store_3d(&p.st_lo, b + f32_bytes + pl_bytes, n0 + cb, r0, 0);
+              }
+              bulk_commit();
+            }
+            close_end += W;
+            ++st_it;
+          }
+        }
+        continue;
+      }
+      // straight from the fragment to global memory (QAGNN_TC_STORE=direct, or outputs TMA cannot address)
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const long long r = row_g + 8 * h;
@@ -371,6 +500,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
         }
       }
     }
+    if (tid == 0) bulk_wait_all();  // no store still reads the staging buffers when the CTA exits
   }
   __syncthreads();
   if (CTAS == 2) cluster_sync_all();  // the peer's multicasts and remote arrivals target this CTA: nobody leaves early
@@ -394,6 +524,15 @@ constexpr int kMlpChunk = 72;                      // W2 rows (output columns) p
 // One consumer thread issues the TMA fills instead, `stages` fills ahead of the consumers.
 constexpr int kMlpThreads = 256;
 constexpr uint32_t kW2Sub = kMlpChunk * BK * 2;    // one W2 plane k block of a chunk: 9216 B (a multiple of 1024)
+// epilogue staging per warpgroup: one chunk of its 64 rows, fp32 or both bf16 planes (staged one after the other when
+// both are asked for: two buffers would leave room for one ring stage only)
+constexpr uint32_t kMlpStBytes = 64 * kMlpChunk * 4;
+constexpr int mlp_ring_stages() {
+  return (int)((kSmemCap - kCtrlBytes - 2 * kMlpStBytes) / ring_stage_bytes(kMlpMaxD)) > 6
+             ? 6
+             : (int)((kSmemCap - kCtrlBytes - 2 * kMlpStBytes) / ring_stage_bytes(kMlpMaxD));
+}
+static_assert(mlp_ring_stages() >= 2, "the fused MLP's epilogue staging leaves room for two ring stages");
 
 struct MlpParams {
   CUtensorMap a_hi, a_lo, w1_hi, w1_lo, w2_hi, w2_lo;
@@ -404,18 +543,10 @@ struct MlpParams {
   int ldc;
   __nv_bfloat16 *c_hi, *c_lo;
   int ldp;
+  // TMA-store epilogue when set: boxes of one 72-column chunk x 64 rows over the fp32 output and the bf16 planes
+  CUtensorMap st_f32, st_hi, st_lo;
+  int tma_store;
 };
-
-// hi = bf16(v), lo = bf16(v - hi) of a column pair, packed low column first (the order of a bf16x2 fragment word)
-__device__ __forceinline__ void split_pair(float v0, float v1, uint32_t& hi, uint32_t& lo) {
-  __nv_bfloat162 h2, l2;
-  h2.x = __float2bfloat16_rn(v0);
-  h2.y = __float2bfloat16_rn(v1);
-  l2.x = __float2bfloat16_rn(v0 - __bfloat162float(h2.x));
-  l2.y = __float2bfloat16_rn(v1 - __bfloat162float(h2.y));
-  hi = *reinterpret_cast<uint32_t*>(&h2);
-  lo = *reinterpret_cast<uint32_t*>(&l2);
-}
 
 // the three split-bf16 passes of the first STEPS k16 steps of the hidden layer against one W2 chunk (hi planes at sw, lo
 // planes lo_off further; k block kb of a plane at kb * kW2Sub)
@@ -447,6 +578,7 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_tc_kernel(const __grid_con
   const uint32_t rank = CTAS == 2 ? cluster_ctarank() : 0u;
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + (size_t)p.stages * stage_bytes);
   uint64_t* empty = full + p.stages;
+  unsigned char* staging = smem + (size_t)p.stages * stage_bytes + kCtrlBytes;  // [2 warpgroups][kMlpStBytes]
 
   const int D = p.D;
   const int nkb = (D + BK - 1) / BK;          // k blocks of both GEMMs (K = D)
@@ -590,6 +722,50 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_tc_kernel(const __grid_con
         wgmma_wait_all();
         fence_acc<kMlpChunk / 2>(acc2);
         release(s);
+        if (p.tma_store) {
+          // through this warpgroup's staging buffer: the fp32 box, then the two plane boxes, each stored with TMA by thread
+          // 0 of the warpgroup (clipped to M rows and D columns); the buffer is rewritten once the last store has read it
+          const uint32_t buf = smem_u32(staging) + (uint32_t)wc * kMlpStBytes;
+          const int rl = warp * 16 + (lane >> 2);
+          const int r0 = (int)(row_g - rl);
+          for (int part = 0; part < 2; ++part) {
+            if (part == 0 ? p.c_f32 == nullptr : p.c_hi == nullptr) continue;
+            if (tid == 0) bulk_wait_read<0>();
+            wg_bar(1 + wc);
+#pragma unroll
+            for (int j = 0; j < kMlpChunk / 8; ++j) {
+              const int cc = 8 * j + q2, gc = ch * kMlpChunk + cc;
+              const float bb0 = gc < D ? __ldg(p.b2 + gc) : 0.f, bb1 = gc < D ? __ldg(p.b2 + gc + 1) : 0.f;
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                const float v0 = act_fn<ACT>(acc2[4 * j + 2 * h] + bb0);
+                const float v1 = act_fn<ACT>(acc2[4 * j + 2 * h + 1] + bb1);
+                const uint32_t e = (uint32_t)((rl + 8 * h) * kMlpChunk + cc);
+                if (part == 0) {
+                  st_shared_f2(buf + 4 * e, v0, v1);
+                } else {
+                  uint32_t hi, lo;
+                  split_pair(v0, v1, hi, lo);
+                  st_shared_u32(buf + 2 * e, hi);
+                  st_shared_u32(buf + kMlpStBytes / 2 + 2 * e, lo);
+                }
+              }
+            }
+            fence_proxy_async();
+            wg_bar(1 + wc);
+            if (tid == 0) {
+              const unsigned char* b = staging + (size_t)wc * kMlpStBytes;
+              if (part == 0) {
+                tma_store_3d(&p.st_f32, b, ch * kMlpChunk, r0, 0);
+              } else {
+                tma_store_3d(&p.st_hi, b, ch * kMlpChunk, r0, 0);
+                tma_store_3d(&p.st_lo, b + kMlpStBytes / 2, ch * kMlpChunk, r0, 0);
+              }
+              bulk_commit();
+            }
+          }
+          continue;
+        }
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           const long long r = row_g + 8 * h;
@@ -611,6 +787,7 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_tc_kernel(const __grid_con
         }
       }
     }
+    if (tid == 0) bulk_wait_all();  // no store still reads the staging buffers when the CTA exits
   }
   __syncthreads();
   if (CTAS == 2) cluster_sync_all();
@@ -662,6 +839,29 @@ bool make_map(CUtensorMap* m, const void* base, long long rows, int K, int ld, i
              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
+
+// Epilogue store map: [planes][rows][inner] elements (rows `ld` elements apart, planes `rows` rows apart), a box of
+// box_w x 64 x 1, no swizzle.  A store writes only the part of its box inside the extents.
+bool make_store_map(CUtensorMap* m, CUtensorMapDataType type, int esize, void* base, int inner, long long rows, int planes,
+                    int ld, int box_w) {
+  EncodeTiledFn enc = encode_fn();
+  if (!enc) return false;
+  cuuint64_t dims[3] = {(cuuint64_t)inner, (cuuint64_t)rows, (cuuint64_t)planes};
+  cuuint64_t strides[2] = {(cuuint64_t)ld * esize, (cuuint64_t)rows * ld * esize};
+  cuuint32_t box[3] = {(cuuint32_t)box_w, 64, 1};
+  cuuint32_t estr[3] = {1, 1, 1};
+  return enc(m, type, 3, base, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
+             CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+}
+
+// Largest chunk width 8 <= w <= max_w that divides span and is a multiple of align > 0 (0: none).
+int chunk_width(int span, int align, int max_w) {
+  for (int w = span < max_w ? span : max_w; w >= 8; --w)
+    if (span % w == 0 && w % align == 0) return w;
+  return 0;
+}
+
+bool aligned16(const void* p) { return ((uintptr_t)p & 15) == 0; }
 
 // Launches one persistent instantiation; attr_set / max_clusters are that instantiation's per-device caches.
 template <typename Params>
@@ -719,6 +919,13 @@ int32_t launch_bn(int ctas, Act act, const cudaLaunchConfig_t& cfg, const TcPara
 int tc_ctas() {
   const char* e = getenv("QAGNN_TC_2CTA");
   return (e && atoi(e) == 0) ? 1 : 2;
+}
+
+// default: the epilogue stores through shared memory with TMA; QAGNN_TC_STORE=direct -> stores straight from the registers
+// (the same values, bit for bit).  Read at every call, so that one process can compare and time both.
+bool tc_store_tma() {
+  const char* e = getenv("QAGNN_TC_STORE");
+  return !(e && strcmp(e, "direct") == 0);
 }
 
 int32_t sm_count(int* sms) {
@@ -785,12 +992,9 @@ int32_t gemm_tc(const TcOperand& A1, const TcOperand& A2, const TcOperand& W, co
   p.kseg[0] = K1;
   p.kseg[1] = K2;
   const int CTAS = tc_ctas();
-  const size_t stage_bytes = 2 * (size_t)BM * BK * 2 + 2 * (size_t)bn * BK * 2;
-  int stages = (int)((kSmemCap - kCtrlBytes) / stage_bytes);
-  if (stages > 6) stages = 6;
-  if (stages < 2) return QAGNN_ERR_UNSUPPORTED;
+  const int stages = ring_stages(bn);
   p.stages = stages;
-  const size_t smem_bytes = stages * stage_bytes + kCtrlBytes;
+  const size_t smem_bytes = stages * ring_stage_bytes(bn) + kCtrlBytes + 2 * st_bufs(bn) * kStBytes;
   bool ok = make_map(&p.a_hi[0], A1.hi, M, K1, A1.ld, BM) && make_map(&p.a_lo[0], A1.lo, M, K1, A1.ld, BM);
   if (K2 > 0) ok = ok && make_map(&p.a_hi[1], A2.hi, M, K2, A2.ld, BM) && make_map(&p.a_lo[1], A2.lo, M, K2, A2.ld, BM);
   ok = ok && make_map(&p.w_hi, W.hi, N, K1 + K2, W.ld, bn / CTAS) && make_map(&p.w_lo, W.lo, N, K1 + K2, W.ld, bn / CTAS);
@@ -807,6 +1011,31 @@ int32_t gemm_tc(const TcOperand& A1, const TcOperand& A2, const TcOperand& W, co
   p.c_hi = (__nv_bfloat16*)out.hi;
   p.c_lo = (__nv_bfloat16*)out.lo;
   p.ldp = out.ldp;
+  if (tc_store_tma()) {
+    // chunks of whole tile columns that never cross a head (head-major) or the tile's n_step: a box must not reach the
+    // neighbouring tile's columns.  Box rows of 16-byte multiples: fp32 chunks of 4 columns, bf16 chunks of 8; with one
+    // staging buffer a chunk must not share a fragment column group with the next, so multiples of 8.
+    const bool f32_out = out.hm_buf != nullptr || out.f32 != nullptr, pl_out = out.hi != nullptr;
+    const int col_bytes = 64 * ((f32_out ? 4 : 0) + (pl_out ? 4 : 0));
+    const int span = out.hm_buf != nullptr ? out.hm.DP : p.n_step;
+    const bool addressable = (!out.hm_buf || aligned16(out.hm_buf)) && (!out.f32 || aligned16(out.f32)) &&
+                             (!pl_out || (aligned16(out.hi) && aligned16(out.lo)));
+    const int w = addressable && (f32_out || pl_out) ? chunk_width(span, pl_out || st_bufs(bn) == 1 ? 8 : 4, (int)kStBytes / col_bytes) : 0;
+    if (w > 0) {
+      bool sok = true;
+      if (out.hm_buf != nullptr)
+        sok = make_store_map(&p.st_f32, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, out.hm_buf, out.hm.DP, M, N / out.hm.DP,
+                             out.hm.DP, w);
+      else if (out.f32 != nullptr)
+        sok = make_store_map(&p.st_f32, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, out.f32, N, M, 1, out.ldc, w);
+      if (pl_out)
+        sok = sok && make_store_map(&p.st_hi, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, out.hi, N, M, 1, out.ldp, w) &&
+              make_store_map(&p.st_lo, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, out.lo, N, M, 1, out.ldp, w);
+      if (!sok) return QAGNN_ERR_CUDA;
+      p.st_w = w;
+      p.st_chunks = p.n_step / w;
+    }
+  }
   int sms = 0;
   QAGNN_RETURN_IF(sm_count(&sms));
   const long long total_tiles = (long long)n_tiles * ((M + (long long)BM * CTAS - 1) / ((long long)BM * CTAS));
@@ -825,7 +1054,7 @@ int32_t gemm_tc(const TcOperand& A1, const TcOperand& A2, const TcOperand& W, co
   lattr[0].val.clusterDim.z = 1;
   cfg.attrs = lattr;
   cfg.numAttrs = CTAS == 2 ? 1 : 0;
-  if (getenv("QAGNN_DEBUG")) fprintf(stderr, "gemm_tc: M=%lld N=%d K1=%d K2=%d act=%d CTAS=%d stages=%d smem=%zu grid=%u bn=%d n_step=%d n_tiles=%d\n", M, N, K1, K2, (int)act, CTAS, stages, smem_bytes, grid, bn, p.n_step, n_tiles);
+  if (getenv("QAGNN_DEBUG")) fprintf(stderr, "gemm_tc: M=%lld N=%d K1=%d K2=%d act=%d CTAS=%d stages=%d smem=%zu grid=%u bn=%d n_step=%d n_tiles=%d st_w=%d\n", M, N, K1, K2, (int)act, CTAS, stages, smem_bytes, grid, bn, p.n_step, n_tiles, p.st_w);
   int32_t rc;
   if (bn == 64) rc = launch_bn<64>(CTAS, act, cfg, p);
   else if (bn == 128) rc = launch_bn<128>(CTAS, act, cfg, p);
@@ -850,11 +1079,8 @@ int32_t mlp_tc(const TcOperand& A, const TcOperand& W1, const float* b1, const T
   const int CTAS = tc_ctas();
   MlpParams p;
   memset(&p, 0, sizeof(p));
-  const size_t stage_bytes = 2 * (size_t)BM * BK * 2 + 2 * (size_t)kMlpMaxD * BK * 2;
-  int stages = (int)((kSmemCap - kCtrlBytes) / stage_bytes);
-  if (stages > 6) stages = 6;
-  if (stages < 2) return QAGNN_ERR_UNSUPPORTED;
-  const size_t smem_bytes = stages * stage_bytes + kCtrlBytes;
+  const int stages = mlp_ring_stages();
+  const size_t smem_bytes = stages * ring_stage_bytes(kMlpMaxD) + kCtrlBytes + 2 * kMlpStBytes;
   bool ok = make_map(&p.a_hi, A.hi, M, D, A.ld, BM) && make_map(&p.a_lo, A.lo, M, D, A.ld, BM);
   ok = ok && make_map(&p.w1_hi, W1.hi, D, D, W1.ld, kMlpMaxD / CTAS) && make_map(&p.w1_lo, W1.lo, D, D, W1.ld, kMlpMaxD / CTAS);
   ok = ok && make_map(&p.w2_hi, W2.hi, D, D, W2.ld, kMlpChunk) && make_map(&p.w2_lo, W2.lo, D, D, W2.ld, kMlpChunk);
@@ -869,6 +1095,17 @@ int32_t mlp_tc(const TcOperand& A, const TcOperand& W1, const float* b1, const T
   p.c_hi = (__nv_bfloat16*)out.hi;
   p.c_lo = (__nv_bfloat16*)out.lo;
   p.ldp = out.ldp;
+  // rows are 16-byte multiples (ldc % 4, ldp % 8 above); the bases must be 16-byte aligned too
+  if (tc_store_tma() && (out.f32 || out.hi) && (!out.f32 || aligned16(out.f32)) &&
+      (!out.hi || (aligned16(out.hi) && aligned16(out.lo)))) {
+    bool sok = true;
+    if (out.f32) sok = make_store_map(&p.st_f32, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, out.f32, D, M, 1, out.ldc, kMlpChunk);
+    if (out.hi)
+      sok = sok && make_store_map(&p.st_hi, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, out.hi, D, M, 1, out.ldp, kMlpChunk) &&
+            make_store_map(&p.st_lo, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, out.lo, D, M, 1, out.ldp, kMlpChunk);
+    if (!sok) return QAGNN_ERR_CUDA;
+    p.tma_store = 1;
+  }
   int sms = 0;
   QAGNN_RETURN_IF(sm_count(&sms));
   const long long total_tiles = (M + (long long)BM * CTAS - 1) / ((long long)BM * CTAS);
