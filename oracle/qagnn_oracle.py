@@ -218,12 +218,9 @@ def multihead_att_pool(sd, prefix, q, k, mask, n_head):
     return out, attn
 
 
-def qagnn_decoder_forward(sd, sent_vecs, concept_ids, node_type_ids, node_scores, adj_lengths, edge_index,
-                          edge_type, k, n_ntype, n_etype, n_attention_head, n_fc_layer, head_count=4,
-                          dtype=torch.float32):
-    """QAGNN.forward (eval), modeling_qagnn.py:141-189.  `sd` holds the decoder's state_dict
-    (keys 'svec2nvec.*', 'concept_emb.*', 'gnn.*', 'pooler.*', 'fc.layers.*')."""
-    sv = sent_vecs.to(dtype)
+def decoder_head(sd, sv, concept_ids, node_scores, adj_lengths, dtype=torch.float32):
+    """modeling_qagnn.py:153-167: the GNN input (context node GELU(svec2nvec(sv)), then the concept rows) and the
+    normalised node scores.  Returns (gnn_input [B, n, D], node_scores [B, n, 1]); adj_lengths = 0 gives NaN scores."""
     gnn_input0 = gelu_tanh(linear(sv, sd, "svec2nvec")).unsqueeze(1)
     emb = sd["concept_emb.emb.weight"].to(dtype)[concept_ids[:, 1:] - 1]
     if "concept_emb.cpt_transform.weight" in sd:  # utils/layers.py:600-603
@@ -236,12 +233,30 @@ def qagnn_decoder_forward(sd, sent_vecs, concept_ids, node_type_ids, node_scores
     ns = ns.squeeze(2) * _mask
     mean_norm = ns.abs().sum(dim=1) / adj_lengths
     ns = (ns / (mean_norm.unsqueeze(1) + 1e-05)).unsqueeze(2)
-    gnn_output = message_passing_forward(sd, gnn_input, edge_index, edge_type, node_type_ids, ns, k, n_ntype,
-                                         n_etype, head_count, dtype, prefix="gnn.")
-    Z = gnn_output[:, 0]
+    return gnn_input, ns
+
+
+def decoder_pool_mask(adj_lengths, node_type_ids):
+    """modeling_qagnn.py:174-176: the pooler's mask [B, n] (True = excluded): nodes past the length and context nodes
+    (type 3); a row with every node masked keeps node 0."""
+    n = node_type_ids.size(1)
     mask = torch.arange(n) >= adj_lengths.unsqueeze(1)
     mask = mask | (node_type_ids == 3)
     mask[mask.all(1), 0] = 0
+    return mask
+
+
+def qagnn_decoder_forward(sd, sent_vecs, concept_ids, node_type_ids, node_scores, adj_lengths, edge_index,
+                          edge_type, k, n_ntype, n_etype, n_attention_head, n_fc_layer, head_count=4,
+                          dtype=torch.float32):
+    """QAGNN.forward (eval), modeling_qagnn.py:141-189.  `sd` holds the decoder's state_dict
+    (keys 'svec2nvec.*', 'concept_emb.*', 'gnn.*', 'pooler.*', 'fc.layers.*')."""
+    sv = sent_vecs.to(dtype)
+    gnn_input, ns = decoder_head(sd, sv, concept_ids, node_scores, adj_lengths, dtype)
+    gnn_output = message_passing_forward(sd, gnn_input, edge_index, edge_type, node_type_ids, ns, k, n_ntype,
+                                         n_etype, head_count, dtype, prefix="gnn.")
+    Z = gnn_output[:, 0]
+    mask = decoder_pool_mask(adj_lengths, node_type_ids)
     graph_vecs, pool_attn = multihead_att_pool(sd, "pooler", sv, gnn_output, mask, n_attention_head)
     concat = torch.cat((graph_vecs, sv, Z), 1)
     h = concat

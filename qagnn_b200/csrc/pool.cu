@@ -208,6 +208,26 @@ __global__ void __launch_bounds__(kPoolThreads, 4) attention_pool_kernel(int n, 
   }
 }
 
+// Largest dynamic shared memory attention_pool_kernel takes; larger shapes are refused (QAGNN_ERR_UNSUPPORTED) and the
+// caller pools with its einsum path.
+constexpr size_t kPoolSmemCap = 200 * 1024;
+
+inline size_t pool_smem_bytes(int n, int D, int nh) {
+  return ((size_t)2 * nh * D + (size_t)nh * n + nh + 16 + (size_t)(kPoolThreads / 32) * nh * D) * sizeof(float);
+}
+
+// Both entry points launch the same kernel, and cudaFuncSetAttribute overwrites the limit rather than raising it, so the
+// limit is set once per device, to the cap, for both of them.
+int32_t prepare_pool_launch(size_t smem) {
+  static bool attr_set[kMaxDevices] = {false};
+  const int dev = current_device();
+  if (smem > 48 * 1024 && !attr_set[dev]) {
+    QAGNN_CHECK_CUDA(cudaFuncSetAttribute(attention_pool_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPoolSmemCap));
+    attr_set[dev] = true;
+  }
+  return QAGNN_OK;
+}
+
 }  // namespace
 }  // namespace qagnn
 
@@ -286,14 +306,9 @@ extern "C" int32_t qagnn_decoder_tail(int32_t B, int32_t n, int32_t D, int32_t n
   if (n_head > 8) return QAGNN_ERR_UNSUPPORTED;
   if (!X || !qs || !node_type || !adj_lengths || !sent_vecs || !wk || !bk || !wv || !bv || !concat || !attn)
     return QAGNN_ERR_INVALID_ARGUMENT;
-  const size_t smem = ((size_t)2 * n_head * D + (size_t)n_head * n + n_head + 16 + (size_t)(kPoolThreads / 32) * n_head * D) * sizeof(float);
-  if (smem > 200 * 1024) return QAGNN_ERR_UNSUPPORTED;
-  static size_t attr[kMaxDevices] = {0};
-  const int dev = current_device();
-  if (smem > 48 * 1024 && smem > attr[dev]) {
-    QAGNN_CHECK_CUDA(cudaFuncSetAttribute(attention_pool_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr[dev] = smem;
-  }
+  const size_t smem = pool_smem_bytes(n, D, n_head);
+  if (smem > kPoolSmemCap) return QAGNN_ERR_UNSUPPORTED;
+  QAGNN_RETURN_IF(prepare_pool_launch(smem));
   attention_pool_kernel<<<B, kPoolThreads, smem, (cudaStream_t)stream>>>(n, D, n_head, X, qs, nullptr, wk, bk, wv, bv, concat, attn, B,
                                                                          node_type, adj_lengths, sent_vecs, S, 2 * D + S);
   QAGNN_CHECK_LAUNCH();
@@ -306,14 +321,9 @@ extern "C" int32_t qagnn_attention_pool(int32_t B, int32_t n, int32_t D, int32_t
   if (B <= 0 || n <= 0 || D <= 0 || n_head <= 0 || D % n_head != 0) return QAGNN_ERR_INVALID_ARGUMENT;
   if (n_head > 8) return QAGNN_ERR_UNSUPPORTED;
   if (!X || !qs || !mask || !wk || !bk || !wv || !bv || !pooled || !attn) return QAGNN_ERR_INVALID_ARGUMENT;
-  const size_t smem = ((size_t)2 * n_head * D + (size_t)n_head * n + n_head + 16 + (size_t)(kPoolThreads / 32) * n_head * D) * sizeof(float);
-  if (smem > 200 * 1024) return QAGNN_ERR_UNSUPPORTED;
-  static size_t attr[kMaxDevices] = {0};
-  const int dev = current_device();
-  if (smem > 48 * 1024 && smem > attr[dev]) {
-    QAGNN_CHECK_CUDA(cudaFuncSetAttribute(attention_pool_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr[dev] = smem;
-  }
+  const size_t smem = pool_smem_bytes(n, D, n_head);
+  if (smem > kPoolSmemCap) return QAGNN_ERR_UNSUPPORTED;
+  QAGNN_RETURN_IF(prepare_pool_launch(smem));
   attention_pool_kernel<<<B, kPoolThreads, smem, (cudaStream_t)stream>>>(n, D, n_head, X, qs, mask, wk, bk, wv, bv, pooled, attn, B);
   QAGNN_CHECK_LAUNCH();
   return QAGNN_OK;

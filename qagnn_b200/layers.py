@@ -74,13 +74,21 @@ class MultiheadAttPoolLayer(nn.Module):
         self.temperature = math.sqrt(self.d_k)
         self.attn_dropout = nn.Dropout(0.1)  # MatrixVectorScaledDotProductAttention's own dropout
         self.dropout = nn.Dropout(dropout)
-        self._fused_ok = True
+        # fewest nodes per graph the fused kernel has refused (its shared memory grows with the node count): longer inputs
+        # go straight to the einsum path, shorter ones still try the kernel
+        self._refused_len = None
+
+    def _fused_may_take(self, l):
+        return self._refused_len is None or l < self._refused_len
+
+    def _note_refused(self, l):
+        self._refused_len = l if self._refused_len is None else min(self._refused_len, l)
 
     def pool_concat(self, q, k, node_type, adj_lengths):
         """Eval-mode decoder tail in ONE kernel (qagnn_decoder_tail): derives the pool mask from adj_lengths / node_type,
         pools, and returns (cat(pooled, q, k[:, 0]) [b, 2*d_k_original + d_q_original], attn) — modeling_qagnn.py:172-187.
         Returns None when the fused kernel cannot take the shape (caller falls back to mask + forward + cat)."""
-        if (self.training or not k.is_cuda or k.dtype != torch.float32 or not self._fused_ok
+        if (self.training or not k.is_cuda or k.dtype != torch.float32 or not self._fused_may_take(k.size(1))
                 or (torch.is_grad_enabled() and (q.requires_grad or k.requires_grad))):
             return None
         from . import _lib
@@ -99,7 +107,7 @@ class MultiheadAttPoolLayer(nn.Module):
                                         _lib.ptr(self.w_vs.weight.detach()), _lib.ptr(self.w_vs.bias.detach()),
                                         _lib.ptr(concat), _lib.ptr(attn), _lib.stream_ptr(k.device))
         if st == -5:
-            self._fused_ok = False
+            self._note_refused(l)
             return None
         _lib.check(st, "qagnn_decoder_tail")
         return concat, attn
@@ -109,7 +117,7 @@ class MultiheadAttPoolLayer(nn.Module):
         nh, dk, dv = self.n_head, self.d_k, self.d_v
         wants_grad = torch.is_grad_enabled() and (q.requires_grad or k.requires_grad)  # the fused kernel is outside autograd
         if (k.is_cuda and not self.training and not wants_grad and mask is not None and k.dtype == torch.float32
-                and self.w_ks.weight.shape[0] == k.shape[2] and self._fused_ok):
+                and self.w_ks.weight.shape[0] == k.shape[2] and self._fused_may_take(l)):
             # fused kernel (one read of k, no ks/vs GEMMs): qagnn_attention_pool
             from . import _lib
             lib = _lib.load()
@@ -124,7 +132,7 @@ class MultiheadAttPoolLayer(nn.Module):
                                               _lib.ptr(self.w_vs.weight.detach()), _lib.ptr(self.w_vs.bias.detach()),
                                               _lib.ptr(pooled), _lib.ptr(attn), _lib.stream_ptr(k.device))
             if st == -5:  # QAGNN_ERR_UNSUPPORTED (node tile does not fit in shared memory): the einsum path below
-                self._fused_ok = False
+                self._note_refused(l)
             else:
                 _lib.check(st, "qagnn_attention_pool")
                 return pooled, attn

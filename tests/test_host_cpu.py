@@ -110,6 +110,25 @@ def test_size_queries_and_argument_checks(lib):
     assert lib.qagnn_mp_forward(C.byref(s), None, None, None, None, None, None, None, None, 0, None) == -1
 
 
+def test_pool_and_head_argument_refusals(lib):
+    """The decoder's pooling and head entry points refuse what their kernels do not take before any CUDA call."""
+    nul = [None] * 14
+    # more than 8 heads: unsupported; D % n_head != 0: invalid
+    assert lib.qagnn_attention_pool(2, 10, 36, 9, *nul[:10]) == -5
+    assert lib.qagnn_decoder_tail(2, 10, 36, 9, 8, *nul[:12]) == -5
+    assert lib.qagnn_attention_pool(2, 10, 10, 4, *nul[:10]) == -1
+    assert lib.qagnn_decoder_tail(2, 10, 10, 4, 8, *nul[:12]) == -1
+    # the head copies rows as float4: D % 4 != 0 is invalid
+    assert lib.qagnn_decoder_head(2, 10, 6, None, 50, *nul[:7]) == -1
+    # one node more than 200 KB of shared memory holds (10 nh D + nh n + nh + 16 floats): refused, so the module pools
+    # with its einsum path.  The pointers are never dereferenced on the host.
+    for nh, D in ((2, 200), (2, 1024), (8, 512)):
+        n = (200 * 1024 // 4 - 10 * nh * D - nh - 16) // nh + 1
+        p = [C.c_void_p(64)] * 12
+        assert lib.qagnn_attention_pool(1, n, D, nh, *p[:10]) == -5
+        assert lib.qagnn_decoder_tail(1, n, D, nh, 8, *p) == -5
+
+
 def test_state_dict_contract_and_cpu_refusal():
     mod = qagnn_b200.QAGNN_Message_Passing(None, 5, 4, 38, 200, 200, 200).eval()
     sd = O.random_state_dict(5, 200)
