@@ -18,6 +18,7 @@
  *   qagnn_mp_core_backward       (modeling_qagnn.py:442,455-484 under qagnn.py:249-278 loss.backward()):
  *                                message passing on node-level projections with the attention kept for backward,
  *                                and its gradient w.r.t. the projections and the two edge tables
+ *                                (_typed: the same on fp16 / bf16 operands, for training under torch.autocast)
  *
  * Conventions
  *   - every pointer is a DEVICE pointer unless its name ends in _host; the caller owns every
@@ -218,6 +219,21 @@ int32_t qagnn_mp_core_forward(const qagnn_shape *shape, const void *prep, const 
 int32_t qagnn_mp_core_backward(const qagnn_shape *shape, const void *prep, const int32_t *combo_order, const float *qkm,
                                const float *ke, const float *me, const float *alpha_scaled, const float *d_aggr,
                                float *d_qkm, float *d_ke, float *d_me, float *scratch, void *stream);
+
+/* The same two calls with the node and table operands stored as `dtype`: qkm, ke, me, aggr, d_aggr, d_qkm, d_ke and d_me are
+ * arrays of that type (the training loop's autocast dtype, so no cast to fp32 runs around the core); alpha_scaled, alpha_out and
+ * scratch stay fp32.  Loads widen exactly and all arithmetic is fp32, as in the fp32 calls: aggr and d_qkm are the fp32 results
+ * rounded once to nearest even, and d_ke / d_me are accumulated in fp32 (atomics, in `scratch`) and rounded once at the end.
+ * QAGNN_DTYPE_F32 runs the fp32 calls above.  `scratch` holds at least qagnn_mp_core_scratch_bytes(shape, dtype) bytes; 16-bit
+ * rows are read and written 4 elements (8 bytes) at a time.  QAGNN_ERR_INVALID_ARGUMENT for an unknown dtype. */
+enum { QAGNN_DTYPE_F32 = 0, QAGNN_DTYPE_F16 = 1, QAGNN_DTYPE_BF16 = 2 };
+size_t qagnn_mp_core_scratch_bytes(const qagnn_shape *shape, int32_t dtype);
+int32_t qagnn_mp_core_forward_typed(const qagnn_shape *shape, int32_t dtype, const void *prep, const void *qkm, const void *ke,
+                                    const void *me, void *aggr, float *alpha_scaled, float *alpha_out, float *scratch,
+                                    void *stream);
+int32_t qagnn_mp_core_backward_typed(const qagnn_shape *shape, int32_t dtype, const void *prep, const int32_t *combo_order,
+                                     const void *qkm, const void *ke, const void *me, const float *alpha_scaled,
+                                     const void *d_aggr, void *d_qkm, void *d_ke, void *d_me, float *scratch, void *stream);
 
 /* What the training path needs per batch besides the prep, without a host synchronisation: a stable counting sort of the
  * by-source positions [0, E') by qagnn_prep_layout.csr_src_combo, with E' = rowptr_src[N] read on the device (shape->N and

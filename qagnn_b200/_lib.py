@@ -63,6 +63,9 @@ EXPORTS = {
     "qagnn_mp_forward": (C.c_int32, [C.POINTER(Shape), _P, _P, _P, _P, _P, _P, _P, _P, C.c_size_t, _P]),
     "qagnn_mp_core_forward": (C.c_int32, [C.POINTER(Shape), _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "qagnn_mp_core_backward": (C.c_int32, [C.POINTER(Shape), _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
+    "qagnn_mp_core_scratch_bytes": (C.c_size_t, [C.POINTER(Shape), C.c_int32]),
+    "qagnn_mp_core_forward_typed": (C.c_int32, [C.POINTER(Shape), C.c_int32, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
+    "qagnn_mp_core_backward_typed": (C.c_int32, [C.POINTER(Shape), C.c_int32, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "qagnn_combo_sort_bytes": (C.c_size_t, [C.POINTER(Shape)]),
     "qagnn_combo_sort": (C.c_int32, [C.POINTER(Shape), _P, _P, _P, _P, C.c_size_t, _P]),
     "qagnn_linear_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int32, C.c_int32, C.c_int32]),
@@ -171,6 +174,10 @@ def f32c(t, name):
     if t.dtype != torch.float32:
         raise TypeError(f"qagnn_b200: `{name}` must be float32 (got {t.dtype})")
     return t.detach().contiguous()
+
+
+# dtype codes of the *_typed entry points (QAGNN_DTYPE_* in include/qagnn_b200.h)
+DTYPE_CODES = {torch.float32: 0, torch.float16: 1, torch.bfloat16: 2}
 
 
 def i64c(t, name):

@@ -190,6 +190,20 @@ int32_t launch_message_passing_backward(const qagnn_shape& s, const int32_t* pre
                                         const float* alpha_s, const float* d_aggr, float* ds, float* d_qkm, float* d_ke,
                                         float* d_me, cudaStream_t st);
 
+// The training core on operands stored as `dtype` (QAGNN_DTYPE_*): qkm, ke, me, aggr, d_aggr, d_qkm, d_ke, d_me of that type;
+// score / alpha / alpha_out / alpha_s and the scratch fp32.  QAGNN_DTYPE_F32 runs exactly the two launchers above.
+int32_t launch_message_passing_typed(const qagnn_shape& s, const int32_t* prep_base, const qagnn_prep_layout& pl,
+                                     int32_t dtype, const void* qkm, const void* ke, const void* me, float* score,
+                                     float* alpha, void* aggr, float* alpha_out, cudaStream_t st);
+int32_t launch_message_passing_backward_typed(const qagnn_shape& s, const int32_t* prep_base, const qagnn_prep_layout& pl,
+                                              int32_t dtype, const int32_t* combo_order, const void* qkm, const void* ke,
+                                              const void* me, const float* alpha_s, const void* d_aggr, float* scratch,
+                                              void* d_qkm, void* d_ke, void* d_me, cudaStream_t st);
+// floats of the [E+N, H] ds array at the start of the backward scratch, rounded up to 256 bytes
+size_t mp_core_ds_floats(const qagnn_shape& s);
+// scratch bytes of qagnn_mp_core_forward_typed / _backward_typed: ds, plus the fp32 d_ke / d_me accumulators of a 16-bit call
+size_t mp_core_scratch_bytes(const qagnn_shape& s, int32_t dtype);
+
 // Exclusive scan of one int per thread over a 1024-thread block; *total = the block's sum.  Every thread must call it.
 __device__ __forceinline__ int block_exclusive_scan_1024(int v, int* total) {
   __shared__ int warp_sums[32];

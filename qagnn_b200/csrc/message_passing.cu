@@ -11,7 +11,7 @@
 //   mp_aggregate_kernel  one warp per TARGET node  : weighted sum of messages
 // No atomics, no global max/sum scratch passes; every summation runs in edge-id order, so results
 // are deterministic and follow the reference's CPU summation order.
-#include "common.cuh"
+#include "storage.cuh"
 
 namespace qagnn {
 
@@ -32,14 +32,13 @@ __device__ __forceinline__ HeadMap head_map(int c, int d) {
   return m;
 }
 
-__device__ __forceinline__ float4 ld4(const float* p) { return *reinterpret_cast<const float4*>(p); }
-
-template <int H, int CH>
+// S: storage type of qkm / ke (float, __half, __nv_bfloat16); the arithmetic is fp32 for every S
+template <int H, int CH, typename S>
 __global__ void __launch_bounds__(256) mp_scores_kernel(int64_t N, int D, const int32_t* __restrict__ rowptr_src,
                                                         const int32_t* __restrict__ csr_src_tgt,
                                                         const int32_t* __restrict__ csr_src_combo,
                                                         const int32_t* __restrict__ perm_src,
-                                                        const float* __restrict__ qkm, const float* __restrict__ ke,
+                                                        const S* __restrict__ qkm, const S* __restrict__ ke,
                                                         float* __restrict__ score, float* __restrict__ alpha,
                                                         float* __restrict__ alpha_out) {
   const int lane = threadIdx.x & 31;
@@ -56,7 +55,7 @@ __global__ void __launch_bounds__(256) mp_scores_kernel(int64_t N, int D, const 
     const int c = lane + 32 * i;
     valid[i] = 4 * c < D;
     hm[i] = head_map(c, d);
-    q[i] = valid[i] ? ld4(qkm + v * ld + 4 * c) : make_float4(0.f, 0.f, 0.f, 0.f);
+    q[i] = valid[i] ? load4(qkm + v * ld + 4 * c) : make_float4(0.f, 0.f, 0.f, 0.f);
   }
 
   const int beg = rowptr_src[v], end = rowptr_src[v + 1];
@@ -75,8 +74,8 @@ __global__ void __launch_bounds__(256) mp_scores_kernel(int64_t N, int D, const 
     for (int i = 0; i < CH; ++i) {
       if (!valid[i]) continue;
       const int c = lane + 32 * i;
-      const float4 kx = ld4(qkm + (int64_t)t * ld + D + 4 * c);
-      const float4 kt = ld4(ke + (int64_t)cb * D + 4 * c);
+      const float4 kx = load4(qkm + (int64_t)t * ld + D + 4 * c);
+      const float4 kt = load4(ke + (int64_t)cb * D + 4 * c);
       const float p0 = q[i].x * (kx.x + kt.x), p1 = q[i].y * (kx.y + kt.y);
       const float p2 = q[i].z * (kx.z + kt.z), p3 = q[i].w * (kx.w + kt.w);
       if (hm[i].first == hm[i].last) {
@@ -132,13 +131,14 @@ __global__ void __launch_bounds__(256) mp_scores_kernel(int64_t N, int D, const 
   }
 }
 
-template <int H, int CH>
+// S: storage type of qkm / me / aggr; aggr is accumulated in fp32 and rounded once
+template <int H, int CH, typename S>
 __global__ void __launch_bounds__(256) mp_aggregate_kernel(int64_t N, int D, const int32_t* __restrict__ rowptr_tgt,
                                                            const int32_t* __restrict__ csr_tgt_src,
                                                            const int32_t* __restrict__ csr_tgt_combo,
                                                            const int32_t* __restrict__ csr_tgt_apos,
-                                                           const float* __restrict__ qkm, const float* __restrict__ me,
-                                                           const float* __restrict__ alpha, float* __restrict__ aggr) {
+                                                           const S* __restrict__ qkm, const S* __restrict__ me,
+                                                           const float* __restrict__ alpha, S* __restrict__ aggr) {
   const int lane = threadIdx.x & 31;
   const int64_t v = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
   if (v >= N) return;
@@ -163,8 +163,8 @@ __global__ void __launch_bounds__(256) mp_aggregate_kernel(int64_t N, int D, con
     for (int i = 0; i < CH; ++i) {
       if (!valid[i]) continue;
       const int c = lane + 32 * i;
-      const float4 mxv = ld4(qkm + (int64_t)s * ld + 2 * D + 4 * c);
-      const float4 mt = ld4(me + (int64_t)cb * D + 4 * c);
+      const float4 mxv = load4(qkm + (int64_t)s * ld + 2 * D + 4 * c);
+      const float4 mt = load4(me + (int64_t)cb * D + 4 * c);
       float w0, w1, w2, w3;
       if (hm[i].first == hm[i].last) {
         w0 = w1 = w2 = w3 = ap[hm[i].first];
@@ -180,43 +180,41 @@ __global__ void __launch_bounds__(256) mp_aggregate_kernel(int64_t N, int D, con
 #pragma unroll
   for (int i = 0; i < CH; ++i) {
     if (!valid[i]) continue;
-    *reinterpret_cast<float4*>(aggr + v * D + 4 * (lane + 32 * i)) = acc[i];
+    store4(aggr + v * D + 4 * (lane + 32 * i), acc[i]);
   }
 }
 
-template <int H, int CH>
-int32_t launch_hc(const qagnn_shape& s, const int32_t* base, const qagnn_prep_layout& pl, const float* qkm,
-                  const float* ke, const float* me, float* score, float* alpha, float* aggr, float* alpha_out,
+template <int H, int CH, typename S>
+int32_t launch_hc(const qagnn_shape& s, const int32_t* base, const qagnn_prep_layout& pl, const S* qkm,
+                  const S* ke, const S* me, float* score, float* alpha, S* aggr, float* alpha_out,
                   cudaStream_t st) {
   auto I = [&](size_t off) { return (const int32_t*)((const char*)base + off); };
   const int block = 256;
   const unsigned grid = (unsigned)((s.N * 32 + block - 1) / block);
-  mp_scores_kernel<H, CH><<<grid, block, 0, st>>>(s.N, s.D, I(pl.rowptr_src), I(pl.csr_src_tgt), I(pl.csr_src_combo),
+  mp_scores_kernel<H, CH, S><<<grid, block, 0, st>>>(s.N, s.D, I(pl.rowptr_src), I(pl.csr_src_tgt), I(pl.csr_src_combo),
                                                   I(pl.perm_src), qkm, ke, score, alpha, alpha_out);
   QAGNN_CHECK_LAUNCH();
-  mp_aggregate_kernel<H, CH><<<grid, block, 0, st>>>(s.N, s.D, I(pl.rowptr_tgt), I(pl.csr_tgt_src),
+  mp_aggregate_kernel<H, CH, S><<<grid, block, 0, st>>>(s.N, s.D, I(pl.rowptr_tgt), I(pl.csr_tgt_src),
                                                      I(pl.csr_tgt_combo), I(pl.csr_tgt_apos), qkm, me, alpha, aggr);
   QAGNN_CHECK_LAUNCH();
   return QAGNN_OK;
 }
 
-template <int H>
-int32_t launch_h(const qagnn_shape& s, const int32_t* base, const qagnn_prep_layout& pl, const float* qkm,
-                 const float* ke, const float* me, float* score, float* alpha, float* aggr, float* alpha_out,
+template <int H, typename S>
+int32_t launch_h(const qagnn_shape& s, const int32_t* base, const qagnn_prep_layout& pl, const S* qkm,
+                 const S* ke, const S* me, float* score, float* alpha, S* aggr, float* alpha_out,
                  cudaStream_t st) {
   const int ch = (s.D + 127) / 128;
-  if (ch <= 1) return launch_hc<H, 1>(s, base, pl, qkm, ke, me, score, alpha, aggr, alpha_out, st);
-  if (ch <= 2) return launch_hc<H, 2>(s, base, pl, qkm, ke, me, score, alpha, aggr, alpha_out, st);
-  if (ch <= 4) return launch_hc<H, 4>(s, base, pl, qkm, ke, me, score, alpha, aggr, alpha_out, st);
-  if (ch <= 8) return launch_hc<H, 8>(s, base, pl, qkm, ke, me, score, alpha, aggr, alpha_out, st);
+  if (ch <= 1) return launch_hc<H, 1, S>(s, base, pl, qkm, ke, me, score, alpha, aggr, alpha_out, st);
+  if (ch <= 2) return launch_hc<H, 2, S>(s, base, pl, qkm, ke, me, score, alpha, aggr, alpha_out, st);
+  if (ch <= 4) return launch_hc<H, 4, S>(s, base, pl, qkm, ke, me, score, alpha, aggr, alpha_out, st);
+  if (ch <= 8) return launch_hc<H, 8, S>(s, base, pl, qkm, ke, me, score, alpha, aggr, alpha_out, st);
   return QAGNN_ERR_UNSUPPORTED;
 }
 
-}  // namespace
-
-int32_t launch_message_passing(const qagnn_shape& s, const int32_t* prep_base, const qagnn_prep_layout& pl,
-                               const float* qkm, const float* ke, const float* me, float* score, float* alpha,
-                               float* aggr, float* alpha_out, cudaStream_t st) {
+template <typename S>
+int32_t launch_mp(const qagnn_shape& s, const int32_t* prep_base, const qagnn_prep_layout& pl, const S* qkm, const S* ke,
+                  const S* me, float* score, float* alpha, S* aggr, float* alpha_out, cudaStream_t st) {
   if (s.D % 4 != 0 || s.D > 1024) return QAGNN_ERR_UNSUPPORTED;
   switch (s.H) {
     case 1: return launch_h<1>(s, prep_base, pl, qkm, ke, me, score, alpha, aggr, alpha_out, st);
@@ -225,6 +223,31 @@ int32_t launch_message_passing(const qagnn_shape& s, const int32_t* prep_base, c
     case 8: return launch_h<8>(s, prep_base, pl, qkm, ke, me, score, alpha, aggr, alpha_out, st);
     case 16: return launch_h<16>(s, prep_base, pl, qkm, ke, me, score, alpha, aggr, alpha_out, st);
     default: return QAGNN_ERR_UNSUPPORTED;
+  }
+}
+
+}  // namespace
+
+int32_t launch_message_passing(const qagnn_shape& s, const int32_t* prep_base, const qagnn_prep_layout& pl,
+                               const float* qkm, const float* ke, const float* me, float* score, float* alpha,
+                               float* aggr, float* alpha_out, cudaStream_t st) {
+  return launch_mp(s, prep_base, pl, qkm, ke, me, score, alpha, aggr, alpha_out, st);
+}
+
+int32_t launch_message_passing_typed(const qagnn_shape& s, const int32_t* prep_base, const qagnn_prep_layout& pl,
+                                     int32_t dtype, const void* qkm, const void* ke, const void* me, float* score,
+                                     float* alpha, void* aggr, float* alpha_out, cudaStream_t st) {
+  switch (dtype) {
+    case QAGNN_DTYPE_F32:
+      return launch_mp(s, prep_base, pl, (const float*)qkm, (const float*)ke, (const float*)me, score, alpha, (float*)aggr,
+                       alpha_out, st);
+    case QAGNN_DTYPE_F16:
+      return launch_mp(s, prep_base, pl, (const __half*)qkm, (const __half*)ke, (const __half*)me, score, alpha,
+                       (__half*)aggr, alpha_out, st);
+    case QAGNN_DTYPE_BF16:
+      return launch_mp(s, prep_base, pl, (const __nv_bfloat16*)qkm, (const __nv_bfloat16*)ke, (const __nv_bfloat16*)me,
+                       score, alpha, (__nv_bfloat16*)aggr, alpha_out, st);
+    default: return QAGNN_ERR_INVALID_ARGUMENT;
   }
 }
 

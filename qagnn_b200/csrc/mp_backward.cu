@@ -14,7 +14,9 @@
 //   mp_bwd_target_kernel   one warp per TARGET node: dKx                                                    no atomics
 //   mp_bwd_table_kernel    one warp per run of 64 edges in COMBO order: register partial sums, one vector
 //                          atomic add per (run, combo change) into dKe / dMe — the only atomics, a few thousand adds
-#include "common.cuh"
+#include <type_traits>
+
+#include "storage.cuh"
 
 namespace qagnn {
 
@@ -32,7 +34,6 @@ __device__ __forceinline__ HeadMap4 head_map4(int c, int d) {
   m.last = m.hid[3];
   return m;
 }
-__device__ __forceinline__ float4 ld4(const float* p) { return *reinterpret_cast<const float4*>(p); }
 
 // per-head partial sums of the 4 products of one float4 chunk
 template <int H>
@@ -59,27 +60,30 @@ __device__ __forceinline__ float pick(const float (&w)[H], int h) {
   return r;
 }
 
-template <int H, int CH>
+// S: storage type of the node and table operands (float, __half, __nv_bfloat16): loads widen exactly, the arithmetic is
+// fp32 for every S, and d_qkm is rounded once when stored.  ds and alpha_s stay fp32.
+template <int H, int CH, typename S>
 __global__ void __launch_bounds__(256) mp_bwd_source_kernel(int64_t N, int D, const int32_t* __restrict__ rowptr_src,
                                                             const int32_t* __restrict__ csr_src_tgt,
                                                             const int32_t* __restrict__ csr_src_combo,
-                                                            const float* __restrict__ qkm, const float* __restrict__ ke,
-                                                            const float* __restrict__ me, const float* __restrict__ alpha_s,
-                                                            const float* __restrict__ d_aggr, float* __restrict__ ds,
-                                                            float* __restrict__ d_qkm) {
+                                                            const S* __restrict__ qkm, const S* __restrict__ ke,
+                                                            const S* __restrict__ me, const float* __restrict__ alpha_s,
+                                                            const S* __restrict__ d_aggr, float* __restrict__ ds,
+                                                            S* __restrict__ d_qkm) {
   const int lane = threadIdx.x & 31;
   const int64_t u = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
   if (u >= N) return;
   const int d = D / H, ld = 3 * D;
   HeadMap4 hm[CH];
   bool valid[CH];
-  float4 mx[CH], dq[CH], dmx[CH];
+  typename Packed4<S>::type mxp[CH];  // Mx[u], widened at each use
+  float4 dq[CH], dmx[CH];
 #pragma unroll
   for (int i = 0; i < CH; ++i) {
     const int c = lane + 32 * i;
     valid[i] = 4 * c < D;
     hm[i] = head_map4(c, d);
-    mx[i] = valid[i] ? ld4(qkm + u * ld + 2 * D + 4 * c) : make_float4(0.f, 0.f, 0.f, 0.f);
+    mxp[i] = valid[i] ? load_packed4(qkm + u * ld + 2 * D + 4 * c) : zero_packed4<S>();
     dq[i] = dmx[i] = make_float4(0.f, 0.f, 0.f, 0.f);
   }
   const int beg = rowptr_src[u], end = rowptr_src[u + 1];
@@ -100,9 +104,10 @@ __global__ void __launch_bounds__(256) mp_bwd_source_kernel(int64_t N, int D, co
     for (int i = 0; i < CH; ++i) {
       if (!valid[i]) continue;
       const int c = lane + 32 * i;
-      const float4 g = ld4(d_aggr + (int64_t)t * D + 4 * c);
-      const float4 mt = ld4(me + (int64_t)cb * D + 4 * c);
-      add_parts<H>(part, hm[i], g.x * (mx[i].x + mt.x), g.y * (mx[i].y + mt.y), g.z * (mx[i].z + mt.z), g.w * (mx[i].w + mt.w));
+      const float4 g = load4(d_aggr + (int64_t)t * D + 4 * c);
+      const float4 mt = load4(me + (int64_t)cb * D + 4 * c);
+      const float4 mx = widen4(mxp[i], qkm);
+      add_parts<H>(part, hm[i], g.x * (mx.x + mt.x), g.y * (mx.y + mt.y), g.z * (mx.z + mt.z), g.w * (mx.w + mt.w));
       dmx[i].x += pick<H>(as, hm[i].hid[0]) * g.x;
       dmx[i].y += pick<H>(as, hm[i].hid[1]) * g.y;
       dmx[i].z += pick<H>(as, hm[i].hid[2]) * g.z;
@@ -131,8 +136,8 @@ __global__ void __launch_bounds__(256) mp_bwd_source_kernel(int64_t N, int D, co
     for (int i = 0; i < CH; ++i) {
       if (!valid[i]) continue;
       const int c = lane + 32 * i;
-      const float4 kx = ld4(qkm + (int64_t)t * ld + D + 4 * c);
-      const float4 kt = ld4(ke + (int64_t)cb * D + 4 * c);
+      const float4 kx = load4(qkm + (int64_t)t * ld + D + 4 * c);
+      const float4 kt = load4(ke + (int64_t)cb * D + 4 * c);
       dq[i].x += pick<H>(dsv, hm[i].hid[0]) * (kx.x + kt.x);
       dq[i].y += pick<H>(dsv, hm[i].hid[1]) * (kx.y + kt.y);
       dq[i].z += pick<H>(dsv, hm[i].hid[2]) * (kx.z + kt.z);
@@ -150,17 +155,17 @@ __global__ void __launch_bounds__(256) mp_bwd_source_kernel(int64_t N, int D, co
   for (int i = 0; i < CH; ++i) {
     if (!valid[i]) continue;
     const int c = lane + 32 * i;
-    *reinterpret_cast<float4*>(d_qkm + u * ld + 4 * c) = dq[i];
-    *reinterpret_cast<float4*>(d_qkm + u * ld + 2 * D + 4 * c) = dmx[i];
+    store4(d_qkm + u * ld + 4 * c, dq[i]);
+    store4(d_qkm + u * ld + 2 * D + 4 * c, dmx[i]);
   }
 }
 
-template <int H, int CH>
+template <int H, int CH, typename S>
 __global__ void __launch_bounds__(256) mp_bwd_target_kernel(int64_t N, int D, const int32_t* __restrict__ rowptr_tgt,
                                                             const int32_t* __restrict__ csr_tgt_src,
                                                             const int32_t* __restrict__ csr_tgt_apos,
-                                                            const float* __restrict__ qkm, const float* __restrict__ ds,
-                                                            float* __restrict__ d_qkm) {
+                                                            const S* __restrict__ qkm, const float* __restrict__ ds,
+                                                            S* __restrict__ d_qkm) {
   const int lane = threadIdx.x & 31;
   const int64_t v = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
   if (v >= N) return;
@@ -186,7 +191,7 @@ __global__ void __launch_bounds__(256) mp_bwd_target_kernel(int64_t N, int D, co
     for (int i = 0; i < CH; ++i) {
       if (!valid[i]) continue;
       const int c = lane + 32 * i;
-      const float4 q = ld4(qkm + (int64_t)s * ld + 4 * c);
+      const float4 q = load4(qkm + (int64_t)s * ld + 4 * c);
       acc[i].x += pick<H>(dsv, hm[i].hid[0]) * q.x;
       acc[i].y += pick<H>(dsv, hm[i].hid[1]) * q.y;
       acc[i].z += pick<H>(dsv, hm[i].hid[2]) * q.z;
@@ -196,7 +201,7 @@ __global__ void __launch_bounds__(256) mp_bwd_target_kernel(int64_t N, int D, co
 #pragma unroll
   for (int i = 0; i < CH; ++i) {
     if (!valid[i]) continue;
-    *reinterpret_cast<float4*>(d_qkm + v * ld + D + 4 * (lane + 32 * i)) = acc[i];
+    store4(d_qkm + v * ld + D + 4 * (lane + 32 * i), acc[i]);
   }
 }
 
@@ -206,15 +211,16 @@ __device__ __forceinline__ void atomic_add4(float* p, const float4& v) {
   atomicAdd(p, v.x); atomicAdd(p + 1, v.y); atomicAdd(p + 2, v.z); atomicAdd(p + 3, v.w);
 }
 
-template <int H, int CH>
+// d_ke / d_me are fp32 for every S (the accumulators of a 16-bit call, rounded afterwards by round_rows_kernel)
+template <int H, int CH, typename S>
 __global__ void __launch_bounds__(256) mp_bwd_table_kernel(int64_t N, int D, const int32_t* __restrict__ rowptr_src,
                                                            const int32_t* __restrict__ combo_order,
                                                            const int32_t* __restrict__ csr_src_tgt,
                                                            const int32_t* __restrict__ csr_src_combo,
                                                            const int32_t* __restrict__ perm_src,
-                                                           const int32_t* __restrict__ src, const float* __restrict__ qkm,
+                                                           const int32_t* __restrict__ src, const S* __restrict__ qkm,
                                                            const float* __restrict__ alpha_s, const float* __restrict__ ds,
-                                                           const float* __restrict__ d_aggr, float* __restrict__ d_ke,
+                                                           const S* __restrict__ d_aggr, float* __restrict__ d_ke,
                                                            float* __restrict__ d_me) {
   const int lane = threadIdx.x & 31;
   const int64_t w = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
@@ -263,8 +269,8 @@ __global__ void __launch_bounds__(256) mp_bwd_table_kernel(int64_t N, int D, con
     for (int k = 0; k < CH; ++k) {
       if (!valid[k]) continue;
       const int c = lane + 32 * k;
-      const float4 q = ld4(qkm + (int64_t)s * ld + 4 * c);
-      const float4 g = ld4(d_aggr + (int64_t)t * D + 4 * c);
+      const float4 q = load4(qkm + (int64_t)s * ld + 4 * c);
+      const float4 g = load4(d_aggr + (int64_t)t * D + 4 * c);
       ak[k].x += pick<H>(dsv, hm[k].hid[0]) * q.x; am[k].x += pick<H>(as, hm[k].hid[0]) * g.x;
       ak[k].y += pick<H>(dsv, hm[k].hid[1]) * q.y; am[k].y += pick<H>(as, hm[k].hid[1]) * g.y;
       ak[k].z += pick<H>(dsv, hm[k].hid[2]) * q.z; am[k].z += pick<H>(as, hm[k].hid[2]) * g.z;
@@ -274,10 +280,18 @@ __global__ void __launch_bounds__(256) mp_bwd_table_kernel(int64_t N, int D, con
   if (cur >= 0) flush(cur);
 }
 
-template <int H, int CH>
+// out[i] = acc[i] rounded to nearest even, 4 elements per thread (n % 4 == 0)
+template <typename S>
+__global__ void __launch_bounds__(256) round_rows_kernel(int64_t n4, const float* __restrict__ acc, S* __restrict__ out) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x)
+    store4(out + 4 * i, load4(acc + 4 * i));
+}
+
+// d_ke / d_me: fp32 outputs (S = float), or fp32 accumulators that are rounded into the S outputs ke_out / me_out
+template <int H, int CH, typename S>
 int32_t launch_bwd_hc(const qagnn_shape& s, const int32_t* base, const qagnn_prep_layout& pl, const int32_t* combo_order,
-                      const float* qkm, const float* ke, const float* me, const float* alpha_s, const float* d_aggr,
-                      float* ds, float* d_qkm, float* d_ke, float* d_me, cudaStream_t st) {
+                      const S* qkm, const S* ke, const S* me, const float* alpha_s, const S* d_aggr,
+                      float* ds, S* d_qkm, float* d_ke, float* d_me, S* ke_out, S* me_out, cudaStream_t st) {
   auto I = [&](size_t off) { return (const int32_t*)((const char*)base + off); };
   const int block = 256;
   const unsigned grid = (unsigned)((s.N * 32 + block - 1) / block);
@@ -285,46 +299,105 @@ int32_t launch_bwd_hc(const qagnn_shape& s, const int32_t* base, const qagnn_pre
   const int C = s.R * s.T * s.T + s.T;
   QAGNN_CHECK_CUDA(cudaMemsetAsync(d_ke, 0, (size_t)C * s.D * sizeof(float), st));
   QAGNN_CHECK_CUDA(cudaMemsetAsync(d_me, 0, (size_t)C * s.D * sizeof(float), st));
-  mp_bwd_source_kernel<H, CH><<<grid, block, 0, st>>>(s.N, s.D, I(pl.rowptr_src), I(pl.csr_src_tgt), I(pl.csr_src_combo), qkm,
+  mp_bwd_source_kernel<H, CH, S><<<grid, block, 0, st>>>(s.N, s.D, I(pl.rowptr_src), I(pl.csr_src_tgt), I(pl.csr_src_combo), qkm,
                                                       ke, me, alpha_s, d_aggr, ds, d_qkm);
   QAGNN_CHECK_LAUNCH();
-  mp_bwd_target_kernel<H, CH><<<grid, block, 0, st>>>(s.N, s.D, I(pl.rowptr_tgt), I(pl.csr_tgt_src), I(pl.csr_tgt_apos), qkm, ds,
+  mp_bwd_target_kernel<H, CH, S><<<grid, block, 0, st>>>(s.N, s.D, I(pl.rowptr_tgt), I(pl.csr_tgt_src), I(pl.csr_tgt_apos), qkm, ds,
                                                       d_qkm);
   QAGNN_CHECK_LAUNCH();
   const int64_t runs = (Ep + kTableRun - 1) / kTableRun;
-  mp_bwd_table_kernel<H, CH><<<(unsigned)((runs * 32 + block - 1) / block), block, 0, st>>>(
+  mp_bwd_table_kernel<H, CH, S><<<(unsigned)((runs * 32 + block - 1) / block), block, 0, st>>>(
       s.N, s.D, I(pl.rowptr_src), combo_order, I(pl.csr_src_tgt), I(pl.csr_src_combo), I(pl.perm_src), I(pl.src), qkm, alpha_s, ds, d_aggr, d_ke,
       d_me);
   QAGNN_CHECK_LAUNCH();
+  if constexpr (!std::is_same<S, float>::value) {
+    const int64_t n4 = (int64_t)C * s.D / 4;
+    const int64_t blocks = (n4 + block - 1) / block;
+    const unsigned g = (unsigned)(blocks < 8 * kNumSMs ? blocks : 8 * kNumSMs);
+    round_rows_kernel<S><<<g, block, 0, st>>>(n4, d_ke, ke_out);
+    QAGNN_CHECK_LAUNCH();
+    round_rows_kernel<S><<<g, block, 0, st>>>(n4, d_me, me_out);
+    QAGNN_CHECK_LAUNCH();
+  }
   return QAGNN_OK;
 }
 
-template <int H>
+template <int H, typename S>
 int32_t launch_bwd_h(const qagnn_shape& s, const int32_t* base, const qagnn_prep_layout& pl, const int32_t* combo_order,
-                     const float* qkm, const float* ke, const float* me, const float* alpha_s, const float* d_aggr, float* ds,
-                     float* d_qkm, float* d_ke, float* d_me, cudaStream_t st) {
+                     const S* qkm, const S* ke, const S* me, const float* alpha_s, const S* d_aggr, float* ds,
+                     S* d_qkm, float* d_ke, float* d_me, S* ke_out, S* me_out, cudaStream_t st) {
   const int ch = (s.D + 127) / 128;
-  if (ch <= 1) return launch_bwd_hc<H, 1>(s, base, pl, combo_order, qkm, ke, me, alpha_s, d_aggr, ds, d_qkm, d_ke, d_me, st);
-  if (ch <= 2) return launch_bwd_hc<H, 2>(s, base, pl, combo_order, qkm, ke, me, alpha_s, d_aggr, ds, d_qkm, d_ke, d_me, st);
-  if (ch <= 4) return launch_bwd_hc<H, 4>(s, base, pl, combo_order, qkm, ke, me, alpha_s, d_aggr, ds, d_qkm, d_ke, d_me, st);
-  if (ch <= 8) return launch_bwd_hc<H, 8>(s, base, pl, combo_order, qkm, ke, me, alpha_s, d_aggr, ds, d_qkm, d_ke, d_me, st);
+  if (ch <= 1) return launch_bwd_hc<H, 1, S>(s, base, pl, combo_order, qkm, ke, me, alpha_s, d_aggr, ds, d_qkm, d_ke, d_me, ke_out,
+                                             me_out, st);
+  if (ch <= 2) return launch_bwd_hc<H, 2, S>(s, base, pl, combo_order, qkm, ke, me, alpha_s, d_aggr, ds, d_qkm, d_ke, d_me, ke_out,
+                                             me_out, st);
+  if (ch <= 4) return launch_bwd_hc<H, 4, S>(s, base, pl, combo_order, qkm, ke, me, alpha_s, d_aggr, ds, d_qkm, d_ke, d_me, ke_out,
+                                             me_out, st);
+  if (ch <= 8) return launch_bwd_hc<H, 8, S>(s, base, pl, combo_order, qkm, ke, me, alpha_s, d_aggr, ds, d_qkm, d_ke, d_me, ke_out,
+                                             me_out, st);
   return QAGNN_ERR_UNSUPPORTED;
 }
 
+template <typename S>
+int32_t launch_bwd(const qagnn_shape& s, const int32_t* prep_base, const qagnn_prep_layout& pl, const int32_t* combo_order,
+                   const S* qkm, const S* ke, const S* me, const float* alpha_s, const S* d_aggr, float* ds, S* d_qkm,
+                   float* d_ke, float* d_me, S* ke_out, S* me_out, cudaStream_t st) {
+  if (s.D % 4 != 0 || s.D > 1024) return QAGNN_ERR_UNSUPPORTED;
+#define QAGNN_BWD_ARGS s, prep_base, pl, combo_order, qkm, ke, me, alpha_s, d_aggr, ds, d_qkm, d_ke, d_me, ke_out, me_out, st
+  switch (s.H) {
+    case 1: return launch_bwd_h<1>(QAGNN_BWD_ARGS);
+    case 2: return launch_bwd_h<2>(QAGNN_BWD_ARGS);
+    case 4: return launch_bwd_h<4>(QAGNN_BWD_ARGS);
+    case 8: return launch_bwd_h<8>(QAGNN_BWD_ARGS);
+    case 16: return launch_bwd_h<16>(QAGNN_BWD_ARGS);
+    default: return QAGNN_ERR_UNSUPPORTED;
+  }
+#undef QAGNN_BWD_ARGS
+}
+
+// a 16-bit call accumulates d_ke / d_me in fp32 after the [E+N, H] floats of ds in the scratch, then rounds them once
+template <typename S>
+int32_t launch_bwd_16(const qagnn_shape& s, const int32_t* prep_base, const qagnn_prep_layout& pl, const int32_t* combo_order,
+                      const void* qkm, const void* ke, const void* me, const float* alpha_s, const void* d_aggr, float* scratch,
+                      void* d_qkm, void* d_ke, void* d_me, cudaStream_t st) {
+  const size_t C = (size_t)s.R * s.T * s.T + s.T;
+  float* acc = scratch + mp_core_ds_floats(s);
+  return launch_bwd(s, prep_base, pl, combo_order, (const S*)qkm, (const S*)ke, (const S*)me, alpha_s, (const S*)d_aggr, scratch,
+                    (S*)d_qkm, acc, acc + C * s.D, (S*)d_ke, (S*)d_me, st);
+}
+
 }  // namespace
+
+size_t mp_core_ds_floats(const qagnn_shape& s) { return align_up((size_t)(s.N + s.E) * s.H, kAlign / sizeof(float)); }
+
+size_t mp_core_scratch_bytes(const qagnn_shape& s, int32_t dtype) {
+  const size_t C = (size_t)s.R * s.T * s.T + s.T;
+  return sizeof(float) * (mp_core_ds_floats(s) + (dtype == QAGNN_DTYPE_F32 ? 0 : 2 * C * s.D));
+}
 
 int32_t launch_message_passing_backward(const qagnn_shape& s, const int32_t* prep_base, const qagnn_prep_layout& pl,
                                         const int32_t* combo_order, const float* qkm, const float* ke, const float* me,
                                         const float* alpha_s, const float* d_aggr, float* ds, float* d_qkm, float* d_ke,
                                         float* d_me, cudaStream_t st) {
-  if (s.D % 4 != 0 || s.D > 1024) return QAGNN_ERR_UNSUPPORTED;
-  switch (s.H) {
-    case 1: return launch_bwd_h<1>(s, prep_base, pl, combo_order, qkm, ke, me, alpha_s, d_aggr, ds, d_qkm, d_ke, d_me, st);
-    case 2: return launch_bwd_h<2>(s, prep_base, pl, combo_order, qkm, ke, me, alpha_s, d_aggr, ds, d_qkm, d_ke, d_me, st);
-    case 4: return launch_bwd_h<4>(s, prep_base, pl, combo_order, qkm, ke, me, alpha_s, d_aggr, ds, d_qkm, d_ke, d_me, st);
-    case 8: return launch_bwd_h<8>(s, prep_base, pl, combo_order, qkm, ke, me, alpha_s, d_aggr, ds, d_qkm, d_ke, d_me, st);
-    case 16: return launch_bwd_h<16>(s, prep_base, pl, combo_order, qkm, ke, me, alpha_s, d_aggr, ds, d_qkm, d_ke, d_me, st);
-    default: return QAGNN_ERR_UNSUPPORTED;
+  return launch_bwd<float>(s, prep_base, pl, combo_order, qkm, ke, me, alpha_s, d_aggr, ds, d_qkm, d_ke, d_me, nullptr, nullptr,
+                           st);
+}
+
+int32_t launch_message_passing_backward_typed(const qagnn_shape& s, const int32_t* prep_base, const qagnn_prep_layout& pl,
+                                              int32_t dtype, const int32_t* combo_order, const void* qkm, const void* ke,
+                                              const void* me, const float* alpha_s, const void* d_aggr, float* scratch,
+                                              void* d_qkm, void* d_ke, void* d_me, cudaStream_t st) {
+  switch (dtype) {
+    case QAGNN_DTYPE_F32:
+      return launch_message_passing_backward(s, prep_base, pl, combo_order, (const float*)qkm, (const float*)ke, (const float*)me,
+                                             alpha_s, (const float*)d_aggr, scratch, (float*)d_qkm, (float*)d_ke, (float*)d_me,
+                                             st);
+    case QAGNN_DTYPE_F16:
+      return launch_bwd_16<__half>(s, prep_base, pl, combo_order, qkm, ke, me, alpha_s, d_aggr, scratch, d_qkm, d_ke, d_me, st);
+    case QAGNN_DTYPE_BF16:
+      return launch_bwd_16<__nv_bfloat16>(s, prep_base, pl, combo_order, qkm, ke, me, alpha_s, d_aggr, scratch, d_qkm, d_ke,
+                                          d_me, st);
+    default: return QAGNN_ERR_INVALID_ARGUMENT;
   }
 }
 

@@ -213,8 +213,10 @@ class TrainStep:
     gradients accumulate into `.grad` as in eager mode; dL/dsent_vecs reaches `sent_vecs`, and dL/dnode_scores reaches
     `node_scores` when it requires grad.  `pool_attn` is returned without a gradient.  Both outputs are static buffers that
     the next call overwrites.  Dropout draws a new mask on every replay and BatchNorm running statistics advance on every
-    replay, as in eager mode.  `autocast_dtype` (None or torch.float16) runs capture and calls under
-    torch.autocast(cache_enabled=False); the message passing keeps fp32 inside.  Construction runs two warm-up iterations
+    replay, as in eager mode.  `autocast_dtype` (None, torch.float16 or torch.bfloat16) runs capture and calls under
+    torch.autocast(cache_enabled=False); the message-passing kernels read and write that dtype and compute in fp32 inside, and
+    the edge encoder's BatchNorm moments stay fp32.  fp16 needs a GradScaler as above; bf16 has fp32's exponent range and needs
+    none (`loss.backward()`).  Construction runs two warm-up iterations
     and restores the buffers, `.grad` and the CUDA RNG state it found.
 
     Out-of-range indices in a later batch raise IndexError at a later call, as with DecoderStep, without blocking the host;
@@ -228,8 +230,8 @@ class TrainStep:
         sizes the static buffers and is what warm-up and capture run on.  `edge_capacity` K defaults to the width of
         packed_adj's edge buffer; `max_edges` bounds the edges of one sub-graph over the whole split
         (FlatAdjCache.max_graph_edges())."""
-        if autocast_dtype not in (None, torch.float16):
-            raise ValueError("autocast_dtype must be None or torch.float16")
+        if autocast_dtype not in (None, torch.float16, torch.bfloat16):
+            raise ValueError("autocast_dtype must be None, torch.float16 or torch.bfloat16")
         if not decoder.training:
             raise ValueError("TrainStep captures the training forward: call decoder.train() first")
         self.decoder, self.autocast_dtype = decoder, autocast_dtype

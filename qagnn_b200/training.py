@@ -49,7 +49,11 @@ def edge_table_train(enc, onehot_tab, combo_count, k_calls):
     """tab[c] = edge_encoder(onehot(c)) with BATCH statistics over the E' edges (each combo weighted by its edge count),
     plus the running-statistics update of `k_calls` forward calls of the shared module."""
     lin0, bn, lin3 = enc[0], enc[1], enc[3]
+    # the moments are fp32 under any autocast: n = E' counts edge positions (> 65504 overflows fp16, bf16 rounds counts to
+    # 8 bits), and h widens exactly, so only its own rounding to the autocast dtype remains
     h = lin0(onehot_tab)                                        # [C, D]
+    if h.dtype in (torch.float16, torch.bfloat16):
+        h = h.float()
     w = combo_count.to(h.dtype)
     n = w.sum()
     mean = (w[:, None] * h).sum(0) / n
@@ -66,27 +70,53 @@ def edge_table_train(enc, onehot_tab, combo_count, k_calls):
     return lin3(F.relu(y))
 
 
-class _MPCore(torch.autograd.Function):
-    """aggr = propagate(...) on node-level projections; forward and backward in libqagnn_b200.so."""
+def _core_dtype(*ts):
+    """Storage dtype of one core call: the widest dtype of its operands (fp16 with bf16 widens to fp32).  Under autocast,
+    operands of another floating dtype (fp64) are cast to fp32, as torch.amp.custom_fwd(cast_inputs=torch.float32) casts."""
+    dt = functools.reduce(torch.promote_types, (t.dtype for t in ts))
+    if dt not in _lib.DTYPE_CODES:
+        if not torch.is_autocast_enabled("cuda"):
+            raise TypeError(f"qagnn_b200: the message-passing core takes float32, float16 or bfloat16 operands (got {dt})")
+        dt = torch.float32
+    return dt
 
-    # under torch.autocast (qagnn.py:91 runs the forward in fp16 autocast when --fp16 is set) the dense layers around this
-    # function may hand it half tensors: the graph part always computes in fp32, like the reference's scatter ops do
+
+def _operand(t, dt, name):
+    _lib.require_cuda(t, name)
+    t = t.detach().to(dt).contiguous()
+    return t if t.data_ptr() % 16 == 0 else t.clone()  # the kernels read rows 4 elements at a time
+
+
+class _MPCore(torch.autograd.Function):
+    """aggr = propagate(...) on node-level projections; forward and backward in libqagnn_b200.so.
+
+    Under torch.autocast (qagnn.py:91 runs the forward in fp16 autocast when --fp16 is set) the dense layers around this
+    function hand it qkm / ke / me in the autocast dtype: the kernels read and write that dtype directly (no cast to fp32 and
+    back around them) and compute in fp32 inside, like the reference's scatter ops do.  aggr and the three gradients come back
+    in that dtype, rounded once from the fp32 results; alpha is fp32.  fp32 operands run the fp32 entry points."""
+
     @staticmethod
-    @torch.amp.custom_fwd(device_type="cuda", cast_inputs=torch.float32)
+    @torch.amp.custom_fwd(device_type="cuda")
     def forward(ctx, qkm, ke, me, prep, shape_args, want_alpha):
         lib = _lib.load()
-        qkm_c, ke_c, me_c = _lib.f32c(qkm, "qkm"), _lib.f32c(ke, "ke"), _lib.f32c(me, "me")
+        dt = _core_dtype(qkm, ke, me)
+        qkm_c, ke_c, me_c = _operand(qkm, dt, "qkm"), _operand(ke, dt, "ke"), _operand(me, dt, "me")
         N, E, D, H, T, R = shape_args
         dev = qkm_c.device
         shape = _lib.Shape(N, E, D, H, T, R, 1, 0)
-        aggr = torch.empty(N, D, dtype=torch.float32, device=dev)
+        aggr = torch.empty(N, D, dtype=dt, device=dev)
         alpha_s = torch.empty(N + E, H, dtype=torch.float32, device=dev)
         alpha = torch.empty(N + E, H, dtype=torch.float32, device=dev) if want_alpha else None
         scratch = torch.empty(N + E, H, dtype=torch.float32, device=dev)
         with torch.cuda.device(dev):
-            st = lib.qagnn_mp_core_forward(C.byref(shape), _lib.ptr(prep.buf), _lib.ptr(qkm_c), _lib.ptr(ke_c), _lib.ptr(me_c),
-                                           _lib.ptr(aggr), _lib.ptr(alpha_s), _lib.ptr(alpha), _lib.ptr(scratch),
-                                           _lib.stream_ptr(dev))
+            if dt == torch.float32:
+                st = lib.qagnn_mp_core_forward(C.byref(shape), _lib.ptr(prep.buf), _lib.ptr(qkm_c), _lib.ptr(ke_c), _lib.ptr(me_c),
+                                               _lib.ptr(aggr), _lib.ptr(alpha_s), _lib.ptr(alpha), _lib.ptr(scratch),
+                                               _lib.stream_ptr(dev))
+            else:
+                st = lib.qagnn_mp_core_forward_typed(C.byref(shape), _lib.DTYPE_CODES[dt], _lib.ptr(prep.buf), _lib.ptr(qkm_c),
+                                                     _lib.ptr(ke_c), _lib.ptr(me_c), _lib.ptr(aggr), _lib.ptr(alpha_s),
+                                                     _lib.ptr(alpha), _lib.ptr(scratch), _lib.stream_ptr(dev))
         _lib.check(st, "qagnn_mp_core_forward")
         ctx.save_for_backward(qkm_c, ke_c, me_c, alpha_s)
         ctx.prep, ctx.shape_args = prep, shape_args
@@ -101,17 +131,25 @@ class _MPCore(torch.autograd.Function):
         lib = _lib.load()
         qkm, ke, me, alpha_s = ctx.saved_tensors
         N, E, D, H, T, R = ctx.shape_args
-        dev = qkm.device
+        dt, dev = qkm.dtype, qkm.device
         shape = _lib.Shape(N, E, D, H, T, R, 1, 0)
-        g = _lib.f32c(d_aggr, "d_aggr")
+        g = _operand(d_aggr, dt, "d_aggr")
         d_qkm = torch.empty_like(qkm)
         d_ke, d_me = torch.empty_like(ke), torch.empty_like(me)
-        scratch = torch.empty(N + E, H, dtype=torch.float32, device=dev)
         order = ctx.prep.combo_sort()[1]  # device-side E': valid under an edge capacity without a host read
         with torch.cuda.device(dev):
-            st = lib.qagnn_mp_core_backward(C.byref(shape), _lib.ptr(ctx.prep.buf), _lib.ptr(order), _lib.ptr(qkm), _lib.ptr(ke),
-                                            _lib.ptr(me), _lib.ptr(alpha_s), _lib.ptr(g), _lib.ptr(d_qkm), _lib.ptr(d_ke),
-                                            _lib.ptr(d_me), _lib.ptr(scratch), _lib.stream_ptr(dev))
+            if dt == torch.float32:
+                scratch = torch.empty(N + E, H, dtype=torch.float32, device=dev)
+                st = lib.qagnn_mp_core_backward(C.byref(shape), _lib.ptr(ctx.prep.buf), _lib.ptr(order), _lib.ptr(qkm), _lib.ptr(ke),
+                                                _lib.ptr(me), _lib.ptr(alpha_s), _lib.ptr(g), _lib.ptr(d_qkm), _lib.ptr(d_ke),
+                                                _lib.ptr(d_me), _lib.ptr(scratch), _lib.stream_ptr(dev))
+            else:
+                code = _lib.DTYPE_CODES[dt]
+                # [E+N, H] fp32 softmax gradients, then the fp32 accumulators of d_ke / d_me
+                scratch = torch.empty(lib.qagnn_mp_core_scratch_bytes(C.byref(shape), code) // 4, dtype=torch.float32, device=dev)
+                st = lib.qagnn_mp_core_backward_typed(C.byref(shape), code, _lib.ptr(ctx.prep.buf), _lib.ptr(order), _lib.ptr(qkm),
+                                                      _lib.ptr(ke), _lib.ptr(me), _lib.ptr(alpha_s), _lib.ptr(g), _lib.ptr(d_qkm),
+                                                      _lib.ptr(d_ke), _lib.ptr(d_me), _lib.ptr(scratch), _lib.stream_ptr(dev))
         _lib.check(st, "qagnn_mp_core_backward")
         return d_qkm, d_ke, d_me, None, None, None
 

@@ -2,7 +2,8 @@
 pipeline.TrainStep's two CUDA graphs, alternated in one process.
 
 Workloads: the batch of the reference's training recipes (run_qagnn__*.sh: -mbs 2, so 2 questions x 5 choices = 10 sub-graphs
-per backward) and the whole -bs 64 batch (320 sub-graphs), each under fp16 autocast (--fp16 true) and in fp32.  Sub-graphs
+per backward) and the whole -bs 64 batch (320 sub-graphs), each under fp16 autocast (--fp16 true), under bf16 autocast and in
+fp32.  Sub-graphs
 come from the loader-shaped synthetic split of tools/bench_stream_split.py (n = 200, 38 relations), packed at the split's
 edge capacity; decoder k = 5, D = 200, sent_dim 1024, dropout 0.2 (the recipes' values).  The text encoder and the
 optimiser are not part of the step (sent_vecs is a leaf tensor standing in for the encoder's output).
@@ -81,7 +82,7 @@ def main():
             d["sent_vecs"].requires_grad_(True)
             batches.append(d)
         edges = [d["adj"].n_edges for d in batches]
-        for amp in (torch.float16, None):
+        for amp in (torch.float16, torch.bfloat16, None):
             torch.manual_seed(1)
             base = qagnn_b200.QAGNN(None, K_LAYERS, T, R, SENT_DIM, N_CONCEPT, D, D, 2, D, 0, DROPOUT, DROPOUT, DROPOUT)
             base.gnn.load_state_dict(O.random_state_dict(K_LAYERS, D, T, R, "prod", seed=0))
@@ -150,7 +151,7 @@ def main():
             for d in batches:
                 d["sent_vecs"].grad = None
             line = {"gpu": gpu, "questions": bs, "graphs": bs * NC, "n_node": N_NODE, "D": D, "k": K_LAYERS,
-                    "autocast": "fp16" if amp else "fp32", "edge_capacity": K, "max_graph_edges": M,
+                    "autocast": {torch.float16: "fp16", torch.bfloat16: "bf16", None: "fp32"}[amp], "edge_capacity": K, "max_graph_edges": M,
                     "edges_per_batch": [min(edges), max(edges)], "steps": args.steps, "reps": args.reps, **res,
                     "speedup_vs_eager": res["eager"]["ms_per_step"] / res["graphs"]["ms_per_step"],
                     "speedup_vs_eager_nocheck": res["eager_nocheck"]["ms_per_step"] / res["graphs"]["ms_per_step"],
