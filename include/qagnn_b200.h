@@ -202,6 +202,23 @@ int32_t qagnn_mp_forward(const qagnn_shape *shape, const float *H_in, const int6
                          const float *node_score, const void *prep, const void *folded, float *out,
                          float *x_layers_out, void *workspace, size_t workspace_bytes, void *stream);
 
+/* The eval forward under bf16 autocast.  `dtype` (QAGNN_DTYPE_*, below) is the storage type of out and selects the GEMMs;
+ * `in_dtype` that of x / extra / H_in (QAGNN_DTYPE_F32 or QAGNN_DTYPE_BF16; an fp32 input is rounded to nearest even as it is
+ * written into the GEMM operand, as autocast's cast would round it).  QAGNN_DTYPE_F32 (with fp32 inputs) runs
+ * qagnn_gatconve_forward / qagnn_mp_forward.  QAGNN_DTYPE_BF16: every GEMM of the tensor-core path
+ * (emb_score, the projection with its per-type bias rows, mlp.0 / mlp.3 or the fused MLP, Vh|Vx) takes the bf16 operands
+ * that path feeds it - the inputs as given, the folded weights rounded to nearest even - and accumulates in fp32 in the same
+ * k order; bias and activation are fp32 in the epilogue.  The folds, the Q|Kx|Mx tiles, logits, softmax and aggr sums stay
+ * fp32 (the message passing is the fp32 one).  out is the fp32 epilogue value rounded to nearest even; x_layers_out,
+ * alpha_out and aggr_out stay fp32.  Shapes without the wgmma GEMM (D % 8 != 0, QAGNN_GEMM=ffma) run the fp32 path on the
+ * widened inputs and round its output.  QAGNN_DTYPE_F16: QAGNN_ERR_INVALID_ARGUMENT. */
+int32_t qagnn_gatconve_forward_typed(const qagnn_shape *shape, int32_t dtype, int32_t in_dtype, int32_t layer, const void *x,
+                                     const void *extra, const void *prep, const void *folded, void *out, float *alpha_out,
+                                     float *aggr_out, void *workspace, size_t workspace_bytes, void *stream);
+int32_t qagnn_mp_forward_typed(const qagnn_shape *shape, int32_t dtype, int32_t in_dtype, const void *H_in,
+                               const int64_t *node_type, const float *node_score, const void *prep, const void *folded,
+                               void *out, float *x_layers_out, void *workspace, size_t workspace_bytes, void *stream);
+
 /* ---- training (SURVEY.md §8f #3) --------------------------------------------------------------- */
 
 /* Message passing of one layer on caller-computed node-level projections, keeping what backward needs.
@@ -254,6 +271,12 @@ size_t qagnn_linear_workspace_bytes(int64_t M, int32_t N, int32_t K1, int32_t K2
 int32_t qagnn_linear_bf16x3(const float *A1, int32_t lda1, int32_t K1, const float *A2, int32_t lda2, int32_t K2,
                             const float *W, int32_t ldw, const float *bias, float *C, int32_t ldc, int64_t M, int32_t N,
                             int32_t act, void *workspace, size_t workspace_bytes, void *stream);
+/* The single-pass GEMM of the bf16 forward on its own: bf16 A1 / A2 / W (row strides lda1 / lda2 / ldw, multiples of 8,
+ * 16-byte aligned bases), fp32 bias, one wgmma per k16 step with fp32 accumulation.  Writes C (fp32, ldc) and/or C_bf16
+ * (the fp32 value rounded to nearest even, ldp); either may be NULL but not both. */
+int32_t qagnn_linear_bf16(const void *A1, int32_t lda1, int32_t K1, const void *A2, int32_t lda2, int32_t K2, const void *W,
+                          int32_t ldw, const float *bias, float *C, int32_t ldc, void *C_bf16, int32_t ldp, int64_t M, int32_t N,
+                          int32_t act, void *stream);
 
 /* The step after the path (SURVEY.md §8f #2): QAGNN's masked multi-head attention pooling of the node representations,
  * MultiheadAttPoolLayer.forward (utils/layers.py:344-371, called at modeling_qagnn.py:180), eval mode, fused into one
@@ -270,6 +293,16 @@ int32_t qagnn_attention_pool(int32_t B, int32_t n, int32_t D, int32_t n_head, co
 int32_t qagnn_decoder_tail(int32_t B, int32_t n, int32_t D, int32_t n_head, int32_t S, const float *X, const float *qs,
                            const int64_t *node_type, const int64_t *adj_lengths, const float *sent_vecs, const float *wk,
                            const float *bk, const float *wv, const float *bv, float *concat, float *attn, void *stream);
+
+/* qagnn_attention_pool / qagnn_decoder_tail with X stored as `x_dtype` (QAGNN_DTYPE_F32 or QAGNN_DTYPE_BF16: the bf16 eval
+ * forward's output, widened exactly); every other operand and output as above. */
+int32_t qagnn_attention_pool_typed(int32_t x_dtype, int32_t B, int32_t n, int32_t D, int32_t n_head, const void *X,
+                                   const float *qs, const uint8_t *mask, const float *wk, const float *bk, const float *wv,
+                                   const float *bv, float *pooled, float *attn, void *stream);
+int32_t qagnn_decoder_tail_typed(int32_t x_dtype, int32_t B, int32_t n, int32_t D, int32_t n_head, int32_t S, const void *X,
+                                 const float *qs, const int64_t *node_type, const int64_t *adj_lengths, const float *sent_vecs,
+                                 const float *wk, const float *bk, const float *wv, const float *bv, float *concat, float *attn,
+                                 void *stream);
 
 /* The step before the path (SURVEY.md §8f #2): QAGNN.forward's input assembly (modeling_qagnn.py:153-167), eval mode, one kernel:
  *   H_out[b,0,:] = ctx[b,:] (= GELU(svec2nvec(sent_vecs)), caller-computed [B,D]);  H_out[b,i,:] = table[concept_ids[b,i]-1], i >= 1,

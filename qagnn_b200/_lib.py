@@ -58,9 +58,13 @@ EXPORTS = {
                                        C.POINTER(MPParams), _P, C.c_size_t, _P]),
     "qagnn_forward_workspace_bytes": (C.c_size_t, [C.POINTER(Shape)]),
     "qagnn_gatconve_forward": (C.c_int32, [C.POINTER(Shape), C.c_int32, _P, _P, _P, _P, _P, _P, _P, _P, C.c_size_t, _P]),
+    "qagnn_gatconve_forward_typed": (C.c_int32, [C.POINTER(Shape), C.c_int32, C.c_int32, C.c_int32, _P, _P, _P, _P, _P, _P,
+                                                 _P, _P, C.c_size_t, _P]),
     "qagnn_mp_path": (C.c_int32, [C.POINTER(Shape)]),
     "qagnn_node_feature_extra": (C.c_int32, [C.POINTER(Shape), _P, _P, _P, _P, _P, C.c_size_t, _P]),
     "qagnn_mp_forward": (C.c_int32, [C.POINTER(Shape), _P, _P, _P, _P, _P, _P, _P, _P, C.c_size_t, _P]),
+    "qagnn_mp_forward_typed": (C.c_int32, [C.POINTER(Shape), C.c_int32, C.c_int32, _P, _P, _P, _P, _P, _P, _P, _P, C.c_size_t,
+                                           _P]),
     "qagnn_mp_core_forward": (C.c_int32, [C.POINTER(Shape), _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "qagnn_mp_core_backward": (C.c_int32, [C.POINTER(Shape), _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "qagnn_mp_core_scratch_bytes": (C.c_size_t, [C.POINTER(Shape), C.c_int32]),
@@ -71,9 +75,15 @@ EXPORTS = {
     "qagnn_linear_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int32, C.c_int32, C.c_int32]),
     "qagnn_linear_bf16x3": (C.c_int32, [_P, C.c_int32, C.c_int32, _P, C.c_int32, C.c_int32, _P, C.c_int32, _P, _P, C.c_int32,
                                         C.c_int64, C.c_int32, C.c_int32, _P, C.c_size_t, _P]),
+    "qagnn_linear_bf16": (C.c_int32, [_P, C.c_int32, C.c_int32, _P, C.c_int32, C.c_int32, _P, C.c_int32, _P, _P, C.c_int32, _P,
+                                      C.c_int32, C.c_int64, C.c_int32, C.c_int32, _P]),
     "qagnn_attention_pool": (C.c_int32, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
+    "qagnn_attention_pool_typed": (C.c_int32, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P, _P, _P, _P, _P, _P,
+                                               _P, _P, _P, _P]),
     "qagnn_decoder_tail": (C.c_int32, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P,
                                        _P, _P]),
+    "qagnn_decoder_tail_typed": (C.c_int32, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P, _P, _P, _P,
+                                             _P, _P, _P, _P, _P, _P, _P, _P]),
     "qagnn_decoder_head": (C.c_int32, [C.c_int32, C.c_int32, C.c_int32, _P, C.c_int64, _P, _P, _P, _P, _P, _P, _P]),
     "qagnn_launch_count": (C.c_int64, []),
     "qagnn_profile_enable": (C.c_int32, [C.c_int32]),
@@ -178,6 +188,23 @@ def f32c(t, name):
 
 # dtype codes of the *_typed entry points (QAGNN_DTYPE_* in include/qagnn_b200.h)
 DTYPE_CODES = {torch.float32: 0, torch.float16: 1, torch.bfloat16: 2}
+
+
+def autocast_dtype():
+    """The CUDA autocast dtype when autocast is on, else None."""
+    return torch.get_autocast_dtype("cuda") if torch.is_autocast_enabled("cuda") else None
+
+
+def eval_dtype(t, name):
+    """(tensor, forward dtype) for an eval forward's input.  Under bf16 autocast: an fp32 or bf16 CUDA tensor as it is (the
+    library rounds an fp32 one to bf16 as it writes the GEMM operand, as autocast's cast would) and torch.bfloat16; otherwise
+    an fp32 tensor (f32c) and torch.float32.  Any other autocast dtype runs the fp32 kernels."""
+    if autocast_dtype() == torch.bfloat16:
+        require_cuda(t, name)
+        if t.dtype not in (torch.float32, torch.bfloat16):
+            raise TypeError(f"qagnn_b200: `{name}` must be float32 or bfloat16 under bf16 autocast (got {t.dtype})")
+        return t.detach().contiguous(), torch.bfloat16
+    return f32c(t, name), torch.float32
 
 
 def i64c(t, name):

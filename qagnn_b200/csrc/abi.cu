@@ -123,7 +123,7 @@ __global__ void sin_basis_planes_kernel(int64_t N, int Dh, int ld, const float* 
     h2.x = __float2bfloat16_rn(a); h2.y = __float2bfloat16_rn(b);
     l2.x = __float2bfloat16_rn(a - __bfloat162float(h2.x)); l2.y = __float2bfloat16_rn(b - __bfloat162float(h2.y));
     *reinterpret_cast<__nv_bfloat162*>(hi + v * ld + j) = h2;
-    *reinterpret_cast<__nv_bfloat162*>(lo + v * ld + j) = l2;
+    if (lo != nullptr) *reinterpret_cast<__nv_bfloat162*>(lo + v * ld + j) = l2;  // null: hi plane alone (single pass)
   }
 }
 
@@ -135,9 +135,14 @@ __global__ void copy_plane_columns_kernel(int64_t N, int w4, int ld8, const uint
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < N * w4; i += (int64_t)gridDim.x * blockDim.x) {
     const int64_t r = i / w4;
     const int c = (int)(i - r * w4);
-    const uint2 h = sh[r * ld8 + c], l = sl[r * ld8 + c];
-    d1h[r * ld8 + c] = h; d1l[r * ld8 + c] = l;
-    d2h[r * ld8 + c] = h; d2l[r * ld8 + c] = l;
+    const uint2 h = sh[r * ld8 + c];
+    d1h[r * ld8 + c] = h;
+    d2h[r * ld8 + c] = h;
+    if (sl != nullptr) {  // null: hi planes alone (single pass)
+      const uint2 l = sl[r * ld8 + c];
+      d1l[r * ld8 + c] = l;
+      d2l[r * ld8 + c] = l;
+    }
   }
 }
 
@@ -175,7 +180,7 @@ __global__ void __launch_bounds__(256) node_feature_fused_kernel(int64_t N, int 
         l[c] = __float2bfloat16_rn(x[c] - __bfloat162float(h[c]));
       }
       *reinterpret_cast<uint2*>(ex_hi + v * D + col) = *reinterpret_cast<const uint2*>(h);
-      *reinterpret_cast<uint2*>(ex_lo + v * D + col) = *reinterpret_cast<const uint2*>(l);
+      if (ex_lo != nullptr) *reinterpret_cast<uint2*>(ex_lo + v * D + col) = *reinterpret_cast<const uint2*>(l);
     }
   };
   // register tile: 4 nodes x 4 outputs per thread -> two LDS.128 per 16 FMAs
@@ -313,13 +318,16 @@ struct Planes {
 };
 
 // one GATConvE layer on split-bf16 planes.  x / extra are [N, D] plane pairs; the layer output goes to any of
-// out_f32 (fp32 [N, D]) and out_planes.
+// out_f32 (fp32 [N, D]) and out_planes.  passes = 1: every GEMM runs on the hi planes alone (lo planes neither read nor
+// written, out_lo ignored); the message passing is the same either way.
 int32_t layer_forward_tc(const qagnn_shape& s, const FoldLayout& L, const WorkLayout& W, int layer, Planes x, Planes extra,
                          const void* prep, const qagnn_prep_layout& pl, const float* folded, float* out_f32,
                          void* out_hi, void* out_lo, float* alpha_out, float* aggr_out, float* ws, Act final_act,
-                         bool tiled, cudaStream_t st, const int64_t* type_bias_classes = nullptr, int out_ldp = 0) {
+                         bool tiled, cudaStream_t st, const int64_t* type_bias_classes = nullptr, int out_ldp = 0,
+                         int passes = 3) {
   const int D = s.D;
   if (out_ldp == 0) out_ldp = D;
+  float* const ap_lo = passes == 1 ? nullptr : ws + W.ap_lo;
   const float* lb = folded + L.layer0 + (size_t)layer * L.layer_stride;
   float* qkm = ws + W.qkm;
   const bool fused_split = tiled && (D / s.H) % 2 == 0;  // the tiled kernel emits the bf16 planes of aggr itself
@@ -337,18 +345,18 @@ int32_t layer_forward_tc(const qagnn_shape& s, const FoldLayout& L, const WorkLa
       o.hm_buf = qkm;
       o.hm = HeadMajorOut{1, D, D / s.H, DP, s.H};
       o.row_class = type_bias_classes; o.class_stride = 3 * s.H * DP; o.n_class = s.T;
-      QAGNN_RETURN_IF(gemm_tc(Ax, none, Wp, lb + L.tbias, s.N, 3 * s.H * DP, ACT_NONE, o, st));
+      QAGNN_RETURN_IF(gemm_tc(Ax, none, Wp, lb + L.tbias, s.N, 3 * s.H * DP, ACT_NONE, o, st, passes));
     } else if (tiled) {  // per-head padded weight rows -> the GEMM writes [3][H][N][DP] (pads = exact zeros) itself
       const int DP = head_dim_padded(D / s.H);
       TcOperand Wp{lb + L.wph_hi, lb + L.wph_lo, 2 * D, 2 * D};
       o.hm_buf = qkm;
       o.hm = HeadMajorOut{1, D, D / s.H, DP, s.H};
-      QAGNN_RETURN_IF(gemm_tc(A1, A2, Wp, lb + L.bph, s.N, 3 * s.H * DP, ACT_NONE, o, st));
+      QAGNN_RETURN_IF(gemm_tc(A1, A2, Wp, lb + L.bph, s.N, 3 * s.H * DP, ACT_NONE, o, st, passes));
     } else {
       TcOperand Wp{lb + L.wp_hi, lb + L.wp_lo, 2 * D, 2 * D};
       o.f32 = qkm;
       o.ldc = 3 * D;
-      QAGNN_RETURN_IF(gemm_tc(A1, A2, Wp, lb + L.bp, s.N, 3 * D, ACT_NONE, o, st));
+      QAGNN_RETURN_IF(gemm_tc(A1, A2, Wp, lb + L.bp, s.N, 3 * D, ACT_NONE, o, st, passes));
     }
   }
   {  // logits -> per-source softmax -> out-degree rescale -> per-target sum   (:442, :469-484)
@@ -357,7 +365,7 @@ int32_t layer_forward_tc(const qagnn_shape& s, const FoldLayout& L, const WorkLa
     if (tiled) {
       QAGNN_RETURN_IF(launch_message_passing_headtile(s, (const int32_t*)prep, pl, qkm, lb + L.keh, lb + L.meh,
                                                       ws + W.score, ws + W.alpha2, aggr, alpha_out,
-                                                      fused_split ? ws + W.ap_hi : nullptr, ws + W.ap_lo, st));
+                                                      fused_split ? ws + W.ap_hi : nullptr, ap_lo, st));
     } else if (use_slice(s)) {
       QAGNN_RETURN_IF(launch_message_passing_slice(s, (const int32_t*)prep, pl, qkm, lb + L.ke, lb + L.me, ws + W.score, aggr,
                                                    alpha_out, st));
@@ -368,21 +376,21 @@ int32_t layer_forward_tc(const qagnn_shape& s, const FoldLayout& L, const WorkLa
   }
   {  // node MLP: Linear -> BatchNorm(eval, folded) -> ReLU -> Linear          (:443, :408)
     ProfScope ps(QAGNN_PROF_NODE_MLP, st);
-    if (!fused_split) QAGNN_RETURN_IF(split_bf16(aggr, D, s.N, D, ws + W.ap_hi, ws + W.ap_lo, D, st));
+    if (!fused_split) QAGNN_RETURN_IF(split_bf16(aggr, D, s.N, D, ws + W.ap_hi, ap_lo, D, st));
     TcOperand A{ws + W.ap_hi, ws + W.ap_lo, D, D}, none{nullptr, nullptr, 0, 0};
     TcOperand W1{lb + L.w1_hi, lb + L.w1_lo, D, D}, W2{lb + L.w2_hi, lb + L.w2_lo, D, D};
     if (use_mlp_fused(D)) {  // one launch, the hidden layer never leaves registers
       TcOutput o{};
       o.f32 = out_f32; o.ldc = D; o.hi = out_hi; o.lo = out_lo; o.ldp = out_ldp;
-      return mlp_tc(A, W1, lb + L.b1, W2, lb + L.b2, s.N, final_act, o, st);
+      return mlp_tc(A, W1, lb + L.b1, W2, lb + L.b2, s.N, final_act, o, st, passes);
     }
     TcOutput o1{};
     o1.hi = ws + W.mp_hi; o1.lo = ws + W.mp_lo; o1.ldp = D;
-    QAGNN_RETURN_IF(gemm_tc(A, none, W1, lb + L.b1, s.N, D, ACT_RELU, o1, st));
+    QAGNN_RETURN_IF(gemm_tc(A, none, W1, lb + L.b1, s.N, D, ACT_RELU, o1, st, passes));
     TcOperand Hm{ws + W.mp_hi, ws + W.mp_lo, D, D};
     TcOutput o2{};
     o2.f32 = out_f32; o2.ldc = D; o2.hi = out_hi; o2.lo = out_lo; o2.ldp = out_ldp;
-    QAGNN_RETURN_IF(gemm_tc(Hm, none, W2, lb + L.b2, s.N, D, final_act, o2, st));
+    QAGNN_RETURN_IF(gemm_tc(Hm, none, W2, lb + L.b2, s.N, D, final_act, o2, st, passes));
   }
   return QAGNN_OK;
 }
@@ -418,6 +426,45 @@ int32_t extra_forward(const qagnn_shape& s, const FoldLayout& L, const WorkLayou
   if (ex_hi != nullptr) QAGNN_RETURN_IF(split_bf16(extra, D, s.N, D, ex_hi, ex_lo, D, st));
   return QAGNN_OK;
 }
+
+__global__ void bf16_to_f32_kernel(int64_t n, const __nv_bfloat16* __restrict__ in, float* __restrict__ out) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
+    out[i] = __bfloat162float(in[i]);
+}
+__global__ void f32_to_bf16_kernel(int64_t n, const float* __restrict__ in, __nv_bfloat16* __restrict__ out) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
+    out[i] = __float2bfloat16_rn(in[i]);
+}
+// exact widening / round-to-nearest-even narrowing of n elements (the bf16 entry points on shapes without the wgmma GEMM)
+int32_t convert(int64_t n, const void* in, void* out, bool widen, cudaStream_t st) {
+  if (n <= 0) return QAGNN_OK;
+  int64_t g = (n + 255) / 256;
+  if (g > kNumSMs * 32) g = kNumSMs * 32;
+  if (widen) bf16_to_f32_kernel<<<(unsigned)g, 256, 0, st>>>(n, (const __nv_bfloat16*)in, (float*)out);
+  else f32_to_bf16_kernel<<<(unsigned)g, 256, 0, st>>>(n, (const float*)in, (__nv_bfloat16*)out);
+  QAGNN_CHECK_LAUNCH();
+  return QAGNN_OK;
+}
+
+// bf16 rows [rows, cols] (row stride `ld` elements) copied into a hi plane with row stride `ldp`: a bf16 operand is its own
+// hi plane (bf16_rn is the identity on it)
+int32_t copy_rows_bf16(const void* src, int ld, void* dst, int ldp, int64_t rows, int cols, cudaStream_t st) {
+  if (rows <= 0) return QAGNN_OK;
+  QAGNN_CHECK_CUDA(cudaMemcpy2DAsync(dst, (size_t)ldp * 2, src, (size_t)ld * 2, (size_t)cols * 2, (size_t)rows,
+                                     cudaMemcpyDeviceToDevice, st));
+  return QAGNN_OK;
+}
+
+// The hi plane [rows, cols] (row stride ldp) of a bf16 or fp32 operand (row stride cols): a bf16 operand is copied, an fp32
+// one rounded to nearest even by split_bf16 without its lo plane - autocast's cast, in the same pass that writes the plane
+int32_t hi_plane_of(const void* src, bool src_bf16, void* dst, int ldp, int64_t rows, int cols, cudaStream_t st) {
+  if (src_bf16) return copy_rows_bf16(src, cols, dst, ldp, rows, cols, st);
+  return split_bf16((const float*)src, cols, rows, cols, dst, nullptr, ldp, st);
+}
+
+// The bf16 entry points on shapes without the wgmma GEMM run the fp32 path on widened inputs: the split-bf16 plane buffers,
+// which that path never touches, hold the fp32 inputs and output there ([hp_hi, ap_hi) spans at least 4 N*D floats).
+float* fp32_staging(const WorkLayout& W, float* ws) { return ws + W.hp_hi; }
 
 }  // namespace
 }  // namespace qagnn
@@ -495,6 +542,57 @@ extern "C" int32_t qagnn_gatconve_forward(const qagnn_shape* shape, int32_t laye
                        ACT_NONE, tiled, st);
 }
 
+extern "C" int32_t qagnn_gatconve_forward_typed(const qagnn_shape* shape, int32_t dtype, int32_t in_dtype, int32_t layer,
+                                                const void* x, const void* extra, const void* prep, const void* folded,
+                                                void* out, float* alpha_out, float* aggr_out, void* workspace,
+                                                size_t workspace_bytes, void* stream) {
+  if (in_dtype != QAGNN_DTYPE_F32 && in_dtype != QAGNN_DTYPE_BF16) return QAGNN_ERR_INVALID_ARGUMENT;
+  if (dtype == QAGNN_DTYPE_F32) {
+    if (in_dtype != QAGNN_DTYPE_F32) return QAGNN_ERR_INVALID_ARGUMENT;
+    return qagnn_gatconve_forward(shape, layer, (const float*)x, (const float*)extra, prep, folded, (float*)out, alpha_out,
+                                  aggr_out, workspace, workspace_bytes, stream);
+  }
+  if (dtype != QAGNN_DTYPE_BF16) return QAGNN_ERR_INVALID_ARGUMENT;
+  const bool in_bf16 = in_dtype == QAGNN_DTYPE_BF16;
+  QAGNN_RETURN_IF(check_shape_fwd(shape));
+  if (!x || !extra || !prep || !folded || !out || !workspace) return QAGNN_ERR_INVALID_ARGUMENT;
+  if (layer < 0 || layer >= shape->k) return QAGNN_ERR_INVALID_ARGUMENT;
+  const FoldLayout L = make_fold_layout(*shape);
+  const WorkLayout W = make_work_layout(*shape);
+  if (workspace_bytes < W.total * sizeof(float)) return QAGNN_ERR_WORKSPACE;
+  qagnn_prep_layout pl;
+  QAGNN_RETURN_IF(qagnn_graph_prep_layout(shape->N, shape->E, &pl));
+  const bool tiled = use_headtile(*shape);
+  cudaStream_t st = (cudaStream_t)stream;
+  float* ws = (float*)workspace;
+  const int D = shape->D;
+  const int64_t ND = shape->N * (int64_t)D;
+  if (use_tc(*shape)) {  // x / extra as hi planes, every GEMM single-pass
+    QAGNN_RETURN_IF(hi_plane_of(x, in_bf16, ws + W.xp_hi[0], D, shape->N, D, st));
+    QAGNN_RETURN_IF(hi_plane_of(extra, in_bf16, ws + W.ep_hi, D, shape->N, D, st));
+    return layer_forward_tc(*shape, L, W, layer, Planes{ws + W.xp_hi[0], nullptr}, Planes{ws + W.ep_hi, nullptr}, prep, pl,
+                            (const float*)folded, nullptr, out, nullptr, alpha_out, aggr_out, ws, ACT_NONE, tiled, st,
+                            nullptr, 0, 1);
+  }
+  // the fp32 path on the rounded inputs (widened exactly), its output rounded once
+  float* x32 = fp32_staging(W, ws);
+  float* ex32 = x32 + ND;
+  float* out32 = ex32 + ND;
+  if (in_bf16) {
+    QAGNN_RETURN_IF(convert(ND, x, x32, true, st));
+    QAGNN_RETURN_IF(convert(ND, extra, ex32, true, st));
+  } else {  // bf16_rn of the fp32 inputs, back in fp32
+    QAGNN_RETURN_IF(convert(ND, x, out32, false, st));
+    QAGNN_RETURN_IF(convert(ND, out32, x32, true, st));
+    QAGNN_RETURN_IF(convert(ND, extra, out32, false, st));
+    QAGNN_RETURN_IF(convert(ND, out32, ex32, true, st));
+  }
+  if (tiled) QAGNN_RETURN_IF(zero_head_pads(*shape, ws + W.qkm, st));
+  QAGNN_RETURN_IF(layer_forward(*shape, L, W, layer, x32, ex32, prep, pl, (const float*)folded, out32, alpha_out, aggr_out, ws,
+                                ACT_NONE, tiled, st));
+  return convert(ND, out32, out, false, st);
+}
+
 extern "C" int32_t qagnn_mp_path(const qagnn_shape* shape) {
   QAGNN_RETURN_IF(check_shape_fwd(shape));
   if (use_headtile(*shape)) return QAGNN_MP_PATH_TILED;
@@ -513,23 +611,29 @@ extern "C" int32_t qagnn_node_feature_extra(const qagnn_shape* shape, const int6
                        (cudaStream_t)stream);
 }
 
-extern "C" int32_t qagnn_mp_forward(const qagnn_shape* shape, const float* H_in, const int64_t* node_type,
-                                    const float* node_score, const void* prep, const void* folded, float* out,
-                                    float* x_layers_out, void* workspace, size_t workspace_bytes, void* stream) {
-  QAGNN_RETURN_IF(check_shape_fwd(shape));
-  if (!H_in || !node_type || !node_score || !prep || !folded || !out || !workspace) return QAGNN_ERR_INVALID_ARGUMENT;
-  const qagnn_shape& s = *shape;
+// QAGNN_Message_Passing.forward; passes = 3: H_in / out fp32 (qagnn_mp_forward), passes = 1: H_in / out bf16 and every
+// GEMM single-pass on the hi planes (qagnn_mp_forward_typed with QAGNN_DTYPE_BF16).
+static int32_t mp_forward(const qagnn_shape& s, int passes, bool h_bf16, const void* H_in_any, const int64_t* node_type,
+                          const float* node_score, const void* prep, const void* folded, void* out_any, float* x_layers_out,
+                          float* ws, cudaStream_t st) {
   const FoldLayout L = make_fold_layout(s);
   const WorkLayout W = make_work_layout(s);
-  if (workspace_bytes < W.total * sizeof(float)) return QAGNN_ERR_WORKSPACE;
   qagnn_prep_layout pl;
   QAGNN_RETURN_IF(qagnn_graph_prep_layout(s.N, s.E, &pl));
-  cudaStream_t st = (cudaStream_t)stream;
-  float* ws = (float*)workspace;
+  const bool single = passes == 1;
   const float* f = (const float*)folded;
   float* extra = ws + W.extra;
   const bool tc = use_tc(s);
   const bool tiled = use_headtile(s);
+  const float* H_in = (const float*)H_in_any;
+  float* out = (float*)out_any;
+  if (single && !tc) {  // the fp32 path on the rounded H (widened exactly), its output rounded once at the end
+    float* h32 = fp32_staging(W, ws);
+    out = h32 + (size_t)s.N * s.D;
+    if (!h_bf16) QAGNN_RETURN_IF(convert((int64_t)s.N * s.D, H_in_any, out, false, st));
+    QAGNN_RETURN_IF(convert((int64_t)s.N * s.D, h_bf16 ? H_in_any : out, h32, true, st));
+    H_in = h32;
+  }
   // fast form: tensor-core emb_score + type-embedding half of node_feature_extra folded into per-type bias rows
   // (QAGNN_MP_FASTPROJ=0 keeps the general [x | extra] projection, for A/B runs and tests)
   const char* efp = getenv("QAGNN_MP_FASTPROJ");
@@ -543,25 +647,27 @@ extern "C" int32_t qagnn_mp_forward(const qagnn_shape* shape, const float* H_in,
       int64_t g = (s.N * (Dh / 2) + 255) / 256;
       if (g > kNumSMs * 32) g = kNumSMs * 32;
       sin_basis_planes_kernel<<<(unsigned)g, 256, 0, st>>>(s.N, Dh, KSh, node_score, f + L.basis, (__nv_bfloat16*)(ws + W.sb_hi),
-                                                           (__nv_bfloat16*)(ws + W.sb_lo));
+                                                           single ? nullptr : (__nv_bfloat16*)(ws + W.sb_lo));
       QAGNN_CHECK_LAUNCH();
       // score_emb = GELU(emb_score(sin basis)) -> columns [D, D + D/2) of the H_in planes                   (:73)
       TcOperand A{ws + W.sb_hi, ws + W.sb_lo, KSh, Dh}, none{nullptr, nullptr, 0, 0}, Wsc{f + L.ws_hi, f + L.ws_lo, KSh, Dh};
       TcOutput o{};
       o.hi = xh[0] + (size_t)D * 2; o.lo = xl[0] + (size_t)D * 2; o.ldp = KS;
-      QAGNN_RETURN_IF(gemm_tc(A, none, Wsc, f + L.bs, s.N, Dh, ACT_GELU, o, st));
+      QAGNN_RETURN_IF(gemm_tc(A, none, Wsc, f + L.bs, s.N, Dh, ACT_GELU, o, st, passes));
       // ... and into the two activation buffers (layer-invariant: modeling_qagnn.py:86)
       {
         const int w4 = Dh * 2 / 8, ld8 = KS * 2 / 8;  // Dh % 4 == 0 and KS % 8 == 0 (checked by `fast`)
         int64_t gc = (s.N * w4 + 255) / 256;
         if (gc > kNumSMs * 16) gc = kNumSMs * 16;
         const size_t off = (size_t)D * 2;
-        copy_plane_columns_kernel<<<(unsigned)gc, 256, 0, st>>>(s.N, w4, ld8, (const uint2*)(xh[0] + off), (const uint2*)(xl[0] + off),
+        copy_plane_columns_kernel<<<(unsigned)gc, 256, 0, st>>>(s.N, w4, ld8, (const uint2*)(xh[0] + off),
+                                                              single ? nullptr : (const uint2*)(xl[0] + off),
                                                               (uint2*)(xh[1] + off), (uint2*)(xl[1] + off), (uint2*)(xh[2] + off),
                                                               (uint2*)(xl[2] + off));
         QAGNN_CHECK_LAUNCH();
       }
-      QAGNN_RETURN_IF(split_bf16(H_in, D, s.N, D, xh[0], xl[0], KS, st));
+      if (single) QAGNN_RETURN_IF(hi_plane_of(H_in_any, h_bf16, xh[0], KS, s.N, D, st));
+      else QAGNN_RETURN_IF(split_bf16(H_in, D, s.N, D, xh[0], xl[0], KS, st));
     }
     const size_t ND = (size_t)s.N * s.D;
     Planes xin{xh[0], xl[0], KS};
@@ -571,20 +677,21 @@ extern "C" int32_t qagnn_mp_forward(const qagnn_shape* shape, const float* H_in,
       void* ohi = xh[1 + (l & 1)];
       void* olo = xl[1 + (l & 1)];
       QAGNN_RETURN_IF(layer_forward_tc(s, L, W, l, xin, ep, prep, pl, f, xo32, ohi, olo, nullptr, nullptr, ws, ACT_GELU, tiled, st,
-                                       node_type, KS));
+                                       node_type, KS, passes));
       xin = Planes{ohi, olo, KS};
     }
     // output = GELU(Vh(H) + Vx(X))                                           (:92)
     ProfScope ps(QAGNN_PROF_PRO_EPILOGUE, st);
     TcOperand A1{xh[0], xl[0], KS, D}, A2{xin.hi, xin.lo, KS, D}, Wv{f + L.vcat_hi, f + L.vcat_lo, 2 * D, 2 * D};
     TcOutput o{};
-    o.f32 = out; o.ldc = D;
-    return gemm_tc(A1, A2, Wv, f + L.vbias, s.N, D, ACT_GELU, o, st);
+    if (single) { o.hi = out_any; o.ldp = D; }
+    else { o.f32 = out; o.ldc = D; }
+    return gemm_tc(A1, A2, Wv, f + L.vbias, s.N, D, ACT_GELU, o, st, passes);
   }
   {
     // tensor-core path: `extra` is only ever consumed as split-bf16 planes, so the prologue writes those directly
     QAGNN_RETURN_IF(extra_forward(s, L, W, node_type, node_score, f, tc && s.D / 2 <= 128 ? nullptr : extra, ws, st,
-                                  tc ? ws + W.ep_hi : nullptr, tc ? ws + W.ep_lo : nullptr));
+                                  tc ? ws + W.ep_hi : nullptr, tc && !single ? ws + W.ep_lo : nullptr));
   }
   if (tiled && !use_tc(s)) QAGNN_RETURN_IF(zero_head_pads(s, ws + W.qkm, st));
   const size_t ND = (size_t)s.N * s.D;
@@ -592,7 +699,8 @@ extern "C" int32_t qagnn_mp_forward(const qagnn_shape* shape, const float* H_in,
     const int D = s.D;
     {
       ProfScope ps(QAGNN_PROF_PRO_EPILOGUE, st);
-      QAGNN_RETURN_IF(split_bf16(H_in, D, s.N, D, ws + W.hp_hi, ws + W.hp_lo, D, st));
+      if (single) QAGNN_RETURN_IF(hi_plane_of(H_in_any, h_bf16, ws + W.hp_hi, D, s.N, D, st));
+      else QAGNN_RETURN_IF(split_bf16(H_in, D, s.N, D, ws + W.hp_hi, ws + W.hp_lo, D, st));
     }
     Planes xin{ws + W.hp_hi, ws + W.hp_lo};
     const Planes ep{ws + W.ep_hi, ws + W.ep_lo};
@@ -601,16 +709,17 @@ extern "C" int32_t qagnn_mp_forward(const qagnn_shape* shape, const float* H_in,
       void* ohi = ws + W.xp_hi[l & 1];
       void* olo = ws + W.xp_lo[l & 1];
       QAGNN_RETURN_IF(layer_forward_tc(s, L, W, l, xin, ep, prep, pl, f, xo32, ohi, olo, nullptr, nullptr, ws, ACT_GELU,
-                                       tiled, st));
+                                       tiled, st, nullptr, 0, passes));
       xin = Planes{ohi, olo};
     }
     // output = GELU(Vh(H) + Vx(X))                                           (:92)
     ProfScope ps(QAGNN_PROF_PRO_EPILOGUE, st);
     TcOperand A1{ws + W.hp_hi, ws + W.hp_lo, D, D}, A2{xin.hi, xin.lo, D, D}, Wv{f + L.vcat_hi, f + L.vcat_lo, 2 * D, 2 * D};
     TcOutput o{};
-    o.f32 = out; o.ldc = D;
+    if (single) { o.hi = out_any; o.ldp = D; }
+    else { o.f32 = out; o.ldc = D; }
     if (s.k == 0) { A2 = A1; }
-    return gemm_tc(A1, A2, Wv, f + L.vbias, s.N, D, ACT_GELU, o, st);
+    return gemm_tc(A1, A2, Wv, f + L.vbias, s.N, D, ACT_GELU, o, st, passes);
   }
   const float* x = H_in;
   for (int l = 0; l < s.k; ++l) {  // mp_helper, :45-50 (dropout is the identity in eval)
@@ -620,7 +729,42 @@ extern "C" int32_t qagnn_mp_forward(const qagnn_shape* shape, const float* H_in,
   }
   // output = GELU(Vh(H) + Vx(X))                                             (:92)
   ProfScope ps(QAGNN_PROF_PRO_EPILOGUE, st);
-  return sgemm_tn(H_in, s.D, s.D, x, s.D, s.D, f + L.vcat, 2 * s.D, f + L.vbias, out, s.D, s.N, s.D, ACT_GELU, st);
+  QAGNN_RETURN_IF(sgemm_tn(H_in, s.D, s.D, x, s.D, s.D, f + L.vcat, 2 * s.D, f + L.vbias, out, s.D, s.N, s.D, ACT_GELU, st));
+  if (single) return convert((int64_t)s.N * s.D, out, out_any, false, st);
+  return QAGNN_OK;
+}
+
+static int32_t check_mp_forward_args(const qagnn_shape* shape, const void* H_in, const int64_t* node_type,
+                                     const float* node_score, const void* prep, const void* folded, const void* out,
+                                     const void* workspace, size_t workspace_bytes) {
+  QAGNN_RETURN_IF(check_shape_fwd(shape));
+  if (!H_in || !node_type || !node_score || !prep || !folded || !out || !workspace) return QAGNN_ERR_INVALID_ARGUMENT;
+  if (workspace_bytes < make_work_layout(*shape).total * sizeof(float)) return QAGNN_ERR_WORKSPACE;
+  return QAGNN_OK;
+}
+
+extern "C" int32_t qagnn_mp_forward(const qagnn_shape* shape, const float* H_in, const int64_t* node_type,
+                                    const float* node_score, const void* prep, const void* folded, float* out,
+                                    float* x_layers_out, void* workspace, size_t workspace_bytes, void* stream) {
+  QAGNN_RETURN_IF(check_mp_forward_args(shape, H_in, node_type, node_score, prep, folded, out, workspace, workspace_bytes));
+  return mp_forward(*shape, 3, false, H_in, node_type, node_score, prep, folded, out, x_layers_out, (float*)workspace,
+                    (cudaStream_t)stream);
+}
+
+extern "C" int32_t qagnn_mp_forward_typed(const qagnn_shape* shape, int32_t dtype, int32_t in_dtype, const void* H_in,
+                                          const int64_t* node_type, const float* node_score, const void* prep,
+                                          const void* folded, void* out, float* x_layers_out, void* workspace,
+                                          size_t workspace_bytes, void* stream) {
+  if (in_dtype != QAGNN_DTYPE_F32 && in_dtype != QAGNN_DTYPE_BF16) return QAGNN_ERR_INVALID_ARGUMENT;
+  if (dtype == QAGNN_DTYPE_F32) {
+    if (in_dtype != QAGNN_DTYPE_F32) return QAGNN_ERR_INVALID_ARGUMENT;
+    return qagnn_mp_forward(shape, (const float*)H_in, node_type, node_score, prep, folded, (float*)out, x_layers_out,
+                            workspace, workspace_bytes, stream);
+  }
+  if (dtype != QAGNN_DTYPE_BF16) return QAGNN_ERR_INVALID_ARGUMENT;
+  QAGNN_RETURN_IF(check_mp_forward_args(shape, H_in, node_type, node_score, prep, folded, out, workspace, workspace_bytes));
+  return mp_forward(*shape, 1, in_dtype == QAGNN_DTYPE_BF16, H_in, node_type, node_score, prep, folded, out, x_layers_out,
+                    (float*)workspace, (cudaStream_t)stream);
 }
 
 extern "C" int32_t qagnn_mp_core_forward(const qagnn_shape* shape, const void* prep, const float* qkm, const float* ke,
@@ -687,6 +831,21 @@ extern "C" size_t qagnn_linear_workspace_bytes(int64_t M, int32_t N, int32_t K1,
   if (M <= 0 || N <= 0 || K1 <= 0 || K2 < 0) return 0;
   const size_t K = (size_t)K1 + K2;
   return align_up(2 * 2 * ((size_t)M * K + (size_t)N * K) + 8 * 1024);
+}
+
+extern "C" int32_t qagnn_linear_bf16(const void* A1, int32_t lda1, int32_t K1, const void* A2, int32_t lda2, int32_t K2,
+                                     const void* Wt, int32_t ldw, const float* bias, float* C, int32_t ldc, void* C_bf16,
+                                     int32_t ldp, int64_t M, int32_t N, int32_t act, void* stream) {
+  if (!A1 || !Wt || (!C && !C_bf16) || M <= 0 || N <= 0 || K1 <= 0 || K2 < 0 || (K2 > 0 && !A2)) return QAGNN_ERR_INVALID_ARGUMENT;
+  if (act < 0 || act > 2) return QAGNN_ERR_INVALID_ARGUMENT;
+  if (!gemm_tc_available() || !gemm_tc_shape_ok(K1, K2, lda1, lda2, ldw, N)) return QAGNN_ERR_UNSUPPORTED;
+  TcOperand o1{A1, nullptr, lda1, K1}, o2{K2 ? A2 : nullptr, nullptr, lda2, K2}, ow{Wt, nullptr, ldw, K1 + K2};
+  TcOutput out{};
+  out.f32 = C;
+  out.ldc = ldc;
+  out.hi = C_bf16;
+  out.ldp = ldp;
+  return gemm_tc(o1, o2, ow, bias, M, N, (Act)act, out, (cudaStream_t)stream, 1);
 }
 
 extern "C" int32_t qagnn_linear_bf16x3(const float* A1, int32_t lda1, int32_t K1, const float* A2, int32_t lda2, int32_t K2,

@@ -156,13 +156,16 @@ bool gemm_tc_shape_ok(int K1, int K2, int lda1, int lda2, int ldw, int N);
 // wgmma), so a tile holds whole heads of one `which`.  0 when no head fits (DP > 256) or DP is odd.
 int hm_n_step(const HeadMajorOut& hm);
 int32_t split_bf16(const float* a, int lda, long long M, int K, void* hi, void* lo, int ldp, cudaStream_t st);
+// passes = 3: split-bf16 (hi*hi + hi*lo + lo*hi); passes = 1: the hi planes alone (bf16 operands, fp32 accumulation) - the
+// lo planes of the operands and of the output are then neither read nor written and may be null
 int32_t gemm_tc(const TcOperand& A1, const TcOperand& A2, const TcOperand& W, const float* bias, long long M, int N,
-                Act act, const TcOutput& out, cudaStream_t st);
+                Act act, const TcOutput& out, cudaStream_t st, int passes = 3);
 // Fused node MLP, one launch: out = act2( W2 . ReLU(W1 . A + b1) + b2 ), A [M, D], W1 / W2 [D, D], the hidden layer kept in
-// registers.  Same arithmetic, bit for bit, as the two gemm_tc calls it replaces.  Shapes: D % 8 == 0, 8 <= D <= 208.
+// registers.  Same arithmetic, bit for bit, as the two gemm_tc calls it replaces (with the same pass count).  Shapes:
+// D % 8 == 0, 8 <= D <= 208.
 bool mlp_tc_shape_ok(int D);
 int32_t mlp_tc(const TcOperand& A, const TcOperand& W1, const float* b1, const TcOperand& W2, const float* b2, long long M,
-               Act act2, const TcOutput& out, cudaStream_t st);
+               Act act2, const TcOutput& out, cudaStream_t st, int passes = 3);
 
 // ---- shared-memory-tiled message passing (mp_headtile.cu) ----------------------------------------------
 inline int head_dim_padded(int d) { return (d + 3) / 4 * 4; }

@@ -16,6 +16,10 @@
 // and each k-step issues three MMAs (hi*hi + hi*lo + lo*hi) into the same fp32 accumulator: the
 // dropped terms are O(2^-17) relative, ~50x below the parity bar, at 3 tensor passes instead of
 // the ~30x slower FFMA path (sgemm.cu, kept as the exact-fp32 fallback).
+//
+// Single pass (passes = 1: gemm_bf16_kernel / mlp_bf16_kernel, the eval forward under bf16 autocast): the same kernels on
+// the hi planes alone - a ring stage is [A hi | W hi], one wgmma per k16 step, and the epilogue writes fp32 and/or the hi
+// plane.  The caller has asked for bf16 matmul operands, and hi = bf16_rn(v) is exactly that rounding.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <stdio.h>
@@ -40,11 +44,16 @@ constexpr int kCtrlBytes = 1024;         // mbarriers after the operand ring
 // with them (bn = 208: 2 stages of 86 KB leave 58 KB), else one (bn = 64 / 128 keep 4 / 3 stages, bn = 256 its 2).
 constexpr uint32_t kStBytes = 13312;
 __host__ __device__ constexpr int st_bufs(int bn) { return bn == 208 ? 2 : 1; }
-__host__ __device__ constexpr size_t ring_stage_bytes(int bn) { return 2 * (size_t)BM * BK * 2 + 2 * (size_t)bn * BK * 2; }
-__host__ __device__ constexpr int ring_stages(int bn) {
-  return (kSmemCap - kCtrlBytes - 2 * st_bufs(bn) * kStBytes) / ring_stage_bytes(bn) > 6
+// bf16 planes per operand: hi and lo for the split-bf16 passes (3), hi alone for the single pass (1)
+__host__ __device__ constexpr int planes_of(int passes) { return passes == 1 ? 1 : 2; }
+__host__ __device__ constexpr size_t ring_stage_bytes(int bn, int passes = 3) {
+  return planes_of(passes) * ((size_t)BM * BK * 2 + (size_t)bn * BK * 2);
+}
+// bn = 208: 2 stages of 86 KB (split) or 4 of 43 KB (single pass) beside the two staging buffers per warpgroup
+__host__ __device__ constexpr int ring_stages(int bn, int passes = 3) {
+  return (kSmemCap - kCtrlBytes - 2 * st_bufs(bn) * kStBytes) / ring_stage_bytes(bn, passes) > 6
              ? 6
-             : (int)((kSmemCap - kCtrlBytes - 2 * st_bufs(bn) * kStBytes) / ring_stage_bytes(bn));
+             : (int)((kSmemCap - kCtrlBytes - 2 * st_bufs(bn) * kStBytes) / ring_stage_bytes(bn, passes));
 }
 
 struct TcParams {
@@ -203,17 +212,20 @@ __device__ __forceinline__ void wgmma_bf16<256>(float (&d)[128], uint64_t da, ui
       : "l"(da), "l"(db), "r"(scale_d));
 }
 
-// the three split-bf16 passes (hi*hi, hi*lo, lo*hi) of the first STEPS k16-steps of one k block; A / W plane tiles at
-// sa / sw.  STEPS is a compile-time count: a run-time one makes ptxas fence every wgmma of the chain.
-template <int BN, int STEPS>
+// the three split-bf16 passes (hi*hi, hi*lo, lo*hi) of the first STEPS k16-steps of one k block, or hi*hi alone when
+// P = 1; A / W plane tiles at sa / sw.  STEPS is a compile-time count: a run-time one makes ptxas fence every wgmma of the
+// chain.
+template <int BN, int STEPS, int P = 3>
 __device__ __forceinline__ void mma_kblock(float (&acc)[BN / 2], uint32_t sa, uint32_t sw, uint32_t a_bytes, uint32_t w_bytes) {
 #pragma unroll
   for (int k = 0; k < STEPS; ++k) {
-    const uint64_t da_hi = wgmma_desc(sa + k * 32), da_lo = wgmma_desc(sa + a_bytes + k * 32);
-    const uint64_t dw_hi = wgmma_desc(sw + k * 32), dw_lo = wgmma_desc(sw + w_bytes + k * 32);
+    const uint64_t da_hi = wgmma_desc(sa + k * 32), dw_hi = wgmma_desc(sw + k * 32);
     wgmma_bf16<BN>(acc, da_hi, dw_hi, 1u);
-    wgmma_bf16<BN>(acc, da_hi, dw_lo, 1u);
-    wgmma_bf16<BN>(acc, da_lo, dw_hi, 1u);
+    if constexpr (P == 3) {
+      const uint64_t da_lo = wgmma_desc(sa + a_bytes + k * 32), dw_lo = wgmma_desc(sw + w_bytes + k * 32);
+      wgmma_bf16<BN>(acc, da_hi, dw_lo, 1u);
+      wgmma_bf16<BN>(acc, da_lo, dw_hi, 1u);
+    }
   }
 }
 
@@ -255,255 +267,26 @@ __device__ __forceinline__ void split_pair(float v0, float v1, uint32_t& hi, uin
   hi = *reinterpret_cast<uint32_t*>(&h2);
   lo = *reinterpret_cast<uint32_t*>(&l2);
 }
+// hi = bf16(v) of a column pair alone (single pass: no lo plane)
+__device__ __forceinline__ uint32_t hi_pair(float v0, float v1) {
+  __nv_bfloat162 h2;
+  h2.x = __float2bfloat16_rn(v0);
+  h2.y = __float2bfloat16_rn(v1);
+  return *reinterpret_cast<uint32_t*>(&h2);
+}
 
 // Persistent CTAs (CTAS = 1) or CTA pairs (CTAS = 2, one cluster) walk the (row block, n tile) grid with n fastest.
-// Ring stage = [A hi | A lo | W hi | W lo], each a 1024-byte aligned K-major tile of 64 bf16 per row.
+// Ring stage = [A hi | A lo | W hi | W lo] (P = 3) or [A hi | W hi] (P = 1), each a 1024-byte aligned K-major tile of 64
+// bf16 per row.  Both kernels are the one body in gemm_tc_body.cuh with their pass count.
 template <int ACT, int BN, int CTAS>
 __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_constant__ TcParams p) {
-  extern __shared__ __align__(1024) unsigned char smem[];
-  constexpr uint32_t a_bytes = BM * BK * 2;  // one A plane tile: 16 KB
-  constexpr uint32_t w_bytes = BN * BK * 2;  // one W plane k block
-  constexpr uint32_t stage_bytes = 2 * a_bytes + 2 * w_bytes;
-  constexpr int kBufs = st_bufs(BN);
-  static_assert(ring_stages(BN) >= 2, "the epilogue staging leaves room for two ring stages");
-  const int wg = threadIdx.x >> 7, tid = threadIdx.x & 127;
-  const uint32_t rank = CTAS == 2 ? cluster_ctarank() : 0u;
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + (size_t)p.stages * stage_bytes);  // [stages]  TMA -> MMA
-  uint64_t* empty = full + p.stages;                                                      // [stages]  MMA -> TMA
-  unsigned char* staging = smem + (size_t)p.stages * stage_bytes + kCtrlBytes;           // [2 warpgroups][kBufs]
-
-  // k-blocks across the (up to two) A segments
-  int nkb_seg[2];
-  nkb_seg[0] = (p.kseg[0] + BK - 1) / BK;
-  nkb_seg[1] = p.nseg > 1 ? (p.kseg[1] + BK - 1) / BK : 0;
-  const int nkb = nkb_seg[0] + nkb_seg[1];
-  // k16 steps of the last k block of each segment: only those that reach its K (the rest would multiply TMA's zero fill)
-  const int tail_steps0 = (p.kseg[0] - 1) % BK / 16 + 1;
-  const int tail_steps1 = nkb_seg[1] > 0 ? (p.kseg[1] - 1) % BK / 16 + 1 : BK / 16;
-  const int n_tiles = (p.N + p.n_step - 1) / p.n_step;
-  const long long total_tiles = (p.M + BM * CTAS - 1) / (BM * CTAS) * n_tiles;
-  const long long cl_id = blockIdx.x / CTAS, n_cl = gridDim.x / CTAS;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < p.stages; ++s) {
-      mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 8 * CTAS);  // one arrival per consumer warp of every CTA whose W half lands here
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncthreads();
-  if (CTAS == 2) cluster_sync_all();  // the peer's barriers are initialised before any multicast or remote arrive
-
-  if (wg == 0) {
-    // ===================================== TMA producer =====================================
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
-    if (tid == 0) {
-      long long it = 0;  // k-block counter across tiles
-      for (long long tile = cl_id; tile < total_tiles; tile += n_cl) {
-        const int n0 = (int)(tile % n_tiles) * p.n_step;
-        const int m0 = (int)((tile / n_tiles) * BM * CTAS + rank * BM);
-        for (int kb = 0; kb < nkb; ++kb, ++it) {
-          const int s = (int)(it % p.stages);
-          // the stage is free once the consumers of BOTH CTAs have read it (the W half of this CTA lands in both)
-          if (it >= p.stages) mbar_wait(&empty[s], (uint32_t)((it / p.stages) - 1) & 1u);
-          const int seg = kb < nkb_seg[0] ? 0 : 1;
-          const int k_in_seg = (seg == 0 ? kb : kb - nkb_seg[0]) * BK;
-          const int k_glob = (seg == 0 ? 0 : p.kseg[0]) + k_in_seg;
-          unsigned char* st = smem + (size_t)s * stage_bytes;
-          mbar_expect_tx(&full[s], stage_bytes);
-          tma_load_2d(st, &p.a_hi[seg], k_in_seg, m0, &full[s]);
-          tma_load_2d(st + a_bytes, &p.a_lo[seg], k_in_seg, m0, &full[s]);
-          if (CTAS == 1) {
-            tma_load_2d(st + 2 * a_bytes, &p.w_hi, k_glob, n0, &full[s]);
-            tma_load_2d(st + 2 * a_bytes + w_bytes, &p.w_lo, k_glob, n0, &full[s]);
-          } else {
-            const uint32_t half = w_bytes / 2;
-            tma_load_2d_multicast(st + 2 * a_bytes + rank * half, &p.w_hi, k_glob, n0 + (int)rank * (BN / 2), &full[s], 3);
-            tma_load_2d_multicast(st + 2 * a_bytes + w_bytes + rank * half, &p.w_lo, k_glob, n0 + (int)rank * (BN / 2), &full[s], 3);
-          }
-        }
-      }
-    }
-  } else {
-    // ===================================== consumers (warpgroups 1, 2) =====================================
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
-    const int wc = wg - 1;  // rows wc*64 .. wc*64+63 of the tile
-    const int warp = tid >> 5, lane = tid & 31;
-    // head-major epilogue: column c = 8j + 2(lane & 3) of a tile is element jj of head hh (c = hh * DP + jj).  The divisions
-    // happen once here; the column loop carries (hh, jj) along.
-    const bool hm_mode = p.c_hm != nullptr;
-    const int DP = hm_mode ? p.hm.DP : 8;
-    const int hh0 = 2 * (lane & 3) / DP, jj0 = 2 * (lane & 3) - hh0 * DP;
-    const int q8 = 8 / DP, r8 = 8 - q8 * DP;
-    float acc[BN / 2];
-    long long it = 0;
-    int st_it = 0;  // staged chunks so far: buffer st_it % kBufs
-    for (long long tile = cl_id; tile < total_tiles; tile += n_cl) {
-#pragma unroll
-      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-      for (int kb = 0; kb < nkb; ++kb, ++it) {
-        const int s = (int)(it % p.stages);
-        mbar_wait(&full[s], (uint32_t)(it / p.stages) & 1u);
-        const uint32_t sbase = smem_u32(smem + (size_t)s * stage_bytes);
-        const uint32_t sa = sbase + (uint32_t)wc * 64 * 128, sw = sbase + 2 * a_bytes;
-        const int steps = kb == nkb_seg[0] - 1 ? tail_steps0 : kb == nkb - 1 ? tail_steps1 : BK / 16;
-        fence_acc<BN / 2>(acc);
-        wgmma_fence();
-        // one compile-time chain per step count, each committing its own group
-        switch (steps) {
-          case 1: mma_kblock<BN, 1>(acc, sa, sw, a_bytes, w_bytes); wgmma_commit(); break;
-          case 2: mma_kblock<BN, 2>(acc, sa, sw, a_bytes, w_bytes); wgmma_commit(); break;
-          case 3: mma_kblock<BN, 3>(acc, sa, sw, a_bytes, w_bytes); wgmma_commit(); break;
-          default: mma_kblock<BN, 4>(acc, sa, sw, a_bytes, w_bytes); wgmma_commit(); break;
-        }
-        wgmma_wait_all();
-        fence_acc<BN / 2>(acc);
-        release_stage<CTAS>(&empty[s], lane);
-      }
-      // ---- epilogue: thread holds rows g, g + 8 and column pairs 8j + 2q of the accumulator fragment
-      const int n_tile = (int)(tile % n_tiles);
-      const int n0 = n_tile * p.n_step;
-      const long long row_g = (tile / n_tiles) * BM * CTAS + rank * BM + wc * 64 + warp * 16 + (lane >> 2);
-      // head-major output: the tile's first column starts plane n0 / DP (= which * H + head) of [3][H][N][DP]
-      const int hm_plane0 = hm_mode ? n0 / DP : 0;
-      if (p.st_w > 0) {
-        // through shared memory in chunks of W tile columns (W >= 8 divides n_step and, head-major, DP): the fragment is
-        // walked in column order, as below, so each accumulator dies once written.  A chunk opens (its buffer free) in the
-        // group that holds its first column and closes in the one that holds its last: thread 0 of the warpgroup then
-        // stores its [64][W] fp32 / bf16 hi / bf16 lo boxes with TMA.  A group straddles two chunks only with two buffers.
-        const int W = p.st_w;
-        const int rl = warp * 16 + (lane >> 2);  // fragment rows rl, rl + 8 of the warpgroup's 64
-        const int r0 = (int)(row_g - rl);
-        int boff[2] = {0, 0};  // per-row bias table offsets
-        if (p.bias != nullptr && p.row_class != nullptr) {
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            long long c = row_g + 8 * h < p.M ? p.row_class[row_g + 8 * h] : 0;
-            c = c < 0 ? 0 : (c >= p.n_class ? p.n_class - 1 : c);
-            boff[h] = (int)c * p.class_stride;
-          }
-        }
-        const bool f32_out = hm_mode || p.c_f32 != nullptr, pl_out = p.c_hi != nullptr;
-        const uint32_t f32_bytes = f32_out ? 64u * W * 4 : 0u, pl_bytes = 64u * W * 2;
-        const uint32_t st0 = smem_u32(staging) + (uint32_t)wc * kBufs * kStBytes;
-        int open_end = 0;  // columns [0, open_end) are in chunks opened so far
-        int close_end = W;  // the oldest open chunk is [close_end - W, close_end)
-#pragma unroll
-        for (int j = 0; j < BN / 8; ++j) {
-          if (8 * j >= p.n_step) break;
-          if (open_end < 8 * j + 8) {  // a chunk starts here: wait until the store that read its buffer last is done
-            if (tid == 0) {
-              if (kBufs == 2 && open_end == close_end) bulk_wait_read<0>();  // the chunk before is still open
-              else bulk_wait_read<kBufs - 1>();
-            }
-            wg_bar(1 + wc);
-            open_end += W;
-          }
-          const int c = 8 * j + 2 * (lane & 3), gc = n0 + c;
-          const bool second = c >= close_end;
-          const uint32_t buf = st0 + (uint32_t)((st_it + (second ? 1 : 0)) % kBufs) * kStBytes;
-          const int cc = c - (second ? close_end : close_end - W);
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
-            if (p.bias != nullptr) {  // columns from N on are clipped by the store
-              if (gc < p.N) v0 += __ldg(p.bias + boff[h] + gc);
-              if (gc + 1 < p.N) v1 += __ldg(p.bias + boff[h] + gc + 1);
-            }
-            v0 = act_fn<ACT>(v0);
-            v1 = act_fn<ACT>(v1);
-            const uint32_t e = (uint32_t)((rl + 8 * h) * W + cc);
-            if (f32_out) st_shared_f2(buf + 4 * e, v0, v1);
-            if (pl_out) {
-              uint32_t hi, lo;
-              split_pair(v0, v1, hi, lo);
-              st_shared_u32(buf + f32_bytes + 2 * e, hi);
-              st_shared_u32(buf + f32_bytes + pl_bytes + 2 * e, lo);
-            }
-          }
-          if (close_end <= 8 * j + 8) {  // the oldest open chunk is complete
-            fence_proxy_async();
-            wg_bar(1 + wc);
-            if (tid == 0) {
-              const int cb = close_end - W;
-              const unsigned char* b = staging + (size_t)(wc * kBufs + st_it % kBufs) * kStBytes;
-              if (f32_out) {
-                if (hm_mode) tma_store_3d(&p.st_f32, b, cb % DP, r0, hm_plane0 + cb / DP);
-                else tma_store_3d(&p.st_f32, b, n0 + cb, r0, 0);
-              }
-              if (pl_out) {
-                tma_store_3d(&p.st_hi, b + f32_bytes, n0 + cb, r0, 0);
-                tma_store_3d(&p.st_lo, b + f32_bytes + pl_bytes, n0 + cb, r0, 0);
-              }
-              bulk_commit();
-            }
-            close_end += W;
-            ++st_it;
-          }
-        }
-        continue;
-      }
-      // straight from the fragment to global memory (QAGNN_TC_STORE=direct, or outputs TMA cannot address)
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const long long r = row_g + 8 * h;
-        if (r >= p.M) continue;
-        const float* bias_row = p.bias;  // per-row bias table (node-type classes)
-        if (p.bias != nullptr && p.row_class != nullptr) {
-          long long c = p.row_class[r];
-          c = c < 0 ? 0 : (c >= p.n_class ? p.n_class - 1 : c);
-          bias_row = p.bias + (size_t)c * p.class_stride;
-        }
-        int hh = hh0, jj = jj0;
-#pragma unroll
-        for (int j = 0; j < BN / 8; ++j) {
-          if (hm_mode && j > 0) {  // c += 8 = q8 heads + r8 columns, r8 < DP
-            jj += r8;
-            hh += q8;
-            if (jj >= DP) { jj -= DP; ++hh; }
-          }
-          const int c = 8 * j + 2 * (lane & 3);  // tile column (even); n_step is even, so c + 1 < n_step too
-          const int gc = n0 + c;
-          if (c >= p.n_step || gc >= p.N) continue;
-          const bool two = gc + 1 < p.N;
-          float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
-          if (p.bias != nullptr) {  // bias is indexed by GEMM column (padded like the weight rows)
-            v0 += __ldg(bias_row + gc);
-            if (two) v1 += __ldg(bias_row + gc + 1);
-          }
-          v0 = act_fn<ACT>(v0);
-          v1 = act_fn<ACT>(v1);
-          if (hm_mode) {  // tile = whole heads of one `which`: column c is element jj of plane hm_plane0 + hh
-            float* o = p.c_hm + ((size_t)(hm_plane0 + hh) * p.M + r) * DP + jj;
-            *reinterpret_cast<float2*>(o) = make_float2(v0, v1);
-          } else if (p.c_f32 != nullptr) {
-            float* o = p.c_f32 + (size_t)r * p.ldc + gc;
-            if (two) *reinterpret_cast<float2*>(o) = make_float2(v0, v1);
-            else o[0] = v0;
-          }
-          if (p.c_hi != nullptr) {
-            __nv_bfloat162 h2, l2;
-            h2.x = __float2bfloat16_rn(v0);
-            h2.y = __float2bfloat16_rn(v1);
-            l2.x = __float2bfloat16_rn(v0 - __bfloat162float(h2.x));
-            l2.y = __float2bfloat16_rn(v1 - __bfloat162float(h2.y));
-            __nv_bfloat16* oh = p.c_hi + (size_t)r * p.ldp + gc;
-            __nv_bfloat16* ol = p.c_lo + (size_t)r * p.ldp + gc;
-            if (two) {
-              *reinterpret_cast<__nv_bfloat162*>(oh) = h2;
-              *reinterpret_cast<__nv_bfloat162*>(ol) = l2;
-            } else {
-              oh[0] = h2.x;
-              ol[0] = l2.x;
-            }
-          }
-        }
-      }
-    }
-    if (tid == 0) bulk_wait_all();  // no store still reads the staging buffers when the CTA exits
-  }
-  __syncthreads();
-  if (CTAS == 2) cluster_sync_all();  // the peer's multicasts and remote arrivals target this CTA: nobody leaves early
+  constexpr int P = 3;
+#include "gemm_tc_body.cuh"
+}
+template <int ACT, int BN, int CTAS>
+__global__ void __launch_bounds__(kThreads, 1) gemm_bf16_kernel(const __grid_constant__ TcParams p) {
+  constexpr int P = 1;
+#include "gemm_tc_body.cuh"
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -527,10 +310,10 @@ constexpr uint32_t kW2Sub = kMlpChunk * BK * 2;    // one W2 plane k block of a 
 // epilogue staging per warpgroup: one chunk of its 64 rows, fp32 or both bf16 planes (staged one after the other when
 // both are asked for: two buffers would leave room for one ring stage only)
 constexpr uint32_t kMlpStBytes = 64 * kMlpChunk * 4;
-constexpr int mlp_ring_stages() {
-  return (int)((kSmemCap - kCtrlBytes - 2 * kMlpStBytes) / ring_stage_bytes(kMlpMaxD)) > 6
+constexpr int mlp_ring_stages(int passes = 3) {
+  return (int)((kSmemCap - kCtrlBytes - 2 * kMlpStBytes) / ring_stage_bytes(kMlpMaxD, passes)) > 6
              ? 6
-             : (int)((kSmemCap - kCtrlBytes - 2 * kMlpStBytes) / ring_stage_bytes(kMlpMaxD));
+             : (int)((kSmemCap - kCtrlBytes - 2 * kMlpStBytes) / ring_stage_bytes(kMlpMaxD, passes));
 }
 static_assert(mlp_ring_stages() >= 2, "the fused MLP's epilogue staging leaves room for two ring stages");
 
@@ -549,31 +332,36 @@ struct MlpParams {
 };
 
 // the three split-bf16 passes of the first STEPS k16 steps of the hidden layer against one W2 chunk (hi planes at sw, lo
-// planes lo_off further; k block kb of a plane at kb * kW2Sub)
-template <int STEPS>
+// planes lo_off further; k block kb of a plane at kb * kW2Sub), or hh * W2 hi alone when P = 1 (hl is then unused)
+template <int STEPS, int P = 3, int HL>
 __device__ __forceinline__ void mma_chunk(float (&acc)[kMlpChunk / 2], const uint32_t (&hh)[kMlpMaxD / 4],
-                                          const uint32_t (&hl)[kMlpMaxD / 4], uint32_t sw, uint32_t lo_off) {
+                                          const uint32_t (&hl)[HL], uint32_t sw, uint32_t lo_off) {
 #pragma unroll
   for (int t = 0; t < STEPS; ++t) {
     const uint32_t off = (uint32_t)(t >> 2) * kW2Sub + (uint32_t)(t & 3) * 32;
-    const uint64_t dw_hi = wgmma_desc(sw + off), dw_lo = wgmma_desc(sw + lo_off + off);
+    const uint64_t dw_hi = wgmma_desc(sw + off);
     wgmma_bf16_rs<kMlpChunk>(acc, hh[4 * t], hh[4 * t + 1], hh[4 * t + 2], hh[4 * t + 3], dw_hi);
-    wgmma_bf16_rs<kMlpChunk>(acc, hh[4 * t], hh[4 * t + 1], hh[4 * t + 2], hh[4 * t + 3], dw_lo);
-    wgmma_bf16_rs<kMlpChunk>(acc, hl[4 * t], hl[4 * t + 1], hl[4 * t + 2], hl[4 * t + 3], dw_hi);
+    if constexpr (P == 3) {
+      const uint64_t dw_lo = wgmma_desc(sw + lo_off + off);
+      wgmma_bf16_rs<kMlpChunk>(acc, hh[4 * t], hh[4 * t + 1], hh[4 * t + 2], hh[4 * t + 3], dw_lo);
+      wgmma_bf16_rs<kMlpChunk>(acc, hl[4 * t], hl[4 * t + 1], hl[4 * t + 2], hl[4 * t + 3], dw_hi);
+    }
   }
 }
 
 // Ring fills per 128-row tile: the k blocks of GEMM1 ([aggr hi | aggr lo | W1 hi | W1 lo], as gemm_tc_kernel at BN = 208),
 // then one fill per W2 chunk ([W2 hi kb 0..nkb-1 | W2 lo kb 0..nkb-1], 72 rows each).  Thread 0 issues them.  With CTA
-// pairs each CTA loads half of W1's rows and every other W2 k block, multicast into both.
-template <int ACT, int CTAS>
-__global__ void __launch_bounds__(kMlpThreads, 1) mlp_tc_kernel(const __grid_constant__ MlpParams p) {
+// pairs each CTA loads half of W1's rows and every other W2 k block, multicast into both.  P = 1 (mlp_bf16_kernel): the
+// hi planes alone, and the hidden layer is one bf16 fragment (52 words at D = 208 instead of 104).
+template <int ACT, int CTAS, int P>
+__device__ __forceinline__ void mlp_body(const MlpParams& p) {
   extern __shared__ __align__(1024) unsigned char smem[];
   constexpr int BN = kMlpMaxD;
+  constexpr int NP = planes_of(P);
   constexpr uint32_t a_bytes = BM * BK * 2;
   constexpr uint32_t w_bytes = BN * BK * 2;
-  constexpr uint32_t stage_bytes = 2 * a_bytes + 2 * w_bytes;
-  static_assert(2 * 4 * kW2Sub <= stage_bytes, "a W2 chunk fills one ring stage");
+  constexpr uint32_t stage_bytes = NP * a_bytes + NP * w_bytes;
+  static_assert(NP * 4 * kW2Sub <= stage_bytes, "a W2 chunk fills one ring stage");
   const int wg = threadIdx.x >> 7, tid = threadIdx.x & 127;
   const uint32_t rank = CTAS == 2 ? cluster_ctarank() : 0u;
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + (size_t)p.stages * stage_bytes);
@@ -585,7 +373,7 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_tc_kernel(const __grid_con
   const int tail_steps = (D - 1) % BK / 16 + 1;
   const int ksteps = (D + 15) / 16;           // k16 steps of GEMM2 = hidden fragment groups in use
   const int nch = (D + kMlpChunk - 1) / kMlpChunk;
-  const uint32_t chunk_bytes = 2u * (uint32_t)nkb * kW2Sub;
+  const uint32_t chunk_bytes = (uint32_t)NP * (uint32_t)nkb * kW2Sub;
   const long long total_tiles = (p.M + BM * CTAS - 1) / (BM * CTAS);
   const long long cl_id = blockIdx.x / CTAS, n_cl = gridDim.x / CTAS;
 
@@ -611,14 +399,15 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_tc_kernel(const __grid_con
       const int kb = sub, m0 = (int)(tile * BM * CTAS + rank * BM);
       mbar_expect_tx(bar, stage_bytes);
       tma_load_2d(st, &p.a_hi, kb * BK, m0, bar);
-      tma_load_2d(st + a_bytes, &p.a_lo, kb * BK, m0, bar);
+      if constexpr (P == 3) tma_load_2d(st + a_bytes, &p.a_lo, kb * BK, m0, bar);
       if (CTAS == 1) {
-        tma_load_2d(st + 2 * a_bytes, &p.w1_hi, kb * BK, 0, bar);
-        tma_load_2d(st + 2 * a_bytes + w_bytes, &p.w1_lo, kb * BK, 0, bar);
+        tma_load_2d(st + NP * a_bytes, &p.w1_hi, kb * BK, 0, bar);
+        if constexpr (P == 3) tma_load_2d(st + 2 * a_bytes + w_bytes, &p.w1_lo, kb * BK, 0, bar);
       } else {
         const uint32_t half = w_bytes / 2;
-        tma_load_2d_multicast(st + 2 * a_bytes + rank * half, &p.w1_hi, kb * BK, (int)rank * (BN / 2), bar, 3);
-        tma_load_2d_multicast(st + 2 * a_bytes + w_bytes + rank * half, &p.w1_lo, kb * BK, (int)rank * (BN / 2), bar, 3);
+        tma_load_2d_multicast(st + NP * a_bytes + rank * half, &p.w1_hi, kb * BK, (int)rank * (BN / 2), bar, 3);
+        if constexpr (P == 3)
+          tma_load_2d_multicast(st + 2 * a_bytes + w_bytes + rank * half, &p.w1_lo, kb * BK, (int)rank * (BN / 2), bar, 3);
       }
     } else {  // W2 chunk: [W2 hi kb 0 .. nkb-1 | W2 lo kb 0 .. nkb-1]
       const int ch = sub - nkb;
@@ -628,10 +417,10 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_tc_kernel(const __grid_con
         unsigned char* lo = st + (size_t)(nkb + kb) * kW2Sub;
         if (CTAS == 1) {
           tma_load_2d(hi, &p.w2_hi, kb * BK, ch * kMlpChunk, bar);
-          tma_load_2d(lo, &p.w2_lo, kb * BK, ch * kMlpChunk, bar);
+          if constexpr (P == 3) tma_load_2d(lo, &p.w2_lo, kb * BK, ch * kMlpChunk, bar);
         } else {
           tma_load_2d_multicast(hi, &p.w2_hi, kb * BK, ch * kMlpChunk, bar, 3);
-          tma_load_2d_multicast(lo, &p.w2_lo, kb * BK, ch * kMlpChunk, bar, 3);
+          if constexpr (P == 3) tma_load_2d_multicast(lo, &p.w2_lo, kb * BK, ch * kMlpChunk, bar, 3);
         }
       }
     }
@@ -663,22 +452,22 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_tc_kernel(const __grid_con
         const int s = (int)(it % p.stages);
         mbar_wait(&full[s], (uint32_t)(it / p.stages) & 1u);
         const uint32_t sbase = smem_u32(smem + (size_t)s * stage_bytes);
-        const uint32_t sa = sbase + (uint32_t)wc * 64 * 128, sw = sbase + 2 * a_bytes;
+        const uint32_t sa = sbase + (uint32_t)wc * 64 * 128, sw = sbase + NP * a_bytes;
         const int steps = kb == nkb - 1 ? tail_steps : BK / 16;
         fence_acc<BN / 2>(acc1);
         wgmma_fence();
         switch (steps) {
-          case 1: mma_kblock<BN, 1>(acc1, sa, sw, a_bytes, w_bytes); wgmma_commit(); break;
-          case 2: mma_kblock<BN, 2>(acc1, sa, sw, a_bytes, w_bytes); wgmma_commit(); break;
-          case 3: mma_kblock<BN, 3>(acc1, sa, sw, a_bytes, w_bytes); wgmma_commit(); break;
-          default: mma_kblock<BN, 4>(acc1, sa, sw, a_bytes, w_bytes); wgmma_commit(); break;
+          case 1: mma_kblock<BN, 1, P>(acc1, sa, sw, a_bytes, w_bytes); wgmma_commit(); break;
+          case 2: mma_kblock<BN, 2, P>(acc1, sa, sw, a_bytes, w_bytes); wgmma_commit(); break;
+          case 3: mma_kblock<BN, 3, P>(acc1, sa, sw, a_bytes, w_bytes); wgmma_commit(); break;
+          default: mma_kblock<BN, 4, P>(acc1, sa, sw, a_bytes, w_bytes); wgmma_commit(); break;
         }
         wgmma_wait_all();
         fence_acc<BN / 2>(acc1);
         release(s);
       }
       // ---- hidden layer in registers: fragment group j (columns 8j + q2, +1; rows g and g + 8) -> words 2j, 2j + 1
-      uint32_t hh[BN / 4], hl[BN / 4];
+      uint32_t hh[BN / 4], hl[P == 3 ? BN / 4 : 1];
 #pragma unroll
       for (int j = 0; j < BN / 8; ++j) {
         const int c = 8 * j + q2;
@@ -689,7 +478,8 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_tc_kernel(const __grid_con
           float v0 = acc1[4 * j + 2 * h] + bb0, v1 = acc1[4 * j + 2 * h + 1] + bb1;
           v0 = in ? act_fn<ACT_RELU>(v0) : 0.f;
           v1 = in ? act_fn<ACT_RELU>(v1) : 0.f;
-          split_pair(v0, v1, hh[2 * j + h], hl[2 * j + h]);
+          if constexpr (P == 3) split_pair(v0, v1, hh[2 * j + h], hl[2 * j + h]);
+          else hh[2 * j + h] = hi_pair(v0, v1);
         }
       }
       // ---- GEMM2 in N chunks, each followed by its epilogue
@@ -704,19 +494,19 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_tc_kernel(const __grid_con
         fence_acc<kMlpChunk / 2>(acc2);
         wgmma_fence();
         switch (ksteps) {  // compile-time chains: the hidden words are registers, indexed by the step
-          case 1: mma_chunk<1>(acc2, hh, hl, sw, lo_off); break;
-          case 2: mma_chunk<2>(acc2, hh, hl, sw, lo_off); break;
-          case 3: mma_chunk<3>(acc2, hh, hl, sw, lo_off); break;
-          case 4: mma_chunk<4>(acc2, hh, hl, sw, lo_off); break;
-          case 5: mma_chunk<5>(acc2, hh, hl, sw, lo_off); break;
-          case 6: mma_chunk<6>(acc2, hh, hl, sw, lo_off); break;
-          case 7: mma_chunk<7>(acc2, hh, hl, sw, lo_off); break;
-          case 8: mma_chunk<8>(acc2, hh, hl, sw, lo_off); break;
-          case 9: mma_chunk<9>(acc2, hh, hl, sw, lo_off); break;
-          case 10: mma_chunk<10>(acc2, hh, hl, sw, lo_off); break;
-          case 11: mma_chunk<11>(acc2, hh, hl, sw, lo_off); break;
-          case 12: mma_chunk<12>(acc2, hh, hl, sw, lo_off); break;
-          default: mma_chunk<13>(acc2, hh, hl, sw, lo_off); break;
+          case 1: mma_chunk<1, P>(acc2, hh, hl, sw, lo_off); break;
+          case 2: mma_chunk<2, P>(acc2, hh, hl, sw, lo_off); break;
+          case 3: mma_chunk<3, P>(acc2, hh, hl, sw, lo_off); break;
+          case 4: mma_chunk<4, P>(acc2, hh, hl, sw, lo_off); break;
+          case 5: mma_chunk<5, P>(acc2, hh, hl, sw, lo_off); break;
+          case 6: mma_chunk<6, P>(acc2, hh, hl, sw, lo_off); break;
+          case 7: mma_chunk<7, P>(acc2, hh, hl, sw, lo_off); break;
+          case 8: mma_chunk<8, P>(acc2, hh, hl, sw, lo_off); break;
+          case 9: mma_chunk<9, P>(acc2, hh, hl, sw, lo_off); break;
+          case 10: mma_chunk<10, P>(acc2, hh, hl, sw, lo_off); break;
+          case 11: mma_chunk<11, P>(acc2, hh, hl, sw, lo_off); break;
+          case 12: mma_chunk<12, P>(acc2, hh, hl, sw, lo_off); break;
+          default: mma_chunk<13, P>(acc2, hh, hl, sw, lo_off); break;
         }
         wgmma_commit();
         wgmma_wait_all();
@@ -743,11 +533,13 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_tc_kernel(const __grid_con
                 const uint32_t e = (uint32_t)((rl + 8 * h) * kMlpChunk + cc);
                 if (part == 0) {
                   st_shared_f2(buf + 4 * e, v0, v1);
-                } else {
+                } else if constexpr (P == 3) {
                   uint32_t hi, lo;
                   split_pair(v0, v1, hi, lo);
                   st_shared_u32(buf + 2 * e, hi);
                   st_shared_u32(buf + kMlpStBytes / 2 + 2 * e, lo);
+                } else {
+                  st_shared_u32(buf + 2 * e, hi_pair(v0, v1));
                 }
               }
             }
@@ -759,7 +551,7 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_tc_kernel(const __grid_con
                 tma_store_3d(&p.st_f32, b, ch * kMlpChunk, r0, 0);
               } else {
                 tma_store_3d(&p.st_hi, b, ch * kMlpChunk, r0, 0);
-                tma_store_3d(&p.st_lo, b + kMlpStBytes / 2, ch * kMlpChunk, r0, 0);
+                if constexpr (P == 3) tma_store_3d(&p.st_lo, b + kMlpStBytes / 2, ch * kMlpChunk, r0, 0);
               }
               bulk_commit();
             }
@@ -778,10 +570,14 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_tc_kernel(const __grid_con
             const float v1 = act_fn<ACT>(acc2[4 * j + 2 * h + 1] + __ldg(p.b2 + gc + 1));
             if (p.c_f32 != nullptr) *reinterpret_cast<float2*>(p.c_f32 + (size_t)r * p.ldc + gc) = make_float2(v0, v1);
             if (p.c_hi != nullptr) {
-              uint32_t hi, lo;
-              split_pair(v0, v1, hi, lo);
-              *reinterpret_cast<uint32_t*>(p.c_hi + (size_t)r * p.ldp + gc) = hi;
-              *reinterpret_cast<uint32_t*>(p.c_lo + (size_t)r * p.ldp + gc) = lo;
+              if constexpr (P == 3) {
+                uint32_t hi, lo;
+                split_pair(v0, v1, hi, lo);
+                *reinterpret_cast<uint32_t*>(p.c_hi + (size_t)r * p.ldp + gc) = hi;
+                *reinterpret_cast<uint32_t*>(p.c_lo + (size_t)r * p.ldp + gc) = lo;
+              } else {
+                *reinterpret_cast<uint32_t*>(p.c_hi + (size_t)r * p.ldp + gc) = hi_pair(v0, v1);
+              }
             }
           }
         }
@@ -791,6 +587,15 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_tc_kernel(const __grid_con
   }
   __syncthreads();
   if (CTAS == 2) cluster_sync_all();
+}
+
+template <int ACT, int CTAS>
+__global__ void __launch_bounds__(kMlpThreads, 1) mlp_tc_kernel(const __grid_constant__ MlpParams p) {
+  mlp_body<ACT, CTAS, 3>(p);
+}
+template <int ACT, int CTAS>
+__global__ void __launch_bounds__(kMlpThreads, 1) mlp_bf16_kernel(const __grid_constant__ MlpParams p) {
+  mlp_body<ACT, CTAS, 1>(p);
 }
 
 __global__ void split_bf16_kernel(const float* __restrict__ a, int lda, long long M, int K, __nv_bfloat16* __restrict__ hi,
@@ -806,7 +611,7 @@ __global__ void split_bf16_kernel(const float* __restrict__ a, int lda, long lon
     ll.x = __float2bfloat16_rn(v.x - __bfloat162float(h0));
     ll.y = __float2bfloat16_rn(v.y - __bfloat162float(h1));
     *reinterpret_cast<__nv_bfloat162*>(hi + r * ldp + c) = hh;
-    *reinterpret_cast<__nv_bfloat162*>(lo + r * ldp + c) = ll;
+    if (lo != nullptr) *reinterpret_cast<__nv_bfloat162*>(lo + r * ldp + c) = ll;
   }
 }
 
@@ -888,30 +693,39 @@ int32_t launch_persistent(void (*kernel)(Params), int ctas, cudaLaunchConfig_t c
   return QAGNN_OK;
 }
 
-template <int ACT, int BN, int CTAS>
+template <int ACT, int BN, int CTAS, int P>
 int32_t launch(cudaLaunchConfig_t cfg, const TcParams& p) {
   static bool attr_set[kMaxDevices] = {false};
   static int max_clusters[kMaxDevices] = {0};
-  return launch_persistent(gemm_tc_kernel<ACT, BN, CTAS>, CTAS, cfg, p, attr_set, max_clusters);
+  return launch_persistent(P == 3 ? gemm_tc_kernel<ACT, BN, CTAS> : gemm_bf16_kernel<ACT, BN, CTAS>, CTAS, cfg, p, attr_set,
+                           max_clusters);
 }
 
-template <int ACT, int CTAS>
+template <int ACT, int CTAS, int P>
 int32_t launch_mlp(cudaLaunchConfig_t cfg, const MlpParams& p) {
   static bool attr_set[kMaxDevices] = {false};
   static int max_clusters[kMaxDevices] = {0};
-  return launch_persistent(mlp_tc_kernel<ACT, CTAS>, CTAS, cfg, p, attr_set, max_clusters);
+  return launch_persistent(P == 3 ? mlp_tc_kernel<ACT, CTAS> : mlp_bf16_kernel<ACT, CTAS>, CTAS, cfg, p, attr_set, max_clusters);
 }
 
-template <int BN, int CTAS>
+template <int BN, int CTAS, int P>
 int32_t launch_act(Act act, const cudaLaunchConfig_t& cfg, const TcParams& p) {
-  if (act == ACT_NONE) return launch<ACT_NONE, BN, CTAS>(cfg, p);
-  if (act == ACT_RELU) return launch<ACT_RELU, BN, CTAS>(cfg, p);
-  return launch<ACT_GELU, BN, CTAS>(cfg, p);
+  if (act == ACT_NONE) return launch<ACT_NONE, BN, CTAS, P>(cfg, p);
+  if (act == ACT_RELU) return launch<ACT_RELU, BN, CTAS, P>(cfg, p);
+  return launch<ACT_GELU, BN, CTAS, P>(cfg, p);
 }
 
 template <int BN>
-int32_t launch_bn(int ctas, Act act, const cudaLaunchConfig_t& cfg, const TcParams& p) {
-  return ctas == 2 ? launch_act<BN, 2>(act, cfg, p) : launch_act<BN, 1>(act, cfg, p);
+int32_t launch_bn(int ctas, int passes, Act act, const cudaLaunchConfig_t& cfg, const TcParams& p) {
+  if (passes == 1) return ctas == 2 ? launch_act<BN, 2, 1>(act, cfg, p) : launch_act<BN, 1, 1>(act, cfg, p);
+  return ctas == 2 ? launch_act<BN, 2, 3>(act, cfg, p) : launch_act<BN, 1, 3>(act, cfg, p);
+}
+
+template <int CTAS, int P>
+int32_t launch_mlp_act(Act act2, const cudaLaunchConfig_t& cfg, const MlpParams& p) {
+  if (act2 == ACT_NONE) return launch_mlp<ACT_NONE, CTAS, P>(cfg, p);
+  if (act2 == ACT_RELU) return launch_mlp<ACT_RELU, CTAS, P>(cfg, p);
+  return launch_mlp<ACT_GELU, CTAS, P>(cfg, p);
 }
 
 // default: CTA pairs (cluster of 2, W tile multicast, half loaded by each); QAGNN_TC_2CTA=0 -> single CTAs.
@@ -958,6 +772,7 @@ int hm_n_step(const HeadMajorOut& hm) {
   return 0;
 }
 
+// lo may be null: the hi plane alone (the single-pass GEMM's operand)
 int32_t split_bf16(const float* a, int lda, long long M, int K, void* hi, void* lo, int ldp, cudaStream_t st) {
   if (M <= 0 || K <= 0) return QAGNN_OK;
   if (K % 2 != 0 || lda % 2 != 0) return QAGNN_ERR_UNSUPPORTED;
@@ -969,9 +784,11 @@ int32_t split_bf16(const float* a, int lda, long long M, int K, void* hi, void* 
 }
 
 int32_t gemm_tc(const TcOperand& A1, const TcOperand& A2, const TcOperand& W, const float* bias, long long M, int N, Act act,
-                const TcOutput& out, cudaStream_t st) {
+                const TcOutput& out, cudaStream_t st, int passes) {
   if (M <= 0 || N <= 0) return QAGNN_OK;
   if (!gemm_tc_available()) return QAGNN_ERR_UNSUPPORTED;
+  if (passes != 1 && passes != 3) return QAGNN_ERR_INVALID_ARGUMENT;
+  const bool single = passes == 1;
   const int K1 = A1.K, K2 = A2.hi ? A2.K : 0;
   if (!gemm_tc_shape_ok(K1, K2, A1.ld, A2.ld, W.ld, N)) return QAGNN_ERR_UNSUPPORTED;
   TcParams p;
@@ -992,12 +809,14 @@ int32_t gemm_tc(const TcOperand& A1, const TcOperand& A2, const TcOperand& W, co
   p.kseg[0] = K1;
   p.kseg[1] = K2;
   const int CTAS = tc_ctas();
-  const int stages = ring_stages(bn);
+  const int stages = ring_stages(bn, passes);
   p.stages = stages;
-  const size_t smem_bytes = stages * ring_stage_bytes(bn) + kCtrlBytes + 2 * st_bufs(bn) * kStBytes;
-  bool ok = make_map(&p.a_hi[0], A1.hi, M, K1, A1.ld, BM) && make_map(&p.a_lo[0], A1.lo, M, K1, A1.ld, BM);
-  if (K2 > 0) ok = ok && make_map(&p.a_hi[1], A2.hi, M, K2, A2.ld, BM) && make_map(&p.a_lo[1], A2.lo, M, K2, A2.ld, BM);
-  ok = ok && make_map(&p.w_hi, W.hi, N, K1 + K2, W.ld, bn / CTAS) && make_map(&p.w_lo, W.lo, N, K1 + K2, W.ld, bn / CTAS);
+  const size_t smem_bytes = stages * ring_stage_bytes(bn, passes) + kCtrlBytes + 2 * st_bufs(bn) * kStBytes;
+  bool ok = make_map(&p.a_hi[0], A1.hi, M, K1, A1.ld, BM) && (single || make_map(&p.a_lo[0], A1.lo, M, K1, A1.ld, BM));
+  if (K2 > 0)
+    ok = ok && make_map(&p.a_hi[1], A2.hi, M, K2, A2.ld, BM) && (single || make_map(&p.a_lo[1], A2.lo, M, K2, A2.ld, BM));
+  ok = ok && make_map(&p.w_hi, W.hi, N, K1 + K2, W.ld, bn / CTAS) &&
+       (single || make_map(&p.w_lo, W.lo, N, K1 + K2, W.ld, bn / CTAS));
   if (!ok) return QAGNN_ERR_CUDA;
   if ((out.f32 && (out.ldc % 4 != 0)) || (out.hi && (out.ldp % 8 != 0))) return QAGNN_ERR_UNSUPPORTED;
   p.bias = bias;
@@ -1009,17 +828,17 @@ int32_t gemm_tc(const TcOperand& A1, const TcOperand& A2, const TcOperand& W, co
   p.c_hm = out.hm_buf;
   p.hm = out.hm;
   p.c_hi = (__nv_bfloat16*)out.hi;
-  p.c_lo = (__nv_bfloat16*)out.lo;
+  p.c_lo = single ? nullptr : (__nv_bfloat16*)out.lo;
   p.ldp = out.ldp;
   if (tc_store_tma()) {
     // chunks of whole tile columns that never cross a head (head-major) or the tile's n_step: a box must not reach the
     // neighbouring tile's columns.  Box rows of 16-byte multiples: fp32 chunks of 4 columns, bf16 chunks of 8; with one
     // staging buffer a chunk must not share a fragment column group with the next, so multiples of 8.
     const bool f32_out = out.hm_buf != nullptr || out.f32 != nullptr, pl_out = out.hi != nullptr;
-    const int col_bytes = 64 * ((f32_out ? 4 : 0) + (pl_out ? 4 : 0));
+    const int col_bytes = 64 * ((f32_out ? 4 : 0) + (pl_out ? 2 * planes_of(passes) : 0));
     const int span = out.hm_buf != nullptr ? out.hm.DP : p.n_step;
     const bool addressable = (!out.hm_buf || aligned16(out.hm_buf)) && (!out.f32 || aligned16(out.f32)) &&
-                             (!pl_out || (aligned16(out.hi) && aligned16(out.lo)));
+                             (!pl_out || (aligned16(out.hi) && (single || aligned16(out.lo))));
     const int w = addressable && (f32_out || pl_out) ? chunk_width(span, pl_out || st_bufs(bn) == 1 ? 8 : 4, (int)kStBytes / col_bytes) : 0;
     if (w > 0) {
       bool sok = true;
@@ -1030,7 +849,7 @@ int32_t gemm_tc(const TcOperand& A1, const TcOperand& A2, const TcOperand& W, co
         sok = make_store_map(&p.st_f32, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, out.f32, N, M, 1, out.ldc, w);
       if (pl_out)
         sok = sok && make_store_map(&p.st_hi, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, out.hi, N, M, 1, out.ldp, w) &&
-              make_store_map(&p.st_lo, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, out.lo, N, M, 1, out.ldp, w);
+              (single || make_store_map(&p.st_lo, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, out.lo, N, M, 1, out.ldp, w));
       if (!sok) return QAGNN_ERR_CUDA;
       p.st_w = w;
       p.st_chunks = p.n_step / w;
@@ -1054,12 +873,12 @@ int32_t gemm_tc(const TcOperand& A1, const TcOperand& A2, const TcOperand& W, co
   lattr[0].val.clusterDim.z = 1;
   cfg.attrs = lattr;
   cfg.numAttrs = CTAS == 2 ? 1 : 0;
-  if (getenv("QAGNN_DEBUG")) fprintf(stderr, "gemm_tc: M=%lld N=%d K1=%d K2=%d act=%d CTAS=%d stages=%d smem=%zu grid=%u bn=%d n_step=%d n_tiles=%d st_w=%d\n", M, N, K1, K2, (int)act, CTAS, stages, smem_bytes, grid, bn, p.n_step, n_tiles, p.st_w);
+  if (getenv("QAGNN_DEBUG")) fprintf(stderr, "gemm_tc: M=%lld N=%d K1=%d K2=%d act=%d CTAS=%d passes=%d stages=%d smem=%zu grid=%u bn=%d n_step=%d n_tiles=%d st_w=%d\n", M, N, K1, K2, (int)act, CTAS, passes, stages, smem_bytes, grid, bn, p.n_step, n_tiles, p.st_w);
   int32_t rc;
-  if (bn == 64) rc = launch_bn<64>(CTAS, act, cfg, p);
-  else if (bn == 128) rc = launch_bn<128>(CTAS, act, cfg, p);
-  else if (bn == 208) rc = launch_bn<208>(CTAS, act, cfg, p);
-  else rc = launch_bn<256>(CTAS, act, cfg, p);
+  if (bn == 64) rc = launch_bn<64>(CTAS, passes, act, cfg, p);
+  else if (bn == 128) rc = launch_bn<128>(CTAS, passes, act, cfg, p);
+  else if (bn == 208) rc = launch_bn<208>(CTAS, passes, act, cfg, p);
+  else rc = launch_bn<256>(CTAS, passes, act, cfg, p);
   QAGNN_RETURN_IF(rc);
   QAGNN_CHECK_LAUNCH();
   return QAGNN_OK;
@@ -1068,9 +887,11 @@ int32_t gemm_tc(const TcOperand& A1, const TcOperand& A2, const TcOperand& W, co
 bool mlp_tc_shape_ok(int D) { return D >= 8 && D % 8 == 0 && D <= kMlpMaxD; }
 
 int32_t mlp_tc(const TcOperand& A, const TcOperand& W1, const float* b1, const TcOperand& W2, const float* b2, long long M,
-               Act act2, const TcOutput& out, cudaStream_t st) {
+               Act act2, const TcOutput& out, cudaStream_t st, int passes) {
   if (M <= 0) return QAGNN_OK;
   if (!gemm_tc_available()) return QAGNN_ERR_UNSUPPORTED;
+  if (passes != 1 && passes != 3) return QAGNN_ERR_INVALID_ARGUMENT;
+  const bool single = passes == 1;
   const int D = A.K;
   if (!mlp_tc_shape_ok(D) || W1.K != D || W2.K != D || b1 == nullptr || b2 == nullptr) return QAGNN_ERR_UNSUPPORTED;
   if (A.ld % 8 != 0 || W1.ld % 8 != 0 || W2.ld % 8 != 0) return QAGNN_ERR_UNSUPPORTED;
@@ -1079,11 +900,12 @@ int32_t mlp_tc(const TcOperand& A, const TcOperand& W1, const float* b1, const T
   const int CTAS = tc_ctas();
   MlpParams p;
   memset(&p, 0, sizeof(p));
-  const int stages = mlp_ring_stages();
-  const size_t smem_bytes = stages * ring_stage_bytes(kMlpMaxD) + kCtrlBytes + 2 * kMlpStBytes;
-  bool ok = make_map(&p.a_hi, A.hi, M, D, A.ld, BM) && make_map(&p.a_lo, A.lo, M, D, A.ld, BM);
-  ok = ok && make_map(&p.w1_hi, W1.hi, D, D, W1.ld, kMlpMaxD / CTAS) && make_map(&p.w1_lo, W1.lo, D, D, W1.ld, kMlpMaxD / CTAS);
-  ok = ok && make_map(&p.w2_hi, W2.hi, D, D, W2.ld, kMlpChunk) && make_map(&p.w2_lo, W2.lo, D, D, W2.ld, kMlpChunk);
+  const int stages = mlp_ring_stages(passes);
+  const size_t smem_bytes = stages * ring_stage_bytes(kMlpMaxD, passes) + kCtrlBytes + 2 * kMlpStBytes;
+  bool ok = make_map(&p.a_hi, A.hi, M, D, A.ld, BM) && (single || make_map(&p.a_lo, A.lo, M, D, A.ld, BM));
+  ok = ok && make_map(&p.w1_hi, W1.hi, D, D, W1.ld, kMlpMaxD / CTAS) &&
+       (single || make_map(&p.w1_lo, W1.lo, D, D, W1.ld, kMlpMaxD / CTAS));
+  ok = ok && make_map(&p.w2_hi, W2.hi, D, D, W2.ld, kMlpChunk) && (single || make_map(&p.w2_lo, W2.lo, D, D, W2.ld, kMlpChunk));
   if (!ok) return QAGNN_ERR_CUDA;
   p.D = D;
   p.stages = stages;
@@ -1093,16 +915,16 @@ int32_t mlp_tc(const TcOperand& A, const TcOperand& W1, const float* b1, const T
   p.c_f32 = out.f32;
   p.ldc = out.ldc;
   p.c_hi = (__nv_bfloat16*)out.hi;
-  p.c_lo = (__nv_bfloat16*)out.lo;
+  p.c_lo = single ? nullptr : (__nv_bfloat16*)out.lo;
   p.ldp = out.ldp;
   // rows are 16-byte multiples (ldc % 4, ldp % 8 above); the bases must be 16-byte aligned too
   if (tc_store_tma() && (out.f32 || out.hi) && (!out.f32 || aligned16(out.f32)) &&
-      (!out.hi || (aligned16(out.hi) && aligned16(out.lo)))) {
+      (!out.hi || (aligned16(out.hi) && (single || aligned16(out.lo))))) {
     bool sok = true;
     if (out.f32) sok = make_store_map(&p.st_f32, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, out.f32, D, M, 1, out.ldc, kMlpChunk);
     if (out.hi)
       sok = sok && make_store_map(&p.st_hi, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, out.hi, D, M, 1, out.ldp, kMlpChunk) &&
-            make_store_map(&p.st_lo, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, out.lo, D, M, 1, out.ldp, kMlpChunk);
+            (single || make_store_map(&p.st_lo, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, out.lo, D, M, 1, out.ldp, kMlpChunk));
     if (!sok) return QAGNN_ERR_CUDA;
     p.tma_store = 1;
   }
@@ -1123,10 +945,10 @@ int32_t mlp_tc(const TcOperand& A, const TcOperand& W1, const float* b1, const T
   lattr[0].val.clusterDim.z = 1;
   cfg.attrs = lattr;
   cfg.numAttrs = CTAS == 2 ? 1 : 0;
-  if (getenv("QAGNN_DEBUG")) fprintf(stderr, "mlp_tc: M=%lld D=%d act2=%d CTAS=%d stages=%d smem=%zu grid=%u\n", M, D, (int)act2, CTAS, stages, smem_bytes, cfg.gridDim.x);
+  if (getenv("QAGNN_DEBUG")) fprintf(stderr, "mlp_tc: M=%lld D=%d act2=%d CTAS=%d passes=%d stages=%d smem=%zu grid=%u\n", M, D, (int)act2, CTAS, passes, stages, smem_bytes, cfg.gridDim.x);
   int32_t rc;
-  if (CTAS == 2) rc = act2 == ACT_NONE ? launch_mlp<ACT_NONE, 2>(cfg, p) : act2 == ACT_RELU ? launch_mlp<ACT_RELU, 2>(cfg, p) : launch_mlp<ACT_GELU, 2>(cfg, p);
-  else rc = act2 == ACT_NONE ? launch_mlp<ACT_NONE, 1>(cfg, p) : act2 == ACT_RELU ? launch_mlp<ACT_RELU, 1>(cfg, p) : launch_mlp<ACT_GELU, 1>(cfg, p);
+  if (single) rc = CTAS == 2 ? launch_mlp_act<2, 1>(act2, cfg, p) : launch_mlp_act<1, 1>(act2, cfg, p);
+  else rc = CTAS == 2 ? launch_mlp_act<2, 3>(act2, cfg, p) : launch_mlp_act<1, 3>(act2, cfg, p);
   QAGNN_RETURN_IF(rc);
   QAGNN_CHECK_LAUNCH();
   return QAGNN_OK;

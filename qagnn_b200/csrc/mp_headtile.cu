@@ -509,12 +509,12 @@ __global__ void __launch_bounds__((WMAX + 1) * 32, 1) mp_headtile_kernel(const H
             h01.x = __float2bfloat16_rn(v0); h01.y = __float2bfloat16_rn(v1);
             l01.x = __float2bfloat16_rn(v0 - __bfloat162float(h01.x)); l01.y = __float2bfloat16_rn(v1 - __bfloat162float(h01.y));
             *reinterpret_cast<__nv_bfloat162*>(oh) = h01;
-            *reinterpret_cast<__nv_bfloat162*>(ol) = l01;
+            if (p.aggr_lo != nullptr) *reinterpret_cast<__nv_bfloat162*>(ol) = l01;  // null: the hi plane alone (single pass)
             if (c0 + 2 < p.d) {
               h23.x = __float2bfloat16_rn(v2); h23.y = __float2bfloat16_rn(v3);
               l23.x = __float2bfloat16_rn(v2 - __bfloat162float(h23.x)); l23.y = __float2bfloat16_rn(v3 - __bfloat162float(h23.y));
               *reinterpret_cast<__nv_bfloat162*>(oh + 2) = h23;
-              *reinterpret_cast<__nv_bfloat162*>(ol + 2) = l23;
+              if (p.aggr_lo != nullptr) *reinterpret_cast<__nv_bfloat162*>(ol + 2) = l23;
             }
           }
         }

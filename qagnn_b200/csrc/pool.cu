@@ -10,15 +10,22 @@
 // Σ_i a_i (W_v,h x_i + b_v,h) = W_v,h (Σ_i a_i x_i) + b_v,h   (Σ_i a_i = 1).  One CTA per graph then reads the
 // graph's [n, D] node tile ONCE: logits for all heads, masked softmax, attention-weighted node sum; the two tiny
 // per-graph matrix-vector products run in the same CTA.  No N-sized GEMM, no ks/vs round trip through HBM.
+#include <cuda_bf16.h>
+
 #include "common.cuh"
 
 namespace qagnn {
 namespace {
 
+// node features X as fp32 or bf16 (the bf16 eval forward's output): bf16 widens exactly
+__device__ __forceinline__ float xval(float v) { return v; }
+__device__ __forceinline__ float xval(__nv_bfloat16 v) { return __bfloat162float(v); }
+
 constexpr int kPoolThreads = 256;  // latency-bound kernel: <= 64 registers so that 4 CTAs (graphs) share an SM
 
 // dynamic smem: qk[nh][D] | logit[nh][n] | xs[nh][D] | cst[nh, padded to 8] | part[warps][nh][D]
-__global__ void __launch_bounds__(kPoolThreads, 4) attention_pool_kernel(int n, int D, int nh, const float* __restrict__ X,
+template <typename XT>
+__global__ void __launch_bounds__(kPoolThreads, 4) attention_pool_kernel(int n, int D, int nh, const XT* __restrict__ X,
                                                                         const float* __restrict__ qs, const unsigned char* __restrict__ mask,
                                                                         const float* __restrict__ wk, const float* __restrict__ bk,
                                                                         const float* __restrict__ wv, const float* __restrict__ bv,
@@ -37,7 +44,7 @@ __global__ void __launch_bounds__(kPoolThreads, 4) attention_pool_kernel(int n, 
   float* cst = xs + nh * D;        // [nh]      qs_h·b_k,h
   const int b = blockIdx.x, tid = threadIdx.x, dk = D / nh;
   const float inv_temp = 1.0f / sqrtf((float)dk);
-  const float* Xb = X + (size_t)b * n * D;
+  const XT* Xb = X + (size_t)b * n * D;
   const bool tail = mask == nullptr;
   if (!tail) pooled_ld = D;
   int len = n;
@@ -82,7 +89,7 @@ __global__ void __launch_bounds__(kPoolThreads, 4) attention_pool_kernel(int n, 
 #pragma unroll
           for (int c = 0; c < 4; ++c) {
             const int j = j0 + 32 * c + lane;
-            x[r][c] = (i0 + r < n && j < D) ? Xb[(size_t)(i0 + r) * D + j] : 0.f;
+            x[r][c] = (i0 + r < n && j < D) ? xval(Xb[(size_t)(i0 + r) * D + j]) : 0.f;
           }
 #pragma unroll
         for (int hh = 0; hh < 4; ++hh) {
@@ -155,7 +162,7 @@ __global__ void __launch_bounds__(kPoolThreads, 4) attention_pool_kernel(int n, 
 #pragma unroll
         for (int c = 0; c < 4; ++c) {
           const int j = j0 + 32 * c + lane;
-          x[c] = j < D ? Xb[(size_t)i * D + j] : 0.f;
+          x[c] = j < D ? xval(Xb[(size_t)i * D + j]) : 0.f;
         }
 #pragma unroll
         for (int hh = 0; hh < 4; ++hh) {
@@ -204,7 +211,7 @@ __global__ void __launch_bounds__(kPoolThreads, 4) attention_pool_kernel(int n, 
   if (tail) {
     float* row = pooled + (size_t)b * pooled_ld;
     for (int j = tid; j < S; j += kPoolThreads) row[D + j] = sent[(size_t)b * S + j];
-    for (int j = tid; j < D; j += kPoolThreads) row[D + S + j] = Xb[j];
+    for (int j = tid; j < D; j += kPoolThreads) row[D + S + j] = xval(Xb[j]);
   }
 }
 
@@ -217,14 +224,47 @@ inline size_t pool_smem_bytes(int n, int D, int nh) {
 }
 
 // Both entry points launch the same kernel, and cudaFuncSetAttribute overwrites the limit rather than raising it, so the
-// limit is set once per device, to the cap, for both of them.
+// limit is set once per device and X type, to the cap, for both of them.
+template <typename XT>
 int32_t prepare_pool_launch(size_t smem) {
   static bool attr_set[kMaxDevices] = {false};
   const int dev = current_device();
   if (smem > 48 * 1024 && !attr_set[dev]) {
-    QAGNN_CHECK_CUDA(cudaFuncSetAttribute(attention_pool_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPoolSmemCap));
+    QAGNN_CHECK_CUDA(cudaFuncSetAttribute(attention_pool_kernel<XT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPoolSmemCap));
     attr_set[dev] = true;
   }
+  return QAGNN_OK;
+}
+
+template <typename XT>
+int32_t decoder_tail(int32_t B, int32_t n, int32_t D, int32_t n_head, int32_t S, const XT* X, const float* qs,
+                     const int64_t* node_type, const int64_t* adj_lengths, const float* sent_vecs, const float* wk,
+                     const float* bk, const float* wv, const float* bv, float* concat, float* attn, cudaStream_t st) {
+  if (B <= 0 || n <= 0 || D <= 0 || n_head <= 0 || D % n_head != 0 || S < 0) return QAGNN_ERR_INVALID_ARGUMENT;
+  if (n_head > 8) return QAGNN_ERR_UNSUPPORTED;
+  if (!X || !qs || !node_type || !adj_lengths || !sent_vecs || !wk || !bk || !wv || !bv || !concat || !attn)
+    return QAGNN_ERR_INVALID_ARGUMENT;
+  const size_t smem = pool_smem_bytes(n, D, n_head);
+  if (smem > kPoolSmemCap) return QAGNN_ERR_UNSUPPORTED;
+  QAGNN_RETURN_IF(prepare_pool_launch<XT>(smem));
+  attention_pool_kernel<XT><<<B, kPoolThreads, smem, st>>>(n, D, n_head, X, qs, nullptr, wk, bk, wv, bv, concat, attn, B,
+                                                           node_type, adj_lengths, sent_vecs, S, 2 * D + S);
+  QAGNN_CHECK_LAUNCH();
+  return QAGNN_OK;
+}
+
+template <typename XT>
+int32_t attention_pool(int32_t B, int32_t n, int32_t D, int32_t n_head, const XT* X, const float* qs, const uint8_t* mask,
+                       const float* wk, const float* bk, const float* wv, const float* bv, float* pooled, float* attn,
+                       cudaStream_t st) {
+  if (B <= 0 || n <= 0 || D <= 0 || n_head <= 0 || D % n_head != 0) return QAGNN_ERR_INVALID_ARGUMENT;
+  if (n_head > 8) return QAGNN_ERR_UNSUPPORTED;
+  if (!X || !qs || !mask || !wk || !bk || !wv || !bv || !pooled || !attn) return QAGNN_ERR_INVALID_ARGUMENT;
+  const size_t smem = pool_smem_bytes(n, D, n_head);
+  if (smem > kPoolSmemCap) return QAGNN_ERR_UNSUPPORTED;
+  QAGNN_RETURN_IF(prepare_pool_launch<XT>(smem));
+  attention_pool_kernel<XT><<<B, kPoolThreads, smem, st>>>(n, D, n_head, X, qs, mask, wk, bk, wv, bv, pooled, attn, B);
+  QAGNN_CHECK_LAUNCH();
   return QAGNN_OK;
 }
 
@@ -302,29 +342,33 @@ extern "C" int32_t qagnn_decoder_tail(int32_t B, int32_t n, int32_t D, int32_t n
                                       const int64_t* node_type, const int64_t* adj_lengths, const float* sent_vecs,
                                       const float* wk, const float* bk, const float* wv, const float* bv, float* concat,
                                       float* attn, void* stream) {
-  if (B <= 0 || n <= 0 || D <= 0 || n_head <= 0 || D % n_head != 0 || S < 0) return QAGNN_ERR_INVALID_ARGUMENT;
-  if (n_head > 8) return QAGNN_ERR_UNSUPPORTED;
-  if (!X || !qs || !node_type || !adj_lengths || !sent_vecs || !wk || !bk || !wv || !bv || !concat || !attn)
-    return QAGNN_ERR_INVALID_ARGUMENT;
-  const size_t smem = pool_smem_bytes(n, D, n_head);
-  if (smem > kPoolSmemCap) return QAGNN_ERR_UNSUPPORTED;
-  QAGNN_RETURN_IF(prepare_pool_launch(smem));
-  attention_pool_kernel<<<B, kPoolThreads, smem, (cudaStream_t)stream>>>(n, D, n_head, X, qs, nullptr, wk, bk, wv, bv, concat, attn, B,
-                                                                         node_type, adj_lengths, sent_vecs, S, 2 * D + S);
-  QAGNN_CHECK_LAUNCH();
-  return QAGNN_OK;
+  return decoder_tail(B, n, D, n_head, S, X, qs, node_type, adj_lengths, sent_vecs, wk, bk, wv, bv, concat, attn,
+                      (cudaStream_t)stream);
 }
 
 extern "C" int32_t qagnn_attention_pool(int32_t B, int32_t n, int32_t D, int32_t n_head, const float* X, const float* qs,
                                         const uint8_t* mask, const float* wk, const float* bk, const float* wv, const float* bv,
                                         float* pooled, float* attn, void* stream) {
-  if (B <= 0 || n <= 0 || D <= 0 || n_head <= 0 || D % n_head != 0) return QAGNN_ERR_INVALID_ARGUMENT;
-  if (n_head > 8) return QAGNN_ERR_UNSUPPORTED;
-  if (!X || !qs || !mask || !wk || !bk || !wv || !bv || !pooled || !attn) return QAGNN_ERR_INVALID_ARGUMENT;
-  const size_t smem = pool_smem_bytes(n, D, n_head);
-  if (smem > kPoolSmemCap) return QAGNN_ERR_UNSUPPORTED;
-  QAGNN_RETURN_IF(prepare_pool_launch(smem));
-  attention_pool_kernel<<<B, kPoolThreads, smem, (cudaStream_t)stream>>>(n, D, n_head, X, qs, mask, wk, bk, wv, bv, pooled, attn, B);
-  QAGNN_CHECK_LAUNCH();
-  return QAGNN_OK;
+  return attention_pool(B, n, D, n_head, X, qs, mask, wk, bk, wv, bv, pooled, attn, (cudaStream_t)stream);
+}
+
+extern "C" int32_t qagnn_decoder_tail_typed(int32_t x_dtype, int32_t B, int32_t n, int32_t D, int32_t n_head, int32_t S,
+                                            const void* X, const float* qs, const int64_t* node_type, const int64_t* adj_lengths,
+                                            const float* sent_vecs, const float* wk, const float* bk, const float* wv,
+                                            const float* bv, float* concat, float* attn, void* stream) {
+  if (x_dtype == QAGNN_DTYPE_F32)
+    return decoder_tail(B, n, D, n_head, S, (const float*)X, qs, node_type, adj_lengths, sent_vecs, wk, bk, wv, bv, concat,
+                        attn, (cudaStream_t)stream);
+  if (x_dtype != QAGNN_DTYPE_BF16) return QAGNN_ERR_INVALID_ARGUMENT;
+  return decoder_tail(B, n, D, n_head, S, (const __nv_bfloat16*)X, qs, node_type, adj_lengths, sent_vecs, wk, bk, wv, bv, concat,
+                      attn, (cudaStream_t)stream);
+}
+
+extern "C" int32_t qagnn_attention_pool_typed(int32_t x_dtype, int32_t B, int32_t n, int32_t D, int32_t n_head, const void* X,
+                                              const float* qs, const uint8_t* mask, const float* wk, const float* bk,
+                                              const float* wv, const float* bv, float* pooled, float* attn, void* stream) {
+  if (x_dtype == QAGNN_DTYPE_F32)
+    return attention_pool(B, n, D, n_head, (const float*)X, qs, mask, wk, bk, wv, bv, pooled, attn, (cudaStream_t)stream);
+  if (x_dtype != QAGNN_DTYPE_BF16) return QAGNN_ERR_INVALID_ARGUMENT;
+  return attention_pool(B, n, D, n_head, (const __nv_bfloat16*)X, qs, mask, wk, bk, wv, bv, pooled, attn, (cudaStream_t)stream);
 }

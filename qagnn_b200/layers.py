@@ -13,6 +13,10 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 
+# node-feature dtypes the fused pooling kernels read: fp32, and bf16 (the eval forward's output under bf16 autocast)
+_POOL_X_DTYPES = (torch.float32, torch.bfloat16)
+
+
 def gelu(x):
     """tanh-approximation GELU, the form the reference uses everywhere (utils/layers.py:10-14)."""
     return F.gelu(x, approximate="tanh")
@@ -88,7 +92,7 @@ class MultiheadAttPoolLayer(nn.Module):
         """Eval-mode decoder tail in ONE kernel (qagnn_decoder_tail): derives the pool mask from adj_lengths / node_type,
         pools, and returns (cat(pooled, q, k[:, 0]) [b, 2*d_k_original + d_q_original], attn) — modeling_qagnn.py:172-187.
         Returns None when the fused kernel cannot take the shape (caller falls back to mask + forward + cat)."""
-        if (self.training or not k.is_cuda or k.dtype != torch.float32 or not self._fused_may_take(k.size(1))
+        if (self.training or not k.is_cuda or k.dtype not in _POOL_X_DTYPES or not self._fused_may_take(k.size(1))
                 or (torch.is_grad_enabled() and (q.requires_grad or k.requires_grad))):
             return None
         from . import _lib
@@ -96,16 +100,17 @@ class MultiheadAttPoolLayer(nn.Module):
         b, l, D = k.shape
         S = q.size(1)
         qc = _lib.f32c(q, "q")
-        qs = self.w_qs(qc).detach().contiguous()
-        kc = _lib.f32c(k, "k")
+        qs = self.w_qs(qc).detach().float().contiguous()  # fp32 for the kernel, also under autocast
+        kc = k.detach().contiguous()  # fp32, or bf16 (the bf16 eval forward's output), widened exactly in the kernel
         concat = torch.empty(b, 2 * D + S, dtype=torch.float32, device=k.device)
         attn = torch.empty(self.n_head * b, l, dtype=torch.float32, device=k.device)
         with torch.cuda.device(k.device):
-            st = lib.qagnn_decoder_tail(b, l, D, self.n_head, S, _lib.ptr(kc), _lib.ptr(qs), _lib.ptr(_lib.i64c(node_type, "node_type")),
-                                        _lib.ptr(_lib.i64c(adj_lengths, "adj_lengths")), _lib.ptr(qc),
-                                        _lib.ptr(self.w_ks.weight.detach()), _lib.ptr(self.w_ks.bias.detach()),
-                                        _lib.ptr(self.w_vs.weight.detach()), _lib.ptr(self.w_vs.bias.detach()),
-                                        _lib.ptr(concat), _lib.ptr(attn), _lib.stream_ptr(k.device))
+            st = lib.qagnn_decoder_tail_typed(_lib.DTYPE_CODES[kc.dtype], b, l, D, self.n_head, S, _lib.ptr(kc), _lib.ptr(qs),
+                                              _lib.ptr(_lib.i64c(node_type, "node_type")),
+                                              _lib.ptr(_lib.i64c(adj_lengths, "adj_lengths")), _lib.ptr(qc),
+                                              _lib.ptr(self.w_ks.weight.detach()), _lib.ptr(self.w_ks.bias.detach()),
+                                              _lib.ptr(self.w_vs.weight.detach()), _lib.ptr(self.w_vs.bias.detach()),
+                                              _lib.ptr(concat), _lib.ptr(attn), _lib.stream_ptr(k.device))
         if st == -5:
             self._note_refused(l)
             return None
@@ -116,21 +121,22 @@ class MultiheadAttPoolLayer(nn.Module):
         b, l, _ = k.shape
         nh, dk, dv = self.n_head, self.d_k, self.d_v
         wants_grad = torch.is_grad_enabled() and (q.requires_grad or k.requires_grad)  # the fused kernel is outside autograd
-        if (k.is_cuda and not self.training and not wants_grad and mask is not None and k.dtype == torch.float32
+        if (k.is_cuda and not self.training and not wants_grad and mask is not None and k.dtype in _POOL_X_DTYPES
                 and self.w_ks.weight.shape[0] == k.shape[2] and self._fused_may_take(l)):
             # fused kernel (one read of k, no ks/vs GEMMs): qagnn_attention_pool
             from . import _lib
             lib = _lib.load()
-            qs = self.w_qs(q).contiguous()
-            kc = _lib.f32c(k, "k")
+            qs = self.w_qs(q).float().contiguous()  # fp32 for the kernel, also under autocast
+            kc = k.detach().contiguous()
             m8 = mask.to(torch.uint8).contiguous()
             pooled = torch.empty(b, nh * dv, dtype=torch.float32, device=k.device)
             attn = torch.empty(nh * b, l, dtype=torch.float32, device=k.device)
             with torch.cuda.device(k.device):
-                st = lib.qagnn_attention_pool(b, l, k.shape[2], nh, _lib.ptr(kc), _lib.ptr(qs.detach()), _lib.ptr(m8),
-                                              _lib.ptr(self.w_ks.weight.detach()), _lib.ptr(self.w_ks.bias.detach()),
-                                              _lib.ptr(self.w_vs.weight.detach()), _lib.ptr(self.w_vs.bias.detach()),
-                                              _lib.ptr(pooled), _lib.ptr(attn), _lib.stream_ptr(k.device))
+                st = lib.qagnn_attention_pool_typed(_lib.DTYPE_CODES[kc.dtype], b, l, k.shape[2], nh, _lib.ptr(kc),
+                                                    _lib.ptr(qs.detach()), _lib.ptr(m8),
+                                                    _lib.ptr(self.w_ks.weight.detach()), _lib.ptr(self.w_ks.bias.detach()),
+                                                    _lib.ptr(self.w_vs.weight.detach()), _lib.ptr(self.w_vs.bias.detach()),
+                                                    _lib.ptr(pooled), _lib.ptr(attn), _lib.stream_ptr(k.device))
             if st == -5:  # QAGNN_ERR_UNSUPPORTED (node tile does not fit in shared memory): the einsum path below
                 self._note_refused(l)
             else:
@@ -194,7 +200,9 @@ class CustomizedEmbedding(nn.Module):
         srcs = [self.emb.weight] + ([self.cpt_transform.weight, self.cpt_transform.bias] if hasattr(self, "cpt_transform") else [])
         key = tuple((t.data_ptr(), t._version, tuple(t.shape)) for t in srcs)
         if getattr(self, "_ptab_key", None) != key:
-            with torch.no_grad():
+            # fp32 whatever autocast the caller runs under: the head kernel reads the table as fp32, and the cache outlives
+            # the call that fills it
+            with torch.no_grad(), torch.autocast("cuda", enabled=False):
                 w = self.emb.weight
                 rows = [self._project(w[i:i + 65536]) for i in range(0, w.size(0), 65536)]  # chunks bound the GEMM workspace
                 self._ptab = torch.cat(rows).contiguous()

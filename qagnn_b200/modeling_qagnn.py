@@ -335,8 +335,11 @@ class GATConvE(nn.Module):
             return TR.gatconve_train(self, x, node_feature_extra, node_type, prep, tab, return_attention_weights)
         _warn_if_grad_wanted("GATConvE", x, node_feature_extra)
         lib = _lib.load()
-        xc = _lib.f32c(x, "x")
-        ex = _lib.f32c(node_feature_extra, "node_feature_extra")
+        # under bf16 autocast: bf16 in and out, single-pass bf16 GEMMs (include/qagnn_b200.h, qagnn_gatconve_forward_typed)
+        xc, dt = _lib.eval_dtype(x, "x")
+        ex, _ = _lib.eval_dtype(node_feature_extra, "node_feature_extra")
+        if ex.dtype != xc.dtype:  # the library takes both inputs in one dtype: bf16 here (dt is bf16 when they can differ)
+            xc, ex = xc.to(dt), ex.to(dt)
         dev = xc.device
         N, D = xc.shape
         if D != self.emb_dim or ex.shape != xc.shape:
@@ -349,14 +352,15 @@ class GATConvE(nn.Module):
         folded = self._folded.get(shape, self.edge_encoder, [self], None, dev)
         ws_bytes = lib.qagnn_forward_workspace_bytes(C.byref(shape))
         ws = self._ws.get(ws_bytes, dev)
-        out = torch.empty_like(xc)
+        out = torch.empty(N, D, dtype=dt, device=dev)
         alpha = torch.empty(N + prep.E, self.head_count, dtype=torch.float32, device=dev) if return_attention_weights else None
-        aggr = torch.empty_like(xc) if return_aggr else None
+        aggr = torch.empty(N, D, dtype=torch.float32, device=dev) if return_aggr else None
         with torch.cuda.device(dev):
-            st = lib.qagnn_gatconve_forward(C.byref(shape), 0, _lib.ptr(xc), _lib.ptr(ex), _lib.ptr(prep.buf),
-                                            _lib.ptr(folded), _lib.ptr(out), _lib.ptr(alpha), _lib.ptr(aggr),
-                                            _lib.ptr(ws), ws.numel(), _lib.stream_ptr(dev))
-        _lib.check(st, "qagnn_gatconve_forward")
+            st = lib.qagnn_gatconve_forward_typed(C.byref(shape), _lib.DTYPE_CODES[dt], _lib.DTYPE_CODES[xc.dtype], 0,
+                                                  _lib.ptr(xc), _lib.ptr(ex),
+                                                  _lib.ptr(prep.buf), _lib.ptr(folded), _lib.ptr(out), _lib.ptr(alpha),
+                                                  _lib.ptr(aggr), _lib.ptr(ws), ws.numel(), _lib.stream_ptr(dev))
+        _lib.check(st, "qagnn_gatconve_forward_typed")
         self._alpha = None
         res = out
         if return_attention_weights:
@@ -474,7 +478,8 @@ class QAGNN_Message_Passing(nn.Module):
         if self.use_cuda_graph and prep is None and not return_layers:
             return self._graphed_forward(H, A, node_type, node_score)
         lib = _lib.load()
-        Hc = _lib.f32c(H, "H")
+        # under bf16 autocast: bf16 in and out, single-pass bf16 GEMMs (include/qagnn_b200.h, qagnn_mp_forward_typed)
+        Hc, dt = _lib.eval_dtype(H, "H")
         if Hc.dim() != 3 or Hc.size(2) != self.hidden_size:
             raise ValueError("H must be [batch, n_node, hidden_size]")
         B, n, D = Hc.shape
@@ -492,13 +497,13 @@ class QAGNN_Message_Passing(nn.Module):
         shape = self._shape(B * n, prep.E, prep.n_per_graph)
         folded = self._folded.get(shape, self.edge_encoder, list(self.gnn_layers), self._mp_tensors(), dev)
         ws = self._ws.get(lib.qagnn_forward_workspace_bytes(C.byref(shape)), dev)
-        out = torch.empty_like(Hc)
+        out = torch.empty(B, n, D, dtype=dt, device=dev)
         layers = torch.empty(self.k, B * n, D, dtype=torch.float32, device=dev) if return_layers else None
         with torch.cuda.device(dev):
-            st = lib.qagnn_mp_forward(C.byref(shape), _lib.ptr(Hc), _lib.ptr(nt), _lib.ptr(sc), _lib.ptr(prep.buf),
-                                      _lib.ptr(folded), _lib.ptr(out), _lib.ptr(layers), _lib.ptr(ws), ws.numel(),
-                                      _lib.stream_ptr(dev))
-        _lib.check(st, "qagnn_mp_forward")
+            st = lib.qagnn_mp_forward_typed(C.byref(shape), _lib.DTYPE_CODES[dt], _lib.DTYPE_CODES[Hc.dtype], _lib.ptr(Hc),
+                                            _lib.ptr(nt), _lib.ptr(sc), _lib.ptr(prep.buf), _lib.ptr(folded), _lib.ptr(out),
+                                            _lib.ptr(layers), _lib.ptr(ws), ws.numel(), _lib.stream_ptr(dev))
+        _lib.check(st, "qagnn_mp_forward_typed")
         if return_layers:
             return out, layers
         return out
@@ -510,8 +515,9 @@ class QAGNN_Message_Passing(nn.Module):
         tensors = [H, A[0], A[1], node_type, node_score]
         if getattr(A, "graph_ptr_dev", None) is not None:
             tensors.append(A.graph_ptr_dev)
+        # the autocast dtype selects the kernels and the output dtype: an fp32 capture must not replay under bf16 autocast
         key = (tuple((t.data_ptr(), tuple(t.shape), t.dtype) for t in tensors),
-               _version_key(list(self.parameters()) + list(self.buffers())))
+               _version_key(list(self.parameters()) + list(self.buffers())), _lib.autocast_dtype())
         entry = self._graphs.get(key)
         if entry is None:
             from .pipeline import capture
@@ -577,7 +583,9 @@ class QAGNN(nn.Module):
             lib = _lib.load()
             B_ = concept_ids.size(0)
             table = self.concept_emb.projected_table()
-            ctx = self.activation(self.svec2nvec(sent_vecs)).contiguous()
+            # the head kernel reads fp32: under autocast ctx comes out in the autocast dtype (its rounding is kept, as the
+            # PyTorch head's torch.cat promotes it to fp32 too)
+            ctx = self.activation(self.svec2nvec(sent_vecs)).float().contiguous()
             cid = _lib.i64c(concept_ids, "concept_ids")
             sc = _lib.f32c(node_scores.reshape(B_, n), "node_scores")
             al = _lib.i64c(adj_lengths, "adj_lengths")

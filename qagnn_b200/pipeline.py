@@ -107,14 +107,22 @@ class DecoderStep:
     FIELDS = ("H", "edge_index", "edge_type", "node_type", "node_score", "sent_vecs", "adj_lengths")
     PACKED_FIELDS = FIELDS + ("graph_ptr",)  # + first edge of every sub-graph, int64 [B + 1] (packed batches)
 
-    def __init__(self, gnn, pooler, fc, inputs, world_size=1, group=None, use_cuda_graph=True, max_edges=-1):
-        """`inputs` may carry "graph_ptr" (device int64 [B + 1]) with `max_edges` = an upper bound of the edges of one sub-graph
+    def __init__(self, gnn, pooler, fc, inputs, world_size=1, group=None, use_cuda_graph=True, max_edges=-1,
+                 autocast_dtype=None):
+        """`autocast_dtype` (None or torch.bfloat16) runs capture and calls under torch.autocast(cache_enabled=False): the
+        message passing then runs its bf16 forward (single-pass bf16 GEMMs, `gnn_out` bf16) and the pooling reads that output
+        directly.
+
+        `inputs` may carry "graph_ptr" (device int64 [B + 1]) with `max_edges` = an upper bound of the edges of one sub-graph
         for every batch that will be written into these buffers: graph prep is then ONE launch (qagnn_graph_prep_packed).
         edge_index / edge_type may then be an edge capacity K wider than any batch (qagnn_b200.data.PackedAdj): the real
         edge count is read from graph_ptr on the device, so one capture serves every batch of a split that fits K and
         `max_edges`.  A capture raises ValueError if the packed prep refuses the shape, since the general prep would freeze
         the edge count of the batch it was captured on."""
+        if autocast_dtype not in (None, torch.bfloat16):
+            raise ValueError("autocast_dtype must be None or torch.bfloat16")
         self.gnn, self.pooler, self.fc = gnn, pooler, fc
+        self.autocast_dtype = autocast_dtype
         self.inp = {k: inputs[k] for k in self.FIELDS}
         self.adj = (self.inp["edge_index"], self.inp["edge_type"])
         if "graph_ptr" in inputs and max_edges >= 0:
@@ -134,8 +142,17 @@ class DecoderStep:
         if use_cuda_graph:
             self._capture()
 
+    def _autocast(self):
+        if self.autocast_dtype is None:
+            return contextlib.nullcontext()
+        return torch.autocast("cuda", dtype=self.autocast_dtype, cache_enabled=False)
+
     @torch.no_grad()
     def _eager(self):
+        with self._autocast():
+            return self._eager_body()
+
+    def _eager_body(self):
         d = self.inp
         out = self.gnn(d["H"], self.adj, d["node_type"], d["node_score"])
         fused = self.pooler.pool_concat(d["sent_vecs"], out, d["node_type"], d["adj_lengths"])  # :172-187 in one kernel

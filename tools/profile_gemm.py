@@ -12,6 +12,12 @@ launch order.  The step is profiled twice: with the fused node MLP (`mlp_tc_kern
 QAGNN_MLP_FUSED=0 (mlp.0 + mlp.3), so the fused kernel is timed beside the pair at the same shape; the "mlp.0+mlp.3" row
 sums the pair's medians and bounds (the pair also writes and reads back the hidden planes).  One JSON line with everything
 follows the table.
+
+    python tools/profile_gemm.py --out DIR --bf16
+
+also profiles the same step under bf16 autocast (DecoderStep(autocast_dtype=torch.bfloat16): the single-pass
+`gemm_bf16_kernel` / `mlp_bf16_kernel`) and prints each call's median kernel time in both forms side by side; the JSON line
+then carries them under "bf16".
 """
 import argparse
 import json
@@ -89,10 +95,42 @@ def cublas_ceiling_us(M, N, K, reps=20):
     return e0.elapsed_time(e1) * 1e3 / reps
 
 
+def profile_gemms(step, steps, trace, kind="tc"):
+    """[(start, (ACT, BN or None for the fused MLP, CTAS), µs)] of the GEMM launches of `steps` eager steps, in launch
+    order, and the launches per step.  kind "tc": the split-bf16 kernels; "bf16": the single-pass ones."""
+    from torch.profiler import ProfilerActivity, profile
+    pat = re.compile(r"gemm_%s_kernel<(\d+), *(\d+), *(\d+)>" % kind)
+    pat_mlp = re.compile(r"mlp_%s_kernel<(\d+), *(\d+)>" % kind)
+    for _ in range(3):
+        step.run()
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
+        for _ in range(steps):
+            step.run()
+        torch.cuda.synchronize()
+    prof.export_chrome_trace(trace)
+    kern = []
+    for e in prof.events():
+        if e.device_type != torch.autograd.DeviceType.CUDA:
+            continue
+        m, mm = pat.search(e.name), pat_mlp.search(e.name)
+        if m:
+            kern.append((e.time_range.start, tuple(int(x) for x in m.groups()), e.time_range.elapsed_us()))
+        elif mm:
+            act, ctas = (int(x) for x in mm.groups())
+            kern.append((e.time_range.start, (act, None, ctas), e.time_range.elapsed_us()))
+    kern.sort()
+    n = len(kern) // steps
+    if n == 0 or len(kern) % steps:
+        raise SystemExit(f"profile_gemm.py: {len(kern)} GEMM launches over {steps} steps")
+    return kern, n
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--out", required=True, help="directory for the trace")
     ap.add_argument("--steps", type=int, default=5, help="profiled eager steps")
+    ap.add_argument("--bf16", action="store_true", help="also profile the step under bf16 autocast (single-pass GEMMs)")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("profile_gemm.py: needs a CUDA device")
@@ -115,35 +153,10 @@ def main():
     d = {k: inp[k].to(dev) for k in DecoderStep.PACKED_FIELDS}
     max_edges = int((inp["graph_ptr"][1:] - inp["graph_ptr"][:-1]).max())
     step = DecoderStep(mod, pooler, fc, d, 1, None, use_cuda_graph=False, max_edges=max_edges)
-    from torch.profiler import ProfilerActivity, profile
-    pat = re.compile(r"gemm_tc_kernel<(\d+), *(\d+), *(\d+)>")
-    pat_mlp = re.compile(r"mlp_tc_kernel<(\d+), *(\d+)>")
     times, templ, per_step = {}, {}, {}
     for fused in ("1", "0"):
         os.environ["QAGNN_MLP_FUSED"] = fused
-        for _ in range(3):
-            step.run()
-        torch.cuda.synchronize()
-        with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
-            for _ in range(args.steps):
-                step.run()
-            torch.cuda.synchronize()
-        trace = os.path.join(args.out, f"gemm_trace_fused{fused}.json")
-        prof.export_chrome_trace(trace)
-        kern = []
-        for e in prof.events():
-            if e.device_type != torch.autograd.DeviceType.CUDA:
-                continue
-            m, mm = pat.search(e.name), pat_mlp.search(e.name)
-            if m:
-                kern.append((e.time_range.start, tuple(int(x) for x in m.groups()), e.time_range.elapsed_us()))
-            elif mm:
-                act, ctas = (int(x) for x in mm.groups())
-                kern.append((e.time_range.start, (act, None, ctas), e.time_range.elapsed_us()))
-        kern.sort()
-        n = len(kern) // args.steps
-        if n == 0 or len(kern) % args.steps:
-            raise SystemExit(f"profile_gemm.py: {len(kern)} GEMM launches over {args.steps} steps")
+        kern, n = profile_gemms(step, args.steps, os.path.join(args.out, f"gemm_trace_fused{fused}.json"))
         per_step[fused] = n
         for s in range(args.steps):
             one = kern[s * n:(s + 1) * n]
@@ -188,8 +201,31 @@ def main():
     total = sum(sum(times[k]) for k in ORDER if k in times and k not in ("mlp.0", "mlp.3", "mlp.0+mlp.3")) / args.steps
     print(f"all GEMM launches of the default (fused) step: {total:.1f} µs per step ({per_step['1']} launches; "
           f"{per_step['0']} with QAGNN_MLP_FUSED=0)")
-    print(json.dumps({"card": info, "gemm_us_per_step": total, "launches_per_step": per_step, "calls": rows,
-                      "trace_dir": args.out}))
+    res = {"card": info, "gemm_us_per_step": total, "launches_per_step": per_step, "calls": rows, "trace_dir": args.out}
+    if args.bf16:
+        step16 = DecoderStep(mod, pooler, fc, d, 1, None, use_cuda_graph=False, max_edges=max_edges,
+                             autocast_dtype=torch.bfloat16)
+        kern, n = profile_gemms(step16, args.steps, os.path.join(args.out, "gemm_trace_bf16.json"), "bf16")
+        t16 = {}
+        for s_ in range(args.steps):
+            one = kern[s_ * n:(s_ + 1) * n]
+            for lab, us in label_calls([(t, us) for _, t, us in one]):
+                t16.setdefault(lab, []).append(us)
+        print(f"\nunder bf16 autocast (gemm_bf16_kernel / mlp_bf16_kernel), same card, {n} launches per step")
+        print(f"{'call':<11} {'fp32 µs':>10} {'bf16 µs':>10} {'fp32/bf16':>10}")
+        cmp_rows = []
+        for lab in ORDER:
+            if lab not in t16 or lab not in times:
+                continue
+            m32 = sorted(times[lab])[len(times[lab]) // 2]
+            m16 = sorted(t16[lab])[len(t16[lab]) // 2]
+            cmp_rows.append(dict(call=lab, fp32_median_us=m32, bf16_median_us=m16, ratio=m32 / m16,
+                                 calls_per_step=len(t16[lab]) // args.steps))
+            print(f"{lab:<11} {m32:>10.1f} {m16:>10.1f} {m32 / m16:>10.2f}")
+        total16 = sum(sum(v) for v in t16.values()) / args.steps
+        print(f"all GEMM launches of the bf16 step: {total16:.1f} µs per step (fp32: {total:.1f})")
+        res["bf16"] = {"gemm_us_per_step": total16, "launches_per_step": n, "calls": cmp_rows}
+    print(json.dumps(res))
 
 
 if __name__ == "__main__":
