@@ -252,6 +252,23 @@ int32_t qagnn_mp_core_backward_typed(const qagnn_shape *shape, int32_t dtype, co
                                      const void *qkm, const void *ke, const void *me, const float *alpha_scaled,
                                      const void *d_aggr, void *d_qkm, void *d_ke, void *d_me, float *scratch, void *stream);
 
+/* qagnn_mp_core_backward_typed with d_ke / d_me summed without atomics, so that every output is the same, bit for bit, on every
+ * run and for every grid size: what training under torch.use_deterministic_algorithms(True) calls.  d_qkm is the same as
+ * qagnn_mp_core_backward_typed's, bit for bit.  combo_count int64 [C] and combo_order int32 [E+N] are qagnn_combo_sort's
+ * outputs for this prep.  Summation order of row c of d_ke / d_me (fp32 sums; a 16-bit call rounds each row once at the end):
+ * the positions [o, o + n) of combo c in combo_order (o = combo_count[0] + ... + combo_count[c-1], n = combo_count[c]) are
+ * cut into runs of 64 positions [64r, 64r + 64); each run's part is summed in combo order; a combo inside one run is that
+ * sum, and one spanning runs r0 < r1 is (P_0 + P_1) + ... + P_7 with P_k = the parts of runs r0 + k, r0 + k + 8, ... added
+ * in ascending order.  A combo without positions gets exact zeros.  E' = rowptr_src[N] is read on the device, so a prep at
+ * an edge capacity works without a host synchronisation, and the call can be captured into a CUDA graph.  `scratch` holds
+ * qagnn_mp_core_backward_det_scratch_bytes(shape, dtype) bytes (0 for an invalid shape or dtype), else
+ * QAGNN_ERR_WORKSPACE. */
+size_t qagnn_mp_core_backward_det_scratch_bytes(const qagnn_shape *shape, int32_t dtype);
+int32_t qagnn_mp_core_backward_det(const qagnn_shape *shape, int32_t dtype, const void *prep, const int32_t *combo_order,
+                                   const int64_t *combo_count, const void *qkm, const void *ke, const void *me,
+                                   const float *alpha_scaled, const void *d_aggr, void *d_qkm, void *d_ke, void *d_me,
+                                   float *scratch, size_t scratch_bytes, void *stream);
+
 /* What the training path needs per batch besides the prep, without a host synchronisation: a stable counting sort of the
  * by-source positions [0, E') by qagnn_prep_layout.csr_src_combo, with E' = rowptr_src[N] read on the device (shape->N and
  * shape->E are those the prep was built with; E may be an edge capacity, see qagnn_graph_prep_packed).

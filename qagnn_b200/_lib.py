@@ -70,6 +70,9 @@ EXPORTS = {
     "qagnn_mp_core_scratch_bytes": (C.c_size_t, [C.POINTER(Shape), C.c_int32]),
     "qagnn_mp_core_forward_typed": (C.c_int32, [C.POINTER(Shape), C.c_int32, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "qagnn_mp_core_backward_typed": (C.c_int32, [C.POINTER(Shape), C.c_int32, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
+    "qagnn_mp_core_backward_det_scratch_bytes": (C.c_size_t, [C.POINTER(Shape), C.c_int32]),
+    "qagnn_mp_core_backward_det": (C.c_int32, [C.POINTER(Shape), C.c_int32, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P,
+                                               C.c_size_t, _P]),
     "qagnn_combo_sort_bytes": (C.c_size_t, [C.POINTER(Shape)]),
     "qagnn_combo_sort": (C.c_int32, [C.POINTER(Shape), _P, _P, _P, _P, C.c_size_t, _P]),
     "qagnn_linear_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int32, C.c_int32, C.c_int32]),

@@ -827,6 +827,28 @@ extern "C" int32_t qagnn_mp_core_backward_typed(const qagnn_shape* shape, int32_
                                                d_aggr, scratch, d_qkm, d_ke, d_me, (cudaStream_t)stream);
 }
 
+extern "C" size_t qagnn_mp_core_backward_det_scratch_bytes(const qagnn_shape* shape, int32_t dtype) {
+  if (check_shape_fwd(shape) != QAGNN_OK || dtype < QAGNN_DTYPE_F32 || dtype > QAGNN_DTYPE_BF16) return 0;
+  return mp_core_det_scratch_bytes(*shape, dtype);
+}
+
+extern "C" int32_t qagnn_mp_core_backward_det(const qagnn_shape* shape, int32_t dtype, const void* prep,
+                                              const int32_t* combo_order, const int64_t* combo_count, const void* qkm,
+                                              const void* ke, const void* me, const float* alpha_scaled, const void* d_aggr,
+                                              void* d_qkm, void* d_ke, void* d_me, float* scratch, size_t scratch_bytes,
+                                              void* stream) {
+  QAGNN_RETURN_IF(check_shape_fwd(shape));
+  if (dtype < QAGNN_DTYPE_F32 || dtype > QAGNN_DTYPE_BF16) return QAGNN_ERR_INVALID_ARGUMENT;
+  if (!prep || !combo_order || !combo_count || !qkm || !ke || !me || !alpha_scaled || !d_aggr || !d_qkm || !d_ke || !d_me ||
+      !scratch)
+    return QAGNN_ERR_INVALID_ARGUMENT;
+  if (scratch_bytes < mp_core_det_scratch_bytes(*shape, dtype)) return QAGNN_ERR_WORKSPACE;
+  qagnn_prep_layout pl;
+  QAGNN_RETURN_IF(qagnn_graph_prep_layout(shape->N, shape->E, &pl));
+  return launch_message_passing_backward_det(*shape, (const int32_t*)prep, pl, dtype, combo_order, combo_count, qkm, ke, me,
+                                             alpha_scaled, d_aggr, scratch, d_qkm, d_ke, d_me, (cudaStream_t)stream);
+}
+
 extern "C" size_t qagnn_linear_workspace_bytes(int64_t M, int32_t N, int32_t K1, int32_t K2) {
   if (M <= 0 || N <= 0 || K1 <= 0 || K2 < 0) return 0;
   const size_t K = (size_t)K1 + K2;

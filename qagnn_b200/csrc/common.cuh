@@ -206,6 +206,14 @@ int32_t launch_message_passing_backward_typed(const qagnn_shape& s, const int32_
 size_t mp_core_ds_floats(const qagnn_shape& s);
 // scratch bytes of qagnn_mp_core_forward_typed / _backward_typed: ds, plus the fp32 d_ke / d_me accumulators of a 16-bit call
 size_t mp_core_scratch_bytes(const qagnn_shape& s, int32_t dtype);
+// The backward with the edge-table gradients summed in an order fixed by the combo order (no atomics): the scratch of
+// launch_message_passing_backward_typed, then the combo offsets and two [2D]-float slots per run of the table kernel
+size_t mp_core_det_scratch_bytes(const qagnn_shape& s, int32_t dtype);
+int32_t launch_message_passing_backward_det(const qagnn_shape& s, const int32_t* prep_base, const qagnn_prep_layout& pl,
+                                            int32_t dtype, const int32_t* combo_order, const int64_t* combo_count,
+                                            const void* qkm, const void* ke, const void* me, const float* alpha_s,
+                                            const void* d_aggr, float* scratch, void* d_qkm, void* d_ke, void* d_me,
+                                            cudaStream_t st);
 
 // Exclusive scan of one int per thread over a 1024-thread block; *total = the block's sum.  Every thread must call it.
 __device__ __forceinline__ int block_exclusive_scan_1024(int v, int* total) {

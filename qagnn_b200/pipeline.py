@@ -239,7 +239,12 @@ class TrainStep:
     Out-of-range indices in a later batch raise IndexError at a later call, as with DecoderStep, without blocking the host;
     that batch's results were computed from clamped indices.  The graphs hold the addresses of the parameters and buffers:
     in-place optimiser steps and load_state_dict keep them, `.to()` / `.cuda()` / `.half()` do not, and a call after one
-    raises RuntimeError (build a new TrainStep).  `use_cuda_graph=False` runs the same code eagerly."""
+    raises RuntimeError (build a new TrainStep).  `use_cuda_graph=False` runs the same code eagerly.
+
+    Under torch.use_deterministic_algorithms(True) at construction, the backward graph holds the message-passing core's
+    deterministic backward (edge-table gradients summed in a fixed order), so two replays of one batch from one CUDA RNG state
+    give the same gradients bit for bit.  `deterministic` records that mode; a graph call after the flag changed raises
+    RuntimeError (build a new TrainStep)."""
 
     def __init__(self, decoder, sent_vecs, concept_ids, node_type_ids, node_scores, adj_lengths, packed_adj, *, max_edges,
                  edge_capacity=None, autocast_dtype=None, use_cuda_graph=True):
@@ -252,6 +257,7 @@ class TrainStep:
         if not decoder.training:
             raise ValueError("TrainStep captures the training forward: call decoder.train() first")
         self.decoder, self.autocast_dtype = decoder, autocast_dtype
+        self.deterministic = torch.are_deterministic_algorithms_enabled()
         dev = node_type_ids.device
         B, n = node_type_ids.shape
         K = int(edge_capacity) if edge_capacity is not None else packed_adj.edge_index.size(1)
@@ -361,6 +367,9 @@ class TrainStep:
             if self._addresses() != self._ptrs:
                 raise RuntimeError("TrainStep: the decoder's parameters or buffers moved since capture (.to() / .cuda() / "
                                    ".half()?); the graphs would read the old addresses. Build a new TrainStep.")
+            if torch.are_deterministic_algorithms_enabled() != self.deterministic:
+                raise RuntimeError(f"TrainStep was captured with torch.use_deterministic_algorithms({self.deterministic}) and "
+                                   "its backward graph holds that mode's kernels; the flag changed since. Build a new TrainStep.")
             if self._status is not None:
                 self._status.check("TrainStep")
         self._copy_batch(sent_vecs, concept_ids, node_type_ids, node_scores, adj_lengths, packed_adj)

@@ -93,7 +93,10 @@ class _MPCore(torch.autograd.Function):
     Under torch.autocast (qagnn.py:91 runs the forward in fp16 autocast when --fp16 is set) the dense layers around this
     function hand it qkm / ke / me in the autocast dtype: the kernels read and write that dtype directly (no cast to fp32 and
     back around them) and compute in fp32 inside, like the reference's scatter ops do.  aggr and the three gradients come back
-    in that dtype, rounded once from the fp32 results; alpha is fp32.  fp32 operands run the fp32 entry points."""
+    in that dtype, rounded once from the fp32 results; alpha is fp32.  fp32 operands run the fp32 entry points.
+
+    Under torch.use_deterministic_algorithms(True) the backward runs qagnn_mp_core_backward_det: d_ke / d_me are summed in an
+    order fixed by the combo order instead of with float atomics, so every gradient is the same, bit for bit, on every run."""
 
     @staticmethod
     @torch.amp.custom_fwd(device_type="cuda")
@@ -136,9 +139,18 @@ class _MPCore(torch.autograd.Function):
         g = _operand(d_aggr, dt, "d_aggr")
         d_qkm = torch.empty_like(qkm)
         d_ke, d_me = torch.empty_like(ke), torch.empty_like(me)
-        order = ctx.prep.combo_sort()[1]  # device-side E': valid under an edge capacity without a host read
+        count, order = ctx.prep.combo_sort()  # device-side E': valid under an edge capacity without a host read
         with torch.cuda.device(dev):
-            if dt == torch.float32:
+            if torch.are_deterministic_algorithms_enabled():
+                # d_ke / d_me summed in an order fixed by the combo order: the same bits on every run
+                code = _lib.DTYPE_CODES[dt]
+                nbytes = lib.qagnn_mp_core_backward_det_scratch_bytes(C.byref(shape), code)
+                scratch = torch.empty(nbytes // 4, dtype=torch.float32, device=dev)
+                st = lib.qagnn_mp_core_backward_det(C.byref(shape), code, _lib.ptr(ctx.prep.buf), _lib.ptr(order), _lib.ptr(count),
+                                                    _lib.ptr(qkm), _lib.ptr(ke), _lib.ptr(me), _lib.ptr(alpha_s), _lib.ptr(g),
+                                                    _lib.ptr(d_qkm), _lib.ptr(d_ke), _lib.ptr(d_me), _lib.ptr(scratch), nbytes,
+                                                    _lib.stream_ptr(dev))
+            elif dt == torch.float32:
                 scratch = torch.empty(N + E, H, dtype=torch.float32, device=dev)
                 st = lib.qagnn_mp_core_backward(C.byref(shape), _lib.ptr(ctx.prep.buf), _lib.ptr(order), _lib.ptr(qkm), _lib.ptr(ke),
                                                 _lib.ptr(me), _lib.ptr(alpha_s), _lib.ptr(g), _lib.ptr(d_qkm), _lib.ptr(d_ke),
