@@ -45,7 +45,7 @@
 extern "C" {
 #endif
 
-#define QAGNN_ABI_VERSION 3 /* 3: + training core, packed graph prep, decoder head / tail (round 2) */
+#define QAGNN_ABI_VERSION 3 /* 3: + training core, packed graph prep, decoder head / tail (round 2); ragged eval entry points */
 
 enum {
   QAGNN_OK = 0,
@@ -161,6 +161,18 @@ int32_t qagnn_graph_prep_packed(const int64_t *edge_index, const int64_t *edge_t
                                 const int64_t *graph_ptr, int32_t max_edges_per_graph, const qagnn_shape *shape, void *prep,
                                 size_t prep_bytes, int32_t validate, void *stream);
 
+/* The packed prep for a RAGGED batch (eval): sub-graph g < n_graphs owns the rows [node_ptr[g], node_ptr[g+1]) of an N-row batch
+ * (shape->N = the node capacity; node_ptr int64 [n_graphs + 1] on the DEVICE, node_ptr[0] = 0) instead of [g*n, (g+1)*n), and its
+ * edges the columns [graph_ptr[g], graph_ptr[g+1]) as above.  shape->n_per_graph = n bounds the rows of one sub-graph (it sizes
+ * the CTA's shared memory; N need not be a multiple of it).  The tail rows [node_ptr[n_graphs], N) belong to no sub-graph and get
+ * their self loops only; the tiled kernel walks them in segments of n rows.  An edge with an endpoint outside its sub-graph's
+ * rows sets bit 8; a node_ptr that is not monotone, has a sub-graph of more than n rows, does not start at 0, ends past N, or
+ * gives a sub-graph with edges no rows sets bit 32 (that sub-graph is then left untouched).  With validate either is
+ * QAGNN_ERR_INDEX_RANGE.  Edge capacity, the status word and QAGNN_ERR_UNSUPPORTED are as for qagnn_graph_prep_packed. */
+int32_t qagnn_graph_prep_ragged(const int64_t *edge_index, const int64_t *edge_type, const int64_t *node_type,
+                                const int64_t *graph_ptr, const int64_t *node_ptr, int32_t n_graphs, int32_t max_edges_per_graph,
+                                const qagnn_shape *shape, void *prep, size_t prep_bytes, int32_t validate, void *stream);
+
 /* ---- weight folding (once per set of weights) --------------------------------------------- */
 
 size_t qagnn_fold_bytes(const qagnn_shape *shape);
@@ -218,6 +230,20 @@ int32_t qagnn_gatconve_forward_typed(const qagnn_shape *shape, int32_t dtype, in
 int32_t qagnn_mp_forward_typed(const qagnn_shape *shape, int32_t dtype, int32_t in_dtype, const void *H_in,
                                const int64_t *node_type, const float *node_score, const void *prep, const void *folded,
                                void *out, float *x_layers_out, void *workspace, size_t workspace_bytes, void *stream);
+
+/* qagnn_gatconve_forward_typed / qagnn_mp_forward_typed on a ragged batch built by qagnn_graph_prep_ragged with the same
+ * n_graphs and node_ptr: every node array has shape->N rows (the node capacity), tail rows included, and the tiled message
+ * passing takes each sub-graph's rows from node_ptr (the column-sliced and CSR kernels take any layout).  Every row of the
+ * output of a sub-graph is what the padded layout computes for that row, within the summation-order bounds of the GEMMs'
+ * row tiling; tail rows are computed like isolated nodes. */
+int32_t qagnn_gatconve_forward_ragged(const qagnn_shape *shape, int32_t dtype, int32_t in_dtype, int32_t n_graphs,
+                                      const int64_t *node_ptr, int32_t layer, const void *x, const void *extra, const void *prep,
+                                      const void *folded, void *out, float *alpha_out, float *aggr_out, void *workspace,
+                                      size_t workspace_bytes, void *stream);
+int32_t qagnn_mp_forward_ragged(const qagnn_shape *shape, int32_t dtype, int32_t in_dtype, int32_t n_graphs,
+                                const int64_t *node_ptr, const void *H_in, const int64_t *node_type, const float *node_score,
+                                const void *prep, const void *folded, void *out, float *x_layers_out, void *workspace,
+                                size_t workspace_bytes, void *stream);
 
 /* ---- training (SURVEY.md §8f #3) --------------------------------------------------------------- */
 
@@ -328,6 +354,22 @@ int32_t qagnn_decoder_tail_typed(int32_t x_dtype, int32_t B, int32_t n, int32_t 
 int32_t qagnn_decoder_head(int32_t B, int32_t n, int32_t D, const int64_t *concept_ids, int64_t n_concept, const float *table,
                            const float *ctx, const float *node_scores, const int64_t *adj_lengths, float *H_out,
                            float *scores_out, void *stream);
+
+/* The decoder head and tail on a ragged batch of B graphs over N_rows packed rows, graph b's rows from node_ptr[b] (device int64
+ * [B + 1], the exclusive cumsum of adj_lengths).  The head reads the padded [B, n] concept_ids / node_scores / node_type as above
+ * and writes positions i < adj_lengths[b] as rows node_ptr[b] + i of H_out [N_rows, D], scores_out [N_rows] and type_out int64
+ * [N_rows], with the values qagnn_decoder_head writes at [b, i]; the tail rows [node_ptr[B], N_rows) get zeros, score 0 and
+ * type 2.  The tail pools graph b over its own rows of X [N_rows, D] (x_dtype as in qagnn_decoder_tail_typed), with node_type
+ * the packed [N_rows] type_out of the head, and writes attn [n_head*B, n] in the padded layout, exact zeros at positions
+ * >= adj_lengths[b]. */
+int32_t qagnn_decoder_head_ragged(int32_t B, int32_t n, int32_t D, int64_t N_rows, const int64_t *concept_ids, int64_t n_concept,
+                                  const float *table, const float *ctx, const float *node_scores, const int64_t *adj_lengths,
+                                  const int64_t *node_type, const int64_t *node_ptr, float *H_out, float *scores_out,
+                                  int64_t *type_out, void *stream);
+int32_t qagnn_decoder_tail_ragged(int32_t x_dtype, int32_t B, int32_t n, int32_t D, int32_t n_head, int32_t S, int64_t N_rows,
+                                  const void *X, const int64_t *node_ptr, const float *qs, const int64_t *node_type,
+                                  const int64_t *adj_lengths, const float *sent_vecs, const float *wk, const float *bk,
+                                  const float *wv, const float *bv, float *concat, float *attn, void *stream);
 
 /* Launch counters since load (kernels this library enqueued); for bench.py's gpu_launches. */
 int64_t qagnn_launch_count(void);

@@ -53,6 +53,8 @@ EXPORTS = {
     "qagnn_graph_prep_bytes": (C.c_size_t, [C.c_int64, C.c_int64]),
     "qagnn_graph_prep": (C.c_int32, [_P, _P, _P, C.POINTER(Shape), _P, C.c_size_t, C.c_int32, _P]),
     "qagnn_graph_prep_packed": (C.c_int32, [_P, _P, _P, _P, C.c_int32, C.POINTER(Shape), _P, C.c_size_t, C.c_int32, _P]),
+    "qagnn_graph_prep_ragged": (C.c_int32, [_P, _P, _P, _P, _P, C.c_int32, C.c_int32, C.POINTER(Shape), _P, C.c_size_t,
+                                            C.c_int32, _P]),
     "qagnn_fold_bytes": (C.c_size_t, [C.POINTER(Shape)]),
     "qagnn_fold_weights": (C.c_int32, [C.POINTER(Shape), C.POINTER(EdgeEncoderParams), C.POINTER(LayerParams),
                                        C.POINTER(MPParams), _P, C.c_size_t, _P]),
@@ -65,6 +67,10 @@ EXPORTS = {
     "qagnn_mp_forward": (C.c_int32, [C.POINTER(Shape), _P, _P, _P, _P, _P, _P, _P, _P, C.c_size_t, _P]),
     "qagnn_mp_forward_typed": (C.c_int32, [C.POINTER(Shape), C.c_int32, C.c_int32, _P, _P, _P, _P, _P, _P, _P, _P, C.c_size_t,
                                            _P]),
+    "qagnn_gatconve_forward_ragged": (C.c_int32, [C.POINTER(Shape), C.c_int32, C.c_int32, C.c_int32, _P, C.c_int32, _P, _P, _P,
+                                                  _P, _P, _P, _P, _P, C.c_size_t, _P]),
+    "qagnn_mp_forward_ragged": (C.c_int32, [C.POINTER(Shape), C.c_int32, C.c_int32, C.c_int32, _P, _P, _P, _P, _P, _P, _P, _P, _P,
+                                            C.c_size_t, _P]),
     "qagnn_mp_core_forward": (C.c_int32, [C.POINTER(Shape), _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "qagnn_mp_core_backward": (C.c_int32, [C.POINTER(Shape), _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "qagnn_mp_core_scratch_bytes": (C.c_size_t, [C.POINTER(Shape), C.c_int32]),
@@ -88,6 +94,10 @@ EXPORTS = {
     "qagnn_decoder_tail_typed": (C.c_int32, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P, _P, _P, _P,
                                              _P, _P, _P, _P, _P, _P, _P, _P]),
     "qagnn_decoder_head": (C.c_int32, [C.c_int32, C.c_int32, C.c_int32, _P, C.c_int64, _P, _P, _P, _P, _P, _P, _P]),
+    "qagnn_decoder_head_ragged": (C.c_int32, [C.c_int32, C.c_int32, C.c_int32, C.c_int64, _P, C.c_int64, _P, _P, _P, _P, _P, _P,
+                                              _P, _P, _P, _P]),
+    "qagnn_decoder_tail_ragged": (C.c_int32, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int64, _P, _P,
+                                              _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "qagnn_launch_count": (C.c_int64, []),
     "qagnn_profile_enable": (C.c_int32, [C.c_int32]),
     "qagnn_profile_read": (C.c_int32, [C.POINTER(C.c_double), C.POINTER(C.c_int64)]),

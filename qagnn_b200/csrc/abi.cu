@@ -251,10 +251,10 @@ int32_t check_shape_fwd(const qagnn_shape* s) {
 // Path selection: the shared-memory-tiled kernel when the batch is made of equal small sub-graphs
 // (shape.n_per_graph > 0 and the tiles fit), else the general CSR kernels.  QAGNN_MP_PATH=csr forces
 // the general path (A/B measurements).
-bool use_headtile(const qagnn_shape& s) {
+bool use_headtile(const qagnn_shape& s, const Ragged& rg = Ragged{}) {
   const char* e = getenv("QAGNN_MP_PATH");  // read at every call: tests cover every path in one process
   const bool forced = e && (strcmp(e, "csr") == 0 || strcmp(e, "basic") == 0);
-  return !forced && headtile_supported(s);
+  return !forced && headtile_supported(s, rg);
 }
 // Without per-graph tiles: the column-sliced kernels (edge tables in shared memory) when the head width allows, else the
 // basic CSR kernels; QAGNN_MP_PATH=basic forces the latter.
@@ -267,7 +267,7 @@ bool use_slice(const qagnn_shape& s) {
 int32_t layer_forward(const qagnn_shape& s, const FoldLayout& L, const WorkLayout& W, int layer, const float* x,
                       const float* extra, const void* prep, const qagnn_prep_layout& pl, const float* folded,
                       float* out, float* alpha_out, float* aggr_out, float* ws, Act final_act, bool tiled,
-                      cudaStream_t st) {
+                      cudaStream_t st, const Ragged& rg = Ragged{}) {
   const int D = s.D;
   const float* lb = folded + L.layer0 + (size_t)layer * L.layer_stride;
   float* qkm = ws + W.qkm;
@@ -282,7 +282,7 @@ int32_t layer_forward(const qagnn_shape& s, const FoldLayout& L, const WorkLayou
     QAGNN_RETURN_IF(zero_alpha_holes(s, prep, pl, alpha_out, st));
     if (tiled) {
       QAGNN_RETURN_IF(launch_message_passing_headtile(s, (const int32_t*)prep, pl, qkm, lb + L.keh, lb + L.meh,
-                                                      ws + W.score, ws + W.alpha2, aggr, alpha_out, nullptr, nullptr, st));
+                                                      ws + W.score, ws + W.alpha2, aggr, alpha_out, nullptr, nullptr, st, rg));
     } else if (use_slice(s)) {
       QAGNN_RETURN_IF(launch_message_passing_slice(s, (const int32_t*)prep, pl, qkm, lb + L.ke, lb + L.me, ws + W.score, aggr,
                                                    alpha_out, st));
@@ -324,7 +324,7 @@ int32_t layer_forward_tc(const qagnn_shape& s, const FoldLayout& L, const WorkLa
                          const void* prep, const qagnn_prep_layout& pl, const float* folded, float* out_f32,
                          void* out_hi, void* out_lo, float* alpha_out, float* aggr_out, float* ws, Act final_act,
                          bool tiled, cudaStream_t st, const int64_t* type_bias_classes = nullptr, int out_ldp = 0,
-                         int passes = 3) {
+                         int passes = 3, const Ragged& rg = Ragged{}) {
   const int D = s.D;
   if (out_ldp == 0) out_ldp = D;
   float* const ap_lo = passes == 1 ? nullptr : ws + W.ap_lo;
@@ -365,7 +365,7 @@ int32_t layer_forward_tc(const qagnn_shape& s, const FoldLayout& L, const WorkLa
     if (tiled) {
       QAGNN_RETURN_IF(launch_message_passing_headtile(s, (const int32_t*)prep, pl, qkm, lb + L.keh, lb + L.meh,
                                                       ws + W.score, ws + W.alpha2, aggr, alpha_out,
-                                                      fused_split ? ws + W.ap_hi : nullptr, ap_lo, st));
+                                                      fused_split ? ws + W.ap_hi : nullptr, ap_lo, st, rg));
     } else if (use_slice(s)) {
       QAGNN_RETURN_IF(launch_message_passing_slice(s, (const int32_t*)prep, pl, qkm, lb + L.ke, lb + L.me, ws + W.score, aggr,
                                                    alpha_out, st));
@@ -516,9 +516,9 @@ extern "C" size_t qagnn_forward_workspace_bytes(const qagnn_shape* shape) {
   return align_up(make_work_layout(*shape).total * sizeof(float));
 }
 
-extern "C" int32_t qagnn_gatconve_forward(const qagnn_shape* shape, int32_t layer, const float* x, const float* extra,
-                                          const void* prep, const void* folded, float* out, float* alpha_out,
-                                          float* aggr_out, void* workspace, size_t workspace_bytes, void* stream) {
+static int32_t gatconve_forward(const qagnn_shape* shape, int32_t layer, const float* x, const float* extra, const void* prep,
+                                const void* folded, float* out, float* alpha_out, float* aggr_out, void* workspace,
+                                size_t workspace_bytes, void* stream, const Ragged& rg) {
   QAGNN_RETURN_IF(check_shape_fwd(shape));
   if (!x || !extra || !prep || !folded || !out || !workspace) return QAGNN_ERR_INVALID_ARGUMENT;
   if (layer < 0 || layer >= shape->k) return QAGNN_ERR_INVALID_ARGUMENT;
@@ -527,7 +527,7 @@ extern "C" int32_t qagnn_gatconve_forward(const qagnn_shape* shape, int32_t laye
   if (workspace_bytes < W.total * sizeof(float)) return QAGNN_ERR_WORKSPACE;
   qagnn_prep_layout pl;
   QAGNN_RETURN_IF(qagnn_graph_prep_layout(shape->N, shape->E, &pl));
-  const bool tiled = use_headtile(*shape);
+  const bool tiled = use_headtile(*shape, rg);
   cudaStream_t st = (cudaStream_t)stream;
   float* ws = (float*)workspace;
   if (tiled && !use_tc(*shape)) QAGNN_RETURN_IF(zero_head_pads(*shape, ws + W.qkm, st));
@@ -536,21 +536,28 @@ extern "C" int32_t qagnn_gatconve_forward(const qagnn_shape* shape, int32_t laye
     QAGNN_RETURN_IF(split_bf16(x, D, shape->N, D, ws + W.xp_hi[0], ws + W.xp_lo[0], D, st));
     QAGNN_RETURN_IF(split_bf16(extra, D, shape->N, D, ws + W.ep_hi, ws + W.ep_lo, D, st));
     return layer_forward_tc(*shape, L, W, layer, Planes{ws + W.xp_hi[0], ws + W.xp_lo[0]}, Planes{ws + W.ep_hi, ws + W.ep_lo},
-                            prep, pl, (const float*)folded, out, nullptr, nullptr, alpha_out, aggr_out, ws, ACT_NONE, tiled, st);
+                            prep, pl, (const float*)folded, out, nullptr, nullptr, alpha_out, aggr_out, ws, ACT_NONE, tiled, st,
+                            nullptr, 0, 3, rg);
   }
   return layer_forward(*shape, L, W, layer, x, extra, prep, pl, (const float*)folded, out, alpha_out, aggr_out, ws,
-                       ACT_NONE, tiled, st);
+                       ACT_NONE, tiled, st, rg);
 }
 
-extern "C" int32_t qagnn_gatconve_forward_typed(const qagnn_shape* shape, int32_t dtype, int32_t in_dtype, int32_t layer,
-                                                const void* x, const void* extra, const void* prep, const void* folded,
-                                                void* out, float* alpha_out, float* aggr_out, void* workspace,
-                                                size_t workspace_bytes, void* stream) {
+extern "C" int32_t qagnn_gatconve_forward(const qagnn_shape* shape, int32_t layer, const float* x, const float* extra,
+                                          const void* prep, const void* folded, float* out, float* alpha_out,
+                                          float* aggr_out, void* workspace, size_t workspace_bytes, void* stream) {
+  return gatconve_forward(shape, layer, x, extra, prep, folded, out, alpha_out, aggr_out, workspace, workspace_bytes, stream,
+                          Ragged{});
+}
+
+static int32_t gatconve_forward_typed(const qagnn_shape* shape, int32_t dtype, int32_t in_dtype, int32_t layer, const void* x,
+                                      const void* extra, const void* prep, const void* folded, void* out, float* alpha_out,
+                                      float* aggr_out, void* workspace, size_t workspace_bytes, void* stream, const Ragged& rg) {
   if (in_dtype != QAGNN_DTYPE_F32 && in_dtype != QAGNN_DTYPE_BF16) return QAGNN_ERR_INVALID_ARGUMENT;
   if (dtype == QAGNN_DTYPE_F32) {
     if (in_dtype != QAGNN_DTYPE_F32) return QAGNN_ERR_INVALID_ARGUMENT;
-    return qagnn_gatconve_forward(shape, layer, (const float*)x, (const float*)extra, prep, folded, (float*)out, alpha_out,
-                                  aggr_out, workspace, workspace_bytes, stream);
+    return gatconve_forward(shape, layer, (const float*)x, (const float*)extra, prep, folded, (float*)out, alpha_out, aggr_out,
+                            workspace, workspace_bytes, stream, rg);
   }
   if (dtype != QAGNN_DTYPE_BF16) return QAGNN_ERR_INVALID_ARGUMENT;
   const bool in_bf16 = in_dtype == QAGNN_DTYPE_BF16;
@@ -562,7 +569,7 @@ extern "C" int32_t qagnn_gatconve_forward_typed(const qagnn_shape* shape, int32_
   if (workspace_bytes < W.total * sizeof(float)) return QAGNN_ERR_WORKSPACE;
   qagnn_prep_layout pl;
   QAGNN_RETURN_IF(qagnn_graph_prep_layout(shape->N, shape->E, &pl));
-  const bool tiled = use_headtile(*shape);
+  const bool tiled = use_headtile(*shape, rg);
   cudaStream_t st = (cudaStream_t)stream;
   float* ws = (float*)workspace;
   const int D = shape->D;
@@ -572,7 +579,7 @@ extern "C" int32_t qagnn_gatconve_forward_typed(const qagnn_shape* shape, int32_
     QAGNN_RETURN_IF(hi_plane_of(extra, in_bf16, ws + W.ep_hi, D, shape->N, D, st));
     return layer_forward_tc(*shape, L, W, layer, Planes{ws + W.xp_hi[0], nullptr}, Planes{ws + W.ep_hi, nullptr}, prep, pl,
                             (const float*)folded, nullptr, out, nullptr, alpha_out, aggr_out, ws, ACT_NONE, tiled, st,
-                            nullptr, 0, 1);
+                            nullptr, 0, 1, rg);
   }
   // the fp32 path on the rounded inputs (widened exactly), its output rounded once
   float* x32 = fp32_staging(W, ws);
@@ -589,8 +596,34 @@ extern "C" int32_t qagnn_gatconve_forward_typed(const qagnn_shape* shape, int32_
   }
   if (tiled) QAGNN_RETURN_IF(zero_head_pads(*shape, ws + W.qkm, st));
   QAGNN_RETURN_IF(layer_forward(*shape, L, W, layer, x32, ex32, prep, pl, (const float*)folded, out32, alpha_out, aggr_out, ws,
-                                ACT_NONE, tiled, st));
+                                ACT_NONE, tiled, st, rg));
   return convert(ND, out32, out, false, st);
+}
+
+extern "C" int32_t qagnn_gatconve_forward_typed(const qagnn_shape* shape, int32_t dtype, int32_t in_dtype, int32_t layer,
+                                                const void* x, const void* extra, const void* prep, const void* folded,
+                                                void* out, float* alpha_out, float* aggr_out, void* workspace,
+                                                size_t workspace_bytes, void* stream) {
+  return gatconve_forward_typed(shape, dtype, in_dtype, layer, x, extra, prep, folded, out, alpha_out, aggr_out, workspace,
+                                workspace_bytes, stream, Ragged{});
+}
+
+// a ragged batch: n_graphs sub-graphs of at most shape->n_per_graph rows at node_ptr, the rest of the N rows a tail
+static int32_t check_ragged(const qagnn_shape* shape, int32_t n_graphs, const int64_t* node_ptr, Ragged& rg) {
+  if (!shape || !node_ptr || n_graphs <= 0 || n_graphs > shape->N || shape->n_per_graph <= 0) return QAGNN_ERR_INVALID_ARGUMENT;
+  rg.node_ptr = node_ptr;
+  rg.B = n_graphs;
+  return QAGNN_OK;
+}
+
+extern "C" int32_t qagnn_gatconve_forward_ragged(const qagnn_shape* shape, int32_t dtype, int32_t in_dtype, int32_t n_graphs,
+                                                 const int64_t* node_ptr, int32_t layer, const void* x, const void* extra,
+                                                 const void* prep, const void* folded, void* out, float* alpha_out,
+                                                 float* aggr_out, void* workspace, size_t workspace_bytes, void* stream) {
+  Ragged rg;
+  QAGNN_RETURN_IF(check_ragged(shape, n_graphs, node_ptr, rg));
+  return gatconve_forward_typed(shape, dtype, in_dtype, layer, x, extra, prep, folded, out, alpha_out, aggr_out, workspace,
+                                workspace_bytes, stream, rg);
 }
 
 extern "C" int32_t qagnn_mp_path(const qagnn_shape* shape) {
@@ -615,7 +648,7 @@ extern "C" int32_t qagnn_node_feature_extra(const qagnn_shape* shape, const int6
 // GEMM single-pass on the hi planes (qagnn_mp_forward_typed with QAGNN_DTYPE_BF16).
 static int32_t mp_forward(const qagnn_shape& s, int passes, bool h_bf16, const void* H_in_any, const int64_t* node_type,
                           const float* node_score, const void* prep, const void* folded, void* out_any, float* x_layers_out,
-                          float* ws, cudaStream_t st) {
+                          float* ws, cudaStream_t st, const Ragged& rg = Ragged{}) {
   const FoldLayout L = make_fold_layout(s);
   const WorkLayout W = make_work_layout(s);
   qagnn_prep_layout pl;
@@ -624,7 +657,7 @@ static int32_t mp_forward(const qagnn_shape& s, int passes, bool h_bf16, const v
   const float* f = (const float*)folded;
   float* extra = ws + W.extra;
   const bool tc = use_tc(s);
-  const bool tiled = use_headtile(s);
+  const bool tiled = use_headtile(s, rg);
   const float* H_in = (const float*)H_in_any;
   float* out = (float*)out_any;
   if (single && !tc) {  // the fp32 path on the rounded H (widened exactly), its output rounded once at the end
@@ -677,7 +710,7 @@ static int32_t mp_forward(const qagnn_shape& s, int passes, bool h_bf16, const v
       void* ohi = xh[1 + (l & 1)];
       void* olo = xl[1 + (l & 1)];
       QAGNN_RETURN_IF(layer_forward_tc(s, L, W, l, xin, ep, prep, pl, f, xo32, ohi, olo, nullptr, nullptr, ws, ACT_GELU, tiled, st,
-                                       node_type, KS, passes));
+                                       node_type, KS, passes, rg));
       xin = Planes{ohi, olo, KS};
     }
     // output = GELU(Vh(H) + Vx(X))                                           (:92)
@@ -709,7 +742,7 @@ static int32_t mp_forward(const qagnn_shape& s, int passes, bool h_bf16, const v
       void* ohi = ws + W.xp_hi[l & 1];
       void* olo = ws + W.xp_lo[l & 1];
       QAGNN_RETURN_IF(layer_forward_tc(s, L, W, l, xin, ep, prep, pl, f, xo32, ohi, olo, nullptr, nullptr, ws, ACT_GELU,
-                                       tiled, st, nullptr, 0, passes));
+                                       tiled, st, nullptr, 0, passes, rg));
       xin = Planes{ohi, olo};
     }
     // output = GELU(Vh(H) + Vx(X))                                           (:92)
@@ -724,7 +757,7 @@ static int32_t mp_forward(const qagnn_shape& s, int passes, bool h_bf16, const v
   const float* x = H_in;
   for (int l = 0; l < s.k; ++l) {  // mp_helper, :45-50 (dropout is the identity in eval)
     float* xo = x_layers_out ? x_layers_out + (size_t)l * ND : ws + ((l & 1) ? W.xb : W.xa);
-    QAGNN_RETURN_IF(layer_forward(s, L, W, l, x, extra, prep, pl, f, xo, nullptr, nullptr, ws, ACT_GELU, tiled, st));
+    QAGNN_RETURN_IF(layer_forward(s, L, W, l, x, extra, prep, pl, f, xo, nullptr, nullptr, ws, ACT_GELU, tiled, st, rg));
     x = xo;
   }
   // output = GELU(Vh(H) + Vx(X))                                             (:92)
@@ -765,6 +798,21 @@ extern "C" int32_t qagnn_mp_forward_typed(const qagnn_shape* shape, int32_t dtyp
   QAGNN_RETURN_IF(check_mp_forward_args(shape, H_in, node_type, node_score, prep, folded, out, workspace, workspace_bytes));
   return mp_forward(*shape, 1, in_dtype == QAGNN_DTYPE_BF16, H_in, node_type, node_score, prep, folded, out, x_layers_out,
                     (float*)workspace, (cudaStream_t)stream);
+}
+
+extern "C" int32_t qagnn_mp_forward_ragged(const qagnn_shape* shape, int32_t dtype, int32_t in_dtype, int32_t n_graphs,
+                                           const int64_t* node_ptr, const void* H_in, const int64_t* node_type,
+                                           const float* node_score, const void* prep, const void* folded, void* out,
+                                           float* x_layers_out, void* workspace, size_t workspace_bytes, void* stream) {
+  Ragged rg;
+  QAGNN_RETURN_IF(check_ragged(shape, n_graphs, node_ptr, rg));
+  if (in_dtype != QAGNN_DTYPE_F32 && in_dtype != QAGNN_DTYPE_BF16) return QAGNN_ERR_INVALID_ARGUMENT;
+  if (dtype != QAGNN_DTYPE_F32 && dtype != QAGNN_DTYPE_BF16) return QAGNN_ERR_INVALID_ARGUMENT;
+  if (dtype == QAGNN_DTYPE_F32 && in_dtype != QAGNN_DTYPE_F32) return QAGNN_ERR_INVALID_ARGUMENT;
+  QAGNN_RETURN_IF(check_mp_forward_args(shape, H_in, node_type, node_score, prep, folded, out, workspace, workspace_bytes));
+  const bool single = dtype == QAGNN_DTYPE_BF16;
+  return mp_forward(*shape, single ? 1 : 3, in_dtype == QAGNN_DTYPE_BF16, H_in, node_type, node_score, prep, folded, out,
+                    x_layers_out, (float*)workspace, (cudaStream_t)stream, rg);
 }
 
 extern "C" int32_t qagnn_mp_core_forward(const qagnn_shape* shape, const void* prep, const float* qkm, const float* ke,

@@ -167,15 +167,41 @@ bool mlp_tc_shape_ok(int D);
 int32_t mlp_tc(const TcOperand& A, const TcOperand& W1, const float* b1, const TcOperand& W2, const float* b2, long long M,
                Act act2, const TcOutput& out, cudaStream_t st, int passes = 3);
 
+// ---- ragged batches (qagnn_graph_prep_ragged) ------------------------------------------------------------
+// Sub-graph g < B owns rows [node_ptr[g], node_ptr[g+1]) of an N-row batch (N = the node capacity); the tail rows
+// [node_ptr[B], N) belong to no graph and are cut into segments of at most n rows, B + j for j = 0, 1, ...  Values are clamped
+// into [0, N] and to n rows per segment, so a bad node_ptr never moves an access out of range (graph prep reports it).
+struct Ragged {
+  const int64_t* node_ptr = nullptr;  // device int64 [B + 1]; nullptr = the uniform layout (g * n_per_graph)
+  int B = 0;
+};
+__host__ __device__ inline int64_t ragged_clamp(int64_t v, int64_t lo, int64_t hi) { return v < lo ? lo : (v > hi ? hi : v); }
+// most segments a ragged batch of B graphs over N rows can have (every graph has at least one row)
+inline int64_t ragged_max_segments(int64_t N, int B, int n) { return B + (N - B + n - 1) / n; }
+__device__ inline void ragged_segment(const int64_t* node_ptr, int B, int n, int64_t N, int64_t g, int64_t& v0, int& ng) {
+  if (g < B) {
+    const int64_t a = ragged_clamp(node_ptr[g], 0, N), b = ragged_clamp(node_ptr[g + 1], a, N);
+    v0 = a;
+    ng = (int)(b - a < n ? b - a : n);
+  } else {
+    v0 = ragged_clamp(ragged_clamp(node_ptr[B], 0, N) + (g - B) * n, 0, N);
+    ng = (int)(N - v0 < n ? N - v0 : n);
+  }
+}
+// segments in use: the B graphs and the tail segments up to row N
+__device__ inline int64_t ragged_segments(const int64_t* node_ptr, int B, int n, int64_t N) {
+  return B + (N - ragged_clamp(node_ptr[B], 0, N) + n - 1) / n;
+}
+
 // ---- shared-memory-tiled message passing (mp_headtile.cu) ----------------------------------------------
 inline int head_dim_padded(int d) { return (d + 3) / 4 * 4; }
 inline int round_up8(int k) { return (k + 7) / 8 * 8; }
 // true when the per-head persistent kernel can run this shape on this device
-bool headtile_supported(const qagnn_shape& s);
+bool headtile_supported(const qagnn_shape& s, const Ragged& rg = Ragged{});
 int32_t launch_message_passing_headtile(const qagnn_shape& s, const int32_t* prep_base, const qagnn_prep_layout& pl,
                                         const float* qkmh, const float* keh, const float* meh, float* score,
                                         float* alpha2, float* aggr, float* alpha_out, void* aggr_hi, void* aggr_lo,
-                                        cudaStream_t st);
+                                        cudaStream_t st, const Ragged& rg = Ragged{});
 int32_t zero_head_pads(const qagnn_shape& s, float* qkmh, cudaStream_t st);
 
 int32_t launch_message_passing(const qagnn_shape& s, const int32_t* prep_base, const qagnn_prep_layout& pl,

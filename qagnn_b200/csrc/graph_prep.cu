@@ -306,15 +306,20 @@ __global__ void __launch_bounds__(256) prep_degree_order_kernel(int npg, const i
 // array then ends at E' = graph_ptr[G] + N, and the positions a sub-graph writes do not depend on E at all.
 struct PackedPrepArgs {
   const int64_t *edge_index, *edge_type, *node_type, *graph_ptr;
+  const int64_t* node_ptr;  // ragged batches: first row of every sub-graph, [B + 1]
   int64_t N, E;
-  int T, R, npg, cap;
+  int T, R, npg, cap, B;    // B: sub-graphs of a ragged batch (the grid adds the tail segments)
   int32_t *src, *tgt, *combo, *rowptr_src, *rowptr_tgt, *perm_src, *perm_tgt, *csr_src_tgt, *csr_src_combo, *csr_tgt_src,
       *csr_tgt_combo, *csr_tgt_apos, *pk_src, *pk_tgt, *csr_src_tpos, *order_src, *order_tgt, *status;
   uint2 *ninfo_src, *ninfo_tgt;
 };
 
 constexpr int kPackedThreads = 256;
+constexpr int kNodePtrBit = 32;  // status bit: node_ptr not monotone, a sub-graph over n rows, or node_ptr[B] past N
 
+// RAGGED: sub-graph g owns rows [node_ptr[g], node_ptr[g+1]) (at most npg of them) instead of [g*npg, (g+1)*npg); CTAs
+// g >= B build the tail segments (rows past node_ptr[B]: self loops only, see ragged_segment in common.cuh).
+template <bool RAGGED>
 __global__ void __launch_bounds__(kPackedThreads) prep_packed_graph_kernel(const PackedPrepArgs a) {
   extern __shared__ int32_t sm_pp[];
   const int n = a.npg, cap = a.cap, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarps = kPackedThreads / 32;
@@ -335,30 +340,50 @@ __global__ void __launch_bounds__(kPackedThreads) prep_packed_graph_kernel(const
   __shared__ int hist[256], hbase[256];
 
   const int64_t g = blockIdx.x, G = gridDim.x;
-  // a.E is the edge CAPACITY of edge_index / edge_type; the batch's edges are the first graph_ptr[G] columns (clamped: a
+  const int64_t Bg = RAGGED ? a.B : G;  // sub-graphs with edges
+  // a.E is the edge CAPACITY of edge_index / edge_type; the batch's edges are the first graph_ptr[B] columns (clamped: a
   // graph_ptr past the capacity sets bit 16 in the CTA of the last sub-graph below).  The ids of the unused columns keep
   // src / tgt / combo = -1; the self loops stay at ids E + v, behind every real edge.
-  const int64_t e_real = min(max(a.graph_ptr[G], (int64_t)0), a.E);
-  if (g == G - 1 && tid == 0) { a.rowptr_src[a.N] = (int32_t)(e_real + a.N); a.rowptr_tgt[a.N] = (int32_t)(e_real + a.N); }
+  const int64_t e_real = min(max(a.graph_ptr[Bg], (int64_t)0), a.E);
+  if (g == (RAGGED ? 0 : G - 1) && tid == 0) {
+    a.rowptr_src[a.N] = (int32_t)(e_real + a.N); a.rowptr_tgt[a.N] = (int32_t)(e_real + a.N);
+  }
   for (int64_t e = e_real + g * kPackedThreads + tid; e < a.E; e += G * kPackedThreads) {
     a.src[e] = -1; a.tgt[e] = -1; a.combo[e] = -1;
   }
-  const int64_t e0 = a.graph_ptr[g], e1 = a.graph_ptr[g + 1];
-  const int eg = (int)(e1 - e0), ep = eg + n;  // real edges, edges incl. self loops (ep <= cap, checked on the host)
-  const int64_t v0 = g * n;
+  int64_t v0 = g * n, e0, e1;
+  int ng = n;  // rows of this sub-graph
+  if (RAGGED) {
+    ragged_segment(a.node_ptr, a.B, n, a.N, g, v0, ng);
+    if (g < Bg) {
+      e0 = a.graph_ptr[g]; e1 = a.graph_ptr[g + 1];
+      const int64_t r0 = a.node_ptr[g], r1 = a.node_ptr[g + 1];
+      const bool bad_ptr = (g == 0 && r0 != 0) || r1 < r0 || r1 - r0 > n || (g == Bg - 1 && r1 > a.N) || (ng == 0 && e1 > e0);
+      if (bad_ptr) {  // nothing of this sub-graph is touched
+        if (tid == 0) atomicOr(a.status, kNodePtrBit);
+        return;
+      }
+    } else {
+      if (ng == 0) return;  // past the tail
+      e0 = e1 = e_real;
+    }
+  } else {
+    e0 = a.graph_ptr[g]; e1 = a.graph_ptr[g + 1];
+  }
+  const int eg = (int)(e1 - e0), ep = eg + ng;  // real edges, edges incl. self loops (ep <= cap, checked on the host)
   const int64_t base = e0 + v0;  // entries of the CSR orders that belong to earlier sub-graphs
   if (e0 < 0 || e1 < e0 || e1 > a.E || ep > cap) {  // graph_ptr disagrees with E / max_edges_per_graph: nothing is touched
     if (tid == 0) atomicOr(a.status, 16);
     return;
   }
   int bad = 0;
-  for (int i = tid; i < n; i += kPackedThreads) {
+  for (int i = tid; i < ng; i += kPackedThreads) {
     int64_t t = a.node_type[v0 + i];
     if (t < 0 || t >= a.T) { bad |= 4; t = min(max(t, (int64_t)0), (int64_t)a.T - 1); }
     ntype[i] = (int32_t)t;
     cnt_s[i] = 0; cnt_t[i] = 0; cur_s[i] = 0; cur_t[i] = 0;
   }
-  if (tid == 0) { cnt_s[n] = 0; cnt_t[n] = 0; }
+  if (tid == 0) { cnt_s[ng] = 0; cnt_t[ng] = 0; }
   __syncthreads();
   // edges -> local ids, combo, counts; global src / tgt / combo in edge-id order
   for (int i = tid; i < ep; i += kPackedThreads) {
@@ -369,9 +394,10 @@ __global__ void __launch_bounds__(kPackedThreads) prep_packed_graph_kernel(const
       int64_t s = a.edge_index[gid], t = a.edge_index[a.E + gid], rr = a.edge_type[gid];
       if (s < 0 || s >= a.N || t < 0 || t >= a.N) { bad |= 1; s = min(max(s, (int64_t)0), a.N - 1); t = min(max(t, (int64_t)0), a.N - 1); }
       if (rr < 0 || rr >= a.R) { bad |= 2; rr = min(max(rr, (int64_t)0), (int64_t)a.R - 1); }
-      if (s / n != g || t / n != g) bad |= 8;  // not an edge of this sub-graph
-      sl = (int)min(max(s - v0, (int64_t)0), (int64_t)n - 1);
-      tl = (int)min(max(t - v0, (int64_t)0), (int64_t)n - 1);
+      if (RAGGED ? (s < v0 || s >= v0 + ng || t < v0 || t >= v0 + ng) : (s / n != g || t / n != g))
+        bad |= 8;  // not an edge of this sub-graph
+      sl = (int)min(max(s - v0, (int64_t)0), (int64_t)ng - 1);
+      tl = (int)min(max(t - v0, (int64_t)0), (int64_t)ng - 1);
       r = (int)rr;
       a.src[gid] = (int32_t)s; a.tgt[gid] = (int32_t)t;
     } else {
@@ -391,7 +417,7 @@ __global__ void __launch_bounds__(kPackedThreads) prep_packed_graph_kernel(const
   // exclusive scan of both count arrays (warp 0: by source, warp 1: by target), n <= 65535
   if (warp < 2) {
     int32_t* cnt = warp == 0 ? cnt_s : cnt_t;
-    const int chunk = (n + 31) / 32, b0 = lane * chunk, b1 = min(n, b0 + chunk);
+    const int chunk = (ng + 31) / 32, b0 = lane * chunk, b1 = min(ng, b0 + chunk);
     int sum = 0;
     for (int i = b0; i < b1; ++i) sum += cnt[i];
     int incl = sum;
@@ -402,10 +428,10 @@ __global__ void __launch_bounds__(kPackedThreads) prep_packed_graph_kernel(const
     }
     int run = incl - sum;
     for (int i = b0; i < b1; ++i) { const int c = cnt[i]; cnt[i] = run; run += c; }
-    if (lane == 31) cnt[n] = incl;
+    if (lane == 31) cnt[ng] = incl;
   }
   __syncthreads();
-  for (int i = tid; i < n; i += kPackedThreads) {
+  for (int i = tid; i < ng; i += kPackedThreads) {
     a.rowptr_src[v0 + i] = (int32_t)(base + cnt_s[i]);
     a.rowptr_tgt[v0 + i] = (int32_t)(base + cnt_t[i]);
   }
@@ -415,9 +441,9 @@ __global__ void __launch_bounds__(kPackedThreads) prep_packed_graph_kernel(const
     tmp_t[cnt_t[ltgt[i]] + atomicAdd(&cur_t[ltgt[i]], 1)] = i;
   }
   __syncthreads();
-  for (int w = warp; w < 2 * n; w += nwarps) {  // one warp per (node, direction); lanes over the segment's positions
-    const bool by_t = w >= n;
-    const int v = by_t ? w - n : w;
+  for (int w = warp; w < 2 * ng; w += nwarps) {  // one warp per (node, direction); lanes over the segment's positions
+    const bool by_t = w >= ng;
+    const int v = by_t ? w - ng : w;
     const int32_t* cnt = by_t ? cnt_t : cnt_s;
     const int32_t* tmp = by_t ? tmp_t : tmp_s;
     int32_t* perm = by_t ? perm_t : perm_s;
@@ -463,14 +489,14 @@ __global__ void __launch_bounds__(kPackedThreads) prep_packed_graph_kernel(const
     __syncthreads();
     hist[tid] = 0;
     __syncthreads();
-    for (int i = tid; i < n; i += kPackedThreads) atomicAdd(&hist[min(cnt[i + 1] - cnt[i], 255)], 1);
+    for (int i = tid; i < ng; i += kPackedThreads) atomicAdd(&hist[min(cnt[i + 1] - cnt[i], 255)], 1);
     __syncthreads();
     if (tid == 0) {
       int run = 0;
       for (int b = 255; b >= 0; --b) { hbase[b] = run; run += hist[b]; }
     }
     __syncthreads();
-    for (int i = tid; i < n; i += kPackedThreads) {
+    for (int i = tid; i < ng; i += kPackedThreads) {
       const int deg = cnt[i + 1] - cnt[i];
       const int slot = atomicAdd(&hbase[min(deg, 255)], 1);
       order[slot] = i;
@@ -605,29 +631,36 @@ extern "C" int32_t qagnn_graph_prep(const int64_t* edge_index, const int64_t* ed
   return QAGNN_OK;
 }
 
-extern "C" int32_t qagnn_graph_prep_packed(const int64_t* edge_index, const int64_t* edge_type, const int64_t* node_type,
-                                           const int64_t* graph_ptr, int32_t max_edges_per_graph, const qagnn_shape* shape,
-                                           void* prep, size_t prep_bytes, int32_t validate, void* stream) {
+namespace qagnn {
+namespace {
+
+// qagnn_graph_prep_packed (node_ptr == nullptr) and qagnn_graph_prep_ragged
+int32_t graph_prep_packed(const int64_t* edge_index, const int64_t* edge_type, const int64_t* node_type, const int64_t* graph_ptr,
+                          const int64_t* node_ptr, int32_t n_graphs, int32_t max_edges_per_graph, const qagnn_shape* shape,
+                          void* prep, size_t prep_bytes, int32_t validate, void* stream) {
+  const bool ragged = node_ptr != nullptr;
   if (!shape || !node_type || !prep || !graph_ptr) return QAGNN_ERR_INVALID_ARGUMENT;
   const int64_t N = shape->N, E = shape->E;
   if (E > 0 && (!edge_index || !edge_type)) return QAGNN_ERR_INVALID_ARGUMENT;
   if (shape->T <= 0 || shape->R <= 0 || max_edges_per_graph < 0) return QAGNN_ERR_INVALID_ARGUMENT;
+  if (ragged && (n_graphs <= 0 || n_graphs > N)) return QAGNN_ERR_INVALID_ARGUMENT;
   const int npg = shape->n_per_graph;
   const int64_t Ccombo = (int64_t)shape->R * shape->T * shape->T + shape->T;
-  if (npg <= 0 || npg > 65535 || N % npg != 0 || Ccombo > 65536) return QAGNN_ERR_UNSUPPORTED;
+  if (npg <= 0 || npg > 65535 || (!ragged && N % npg != 0) || Ccombo > 65536) return QAGNN_ERR_UNSUPPORTED;
   qagnn_prep_layout pl;
   QAGNN_RETURN_IF(qagnn_graph_prep_layout(N, E, &pl));
   if (prep_bytes < pl.total_bytes) return QAGNN_ERR_WORKSPACE;
   const int cap = max_edges_per_graph + npg;
   const size_t smem = ((size_t)5 * npg + 2 + (size_t)9 * cap) * sizeof(int32_t);
   static int smem_c[kMaxDevices] = {0};
-  static size_t attr[kMaxDevices] = {0};
+  static size_t attr[2][kMaxDevices] = {{0}};
   const int dev = current_device();
   if (smem_c[dev] == 0) cudaDeviceGetAttribute(&smem_c[dev], cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
   if (smem + 4096 > (size_t)smem_c[dev]) return QAGNN_ERR_UNSUPPORTED;  // sub-graphs too large for one CTA: use qagnn_graph_prep
-  if (smem + 4096 > 48 * 1024 && smem > attr[dev]) {  // the kernel also has 2 KB of static shared memory
-    QAGNN_CHECK_CUDA(cudaFuncSetAttribute(prep_packed_graph_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr[dev] = smem;
+  if (smem + 4096 > 48 * 1024 && smem > attr[ragged][dev]) {  // the kernel also has 2 KB of static shared memory
+    QAGNN_CHECK_CUDA(cudaFuncSetAttribute(ragged ? prep_packed_graph_kernel<true> : prep_packed_graph_kernel<false>,
+                                          cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    attr[ragged][dev] = smem;
   }
   cudaStream_t st = (cudaStream_t)stream;
   char* base = (char*)prep;
@@ -635,14 +668,18 @@ extern "C" int32_t qagnn_graph_prep_packed(const int64_t* edge_index, const int6
   ProfScope ps(QAGNN_PROF_GRAPH_PREP, st);
   QAGNN_CHECK_CUDA(cudaMemsetAsync(I(pl.status), 0, 16, st));
   PackedPrepArgs a;
-  a.edge_index = edge_index; a.edge_type = edge_type; a.node_type = node_type; a.graph_ptr = graph_ptr;
-  a.N = N; a.E = E; a.T = shape->T; a.R = shape->R; a.npg = npg; a.cap = cap;
+  a.edge_index = edge_index; a.edge_type = edge_type; a.node_type = node_type; a.graph_ptr = graph_ptr; a.node_ptr = node_ptr;
+  a.N = N; a.E = E; a.T = shape->T; a.R = shape->R; a.npg = npg; a.cap = cap; a.B = ragged ? n_graphs : 0;
   a.src = I(pl.src); a.tgt = I(pl.tgt); a.combo = I(pl.combo); a.rowptr_src = I(pl.rowptr_src); a.rowptr_tgt = I(pl.rowptr_tgt);
   a.perm_src = I(pl.perm_src); a.perm_tgt = I(pl.perm_tgt); a.csr_src_tgt = I(pl.csr_src_tgt); a.csr_src_combo = I(pl.csr_src_combo);
   a.csr_tgt_src = I(pl.csr_tgt_src); a.csr_tgt_combo = I(pl.csr_tgt_combo); a.csr_tgt_apos = I(pl.csr_tgt_apos);
   a.pk_src = I(pl.pk_src); a.pk_tgt = I(pl.pk_tgt); a.csr_src_tpos = I(pl.csr_src_tpos); a.order_src = I(pl.order_src);
   a.order_tgt = I(pl.order_tgt); a.status = I(pl.status); a.ninfo_src = (uint2*)I(pl.ninfo_src); a.ninfo_tgt = (uint2*)I(pl.ninfo_tgt);
-  prep_packed_graph_kernel<<<(unsigned)(N / npg), kPackedThreads, smem, st>>>(a);
+  if (ragged) {
+    prep_packed_graph_kernel<true><<<(unsigned)ragged_max_segments(N, n_graphs, npg), kPackedThreads, smem, st>>>(a);
+  } else {
+    prep_packed_graph_kernel<false><<<(unsigned)(N / npg), kPackedThreads, smem, st>>>(a);
+  }
   QAGNN_CHECK_LAUNCH();
   if (validate) {
     int32_t h = 0;
@@ -651,4 +688,23 @@ extern "C" int32_t qagnn_graph_prep_packed(const int64_t* edge_index, const int6
     if (h != 0) return QAGNN_ERR_INDEX_RANGE;
   }
   return QAGNN_OK;
+}
+
+}  // namespace
+}  // namespace qagnn
+
+extern "C" int32_t qagnn_graph_prep_packed(const int64_t* edge_index, const int64_t* edge_type, const int64_t* node_type,
+                                           const int64_t* graph_ptr, int32_t max_edges_per_graph, const qagnn_shape* shape,
+                                           void* prep, size_t prep_bytes, int32_t validate, void* stream) {
+  return graph_prep_packed(edge_index, edge_type, node_type, graph_ptr, nullptr, 0, max_edges_per_graph, shape, prep, prep_bytes,
+                           validate, stream);
+}
+
+extern "C" int32_t qagnn_graph_prep_ragged(const int64_t* edge_index, const int64_t* edge_type, const int64_t* node_type,
+                                           const int64_t* graph_ptr, const int64_t* node_ptr, int32_t n_graphs,
+                                           int32_t max_edges_per_graph, const qagnn_shape* shape, void* prep, size_t prep_bytes,
+                                           int32_t validate, void* stream) {
+  if (!node_ptr) return QAGNN_ERR_INVALID_ARGUMENT;
+  return graph_prep_packed(edge_index, edge_type, node_type, graph_ptr, node_ptr, n_graphs, max_edges_per_graph, shape, prep,
+                           prep_bytes, validate, stream);
 }

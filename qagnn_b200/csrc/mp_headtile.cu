@@ -50,6 +50,8 @@ struct HeadTileParams {
   uint2* alpha2;  // [H][Eps] {tile byte offset of the source row << 16 | table float4 offset, a'} in by-target order
   float *aggr, *alpha_out;
   void *aggr_hi, *aggr_lo;  // optional split-bf16 planes of aggr [N, D] (A operand of the node-MLP GEMM)
+  const int64_t* node_ptr;  // ragged batches: first row of every sub-graph [B + 1]; G is then the most segments
+  int B;
 };
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -120,7 +122,10 @@ __host__ __device__ inline SmemMap make_smem_map(int C, int DP, int n) {
 // Consumer warps per CTA: 24 at <= 80 registers, or 31 (a full 1024-thread CTA) at <= 64.
 constexpr int kWarpsWide = 31, kWarpsNarrow = 24;
 
-template <int CPL, int WMAX>  // CPL: float4 chunks per lane (1: DP <= 32, 2: DP <= 64); WMAX: consumer-warp capacity
+// CPL: float4 chunks per lane (1: DP <= 32, 2: DP <= 64); WMAX: consumer-warp capacity.  RAGGED: graph g is segment g of a
+// ragged batch (ragged_segment in common.cuh: rows [node_ptr[g], node_ptr[g+1]) for g < B, then the tail rows in segments of n)
+// and its tile holds only its own rows; quads past a graph's row count are idle work items.
+template <int CPL, int WMAX, bool RAGGED = false>
 __global__ void __launch_bounds__((WMAX + 1) * 32, 1) mp_headtile_kernel(const HeadTileParams p) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   const int NCH = p.DP / 4;
@@ -134,7 +139,8 @@ __global__ void __launch_bounds__((WMAX + 1) * 32, 1) mp_headtile_kernel(const H
 
   const int h = blockIdx.x % p.H;
   const int slot = blockIdx.x / p.H;
-  const int Gc = slot < p.G ? (p.G - slot + p.S - 1) / p.S : 0;  // graphs slot, slot+S, ...
+  const int G = RAGGED ? (int)ragged_segments(p.node_ptr, p.B, p.n, p.N) : p.G;
+  const int Gc = slot < G ? (G - slot + p.S - 1) / p.S : 0;  // graphs slot, slot+S, ...
   if (Gc == 0) return;
   const int nq = p.nquads, total = Gc * nq;
 
@@ -172,8 +178,16 @@ __global__ void __launch_bounds__((WMAX + 1) * 32, 1) mp_headtile_kernel(const H
       }
       if (t >= 2) mbar_wait(&empty[b], ((t >> 1) - 1) & 1);
       const int g = slot + (ph2 ? t - Gc : t) * p.S;
-      bulk_g2s_chunked((char*)(smem_raw + sm.tile0 + b * sm.tile_bytes),
-                       (const char*)((ph2 ? Mh : Kh) + (size_t)g * p.n * p.DP), sm.tile_bytes, &full[b]);
+      if (RAGGED) {
+        int64_t v0;
+        int ng;
+        ragged_segment(p.node_ptr, p.B, p.n, p.N, g, v0, ng);
+        bulk_g2s_chunked((char*)(smem_raw + sm.tile0 + b * sm.tile_bytes), (const char*)((ph2 ? Mh : Kh) + (size_t)v0 * p.DP),
+                         (uint32_t)ng * p.DP * 4, &full[b]);
+      } else {
+        bulk_g2s_chunked((char*)(smem_raw + sm.tile0 + b * sm.tile_bytes),
+                         (const char*)((ph2 ? Mh : Kh) + (size_t)g * p.n * p.DP), sm.tile_bytes, &full[b]);
+      }
     }
     return;
   }
@@ -212,13 +226,25 @@ __global__ void __launch_bounds__((WMAX + 1) * 32, 1) mp_headtile_kernel(const H
     return __shfl_sync(0xffffffffu, v, 0);
   };
   auto item_graph = [&](int it) { return (int)__umulhi((uint32_t)it, magic); };  // it / nq
+  // first row and row count of this CTA's t-th graph (ragged batches only)
+  auto segment = [&](int t, int& ng) {
+    int64_t v0;
+    ragged_segment(p.node_ptr, p.B, p.n, p.N, slot + (int64_t)t * p.S, v0, ng);
+    return v0;
+  };
   // packed node record of work item `it` for this lane's node: {local id | degree << 16, CSR begin}; degree 0 = idle
   auto load_ninfo = [&](const uint2* ninfo, int it) {
     uint2 r = make_uint2(0u, 0u);
     if (it < total) {
       const int t = item_graph(it);
       const int si = (it - t * nq) * 4 + qi;
-      if (si < p.n) r = __ldg(ninfo + (uint32_t)((slot + t * p.S) * p.n + si));
+      if (RAGGED) {
+        int ng;
+        const int64_t v0 = segment(t, ng);
+        if (si < ng) r = __ldg(ninfo + v0 + si);
+      } else {
+        if (si < p.n) r = __ldg(ninfo + (uint32_t)((slot + t * p.S) * p.n + si));
+      }
     }
     return r;
   };
@@ -238,7 +264,13 @@ __global__ void __launch_bounds__((WMAX + 1) * 32, 1) mp_headtile_kernel(const H
 #pragma unroll
       for (int k = 0; k < CPL; ++k) q[k] = make_float4(0.f, 0.f, 0.f, 0.f);
       if (deg > 0) {  // deg > 0 implies it < total and a valid node
-        const uint32_t v = (uint32_t)((slot + item_graph(it) * p.S) * p.n) + (ni.x & 0xffffu);
+        uint32_t v;
+        if (RAGGED) {
+          int ng;
+          v = (uint32_t)segment(item_graph(it), ng) + (ni.x & 0xffffu);
+        } else {
+          v = (uint32_t)((slot + item_graph(it) * p.S) * p.n) + (ni.x & 0xffffu);
+        }
         const float4* qrow = reinterpret_cast<const float4*>(Qh) + (size_t)v * nch;
 #pragma unroll
         for (int k = 0; k < CPL; ++k)
@@ -274,7 +306,8 @@ __global__ void __launch_bounds__((WMAX + 1) * 32, 1) mp_headtile_kernel(const H
       const int beg = (int)ni0.y;
       int deg = (int)(ni0.x >> 16);
       if (deg == 0xffff) {  // saturated record: read the true out-degree
-        const int64_t v = (int64_t)(slot + t * p.S) * p.n + vl;
+        int ng;
+        const int64_t v = (RAGGED ? segment(t, ng) : (int64_t)(slot + t * p.S) * p.n) + vl;
         deg = p.rowptr_src[v + 1] - p.rowptr_src[v];
       }
       const int maxdeg = __reduce_max_sync(0xffffffffu, deg);
@@ -428,10 +461,12 @@ __global__ void __launch_bounds__((WMAX + 1) * 32, 1) mp_headtile_kernel(const H
         cur_t = t;
       }
       const int quad = it0 - tg * nq;
-      const bool nvalid = quad * 4 + qi < p.n;
+      int ng = p.n;
+      const int64_t gbase = RAGGED ? segment(tg, ng) : (int64_t)(slot + tg * p.S) * p.n;
+      const bool nvalid = quad * 4 + qi < ng;
       const uint32_t vl = ni0.x & 0xffffu;
       const int beg = (int)ni0.y;
-      const int64_t v = (int64_t)(slot + tg * p.S) * p.n + vl;
+      const int64_t v = gbase + vl;
       int deg = (int)(ni0.x >> 16);
       if (deg == 0xffff) deg = p.rowptr_tgt[v + 1] - p.rowptr_tgt[v];  // saturated record: read the true in-degree
       const int maxdeg = __reduce_max_sync(0xffffffffu, deg);
@@ -545,10 +580,13 @@ int forced_warps() {
   return (w >= 1 && w <= kWarpsWide) ? w : 0;
 }
 
-HeadTilePlan make_plan(const qagnn_shape& s) {
+// rg.node_ptr != nullptr: a ragged batch of rg.B graphs of at most n_per_graph rows over the N rows
+HeadTilePlan make_plan(const qagnn_shape& s, const Ragged& rg) {
   HeadTilePlan pl{};
   pl.ok = false;
-  if (s.n_per_graph <= 0 || s.n_per_graph > 65535 || s.N % s.n_per_graph != 0) return pl;
+  const bool ragged = rg.node_ptr != nullptr;
+  if (s.n_per_graph <= 0 || s.n_per_graph > 65535 || (!ragged && s.N % s.n_per_graph != 0)) return pl;
+  if (ragged && (rg.B <= 0 || rg.B > s.N)) return pl;
   const int d = s.D / s.H;
   pl.DP = head_dim_padded(d);
   pl.C = s.R * s.T * s.T + s.T;
@@ -574,7 +612,7 @@ HeadTilePlan make_plan(const qagnn_shape& s) {
   pl.nquads = (s.n_per_graph + 3) / 4;
   // item / nquads by multiply-high: exact while item * nquads < 2^32 (items run to graphs-per-CTA * nquads + 2 per warp)
   pl.nq_magic = (uint32_t)((((uint64_t)1) << 32) / (uint64_t)pl.nquads) + 1u;
-  const long long G = s.N / s.n_per_graph, Gc = (G + pl.S - 1) / pl.S;
+  const long long G = ragged ? ragged_max_segments(s.N, rg.B, s.n_per_graph) : s.N / s.n_per_graph, Gc = (G + pl.S - 1) / pl.S;
   if ((Gc * pl.nquads + 4 * kWarpsWide) * (long long)pl.nquads >= ((long long)1 << 32)) return pl;
   // two graphs' quads can be in flight at once; more warps than that would only spin
   // (24 warps at 72 registers beat 31 at 64 with spills: 112 vs 115 us/layer at cfg2, profiles/r2_mp_tuning.md)
@@ -587,22 +625,23 @@ HeadTilePlan make_plan(const qagnn_shape& s) {
   return pl;
 }
 
-template <int CPL, int WMAX>
+template <int CPL, int WMAX, bool RAGGED = false>
 int32_t launch_t(const HeadTileParams& p, const HeadTilePlan& plan, unsigned grid, unsigned block, cudaStream_t st) {
   static size_t attr_smem[kMaxDevices] = {0};  // the attribute is per device
   const int dev = current_device();
   if (plan.smem > attr_smem[dev]) {
-    QAGNN_CHECK_CUDA(cudaFuncSetAttribute(mp_headtile_kernel<CPL, WMAX>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan.smem));
+    QAGNN_CHECK_CUDA(cudaFuncSetAttribute(mp_headtile_kernel<CPL, WMAX, RAGGED>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                          (int)plan.smem));
     attr_smem[dev] = plan.smem;
   }
-  mp_headtile_kernel<CPL, WMAX><<<grid, block, plan.smem, st>>>(p);
+  mp_headtile_kernel<CPL, WMAX, RAGGED><<<grid, block, plan.smem, st>>>(p);
   QAGNN_CHECK_LAUNCH();
   return QAGNN_OK;
 }
 
 }  // namespace
 
-bool headtile_supported(const qagnn_shape& s) { return make_plan(s).ok; }
+bool headtile_supported(const qagnn_shape& s, const Ragged& rg) { return make_plan(s, rg).ok; }
 
 int32_t zero_head_pads(const qagnn_shape& s, float* qkmh, cudaStream_t st) {
   const int d = s.D / s.H, DP = head_dim_padded(d);
@@ -618,13 +657,14 @@ int32_t zero_head_pads(const qagnn_shape& s, float* qkmh, cudaStream_t st) {
 int32_t launch_message_passing_headtile(const qagnn_shape& s, const int32_t* prep_base, const qagnn_prep_layout& L,
                                         const float* qkmh, const float* keh, const float* meh, float* score,
                                         float* alpha2, float* aggr, float* alpha_out, void* aggr_hi, void* aggr_lo,
-                                        cudaStream_t st) {
-  const HeadTilePlan plan = make_plan(s);
+                                        cudaStream_t st, const Ragged& rg) {
+  const HeadTilePlan plan = make_plan(s, rg);
   if (!plan.ok) return QAGNN_ERR_UNSUPPORTED;
   auto I = [&](size_t off) { return (const int32_t*)((const char*)prep_base + off); };
   HeadTileParams p;
   p.N = s.N; p.Eps = (s.N + s.E + 3) / 4 * 4;
-  p.n = s.n_per_graph; p.G = (int)(s.N / s.n_per_graph); p.H = s.H; p.D = s.D; p.d = s.D / s.H; p.DP = plan.DP;
+  p.n = s.n_per_graph; p.G = (int)(s.N / s.n_per_graph);
+  p.node_ptr = rg.node_ptr; p.B = rg.B; p.H = s.H; p.D = s.D; p.d = s.D / s.H; p.DP = plan.DP;
   p.C = plan.C; p.S = plan.S; p.W = plan.W; p.nquads = plan.nquads; p.nq_magic = plan.nq_magic;
   p.rowptr_src = I(L.rowptr_src); p.rowptr_tgt = I(L.rowptr_tgt); p.pk_src = I(L.pk_src); p.tpos = I(L.csr_src_tpos); p.perm_src = I(L.perm_src);
   p.ninfo_src = (const uint2*)I(L.ninfo_src); p.ninfo_tgt = (const uint2*)I(L.ninfo_tgt);
@@ -633,6 +673,11 @@ int32_t launch_message_passing_headtile(const qagnn_shape& s, const int32_t* pre
   if (aggr_hi != nullptr && p.aggr_hi == nullptr) return QAGNN_ERR_UNSUPPORTED;
   const unsigned grid = (unsigned)(plan.S * s.H), block = (unsigned)(plan.W + 1) * 32;
   const bool wide = plan.W > kWarpsNarrow;  // more than 24 consumer warps: the 64-register build
+  if (rg.node_ptr != nullptr) {
+    if (plan.cpl == 1)
+      return wide ? launch_t<1, kWarpsWide, true>(p, plan, grid, block, st) : launch_t<1, kWarpsNarrow, true>(p, plan, grid, block, st);
+    return wide ? launch_t<2, kWarpsWide, true>(p, plan, grid, block, st) : launch_t<2, kWarpsNarrow, true>(p, plan, grid, block, st);
+  }
   if (plan.cpl == 1) return wide ? launch_t<1, kWarpsWide>(p, plan, grid, block, st) : launch_t<1, kWarpsNarrow>(p, plan, grid, block, st);
   return wide ? launch_t<2, kWarpsWide>(p, plan, grid, block, st) : launch_t<2, kWarpsNarrow>(p, plan, grid, block, st);
 }

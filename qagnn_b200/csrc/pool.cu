@@ -24,7 +24,9 @@ __device__ __forceinline__ float xval(__nv_bfloat16 v) { return __bfloat162float
 constexpr int kPoolThreads = 256;  // latency-bound kernel: <= 64 registers so that 4 CTAs (graphs) share an SM
 
 // dynamic smem: qk[nh][D] | logit[nh][n] | xs[nh][D] | cst[nh, padded to 8] | part[warps][nh][D]
-template <typename XT>
+// RAGGED (decoder tail mode only): X and node_type are a ragged batch of N_rows packed rows, graph b's rows start at
+// node_ptr[b]; only its own rows are read, and the positions past them have exact zero weights, as in the padded layout.
+template <typename XT, bool RAGGED = false>
 __global__ void __launch_bounds__(kPoolThreads, 4) attention_pool_kernel(int n, int D, int nh, const XT* __restrict__ X,
                                                                         const float* __restrict__ qs, const unsigned char* __restrict__ mask,
                                                                         const float* __restrict__ wk, const float* __restrict__ bk,
@@ -33,7 +35,8 @@ __global__ void __launch_bounds__(kPoolThreads, 4) attention_pool_kernel(int n, 
                                                                         const int64_t* __restrict__ node_type = nullptr,
                                                                         const int64_t* __restrict__ adj_lengths = nullptr,
                                                                         const float* __restrict__ sent = nullptr, int S = 0,
-                                                                        int pooled_ld = 0) {
+                                                                        int pooled_ld = 0, const int64_t* __restrict__ node_ptr = nullptr,
+                                                                        int64_t N_rows = 0) {
   // mask == nullptr: "decoder tail" mode (modeling_qagnn.py:172-187) — the pool mask is derived here from adj_lengths and
   // node_type, and the row of cat(graph_vecs, sent_vecs, Z) is written in place: pooled -> columns [0, D) of a
   // [B, pooled_ld = 2D+S] buffer, sent_vecs -> [D, D+S), Z = X[b, 0, :] -> [D+S, 2D+S)
@@ -44,16 +47,23 @@ __global__ void __launch_bounds__(kPoolThreads, 4) attention_pool_kernel(int n, 
   float* cst = xs + nh * D;        // [nh]      qs_h·b_k,h
   const int b = blockIdx.x, tid = threadIdx.x, dk = D / nh;
   const float inv_temp = 1.0f / sqrtf((float)dk);
-  const XT* Xb = X + (size_t)b * n * D;
+  int64_t row0 = (int64_t)b * n;
+  int nr = n;  // rows of X that belong to graph b
+  if (RAGGED) {
+    row0 = min(max(node_ptr[b], (int64_t)0), N_rows);
+    nr = (int)min(min((int64_t)n, N_rows - row0), max(node_ptr[b + 1] - row0, (int64_t)0));
+  }
+  const XT* Xb = X + (size_t)row0 * D;
   const bool tail = mask == nullptr;
   if (!tail) pooled_ld = D;
   int len = n;
   bool all_masked = false;
   if (tail) {
     len = (int)min((int64_t)n, max((int64_t)0, adj_lengths[b]));
+    if (RAGGED) nr = min(nr, len);
     // mask = (i >= len) | (type == 3); a fully masked row keeps node 0 (:174-176)
     int any_open = 0;
-    for (int i = tid; i < len; i += kPoolThreads) any_open |= node_type[(size_t)b * n + i] != 3;
+    for (int i = tid; i < (RAGGED ? nr : len); i += kPoolThreads) any_open |= node_type[RAGGED ? row0 + i : (int64_t)b * n + i] != 3;
     all_masked = __syncthreads_or(any_open) == 0;
   }
   // fold the key projection into the query: qk[h][j] = Σ_{r in head h} qs[b, r] * wk[r, j]
@@ -89,7 +99,7 @@ __global__ void __launch_bounds__(kPoolThreads, 4) attention_pool_kernel(int n, 
 #pragma unroll
           for (int c = 0; c < 4; ++c) {
             const int j = j0 + 32 * c + lane;
-            x[r][c] = (i0 + r < n && j < D) ? xval(Xb[(size_t)(i0 + r) * D + j]) : 0.f;
+            x[r][c] = (i0 + r < (RAGGED ? nr : n) && j < D) ? xval(Xb[(size_t)(i0 + r) * D + j]) : 0.f;
           }
 #pragma unroll
         for (int hh = 0; hh < 4; ++hh) {
@@ -108,7 +118,8 @@ __global__ void __launch_bounds__(kPoolThreads, 4) attention_pool_kernel(int n, 
       for (int r = 0; r < 4; ++r) {
         const int i = i0 + r;
         if (i < n) {
-          const bool masked = tail ? ((i >= len || node_type[(size_t)b * n + i] == 3) && !(all_masked && i == 0))
+          const bool masked = tail ? ((i >= (RAGGED ? nr : len) || node_type[RAGGED ? row0 + i : (int64_t)b * n + i] == 3) &&
+                                      !(all_masked && i == 0))
                                    : mask[(size_t)b * n + i] != 0;
 #pragma unroll
           for (int hh = 0; hh < 4; ++hh) {
@@ -157,7 +168,7 @@ __global__ void __launch_bounds__(kPoolThreads, 4) attention_pool_kernel(int n, 
 #pragma unroll
         for (int hh = 0; hh < 4; ++hh) acc[c][hh] = 0.f;
 #pragma unroll 4
-      for (int i = warp; i < n; i += nwarps) {
+      for (int i = warp; i < (RAGGED ? nr : n); i += nwarps) {  // ragged: the positions past nr have weight 0
         float x[4];
 #pragma unroll
         for (int c = 0; c < 4; ++c) {
@@ -211,7 +222,7 @@ __global__ void __launch_bounds__(kPoolThreads, 4) attention_pool_kernel(int n, 
   if (tail) {
     float* row = pooled + (size_t)b * pooled_ld;
     for (int j = tid; j < S; j += kPoolThreads) row[D + j] = sent[(size_t)b * S + j];
-    for (int j = tid; j < D; j += kPoolThreads) row[D + S + j] = xval(Xb[j]);
+    for (int j = tid; j < D; j += kPoolThreads) row[D + S + j] = (!RAGGED || nr > 0) ? xval(Xb[j]) : 0.f;
   }
 }
 
@@ -225,12 +236,13 @@ inline size_t pool_smem_bytes(int n, int D, int nh) {
 
 // Both entry points launch the same kernel, and cudaFuncSetAttribute overwrites the limit rather than raising it, so the
 // limit is set once per device and X type, to the cap, for both of them.
-template <typename XT>
+template <typename XT, bool RAGGED = false>
 int32_t prepare_pool_launch(size_t smem) {
   static bool attr_set[kMaxDevices] = {false};
   const int dev = current_device();
   if (smem > 48 * 1024 && !attr_set[dev]) {
-    QAGNN_CHECK_CUDA(cudaFuncSetAttribute(attention_pool_kernel<XT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPoolSmemCap));
+    QAGNN_CHECK_CUDA(cudaFuncSetAttribute(attention_pool_kernel<XT, RAGGED>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                          (int)kPoolSmemCap));
     attr_set[dev] = true;
   }
   return QAGNN_OK;
@@ -249,6 +261,25 @@ int32_t decoder_tail(int32_t B, int32_t n, int32_t D, int32_t n_head, int32_t S,
   QAGNN_RETURN_IF(prepare_pool_launch<XT>(smem));
   attention_pool_kernel<XT><<<B, kPoolThreads, smem, st>>>(n, D, n_head, X, qs, nullptr, wk, bk, wv, bv, concat, attn, B,
                                                            node_type, adj_lengths, sent_vecs, S, 2 * D + S);
+  QAGNN_CHECK_LAUNCH();
+  return QAGNN_OK;
+}
+
+// decoder_tail on a ragged X [N_rows, D] (graph b's rows start at node_ptr[b])
+template <typename XT>
+int32_t decoder_tail_ragged(int32_t B, int32_t n, int32_t D, int32_t n_head, int32_t S, int64_t N_rows, const XT* X,
+                            const int64_t* node_ptr, const float* qs, const int64_t* node_type, const int64_t* adj_lengths,
+                            const float* sent_vecs, const float* wk, const float* bk, const float* wv, const float* bv,
+                            float* concat, float* attn, cudaStream_t st) {
+  if (B <= 0 || n <= 0 || D <= 0 || n_head <= 0 || D % n_head != 0 || S < 0 || N_rows <= 0) return QAGNN_ERR_INVALID_ARGUMENT;
+  if (n_head > 8) return QAGNN_ERR_UNSUPPORTED;
+  if (!X || !node_ptr || !qs || !node_type || !adj_lengths || !sent_vecs || !wk || !bk || !wv || !bv || !concat || !attn)
+    return QAGNN_ERR_INVALID_ARGUMENT;
+  const size_t smem = pool_smem_bytes(n, D, n_head);
+  if (smem > kPoolSmemCap) return QAGNN_ERR_UNSUPPORTED;
+  QAGNN_RETURN_IF((prepare_pool_launch<XT, true>(smem)));
+  attention_pool_kernel<XT, true><<<B, kPoolThreads, smem, st>>>(n, D, n_head, X, qs, nullptr, wk, bk, wv, bv, concat, attn, B,
+                                                                 node_type, adj_lengths, sent_vecs, S, 2 * D + S, node_ptr, N_rows);
   QAGNN_CHECK_LAUNCH();
   return QAGNN_OK;
 }
@@ -324,8 +355,94 @@ __global__ void __launch_bounds__(256) decoder_head_kernel(int n, int D, const i
   for (int i = tid; i < n; i += 256) scores_out[(size_t)b * n + i] = ((i < len) ? (-sc[i] - s0) : 0.f) / denom;
 }
 
+// decoder_head_kernel for a ragged batch: graph b's first min(adj_lengths[b], n) positions become the packed rows from
+// node_ptr[b] on of H_out [N_rows, D], scores_out [N_rows] and type_out [N_rows] (the loader's node types), with the same
+// values the padded kernel writes there.  The tail rows [node_ptr[B], N_rows) get zeros, type 2 and score 0; CTA b clears rows
+// node_ptr[B] + b, + B, ...
+__global__ void __launch_bounds__(256) decoder_head_ragged_kernel(int n, int D, int64_t N_rows, const int64_t* __restrict__ concept_ids,
+                                                                   int64_t n_concept, const float* __restrict__ table,
+                                                                   const float* __restrict__ ctx, const float* __restrict__ node_scores,
+                                                                   const int64_t* __restrict__ adj_lengths,
+                                                                   const int64_t* __restrict__ node_type,
+                                                                   const int64_t* __restrict__ node_ptr, float* __restrict__ H_out,
+                                                                   float* __restrict__ scores_out, int64_t* __restrict__ type_out) {
+  __shared__ float red[32];
+  __shared__ float s_total;
+  const int b = blockIdx.x, B = gridDim.x, tid = threadIdx.x;
+  const int64_t* cid = concept_ids + (size_t)b * n;
+  const int D4 = D / 4;
+  const int64_t len = adj_lengths[b];
+  const int64_t row0 = min(max(node_ptr[b], (int64_t)0), N_rows);
+  const int rows = (int)min(min((int64_t)n, max(len, (int64_t)0)), N_rows - row0);
+  float* Hb = H_out + (size_t)row0 * D;
+  for (int i = tid; i < rows * D4; i += 256) {
+    const int row = i / D4, c = i - row * D4;
+    const float* srcp;
+    if (row == 0) {
+      srcp = ctx + (size_t)b * D;
+    } else {
+      int64_t id = cid[row] - 1;
+      id = id < 0 ? 0 : (id >= n_concept ? n_concept - 1 : id);
+      srcp = table + (size_t)id * D;
+    }
+    reinterpret_cast<float4*>(Hb + (size_t)row * D)[c] = __ldg(reinterpret_cast<const float4*>(srcp) + c);
+  }
+  const float* sc = node_scores + (size_t)b * n;
+  const float s0 = -sc[0];
+  float part = 0.f;
+  for (int i = tid; i < n; i += 256) part += (i < len) ? fabsf(-sc[i] - s0) : 0.f;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
+  if ((tid & 31) == 0) red[tid >> 5] = part;
+  __syncthreads();
+  if (tid == 0) {
+    float t = 0.f;
+    for (int w = 0; w < 8; ++w) t += red[w];
+    s_total = t;
+  }
+  __syncthreads();
+  const float denom = s_total / (float)len + 1e-05f;
+  for (int i = tid; i < rows; i += 256) {
+    scores_out[row0 + i] = (-sc[i] - s0) / denom;
+    type_out[row0 + i] = node_type[(size_t)b * n + i];
+  }
+  const int64_t t0 = min(max(node_ptr[B], (int64_t)0), N_rows);
+  for (int64_t r = t0 + b; r < N_rows; r += B) {
+    float4* hr = reinterpret_cast<float4*>(H_out + (size_t)r * D);
+    for (int c = tid; c < D4; c += 256) hr[c] = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (tid == 0) { scores_out[r] = 0.f; type_out[r] = 2; }
+  }
+}
+
 }  // namespace
 }  // namespace qagnn
+
+extern "C" int32_t qagnn_decoder_head_ragged(int32_t B, int32_t n, int32_t D, int64_t N_rows, const int64_t* concept_ids,
+                                             int64_t n_concept, const float* table, const float* ctx, const float* node_scores,
+                                             const int64_t* adj_lengths, const int64_t* node_type, const int64_t* node_ptr,
+                                             float* H_out, float* scores_out, int64_t* type_out, void* stream) {
+  if (B <= 0 || n <= 0 || D <= 0 || D % 4 != 0 || n_concept <= 0 || N_rows <= 0) return QAGNN_ERR_INVALID_ARGUMENT;
+  if (!concept_ids || !table || !ctx || !node_scores || !adj_lengths || !node_type || !node_ptr || !H_out || !scores_out || !type_out)
+    return QAGNN_ERR_INVALID_ARGUMENT;
+  qagnn::decoder_head_ragged_kernel<<<B, 256, 0, (cudaStream_t)stream>>>(n, D, N_rows, concept_ids, n_concept, table, ctx,
+                                                                          node_scores, adj_lengths, node_type, node_ptr, H_out,
+                                                                          scores_out, type_out);
+  QAGNN_CHECK_LAUNCH();
+  return QAGNN_OK;
+}
+
+extern "C" int32_t qagnn_decoder_tail_ragged(int32_t x_dtype, int32_t B, int32_t n, int32_t D, int32_t n_head, int32_t S,
+                                             int64_t N_rows, const void* X, const int64_t* node_ptr, const float* qs,
+                                             const int64_t* node_type, const int64_t* adj_lengths, const float* sent_vecs,
+                                             const float* wk, const float* bk, const float* wv, const float* bv, float* concat,
+                                             float* attn, void* stream) {
+  if (x_dtype == QAGNN_DTYPE_F32)
+    return decoder_tail_ragged(B, n, D, n_head, S, N_rows, (const float*)X, node_ptr, qs, node_type, adj_lengths, sent_vecs, wk,
+                               bk, wv, bv, concat, attn, (cudaStream_t)stream);
+  if (x_dtype != QAGNN_DTYPE_BF16) return QAGNN_ERR_INVALID_ARGUMENT;
+  return decoder_tail_ragged(B, n, D, n_head, S, N_rows, (const __nv_bfloat16*)X, node_ptr, qs, node_type, adj_lengths, sent_vecs,
+                             wk, bk, wv, bv, concat, attn, (cudaStream_t)stream);
+}
 
 extern "C" int32_t qagnn_decoder_head(int32_t B, int32_t n, int32_t D, const int64_t* concept_ids, int64_t n_concept,
                                       const float* table, const float* ctx, const float* node_scores,

@@ -22,7 +22,13 @@ class PackedAdj:
 
     Packed with an edge capacity K, edge_index / edge_type are [2, K] / [K]: the batch's `n_edges` = graph_ptr[-1] edges
     fill the first columns and the rest is zero.  Every batch of a split then has the same shapes, and the one-launch
-    graph prep reads the real edge count from graph_ptr on the device (include/qagnn_b200.h, qagnn_graph_prep_packed)."""
+    graph prep reads the real edge count from graph_ptr on the device (include/qagnn_b200.h, qagnn_graph_prep_packed).
+
+    RAGGED (eval only; built by pack_adj / FlatAdjCache.pack given the batch's adj_lengths): graph g's nodes are the rows
+    [node_ptr[g], node_ptr[g+1]) of the batch, node_ptr int64 [n_graphs + 1] = the exclusive cumsum of adj_lengths, and its
+    edge ids are offset by node_ptr[g] instead of g * n_nodes.  `n_nodes` stays the most rows one graph may have (the loader's
+    max_node_num) and `node_capacity` N_cap is the number of rows of every node array of the batch: rows >= node_ptr[-1] are
+    unused.  The modules take such a batch in .eval() with node arrays of N_cap rows and no padding."""
     edge_index: torch.Tensor
     edge_type: torch.Tensor
     graph_ptr: torch.Tensor
@@ -34,18 +40,29 @@ class PackedAdj:
     n_edges: int = -1                    # edges of the batch = graph_ptr[-1] (host value; -1 = unknown)
     edge_capacity: int = -1              # width of edge_index (host value; -1 = unknown)
 
+    node_ptr: torch.Tensor = None        # ragged batches: first row of every graph, int64 [n_graphs + 1] (host)
+    node_ptr_dev: torch.Tensor = None    # node_ptr on the device of edge_index
+    node_capacity: int = -1              # ragged batches: rows of every node array (N_cap)
+
+    @property
+    def ragged(self):
+        return self.node_ptr is not None or self.node_ptr_dev is not None
+
     def to(self, device, non_blocking=True):
-        gp = self.graph_ptr
-        if torch.cuda.is_available() and torch.device(device).type == "cuda" and not gp.is_cuda and not gp.is_pinned():
-            gp = gp.pin_memory()
-        gpd = gp.to(device, non_blocking=non_blocking)
+        def up(t):
+            if torch.cuda.is_available() and torch.device(device).type == "cuda" and not t.is_cuda and not t.is_pinned():
+                t = t.pin_memory()
+            return t.to(device, non_blocking=non_blocking)
+        gpd = up(self.graph_ptr)
+        npd = up(self.node_ptr) if self.node_ptr is not None else self.node_ptr_dev
         me = self.max_edges if self.max_edges >= 0 else (int((self.graph_ptr[1:] - self.graph_ptr[:-1]).max()) if self.graph_ptr.numel() > 1 else 0)
         if self.buf is not None:
             b = self.buf.to(device, non_blocking=non_blocking)
-            return PackedAdj(b[:2], b[2], self.graph_ptr, self.n_nodes, b, gpd, me, self.n_edges, self.edge_capacity)
+            return PackedAdj(b[:2], b[2], self.graph_ptr, self.n_nodes, b, gpd, me, self.n_edges, self.edge_capacity,
+                             self.node_ptr, npd, self.node_capacity)
         return PackedAdj(self.edge_index.to(device, non_blocking=non_blocking),
                          self.edge_type.to(device, non_blocking=non_blocking), self.graph_ptr, self.n_nodes, None, gpd, me,
-                         self.n_edges, self.edge_capacity)
+                         self.n_edges, self.edge_capacity, self.node_ptr, npd, self.node_capacity)
 
     # LM_QAGNN.forward slices inputs positionally and calls .size() only on tensors before the last two; everywhere an
     # (edge_index, edge_type) pair is expected a PackedAdj unpacks / indexes as that pair
@@ -68,23 +85,64 @@ def _capacity(total, edge_capacity):
     return int(edge_capacity)
 
 
-def pack_adj(edge_index_nested, edge_type_nested, n_nodes, pin=True, edge_capacity=None):
+def node_ptr_of(adj_lengths, n_nodes, n_graphs):
+    """node_ptr int64 [n_graphs + 1] = the exclusive cumsum of a batch's adj_lengths (any shape, one entry per graph); raises
+    ValueError for a length outside [1, n_nodes]."""
+    lens = torch.as_tensor(adj_lengths).reshape(-1).to("cpu", torch.long)
+    if lens.numel() != n_graphs:
+        raise ValueError(f"adj_lengths has {lens.numel()} entries for {n_graphs} graphs")
+    if n_graphs and (int(lens.min()) < 1 or int(lens.max()) > n_nodes):
+        raise ValueError(f"adj_lengths must lie in [1, {n_nodes}] (got {int(lens.min())}..{int(lens.max())})")
+    ptr = torch.zeros(n_graphs + 1, dtype=torch.long)
+    ptr[1:] = torch.cumsum(lens, 0)
+    return ptr
+
+
+def _node_capacity(total, node_capacity):
+    """Rows of a ragged batch's node arrays; raises before anything is copied when the batch does not fit."""
+    if node_capacity is None:
+        return total
+    if int(node_capacity) < total:
+        raise ValueError(f"batch has {total} nodes, more than the node capacity {int(node_capacity)}")
+    return int(node_capacity)
+
+
+def split_node_capacity(adj_lengths, batch_size):
+    """Node capacity of a ragged split read in a FIXED batch order (dev and test splits are not shuffled): the largest
+    sum(adj_lengths) over its batches of `batch_size` questions.  adj_lengths is the split's [Q, num_choice] (or [Q]) tensor.  A
+    bound that held under any shuffle would be close to batch_size * num_choice * n and save nothing."""
+    lens = torch.as_tensor(adj_lengths).to("cpu", torch.long)
+    lens = lens.reshape(lens.size(0), -1).sum(1)
+    return max((int(lens[a:a + batch_size].sum()) for a in range(0, lens.numel(), int(batch_size))), default=0)
+
+
+def pack_adj(edge_index_nested, edge_type_nested, n_nodes, pin=True, edge_capacity=None, adj_lengths=None, node_capacity=None):
     """[batch][num_choice] nested lists (load_sparse_adj_data_with_contextnode format,
     utils/data_utils.py:189-190) -> PackedAdj, equal to LM_QAGNN.batch_graph's output.  With `edge_capacity` K the edges
-    go into one pinned [3, K] buffer with a zero tail (ValueError if the batch has more than K edges)."""
+    go into one pinned [3, K] buffer with a zero tail (ValueError if the batch has more than K edges).
+
+    With the batch's `adj_lengths` the PackedAdj is RAGGED (see PackedAdj): node ids are offset by node_ptr[g] and the node
+    arrays have `node_capacity` rows (default: the batch's node count; ValueError if the batch has more)."""
     flat_ei = [e for row in edge_index_nested for e in row] if isinstance(edge_index_nested[0], (list, tuple)) else list(edge_index_nested)
     flat_et = [e for row in edge_type_nested for e in row] if isinstance(edge_type_nested[0], (list, tuple)) else list(edge_type_nested)
     counts = torch.tensor([e.size(1) for e in flat_ei], dtype=torch.long)
     graph_ptr = torch.zeros(len(flat_ei) + 1, dtype=torch.long)
     graph_ptr[1:] = torch.cumsum(counts, 0)
     total = int(graph_ptr[-1])
-    if edge_capacity is not None:
+    node_ptr, n_cap = None, -1
+    offsets = torch.arange(len(flat_ei)) * n_nodes
+    if adj_lengths is not None:
+        node_ptr = node_ptr_of(adj_lengths, n_nodes, len(flat_ei))
+        n_cap = _node_capacity(int(node_ptr[-1]), node_capacity)
+        offsets = node_ptr[:-1]
+    if edge_capacity is not None or node_ptr is not None:
         K = _capacity(total, edge_capacity)
         buf = torch.zeros(3, K, dtype=torch.long, pin_memory=pin and torch.cuda.is_available())
         if total:
-            buf[:2, :total] = torch.cat(flat_ei, dim=1) + torch.repeat_interleave(torch.arange(len(flat_ei)) * n_nodes, counts)
+            buf[:2, :total] = torch.cat(flat_ei, dim=1) + torch.repeat_interleave(offsets, counts)
             buf[2, :total] = torch.cat(flat_et, dim=0)
-        return PackedAdj(buf[:2], buf[2], graph_ptr, n_nodes, buf, n_edges=total, edge_capacity=K)
+        return PackedAdj(buf[:2], buf[2], graph_ptr, n_nodes, buf, n_edges=total, edge_capacity=K, node_ptr=node_ptr,
+                         node_capacity=n_cap)
     edge_index = torch.empty(2, total, dtype=torch.long, pin_memory=pin and torch.cuda.is_available())
     edge_type = torch.empty(total, dtype=torch.long, pin_memory=pin and torch.cuda.is_available())
     if total:
@@ -278,10 +336,11 @@ class FlatAdjCache:
             return range(self.n_questions())
         raise IndexError("FlatAdjCache stands in for the (edge_index, edge_type) pair: index 0 or 1")
 
-    def pack(self, question_indexes, pin=True, edge_capacity=None):
+    def pack(self, question_indexes, pin=True, edge_capacity=None, adj_lengths=None, node_capacity=None):
         """PackedAdj of the questions `question_indexes` (all their choices, in order) — equal to
         LM_QAGNN.batch_graph applied to the corresponding nested-list slice (modeling_qagnn.py:244-251).  With
-        `edge_capacity` K the buffer is [3, K] with a zero tail (ValueError if the batch has more than K edges)."""
+        `edge_capacity` K the buffer is [3, K] with a zero tail (ValueError if the batch has more than K edges).  With the
+        batch's `adj_lengths` ([bs, num_choice]) the PackedAdj is ragged at `node_capacity` rows, as in pack_adj."""
         q = np.asarray(question_indexes, dtype=np.int64).reshape(-1)
         gids = (q[:, None] * self.num_choice + np.arange(self.num_choice)[None, :]).reshape(-1)
         beg, end = self.graph_ptr[gids], self.graph_ptr[gids + 1]
@@ -290,16 +349,22 @@ class FlatAdjCache:
         ptr[1:] = np.cumsum(counts)
         total = int(ptr[-1])
         K = _capacity(total, edge_capacity)
+        node_ptr, n_cap = None, -1
+        if adj_lengths is not None:
+            node_ptr = node_ptr_of(adj_lengths, self.n_nodes, len(gids))
+            n_cap = _node_capacity(int(node_ptr[-1]), node_capacity)
         # flat positions of every edge of the batch: beg[g] + (0 .. counts[g]-1)
         pos = np.repeat(beg - ptr[:-1], counts) + np.arange(total, dtype=np.int64)
-        off = np.repeat(np.arange(len(gids), dtype=np.int64) * self.n_nodes, counts)
+        first = node_ptr[:-1].numpy() if node_ptr is not None else np.arange(len(gids), dtype=np.int64) * self.n_nodes
+        off = np.repeat(first, counts)
         buf = torch.empty(3, K, dtype=torch.long, pin_memory=pin and torch.cuda.is_available())
         b = buf.numpy()
         np.add(self.src[pos], off, out=b[0, :total], casting="unsafe")
         np.add(self.tgt[pos], off, out=b[1, :total], casting="unsafe")
         b[2, :total] = self.etype[pos]
         b[:, total:] = 0
-        return PackedAdj(buf[:2], buf[2], torch.from_numpy(ptr), self.n_nodes, buf, n_edges=total, edge_capacity=K)
+        return PackedAdj(buf[:2], buf[2], torch.from_numpy(ptr), self.n_nodes, buf, n_edges=total, edge_capacity=K,
+                         node_ptr=node_ptr, node_capacity=n_cap)
 
 
 def load_flat_adj_cache(adj_pk_path, max_node_num, num_choice, args=None):

@@ -117,6 +117,32 @@ class MultiheadAttPoolLayer(nn.Module):
         _lib.check(st, "qagnn_decoder_tail")
         return concat, attn
 
+    def pool_concat_ragged(self, q, k, node_ptr, node_type, adj_lengths, n):
+        """pool_concat on a ragged batch (qagnn_decoder_tail_ragged): k [N_cap, D] and node_type [N_cap] are packed rows, graph b's
+        from node_ptr[b] (device int64 [b + 1]); returns (concat [b, 2D + S], attn [n_head*b, n]) with attn exactly 0 at
+        positions >= adj_lengths[b].  Raises where pool_concat would return None: there is no padded fallback."""
+        from . import _lib
+        if self.training or not k.is_cuda or k.dtype not in _POOL_X_DTYPES:
+            raise ValueError("pool_concat_ragged: eval mode and a CUDA fp32 / bf16 k only")
+        lib = _lib.load()
+        N_cap, D = k.shape
+        b, S = q.size(0), q.size(1)
+        qc = _lib.f32c(q, "q")
+        qs = self.w_qs(qc).detach().float().contiguous()
+        kc = k.detach().contiguous()
+        concat = torch.empty(b, 2 * D + S, dtype=torch.float32, device=k.device)
+        attn = torch.empty(self.n_head * b, n, dtype=torch.float32, device=k.device)
+        with torch.cuda.device(k.device):
+            st = lib.qagnn_decoder_tail_ragged(_lib.DTYPE_CODES[kc.dtype], b, n, D, self.n_head, S, N_cap, _lib.ptr(kc),
+                                               _lib.ptr(_lib.i64c(node_ptr, "node_ptr")), _lib.ptr(qs),
+                                               _lib.ptr(_lib.i64c(node_type, "node_type")),
+                                               _lib.ptr(_lib.i64c(adj_lengths, "adj_lengths")), _lib.ptr(qc),
+                                               _lib.ptr(self.w_ks.weight.detach()), _lib.ptr(self.w_ks.bias.detach()),
+                                               _lib.ptr(self.w_vs.weight.detach()), _lib.ptr(self.w_vs.bias.detach()),
+                                               _lib.ptr(concat), _lib.ptr(attn), _lib.stream_ptr(k.device))
+        _lib.check(st, "qagnn_decoder_tail_ragged")
+        return concat, attn
+
     def forward(self, q, k, mask=None):
         b, l, _ = k.shape
         nh, dk, dv = self.n_head, self.d_k, self.d_v

@@ -67,11 +67,12 @@ class _DeviceBlob:
 
 
 CROSS_GRAPH = 8  # graph prep status bit: an edge crosses a sub-graph boundary
+NODE_PTR = 32    # graph prep status bit: a ragged batch's node_ptr is not monotone, has a graph over n rows or ends past N
 
 
 class GraphPrepIndexError(IndexError):
     """Indices a validating graph prep found out of range.  `bits` is its status word: 1 edge_index, 2 edge_type,
-    4 node_type, CROSS_GRAPH, 16 graph_ptr disagreeing with the edges or with max_edges."""
+    4 node_type, CROSS_GRAPH, 16 graph_ptr disagreeing with the edges or with max_edges, NODE_PTR."""
 
     def __init__(self, bits):
         super().__init__(f"qagnn_graph_prep: index out of range (status bits {bits})")
@@ -82,12 +83,15 @@ class GraphPrep:
     """Owns the opaque graph-prep workspace of one batched graph (qagnn_graph_prep)."""
 
     def __init__(self, edge_index, edge_type, node_type, n_ntype, n_etype, n_per_graph=0, validate=True, graph_ptr=None,
-                 max_edges=-1):
+                 max_edges=-1, node_ptr=None):
         """graph_ptr (device int64 [n_graphs + 1]) + max_edges (host int): the batch is PACKED graph by graph — the whole
         prep is then one kernel launch (qagnn_graph_prep_packed) instead of twelve.  edge_index may then be an edge
         capacity wider than the batch: the real count graph_ptr[-1] is read on the device.  That prep raises QagnnError
         with status -5 when it refuses the shape (sub-graphs too large for one CTA).  Without graph_ptr every column of
-        edge_index is an edge.  A validating prep raises GraphPrepIndexError.  graph_prep() picks which prep a batch gets."""
+        edge_index is an edge.  A validating prep raises GraphPrepIndexError.  graph_prep() picks which prep a batch gets.
+
+        node_ptr (device int64 [n_graphs + 1], with graph_ptr): a RAGGED batch (qagnn_graph_prep_ragged): graph g owns the rows
+        [node_ptr[g], node_ptr[g+1]) of the node_type.numel() rows and n_per_graph bounds its rows."""
         lib = _lib.load()
         ei = _lib.i64c(edge_index, "edge_index")
         et = _lib.i64c(edge_type, "edge_type")
@@ -103,10 +107,20 @@ class GraphPrep:
         self._combo = None
         # built by qagnn_graph_prep_packed: the edge columns past graph_ptr[-1] are unused
         self.packed = graph_ptr is not None and max_edges >= 0 and self.n_per_graph > 0
+        self.node_ptr = node_ptr if self.packed else None
+        self.n_graphs = 0
         shape = _lib.Shape(self.N, self.E, 4, 1, n_ntype, n_etype, 0, self.n_per_graph)
         eptr, tptr = (_lib.ptr(ei), _lib.ptr(et)) if self.E else (None, None)
         with torch.cuda.device(self.device):
-            if self.packed:
+            if self.node_ptr is not None:
+                gp, npt = _lib.i64c(graph_ptr, "graph_ptr"), _lib.i64c(node_ptr, "node_ptr")
+                if gp.numel() != npt.numel() or gp.numel() < 2:
+                    raise ValueError("graph_ptr and node_ptr must both have one entry per graph plus one")
+                self.n_graphs = gp.numel() - 1
+                st = lib.qagnn_graph_prep_ragged(eptr, tptr, _lib.ptr(nt), _lib.ptr(gp), _lib.ptr(npt), self.n_graphs,
+                                                 int(max_edges), C.byref(shape), _lib.ptr(self.buf), self.buf.numel(),
+                                                 int(bool(validate)), _lib.stream_ptr(self.device))
+            elif self.packed:
                 gp = _lib.i64c(graph_ptr, "graph_ptr")
                 if gp.numel() != self.N // self.n_per_graph + 1:
                     raise ValueError("graph_ptr must have one entry per sub-graph plus one")
@@ -118,8 +132,9 @@ class GraphPrep:
                                           int(bool(validate)), _lib.stream_ptr(self.device))
         if st == -3:  # the validating prep has synchronised: its status word says which check failed
             raise GraphPrepIndexError(int(self.status_word().item()))
-        _lib.check(st, "qagnn_graph_prep_packed" if self.packed else "qagnn_graph_prep")
-        self._keep = (ei, et, nt, graph_ptr)
+        _lib.check(st, "qagnn_graph_prep_ragged" if self.node_ptr is not None else
+                   "qagnn_graph_prep_packed" if self.packed else "qagnn_graph_prep")
+        self._keep = (ei, et, nt, graph_ptr, node_ptr)
 
     def real_edges(self):
         """Edges of the batch (self loops excluded).  Below E only for a packed prep on an edge capacity; read from the
@@ -191,6 +206,18 @@ def graph_prep(A, node_type, n, n_ntype, n_etype, validate):
         the batch goes to the general CSR kernels."""
     ei, et, nt = A[0], A[1], node_type.reshape(-1)
     gp = getattr(A, "graph_ptr_dev", None)
+    if getattr(A, "ragged", False):
+        # a ragged batch has no padded layout to fall back to: an edge outside its graph's rows is an error
+        if A.node_ptr_dev is None or gp is None or A.max_edges < 0:
+            raise ValueError("a ragged PackedAdj must be on the device (PackedAdj.to) with graph_ptr and max_edges")
+        try:
+            return GraphPrep(ei, et, nt, n_ntype, n_etype, A.n_nodes, validate, graph_ptr=gp, max_edges=A.max_edges,
+                             node_ptr=A.node_ptr_dev)
+        except _lib.QagnnError as e:
+            if e.status == -5:  # QAGNN_ERR_UNSUPPORTED
+                raise ValueError(f"ragged batch: graphs of {A.n_nodes} nodes and {A.max_edges} edges do not fit the one-CTA "
+                                 "graph prep; run this batch padded") from e
+            raise
     if gp is not None:
         if n > 0 and A.n_nodes == n and A.max_edges >= 0:
             try:
@@ -212,6 +239,13 @@ def graph_prep(A, node_type, n, n_ntype, n_etype, validate):
         if n == 0 or e.bits != CROSS_GRAPH:
             raise
     return GraphPrep(ei, et, nt, n_ntype, n_etype, 0, validate)
+
+
+def _ragged_eval_only(module, what, *tensors):
+    """A ragged batch runs the eval forward only: the reference's training BatchNorm statistics include the padded rows."""
+    if module.training or (torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in tensors)):
+        raise ValueError(f"{what}: a ragged batch runs in .eval() without gradients only; training keeps the padded layout "
+                         "because BatchNorm batch statistics include the padded rows")
 
 
 def _edge_encoder_params(enc):
@@ -312,6 +346,8 @@ class GATConvE(nn.Module):
         gp = getattr(edge_index, "graph_ptr_dev", None)
         if gp is not None:  # a qagnn_b200.data.PackedAdj: one-launch packed prep
             A, n, srcs = edge_index, edge_index.n_nodes, [edge_index.edge_index, edge_index.edge_type, node_type, gp]
+            if edge_index.ragged:
+                srcs.append(edge_index.node_ptr_dev)
         else:
             A, n, srcs = (edge_index, edge_type), 0, [edge_index, edge_type, node_type]
         key = _version_key(srcs)
@@ -325,7 +361,9 @@ class GATConvE(nn.Module):
         Returns out [N, emb_dim], or (out, (edge_index' [2,E+N], alpha [E+N, heads])) with
         return_attention_weights=True (alpha = softmax before the out-degree rescale, :473).  edge_index may be a
         qagnn_b200.data.PackedAdj (edge_type is then ignored), also one packed at an edge capacity: E is then its real
-        edge count."""
+        edge count.  A ragged PackedAdj (eval only) takes x / node_feature_extra [N_cap, emb_dim] and node_type [N_cap]."""
+        if getattr(edge_index, "ragged", False):
+            _ragged_eval_only(self, "GATConvE", x, node_feature_extra)
         if self.training:  # dropout-free layer, BatchNorm batch statistics, autograd through the CUDA message passing
             from . import training as TR
             if prep is None:
@@ -356,10 +394,16 @@ class GATConvE(nn.Module):
         alpha = torch.empty(N + prep.E, self.head_count, dtype=torch.float32, device=dev) if return_attention_weights else None
         aggr = torch.empty(N, D, dtype=torch.float32, device=dev) if return_aggr else None
         with torch.cuda.device(dev):
-            st = lib.qagnn_gatconve_forward_typed(C.byref(shape), _lib.DTYPE_CODES[dt], _lib.DTYPE_CODES[xc.dtype], 0,
-                                                  _lib.ptr(xc), _lib.ptr(ex),
-                                                  _lib.ptr(prep.buf), _lib.ptr(folded), _lib.ptr(out), _lib.ptr(alpha),
-                                                  _lib.ptr(aggr), _lib.ptr(ws), ws.numel(), _lib.stream_ptr(dev))
+            if prep.node_ptr is not None:
+                st = lib.qagnn_gatconve_forward_ragged(C.byref(shape), _lib.DTYPE_CODES[dt], _lib.DTYPE_CODES[xc.dtype],
+                                                       prep.n_graphs, _lib.ptr(prep.node_ptr), 0, _lib.ptr(xc), _lib.ptr(ex),
+                                                       _lib.ptr(prep.buf), _lib.ptr(folded), _lib.ptr(out), _lib.ptr(alpha),
+                                                       _lib.ptr(aggr), _lib.ptr(ws), ws.numel(), _lib.stream_ptr(dev))
+            else:
+                st = lib.qagnn_gatconve_forward_typed(C.byref(shape), _lib.DTYPE_CODES[dt], _lib.DTYPE_CODES[xc.dtype], 0,
+                                                      _lib.ptr(xc), _lib.ptr(ex),
+                                                      _lib.ptr(prep.buf), _lib.ptr(folded), _lib.ptr(out), _lib.ptr(alpha),
+                                                      _lib.ptr(aggr), _lib.ptr(ws), ws.numel(), _lib.stream_ptr(dev))
         _lib.check(st, "qagnn_gatconve_forward_typed")
         self._alpha = None
         res = out
@@ -463,7 +507,13 @@ class QAGNN_Message_Passing(nn.Module):
         node_type: long tensor (batch_size, n_node): 0 question entity, 1 answer entity, 2 other, 3 context
         node_score: tensor (batch_size, n_node, 1)
         returns (batch_size, n_node, d_node)
+
+        With A a ragged qagnn_b200.data.PackedAdj (eval only): H [N_cap, d_node], node_type [N_cap], node_score [N_cap, 1],
+        one row per node of the batch (rows past A.node_ptr[-1] unused); returns [N_cap, d_node].
         """
+        ragged = getattr(A, "ragged", False)
+        if ragged:
+            _ragged_eval_only(self, "QAGNN_Message_Passing", H, node_score)
         for status in self._replayed:  # never waits for the GPU: a replay whose copy has not landed is looked at later
             status.check("QAGNN_Message_Passing")
         self._replayed = [s for s in self._replayed if s.pending is not None]
@@ -480,6 +530,10 @@ class QAGNN_Message_Passing(nn.Module):
         lib = _lib.load()
         # under bf16 autocast: bf16 in and out, single-pass bf16 GEMMs (include/qagnn_b200.h, qagnn_mp_forward_typed)
         Hc, dt = _lib.eval_dtype(H, "H")
+        if ragged:
+            if Hc.dim() != 2 or Hc.size(1) != self.hidden_size:
+                raise ValueError("H of a ragged batch must be [node_capacity, hidden_size]")
+            Hc = Hc.unsqueeze(0)
         if Hc.dim() != 3 or Hc.size(2) != self.hidden_size:
             raise ValueError("H must be [batch, n_node, hidden_size]")
         B, n, D = Hc.shape
@@ -500,10 +554,18 @@ class QAGNN_Message_Passing(nn.Module):
         out = torch.empty(B, n, D, dtype=dt, device=dev)
         layers = torch.empty(self.k, B * n, D, dtype=torch.float32, device=dev) if return_layers else None
         with torch.cuda.device(dev):
-            st = lib.qagnn_mp_forward_typed(C.byref(shape), _lib.DTYPE_CODES[dt], _lib.DTYPE_CODES[Hc.dtype], _lib.ptr(Hc),
-                                            _lib.ptr(nt), _lib.ptr(sc), _lib.ptr(prep.buf), _lib.ptr(folded), _lib.ptr(out),
-                                            _lib.ptr(layers), _lib.ptr(ws), ws.numel(), _lib.stream_ptr(dev))
+            if prep.node_ptr is not None:
+                st = lib.qagnn_mp_forward_ragged(C.byref(shape), _lib.DTYPE_CODES[dt], _lib.DTYPE_CODES[Hc.dtype], prep.n_graphs,
+                                                 _lib.ptr(prep.node_ptr), _lib.ptr(Hc), _lib.ptr(nt), _lib.ptr(sc),
+                                                 _lib.ptr(prep.buf), _lib.ptr(folded), _lib.ptr(out), _lib.ptr(layers),
+                                                 _lib.ptr(ws), ws.numel(), _lib.stream_ptr(dev))
+            else:
+                st = lib.qagnn_mp_forward_typed(C.byref(shape), _lib.DTYPE_CODES[dt], _lib.DTYPE_CODES[Hc.dtype], _lib.ptr(Hc),
+                                                _lib.ptr(nt), _lib.ptr(sc), _lib.ptr(prep.buf), _lib.ptr(folded), _lib.ptr(out),
+                                                _lib.ptr(layers), _lib.ptr(ws), ws.numel(), _lib.stream_ptr(dev))
         _lib.check(st, "qagnn_mp_forward_typed")
+        if ragged:
+            out = out[0]
         if return_layers:
             return out, layers
         return out
@@ -515,6 +577,8 @@ class QAGNN_Message_Passing(nn.Module):
         tensors = [H, A[0], A[1], node_type, node_score]
         if getattr(A, "graph_ptr_dev", None) is not None:
             tensors.append(A.graph_ptr_dev)
+        if getattr(A, "ragged", False):
+            tensors.append(A.node_ptr_dev)
         # the autocast dtype selects the kernels and the output dtype: an fp32 capture must not replay under bf16 autocast
         key = (tuple((t.data_ptr(), tuple(t.shape), t.dtype) for t in tensors),
                _version_key(list(self.parameters()) + list(self.buffers())), _lib.autocast_dtype())
@@ -572,6 +636,9 @@ class QAGNN(nn.Module):
                         cache_output=False):
         """Everything up to (and excluding) the answer MLP: returns (concat [B, 2*concept_dim+sent_dim], pool_attn).
         Split out so a data-parallel caller can all-gather `concat` before `fc` (qagnn_b200.distributed)."""
+        if getattr(adj, "ragged", False):
+            return self._pooled_features_ragged(sent_vecs, concept_ids, node_type_ids, node_scores, adj_lengths, adj, emb_data,
+                                                cache_output)
         n = node_scores.size(1)
         pos = torch.arange(n, device=node_scores.device)
         fused_head = (not self.training and not torch.is_grad_enabled() and emb_data is None and node_scores.is_cuda
@@ -619,6 +686,42 @@ class QAGNN(nn.Module):
         if cache_output:
             self.concept_ids, self.adj, self.pool_attn = concept_ids, adj, pool_attn
         concat = self.dropout_fc(torch.cat((graph_vecs, sent_vecs, Z_vecs), 1))
+        return concat, pool_attn
+
+    def _pooled_features_ragged(self, sent_vecs, concept_ids, node_type_ids, node_scores, adj_lengths, adj, emb_data,
+                                cache_output):
+        """pooled_features on a ragged PackedAdj (eval): the head writes only the valid positions of the padded [B, n] inputs
+        as packed rows (qagnn_decoder_head_ragged), the message passing runs on adj.node_capacity rows and the tail pools each
+        graph over its own rows (qagnn_decoder_tail_ragged); `pool_attn` keeps the padded [n_head*B, n] layout."""
+        _ragged_eval_only(self, "QAGNN", sent_vecs, node_scores)
+        if (emb_data is not None or not node_scores.is_cuda or self.concept_emb.use_contextualized or self.concept_dim % 4 != 0
+                or concept_ids.device != node_scores.device or sent_vecs.dtype != torch.float32):
+            raise ValueError("QAGNN: a ragged batch needs the fused decoder head (CUDA inputs, fp32 sent_vecs, no contextualized "
+                             "embeddings, concept_dim % 4 == 0)")
+        lib = _lib.load()
+        B_, n = concept_ids.shape
+        N_cap = adj.node_capacity
+        dev = node_scores.device
+        table = self.concept_emb.projected_table()
+        ctx = self.activation(self.svec2nvec(sent_vecs)).float().contiguous()
+        node_ptr = _lib.i64c(adj.node_ptr_dev, "node_ptr")
+        if node_ptr.numel() != B_ + 1 or N_cap <= 0:
+            raise ValueError("ragged PackedAdj: node_ptr must have one entry per graph plus one and node_capacity be set")
+        gnn_input = torch.empty(N_cap, self.concept_dim, dtype=torch.float32, device=dev)
+        s = torch.empty(N_cap, dtype=torch.float32, device=dev)
+        nt = torch.empty(N_cap, dtype=torch.int64, device=dev)
+        al = _lib.i64c(adj_lengths, "adj_lengths")
+        with torch.cuda.device(dev):
+            st = lib.qagnn_decoder_head_ragged(B_, n, self.concept_dim, N_cap, _lib.ptr(_lib.i64c(concept_ids, "concept_ids")),
+                                               table.size(0), _lib.ptr(table), _lib.ptr(ctx),
+                                               _lib.ptr(_lib.f32c(node_scores.reshape(B_, n), "node_scores")), _lib.ptr(al),
+                                               _lib.ptr(_lib.i64c(node_type_ids, "node_type_ids")), _lib.ptr(node_ptr),
+                                               _lib.ptr(gnn_input), _lib.ptr(s), _lib.ptr(nt), _lib.stream_ptr(dev))
+        _lib.check(st, "qagnn_decoder_head_ragged")
+        gnn_output = self.gnn(gnn_input, adj, nt, s.unsqueeze(1))
+        concat, pool_attn = self.pooler.pool_concat_ragged(sent_vecs, gnn_output, node_ptr, nt, adj_lengths, n)
+        if cache_output:
+            self.concept_ids, self.adj, self.pool_attn = concept_ids, adj, pool_attn
         return concat, pool_attn
 
     def forward(self, sent_vecs, concept_ids, node_type_ids, node_scores, adj_lengths, adj, emb_data=None,

@@ -106,9 +106,12 @@ class DecoderStep:
 
     FIELDS = ("H", "edge_index", "edge_type", "node_type", "node_score", "sent_vecs", "adj_lengths")
     PACKED_FIELDS = FIELDS + ("graph_ptr",)  # + first edge of every sub-graph, int64 [B + 1] (packed batches)
+    # ragged batches: the packed fields with H [N_cap, D], node_type [N_cap] and node_score [N_cap, 1] holding one row per node
+    # (qagnn_b200.data.PackedAdj with node_ptr); node_ptr itself is rebuilt from adj_lengths on the device in every run
+    RAGGED_FIELDS = PACKED_FIELDS
 
     def __init__(self, gnn, pooler, fc, inputs, world_size=1, group=None, use_cuda_graph=True, max_edges=-1,
-                 autocast_dtype=None):
+                 autocast_dtype=None, max_nodes=None):
         """`autocast_dtype` (None or torch.bfloat16) runs capture and calls under torch.autocast(cache_enabled=False): the
         message passing then runs its bf16 forward (single-pass bf16 GEMMs, `gnn_out` bf16) and the pooling reads that output
         directly.
@@ -118,21 +121,42 @@ class DecoderStep:
         edge_index / edge_type may then be an edge capacity K wider than any batch (qagnn_b200.data.PackedAdj): the real
         edge count is read from graph_ptr on the device, so one capture serves every batch of a split that fits K and
         `max_edges`.  A capture raises ValueError if the packed prep refuses the shape, since the general prep would freeze
-        the edge count of the batch it was captured on."""
+        the edge count of the batch it was captured on.
+
+        A RAGGED step (inputs with 2-D H, RAGGED_FIELDS) runs the batch without padding rows: the node arrays have N_cap =
+        H.size(0) rows (qagnn_b200.data.split_node_capacity), graph b's from node_ptr[b] = sum(adj_lengths[:b]) on, and
+        `max_nodes` n bounds one graph's rows (the loader's max_node_num; `pool_attn` is [n_head*B, n]).  node_ptr is rebuilt
+        from adj_lengths on the device in every run, so one capture at N_cap and the edge capacity serves every full batch of a
+        split.  `gnn_out` is then [N_cap, D].  Single GPU only."""
         if autocast_dtype not in (None, torch.bfloat16):
             raise ValueError("autocast_dtype must be None or torch.bfloat16")
         self.gnn, self.pooler, self.fc = gnn, pooler, fc
         self.autocast_dtype = autocast_dtype
         self.inp = {k: inputs[k] for k in self.FIELDS}
         self.adj = (self.inp["edge_index"], self.inp["edge_type"])
-        if "graph_ptr" in inputs and max_edges >= 0:
+        self.ragged = self.inp["H"].dim() == 2
+        self._node_ptr = None
+        if self.ragged:
+            if world_size > 1:
+                raise ValueError("DecoderStep: ragged batches run on one GPU (world_size == 1)")
+            if "graph_ptr" not in inputs or max_edges < 0 or max_nodes is None:
+                raise ValueError("DecoderStep: a ragged step needs inputs['graph_ptr'], max_edges and max_nodes")
+            from .data import PackedAdj
+            self.inp["graph_ptr"] = inputs["graph_ptr"]
+            al = self.inp["adj_lengths"]
+            self._node_ptr = torch.zeros(al.numel() + 1, dtype=torch.int64, device=al.device)
+            self._update_node_ptr()
+            self.adj = PackedAdj(self.inp["edge_index"], self.inp["edge_type"], None, int(max_nodes), None,
+                                 self.inp["graph_ptr"], int(max_edges), -1, self.inp["edge_index"].size(1), None,
+                                 self._node_ptr, self.inp["H"].size(0))
+        elif "graph_ptr" in inputs and max_edges >= 0:
             from .data import PackedAdj
             self.inp["graph_ptr"] = inputs["graph_ptr"]
             self.adj = PackedAdj(self.inp["edge_index"], self.inp["edge_type"], None, self.inp["H"].size(1), None,
                                  self.inp["graph_ptr"], int(max_edges), -1, self.inp["edge_index"].size(1))
         self.world, self.group = world_size, group
         dev = self.inp["H"].device
-        B, n, D = self.inp["H"].shape
+        B, D = self.inp["sent_vecs"].size(0), self.inp["H"].size(-1)
         S = self.inp["sent_vecs"].size(1)
         self.full = torch.empty(world_size * B, 2 * D + S, device=dev) if world_size > 1 else None
         self.graph = None
@@ -152,8 +176,17 @@ class DecoderStep:
         with self._autocast():
             return self._eager_body()
 
+    def _update_node_ptr(self):
+        torch.cumsum(self.inp["adj_lengths"], 0, out=self._node_ptr[1:])
+
     def _eager_body(self):
         d = self.inp
+        if self.ragged:
+            self._update_node_ptr()
+            out = self.gnn(d["H"], self.adj, d["node_type"], d["node_score"])
+            concat, pool_attn = self.pooler.pool_concat_ragged(d["sent_vecs"], out, self._node_ptr, d["node_type"],
+                                                               d["adj_lengths"], self.adj.n_nodes)
+            return self.fc(concat), pool_attn, out
         out = self.gnn(d["H"], self.adj, d["node_type"], d["node_score"])
         fused = self.pooler.pool_concat(d["sent_vecs"], out, d["node_type"], d["adj_lengths"])  # :172-187 in one kernel
         if fused is not None:
