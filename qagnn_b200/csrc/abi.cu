@@ -345,7 +345,10 @@ int32_t layer_forward_tc(const qagnn_shape& s, const FoldLayout& L, const WorkLa
       o.hm_buf = qkm;
       o.hm = HeadMajorOut{1, D, D / s.H, DP, s.H};
       o.row_class = type_bias_classes; o.class_stride = 3 * s.H * DP; o.n_class = s.T;
-      QAGNN_RETURN_IF(gemm_tc(Ax, none, Wp, lb + L.tbias, s.N, 3 * s.H * DP, ACT_NONE, o, st, passes));
+      // the resident-weight kernel where its slice fits (split-bf16 only), else the general GEMM
+      int32_t rc = passes == 3 ? proj_resident(Ax, Wp, lb + L.tbias, s.N, 3 * s.H * DP, o, st) : QAGNN_ERR_UNSUPPORTED;
+      if (rc == QAGNN_ERR_UNSUPPORTED) rc = gemm_tc(Ax, none, Wp, lb + L.tbias, s.N, 3 * s.H * DP, ACT_NONE, o, st, passes);
+      QAGNN_RETURN_IF(rc);
     } else if (tiled) {  // per-head padded weight rows -> the GEMM writes [3][H][N][DP] (pads = exact zeros) itself
       const int DP = head_dim_padded(D / s.H);
       TcOperand Wp{lb + L.wph_hi, lb + L.wph_lo, 2 * D, 2 * D};

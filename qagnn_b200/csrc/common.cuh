@@ -163,6 +163,12 @@ int32_t gemm_tc(const TcOperand& A1, const TcOperand& A2, const TcOperand& W, co
 // Fused node MLP, one launch: out = act2( W2 . ReLU(W1 . A + b1) + b2 ), A [M, D], W1 / W2 [D, D], the hidden layer kept in
 // registers.  Same arithmetic, bit for bit, as the two gemm_tc calls it replaces (with the same pass count).  Shapes:
 // D % 8 == 0, 8 <= D <= 208.
+// The fast-form projection (head-major output with a per-row class bias, one A segment, split-bf16) on proj_resident_kernel:
+// each CTA keeps one slice of whole heads of W in shared memory and streams only A.  The same arithmetic, bit for bit, as
+// gemm_tc.  QAGNN_ERR_UNSUPPORTED (nothing launched) for shapes it does not take - K > 320, a head wider than 52 padded
+// columns, no class bias - and when QAGNN_PROJ_RESIDENT=0: the caller then runs gemm_tc.
+int32_t proj_resident(const TcOperand& A, const TcOperand& W, const float* bias, long long M, int N, const TcOutput& out,
+                      cudaStream_t st);
 bool mlp_tc_shape_ok(int D);
 int32_t mlp_tc(const TcOperand& A, const TcOperand& W1, const float* b1, const TcOperand& W2, const float* b2, long long M,
                Act act2, const TcOutput& out, cudaStream_t st, int passes = 3);

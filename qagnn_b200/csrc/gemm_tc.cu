@@ -188,6 +188,14 @@ __device__ __forceinline__ void wgmma_bf16<64>(float (&d)[32], uint64_t da, uint
       : "l"(da), "l"(db), "r"(scale_d));
 }
 template <>
+__device__ __forceinline__ void wgmma_bf16<104>(float (&d)[52], uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %54, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n104k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51}, %52, %53, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51])
+      : "l"(da), "l"(db), "r"(scale_d));
+}
+template <>
 __device__ __forceinline__ void wgmma_bf16<128>(float (&d)[64], uint64_t da, uint64_t db, uint32_t scale_d) {
   asm volatile(
       "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
@@ -598,6 +606,202 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_bf16_kernel(const __grid_c
   mlp_body<ACT, CTAS, 1>(p);
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// The fast-form Q|Kx|Mx projection with a resident weight slice:
+//
+//     qkm[3][H][M][DP] = [x | score_emb] @ W^T + tbias[clamp(type)]        split-bf16, K = D + D/2 <= 320
+//
+// gemm_tc_kernel reloads its whole W tile (208 columns x K x 2 planes, 266 KB at D = 200) for every 128-row tile, through
+// the same ring as A, and its two consumer warpgroups sit in their epilogue together while the tensor pipe idles.  Here each
+// persistent CTA owns one n slice of whole heads (kResBN = 104 columns: two heads of DP 52 at D = 200, six slices over
+// Q|Kx|Mx) and loads both of its W planes, every k block, into shared memory once; wgmma reads B from that copy for the
+// whole walk.  The ring carries A alone, one 64-row unit of one warpgroup per stage ([A hi | A lo], 16 KB).  The two
+// consumer warpgroups own alternate units and take turns on the tensor pipe (named barriers 3 and 4), so one warpgroup's
+// epilogue runs under the other's mainloop.  With CTA pairs the two CTAs of a cluster hold neighbouring slices of the same
+// rows, and each loads one A plane multicast into both.  The clusters of one slice group walk the units in the same order as
+// the other groups, so A comes from HBM about once and from L2 thereafter.
+//
+// Every output element sees the same k16 steps in the same order with the same three passes (hi*hi, hi*lo, lo*hi) and the
+// same exact K tail as in gemm_tc_kernel, and the same bias addition, so the two kernels' outputs are equal bit for bit.
+constexpr int kResBN = 104;                                 // wgmma N: one slice of whole heads
+constexpr int kResMaxKb = 5;                                // k blocks the resident slice holds: K <= 320
+constexpr int kResStages = 4;
+constexpr uint32_t kResAPlane = 64 * BK * 2;                // one A plane of one 64-row unit: 8 KB
+constexpr uint32_t kResStage = 2 * kResAPlane;              // ring stage [A hi | A lo]
+constexpr uint32_t kResWPlane = kResBN * BK * 2;            // one W plane k block of the slice: 13 KB
+constexpr uint32_t kResWBytes = kResMaxKb * 2 * kResWPlane;  // resident slice: [kb][hi | lo], 130 KB
+// [resident W | ring | mbarriers | one staging buffer (64 rows x one head of fp32) per consumer warpgroup]
+constexpr size_t kResSmem = kResWBytes + kResStages * kResStage + kCtrlBytes + 2 * kStBytes;
+static_assert(kResSmem <= kSmemCap, "the resident slice, the A ring and the staging buffers fit the opt-in shared memory");
+static_assert(kResWPlane % 1024 == 0 && kResStage % 1024 == 0, "swizzled tiles start on 1024-byte boundaries");
+
+struct ResParams {
+  CUtensorMap a_hi, a_lo, w_hi, w_lo, st_f32;
+  int nkb, tail_steps;
+  int n_step, DP;  // slice columns (whole heads) and padded head width
+  int groups;      // slice groups: slices / CTAS
+  long long M;
+  const float* bias;         // [n_class][N]
+  const int64_t* row_class;  // bias row of row r = clamp(row_class[r], 0, n_class - 1)
+  int class_stride, n_class;
+};
+
+__device__ __forceinline__ void named_bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+__device__ __forceinline__ void named_bar_arrive(int id, int n) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+
+template <int CTAS>
+__global__ void __launch_bounds__(kThreads, 1) proj_resident_kernel(const __grid_constant__ ResParams p) {
+  extern __shared__ __align__(1024) unsigned char smem[];
+  unsigned char* const wres = smem;
+  unsigned char* const ring = smem + kResWBytes;
+  uint64_t* full = reinterpret_cast<uint64_t*>(ring + kResStages * kResStage);  // [stages]  TMA -> MMA
+  uint64_t* empty = full + kResStages;                                           // [stages]  MMA -> TMA
+  uint64_t* w_full = empty + kResStages;                                         // the resident slice has landed
+  unsigned char* const staging = ring + kResStages * kResStage + kCtrlBytes;     // [2 warpgroups][kStBytes]
+  const int wg = threadIdx.x >> 7, tid = threadIdx.x & 127;
+  const uint32_t rank = CTAS == 2 ? cluster_ctarank() : 0u;
+  // cluster cl holds slice group cl % groups and walks the 64-row units first, first + walkers, ...
+  const int cl = blockIdx.x / CTAS, n_cl = gridDim.x / CTAS;
+  const int slice = (cl % p.groups) * CTAS + (int)rank;
+  const long long first = cl / p.groups, walkers = n_cl / p.groups;
+  const long long units = (p.M + 63) / 64;
+  const long long n_mine = first < units ? (units - 1 - first) / walkers + 1 : 0;
+  const int n0 = slice * p.n_step;
+
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < kResStages; ++s) {
+      mbar_init(&full[s], 1);
+      mbar_init(&empty[s], 4 * CTAS);  // one arrival per warp of the consuming warpgroup in every CTA the stage lands in
+    }
+    mbar_init(w_full, 1);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+  if (CTAS == 2) cluster_sync_all();  // the peer's barriers are initialised before any multicast or remote arrive
+
+  if (wg == 0) {
+    // ===================================== TMA producer =====================================
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (tid == 0) {
+      mbar_expect_tx(w_full, (uint32_t)p.nkb * 2 * kResWPlane);
+      for (int kb = 0; kb < p.nkb; ++kb) {
+        tma_load_2d(wres + (size_t)(2 * kb) * kResWPlane, &p.w_hi, kb * BK, n0, w_full);
+        tma_load_2d(wres + (size_t)(2 * kb + 1) * kResWPlane, &p.w_lo, kb * BK, n0, w_full);
+      }
+      long long it = 0;  // fill i * nkb + kb: unit i, k block kb
+      for (long long i = 0; i < n_mine; ++i) {
+        const int m0 = (int)((first + i * walkers) * 64);
+        for (int kb = 0; kb < p.nkb; ++kb, ++it) {
+          const int s = (int)(it % kResStages);
+          // the stage is free once the consuming warpgroup of BOTH CTAs has read it (each CTA's plane lands in both)
+          if (it >= kResStages) mbar_wait(&empty[s], (uint32_t)((it / kResStages) - 1) & 1u);
+          unsigned char* st = ring + (size_t)s * kResStage;
+          mbar_expect_tx(&full[s], kResStage);
+          if (CTAS == 1) {
+            tma_load_2d(st, &p.a_hi, kb * BK, m0, &full[s]);
+            tma_load_2d(st + kResAPlane, &p.a_lo, kb * BK, m0, &full[s]);
+          } else {
+            tma_load_2d_multicast(st + rank * kResAPlane, rank == 0 ? &p.a_hi : &p.a_lo, kb * BK, m0, &full[s], 3);
+          }
+        }
+      }
+    }
+  } else {
+    // ===================================== consumers (warpgroups 1, 2) =====================================
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+    const int wc = wg - 1;  // units wc, wc + 2, ... of this CTA's walk
+    const int warp = tid >> 5, lane = tid & 31;
+    const int q2 = 2 * (lane & 3);
+    const int rl = warp * 16 + (lane >> 2);  // fragment rows rl, rl + 8 of the unit's 64
+    const int DP = p.DP;
+    const uint32_t buf = smem_u32(staging) + (uint32_t)wc * kStBytes;
+    const uint32_t sw0 = smem_u32(wres);
+    mbar_wait(w_full, 0u);
+    float acc[kResBN / 2];
+    for (long long i = wc; i < n_mine; i += 2) {
+      // the other warpgroup's mainloop of unit i - 1 has been issued: this one's turn on the tensor pipe
+      if (i > 0) named_bar_sync(3 + wc, 256);
+#pragma unroll
+      for (int j = 0; j < kResBN / 2; ++j) acc[j] = 0.f;
+      // k blocks 0 .. nkb-2 take four k16 steps and the last one the K tail, peeled so that the group left in flight never
+      // crosses into a run-time branch (ptxas would serialise every wgmma).  A k block's stage is free once its group is done.
+      auto wait_full = [&](int kb) {
+        const long long f = i * p.nkb + kb;
+        mbar_wait(&full[f % kResStages], (uint32_t)(f / kResStages) & 1u);
+        fence_acc<kResBN / 2>(acc);
+        wgmma_fence();
+        return smem_u32(ring + (size_t)(f % kResStages) * kResStage);
+      };
+      auto release_prev = [&](int kb) {  // after k block kb's group is committed: release k block kb - 1
+        if (kb == 0) return;
+        wgmma_wait<1>();
+        fence_acc<kResBN / 2>(acc);
+        release_stage<CTAS>(&empty[(i * p.nkb + kb - 1) % kResStages], lane);
+      };
+      const int kt = p.nkb - 1;
+      for (int kb = 0; kb < kt; ++kb) {
+        const uint32_t sa = wait_full(kb);
+        mma_kblock<kResBN, 4>(acc, sa, sw0 + (uint32_t)(2 * kb) * kResWPlane, kResAPlane, kResWPlane);
+        wgmma_commit();
+        release_prev(kb);
+      }
+      {
+        const uint32_t sa = wait_full(kt), sw = sw0 + (uint32_t)(2 * kt) * kResWPlane;
+        switch (p.tail_steps) {
+          case 1: mma_kblock<kResBN, 1>(acc, sa, sw, kResAPlane, kResWPlane); break;
+          case 2: mma_kblock<kResBN, 2>(acc, sa, sw, kResAPlane, kResWPlane); break;
+          case 3: mma_kblock<kResBN, 3>(acc, sa, sw, kResAPlane, kResWPlane); break;
+          default: mma_kblock<kResBN, 4>(acc, sa, sw, kResAPlane, kResWPlane); break;
+        }
+        wgmma_commit();
+        release_prev(kt);
+      }
+      if (i + 1 < n_mine) named_bar_arrive(3 + (1 - wc), 256);  // hand the tensor pipe to unit i + 1
+      wgmma_wait<0>();
+      fence_acc<kResBN / 2>(acc);
+      release_stage<CTAS>(&empty[(i * p.nkb + kt) % kResStages], lane);
+
+      // ---- epilogue: + type-bias row, one head at a time through the staging buffer, stored with TMA (clipped at M)
+      const long long row_g = (first + i * walkers) * 64 + rl;
+      const int r0 = (int)(row_g - rl);
+      int boff[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        long long c = row_g + 8 * h < p.M ? p.row_class[row_g + 8 * h] : 0;
+        c = c < 0 ? 0 : (c >= p.n_class ? p.n_class - 1 : c);
+        boff[h] = (int)c * p.class_stride;
+      }
+      for (int h0 = 0; h0 < p.n_step; h0 += DP) {
+        if (tid == 0) bulk_wait_read<0>();  // the previous store has read the buffer
+        wg_bar(1 + wc);
+#pragma unroll
+        for (int j = 0; j < kResBN / 8; ++j) {
+          const int c = 8 * j + q2;  // DP is even: a column pair never straddles two heads
+          if (c < h0 || c >= h0 + DP) continue;
+          const int gc = n0 + c;
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const float v0 = acc[4 * j + 2 * h] + __ldg(p.bias + boff[h] + gc);
+            const float v1 = acc[4 * j + 2 * h + 1] + __ldg(p.bias + boff[h] + gc + 1);
+            st_shared_f2(buf + 4u * (uint32_t)((rl + 8 * h) * DP + c - h0), v0, v1);
+          }
+        }
+        fence_proxy_async();
+        wg_bar(1 + wc);
+        if (tid == 0) {
+          tma_store_3d(&p.st_f32, staging + (size_t)wc * kStBytes, 0, r0, (n0 + h0) / DP);
+          bulk_commit();
+        }
+      }
+    }
+    if (tid == 0) bulk_wait_all();  // no store still reads the staging buffers when the CTA exits
+  }
+  __syncthreads();
+  if (CTAS == 2) cluster_sync_all();  // the peer's multicasts and remote arrivals target this CTA: nobody leaves early
+}
+
 __global__ void split_bf16_kernel(const float* __restrict__ a, int lda, long long M, int K, __nv_bfloat16* __restrict__ hi,
                                   __nv_bfloat16* __restrict__ lo, int ldp) {
   const long long total = M * (long long)(K / 2);
@@ -880,6 +1084,99 @@ int32_t gemm_tc(const TcOperand& A1, const TcOperand& A2, const TcOperand& W, co
   else if (bn == 208) rc = launch_bn<208>(CTAS, passes, act, cfg, p);
   else rc = launch_bn<256>(CTAS, passes, act, cfg, p);
   QAGNN_RETURN_IF(rc);
+  QAGNN_CHECK_LAUNCH();
+  return QAGNN_OK;
+}
+
+// default: the fast-form projection runs proj_resident_kernel where it fits; QAGNN_PROJ_RESIDENT=0 -> gemm_tc_kernel.
+// Read at every call, so that tests and A/B runs cover both paths in one process.
+static bool proj_resident_enabled() {
+  const char* e = getenv("QAGNN_PROJ_RESIDENT");
+  return !(e && atoi(e) == 0);
+}
+
+// slice width: hpt * DP for the largest divisor hpt of H with hpt * DP <= 104; 0 when one head's fp32 columns of a 64-row
+// unit overflow a staging buffer or its TMA-store rows are not 16-byte multiples
+static int proj_resident_n_step(const HeadMajorOut& hm) {
+  if (hm.H <= 0 || hm.DP <= 0 || hm.DP % 4 != 0 || 64u * hm.DP * 4 > kStBytes) return 0;
+  for (int hpt = hm.H; hpt >= 1; --hpt)
+    if (hm.H % hpt == 0 && hpt * hm.DP <= kResBN) return hpt * hm.DP;
+  return 0;
+}
+
+static bool proj_resident_ok(const TcOperand& A, const TcOperand& W, const float* bias, int N, const TcOutput& out, int passes) {
+  if (!proj_resident_enabled() || !gemm_tc_available() || passes != 3) return false;
+  if (out.hm_buf == nullptr || !aligned16(out.hm_buf) || bias == nullptr || out.row_class == nullptr) return false;
+  const int n_step = proj_resident_n_step(out.hm);
+  return n_step > 0 && N % n_step == 0 && (A.K + BK - 1) / BK <= kResMaxKb && W.K == A.K &&
+         gemm_tc_shape_ok(A.K, 0, A.ld, 0, W.ld, N);
+}
+
+int32_t proj_resident(const TcOperand& A, const TcOperand& W, const float* bias, long long M, int N, const TcOutput& out,
+                      cudaStream_t st) {
+  if (M <= 0) return QAGNN_OK;
+  if (!proj_resident_ok(A, W, bias, N, out, 3)) return QAGNN_ERR_UNSUPPORTED;
+  const int CTAS = tc_ctas();
+  ResParams p;
+  memset(&p, 0, sizeof(p));
+  p.n_step = proj_resident_n_step(out.hm);
+  p.DP = out.hm.DP;
+  const int slices = N / p.n_step;
+  // CTA pairs hold two slices of the same rows; an odd slice count runs on single CTAs
+  const int ctas = slices % 2 == 0 ? CTAS : 1;
+  p.groups = slices / ctas;
+  p.nkb = (A.K + BK - 1) / BK;
+  p.tail_steps = (A.K - 1) % BK / 16 + 1;
+  p.M = M;
+  p.bias = bias;
+  p.row_class = out.row_class;
+  p.class_stride = out.class_stride;
+  p.n_class = out.n_class > 0 ? out.n_class : 1;
+  bool ok = make_map(&p.a_hi, A.hi, M, A.K, A.ld, 64) && make_map(&p.a_lo, A.lo, M, A.K, A.ld, 64) &&
+            make_map(&p.w_hi, W.hi, N, W.K, W.ld, kResBN) && make_map(&p.w_lo, W.lo, N, W.K, W.ld, kResBN) &&
+            make_store_map(&p.st_f32, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, out.hm_buf, p.DP, M, N / p.DP, p.DP, p.DP);
+  if (!ok) return QAGNN_ERR_CUDA;
+
+  void (*kernel)(ResParams) = ctas == 2 ? proj_resident_kernel<2> : proj_resident_kernel<1>;
+  cudaLaunchConfig_t cfg;
+  memset(&cfg, 0, sizeof(cfg));
+  cfg.blockDim = dim3(kThreads);
+  cfg.dynamicSmemBytes = kResSmem;
+  cfg.stream = st;
+  cudaLaunchAttribute lattr[1];
+  lattr[0].id = cudaLaunchAttributeClusterDimension;
+  lattr[0].val.clusterDim.x = ctas;
+  lattr[0].val.clusterDim.y = 1;
+  lattr[0].val.clusterDim.z = 1;
+  cfg.attrs = lattr;
+  cfg.numAttrs = ctas == 2 ? 1 : 0;
+  // resident CTAs (pairs), per device and CTA setting: every slice group gets the same number of walkers, so the groups
+  // read each unit of A at about the same time
+  static bool attr_set[2][kMaxDevices] = {{false}};
+  static int resident[2][kMaxDevices] = {{0}};
+  const int dev = current_device(), ci = ctas - 1;
+  if (!attr_set[ci][dev]) {
+    QAGNN_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kResSmem));
+    attr_set[ci][dev] = true;
+  }
+  if (resident[ci][dev] == 0) {
+    int n = 0;
+    if (ctas == 2) {
+      cudaLaunchConfig_t q = cfg;
+      q.gridDim = dim3(2);
+      QAGNN_CHECK_CUDA(cudaOccupancyMaxActiveClusters(&n, kernel, &q));
+    } else {
+      QAGNN_RETURN_IF(sm_count(&n));
+    }
+    resident[ci][dev] = n > 0 ? n : 1;
+  }
+  const long long units = (M + 63) / 64;
+  long long walkers = resident[ci][dev] / p.groups;
+  if (walkers > units) walkers = units;
+  if (walkers < 1) return QAGNN_ERR_UNSUPPORTED;  // fewer resident CTAs than slices (not on an H100)
+  cfg.gridDim = dim3((unsigned)(walkers * p.groups * ctas));
+  if (getenv("QAGNN_DEBUG")) fprintf(stderr, "proj_resident: M=%lld N=%d K=%d CTAS=%d slices=%d n_step=%d grid=%u smem=%zu\n", M, N, A.K, ctas, slices, p.n_step, cfg.gridDim.x, kResSmem);
+  QAGNN_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kernel, p));
   QAGNN_CHECK_LAUNCH();
   return QAGNN_OK;
 }

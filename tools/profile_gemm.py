@@ -1,5 +1,6 @@
 #!/usr/bin/env python
-"""Kernel time of every split-bf16 GEMM (`gemm_tc_kernel`, `mlp_tc_kernel`) of one cfg2 step, beside its bounds.
+"""Kernel time of every split-bf16 GEMM (`gemm_tc_kernel`, `mlp_tc_kernel`, `proj_resident_kernel`) of one cfg2 step, beside
+its bounds.
 
     python tools/profile_gemm.py --out DIR [--steps 5]
 
@@ -10,8 +11,9 @@ of three cuBLAS BF16 `torch.mm` calls at the same M, N, K (the card's practical 
 The calls are told apart by the template arguments <ACT, BN, CTAS> and, for mlp.3 and Vh/Vx (both <2, 208, CTAS>), by
 launch order.  The step is profiled twice: with the fused node MLP (`mlp_tc_kernel`, one launch per layer) and with
 QAGNN_MLP_FUSED=0 (mlp.0 + mlp.3), so the fused kernel is timed beside the pair at the same shape; the "mlp.0+mlp.3" row
-sums the pair's medians and bounds (the pair also writes and reads back the hidden planes).  One JSON line with everything
-follows the table.
+sums the pair's medians and bounds (the pair also writes and reads back the hidden planes).  The projection runs on
+`proj_resident_kernel` (<ACT, BN, CTAS> shown as <0, 104, CTAS>); a third profile with QAGNN_PROJ_RESIDENT=0 times it on
+`gemm_tc_kernel` as well, in the "proj.gemm_tc" row.  One JSON line with everything follows the table.
 
     python tools/profile_gemm.py --out DIR --bf16
 
@@ -39,11 +41,12 @@ N_NODES, D, H, DP = 64000, 200, 4, 52
 SHAPES = {
     "emb_score": (N_NODES, D // 2, D // 2, 4),       # bf16 hi + lo planes out
     "projection": (N_NODES, 3 * H * DP, D + D // 2, 4),  # fp32 head-major [3][H][N][DP] out
+    "proj.gemm_tc": (N_NODES, 3 * H * DP, D + D // 2, 4),  # the same call on gemm_tc_kernel (QAGNN_PROJ_RESIDENT=0)
     "mlp.0": (N_NODES, D, D, 4),                     # bf16 hi + lo planes out
     "mlp.3": (N_NODES, D, D, 4),                     # bf16 hi + lo planes out
     "Vh/Vx": (N_NODES, D, 2 * D, 4),                 # fp32 out
 }
-ORDER = ["emb_score", "projection", "mlp.0", "mlp.3", "mlp.0+mlp.3", "mlp fused", "Vh/Vx"]
+ORDER = ["emb_score", "projection", "proj.gemm_tc", "mlp.0", "mlp.3", "mlp.0+mlp.3", "mlp fused", "Vh/Vx"]
 
 
 def card():
@@ -101,6 +104,7 @@ def profile_gemms(step, steps, trace, kind="tc"):
     from torch.profiler import ProfilerActivity, profile
     pat = re.compile(r"gemm_%s_kernel<(\d+), *(\d+), *(\d+)>" % kind)
     pat_mlp = re.compile(r"mlp_%s_kernel<(\d+), *(\d+)>" % kind)
+    pat_res = re.compile(r"proj_resident_kernel<(\d+)>") if kind == "tc" else None
     for _ in range(3):
         step.run()
     torch.cuda.synchronize()
@@ -114,7 +118,10 @@ def profile_gemms(step, steps, trace, kind="tc"):
         if e.device_type != torch.autograd.DeviceType.CUDA:
             continue
         m, mm = pat.search(e.name), pat_mlp.search(e.name)
-        if m:
+        mr = pat_res.search(e.name) if pat_res else None
+        if mr:  # the projection (ACT_NONE) on a 104-column resident W slice
+            kern.append((e.time_range.start, (0, 104, int(mr.group(1))), e.time_range.elapsed_us()))
+        elif m:
             kern.append((e.time_range.start, tuple(int(x) for x in m.groups()), e.time_range.elapsed_us()))
         elif mm:
             act, ctas = (int(x) for x in mm.groups())
@@ -166,6 +173,16 @@ def main():
                 times.setdefault(lab, []).append(us)
                 templ[lab] = t
     os.environ.pop("QAGNN_MLP_FUSED", None)
+    os.environ["QAGNN_PROJ_RESIDENT"] = "0"  # the projection on gemm_tc_kernel, in the same process
+    kern, n = profile_gemms(step, args.steps, os.path.join(args.out, "gemm_trace_proj_gemm_tc.json"))
+    per_step["proj.gemm_tc"] = n
+    for s in range(args.steps):
+        one = kern[s * n:(s + 1) * n]
+        for (lab, us), (_, t, _) in zip(label_calls([(t, us) for _, t, us in one]), one):
+            if lab == "projection":
+                times.setdefault("proj.gemm_tc", []).append(us)
+                templ["proj.gemm_tc"] = t
+    os.environ.pop("QAGNN_PROJ_RESIDENT", None)
     if "mlp.0" in times and "mlp.3" in times:  # the pair, call by call
         times["mlp.0+mlp.3"] = [a + b for a, b in zip(times["mlp.0"], times["mlp.3"])]
         templ["mlp.0+mlp.3"] = templ["mlp.0"]
@@ -173,7 +190,7 @@ def main():
     rows = []
     info = card()
     print(f"card: {info['name']} | nvidia-smi name, power limit, max SM clock: {info['nvidia_smi']}")
-    print(f"{'call':<11} {'<ACT,BN,CTAS>':<14} {'calls/step':>10} {'median µs':>10} {'tensor µs':>10} {'HBM µs':>8} "
+    print(f"{'call':<12} {'<ACT,BN,CTAS>':<14} {'calls/step':>10} {'median µs':>10} {'tensor µs':>10} {'HBM µs':>8} "
           f"{'cuBLAS 3x µs':>12} {'TFLOP/s-eq':>10}")
     for lab in ORDER:
         if lab not in times:
@@ -196,9 +213,9 @@ def main():
                    tensor_bound_us=flops / PEAK_BF16 * 1e6, hbm_bound_us=hbm / PEAK_HBM * 1e6, cublas_3x_us=cub,
                    tflops_equiv=flops / med / 1e6)
         rows.append(row)
-        print(f"{lab:<11} {str(tuple(templ[lab])):<14} {row['calls_per_step']:>10} {med:>10.1f} {row['tensor_bound_us']:>10.1f} "
+        print(f"{lab:<12} {str(tuple(templ[lab])):<14} {row['calls_per_step']:>10} {med:>10.1f} {row['tensor_bound_us']:>10.1f} "
               f"{row['hbm_bound_us']:>8.1f} {cub:>12.1f} {row['tflops_equiv']:>10.1f}")
-    total = sum(sum(times[k]) for k in ORDER if k in times and k not in ("mlp.0", "mlp.3", "mlp.0+mlp.3")) / args.steps
+    total = sum(sum(times[k]) for k in ORDER if k in times and k not in ("mlp.0", "mlp.3", "mlp.0+mlp.3", "proj.gemm_tc")) / args.steps
     print(f"all GEMM launches of the default (fused) step: {total:.1f} µs per step ({per_step['1']} launches; "
           f"{per_step['0']} with QAGNN_MLP_FUSED=0)")
     res = {"card": info, "gemm_us_per_step": total, "launches_per_step": per_step, "calls": rows, "trace_dir": args.out}
