@@ -248,108 +248,163 @@ int32_t check_shape_fwd(const qagnn_shape* s) {
   return QAGNN_OK;
 }
 
-// Path selection: the shared-memory-tiled kernel when the batch is made of equal small sub-graphs
-// (shape.n_per_graph > 0 and the tiles fit), else the general CSR kernels.  QAGNN_MP_PATH=csr forces
-// the general path (A/B measurements).
-bool use_headtile(const qagnn_shape& s, const Ragged& rg = Ragged{}) {
-  const char* e = getenv("QAGNN_MP_PATH");  // read at every call: tests cover every path in one process
-  const bool forced = e && (strcmp(e, "csr") == 0 || strcmp(e, "basic") == 0);
-  return !forced && headtile_supported(s, rg);
-}
-// Without per-graph tiles: the column-sliced kernels (edge tables in shared memory) when the head width allows, else the
-// basic CSR kernels; QAGNN_MP_PATH=basic forces the latter.
-bool use_slice(const qagnn_shape& s) {
-  const char* e = getenv("QAGNN_MP_PATH");
-  return !(e && strcmp(e, "basic") == 0) && slice_supported(s);
+// ---- path decision ------------------------------------------------------------------------------------
+// Every forward entry point runs the kernels of one ForwardPlan, made once per call by plan_forward.  The switches are read at
+// every call: tests and A/B runs cover every path in one process.
+struct ForwardPlan {
+  int passes;      // 3: split-bf16 GEMMs on fp32 data; 1: single-pass bf16 GEMMs (the bf16 entry points)
+  bool tc;         // wgmma GEMMs: the driver exposes TMA descriptors and the row strides meet TMA's 16-byte rule (D % 8 == 0);
+                   // else the exact-fp32 FFMA GEMM.  QAGNN_GEMM=ffma forces the latter.
+  bool tiled;      // shared-memory-tiled message passing: the batch is made of equal small sub-graphs (shape.n_per_graph > 0,
+                   // or a ragged batch) and the tiles fit.  QAGNN_MP_PATH=csr|basic forces the general kernels.
+  bool slice;      // without tiles: the column-sliced kernels (edge tables in shared memory) when the head width allows, else
+                   // the basic CSR kernels.  QAGNN_MP_PATH=basic forces the latter.
+  bool zero_pads;  // tiled on the FFMA GEMM: its head-major projection never writes the pad columns, so the call zeroes them once
+  bool fast;       // qagnn_mp_forward's fast-form projection (tiled, tc, k > 0, D/2 % 4 == 0): emb_score on the tensor cores
+                   // and the type-embedding half of node_feature_extra folded into per-node-type bias rows.
+                   // QAGNN_MP_FASTPROJ=0 keeps the general [x | extra] projection.
+  bool mlp_fused;  // node MLP in one launch with the hidden layer in registers (tc, D <= 208), else mlp.0 and mlp.3 as two
+                   // GEMMs with the hidden planes in the workspace.  QAGNN_MLP_FUSED=0 forces the two launches.
+};
+
+ForwardPlan plan_forward(const qagnn_shape& s, const Ragged& rg, int passes) {
+  const char* path = getenv("QAGNN_MP_PATH");
+  const bool basic = path && strcmp(path, "basic") == 0;
+  const bool general = basic || (path && strcmp(path, "csr") == 0);
+  const char* fastproj = getenv("QAGNN_MP_FASTPROJ");
+  const char* fused = getenv("QAGNN_MLP_FUSED");
+  ForwardPlan p;
+  p.passes = passes;
+  p.tc = gemm_tc_available() && s.D % 8 == 0;
+  p.tiled = !general && headtile_supported(s, rg);
+  p.slice = !p.tiled && !basic && slice_supported(s);
+  p.zero_pads = p.tiled && !p.tc;
+  p.fast = p.tc && p.tiled && s.k > 0 && (s.D / 2) % 4 == 0 && !(fastproj && atoi(fastproj) == 0);
+  p.mlp_fused = p.tc && !(fused && atoi(fused) == 0) && mlp_tc_shape_ok(s.D);
+  return p;
 }
 
-// one GATConvE layer; `final_act` = ACT_NONE for the bare layer, ACT_GELU when called from mp_helper
-int32_t layer_forward(const qagnn_shape& s, const FoldLayout& L, const WorkLayout& W, int layer, const float* x,
-                      const float* extra, const void* prep, const qagnn_prep_layout& pl, const float* folded,
-                      float* out, float* alpha_out, float* aggr_out, float* ws, Act final_act, bool tiled,
-                      cudaStream_t st, const Ragged& rg = Ragged{}) {
+// One forward call: its shape and layouts, its plan, and what every stage reads.
+struct Fwd {
+  qagnn_shape s;
+  FoldLayout L;
+  WorkLayout W;
+  qagnn_prep_layout pl;
+  ForwardPlan plan;
+  bool in_bf16;  // bf16 inputs (a one-pass call only)
+  Ragged rg;
+  const void* prep;
+  const float* folded;
+  float* ws;
+  cudaStream_t st;
+  const float* layer_block(int l) const { return folded + L.layer0 + (size_t)l * L.layer_stride; }
+};
+
+// The checks and setup of every forward entry.  `args_ok`: the entry's own pointer and index checks.  (dtype, in_dtype) is
+// (F32, F32) for the fp32 forward (3 passes) or (BF16, F32 | BF16) for bf16 out (1 pass); any other pair is invalid.  Every
+// invalid argument is reported ahead of a short workspace.
+int32_t setup_forward(const qagnn_shape* shape, int32_t dtype, int32_t in_dtype, bool args_ok, const void* prep,
+                      const void* folded, void* workspace, size_t workspace_bytes, void* stream, const Ragged& rg, Fwd& f) {
+  QAGNN_RETURN_IF(check_shape_fwd(shape));
+  const bool bf16 = dtype == QAGNN_DTYPE_BF16 && (in_dtype == QAGNN_DTYPE_F32 || in_dtype == QAGNN_DTYPE_BF16);
+  const bool f32 = dtype == QAGNN_DTYPE_F32 && in_dtype == QAGNN_DTYPE_F32;
+  if (!(bf16 || f32) || !args_ok) return QAGNN_ERR_INVALID_ARGUMENT;
+  f.s = *shape;
+  f.L = make_fold_layout(f.s);
+  f.W = make_work_layout(f.s);
+  if (workspace_bytes < f.W.total * sizeof(float)) return QAGNN_ERR_WORKSPACE;
+  QAGNN_RETURN_IF(qagnn_graph_prep_layout(f.s.N, f.s.E, &f.pl));
+  f.plan = plan_forward(f.s, rg, bf16 ? 1 : 3);
+  f.in_bf16 = in_dtype == QAGNN_DTYPE_BF16;
+  f.rg = rg;
+  f.prep = prep;
+  f.folded = (const float*)folded;
+  f.ws = (float*)workspace;
+  f.st = (cudaStream_t)stream;
+  return QAGNN_OK;
+}
+
+// logits -> per-source softmax -> out-degree rescale -> per-target sum   (:442, :469-484), on the plan's kernels, from the
+// projection in the workspace.  aggr_hi / aggr_lo: the tiled kernel also writes the bf16 planes of aggr (tensor-core layer).
+int32_t message_passing(const Fwd& f, const float* lb, float* aggr, float* alpha_out, void* aggr_hi, void* aggr_lo) {
+  ProfScope ps(QAGNN_PROF_MESSAGE_PASSING, f.st);
+  QAGNN_RETURN_IF(zero_alpha_holes(f.s, f.prep, f.pl, alpha_out, f.st));
+  const int32_t* prep = (const int32_t*)f.prep;
+  const float* qkm = f.ws + f.W.qkm;
+  float* score = f.ws + f.W.score;
+  if (f.plan.tiled)
+    return launch_message_passing_headtile(f.s, prep, f.pl, qkm, lb + f.L.keh, lb + f.L.meh, score, f.ws + f.W.alpha2, aggr,
+                                           alpha_out, aggr_hi, aggr_lo, f.st, f.rg);
+  if (f.plan.slice)
+    return launch_message_passing_slice(f.s, prep, f.pl, qkm, lb + f.L.ke, lb + f.L.me, score, aggr, alpha_out, f.st);
+  return launch_message_passing_typed(f.s, prep, f.pl, QAGNN_DTYPE_F32, qkm, lb + f.L.ke, lb + f.L.me, score, f.ws + f.W.alpha,
+                                      aggr, alpha_out, f.st);
+}
+
+// one GATConvE layer on the exact-fp32 FFMA GEMM; `final_act` = ACT_NONE for the bare layer, ACT_GELU when called from mp_helper
+int32_t layer_forward(const Fwd& f, int layer, const float* x, const float* extra, float* out, float* alpha_out,
+                      float* aggr_out, Act final_act) {
+  const qagnn_shape& s = f.s;
+  const FoldLayout& L = f.L;
+  const WorkLayout& W = f.W;
   const int D = s.D;
-  const float* lb = folded + L.layer0 + (size_t)layer * L.layer_stride;
-  float* qkm = ws + W.qkm;
+  const float* lb = f.layer_block(layer);
+  float* ws = f.ws;
   float* aggr = aggr_out ? aggr_out : ws + W.aggr;
   {  // Q | Kx | Mx = [x ‖ extra] @ Wp^T + bp                     (:440, :464-466 node part, :469)
-    ProfScope ps(QAGNN_PROF_PROJECTION, st);
-    HeadMajorOut hm{tiled ? 1 : 0, D, D / s.H, head_dim_padded(D / s.H), s.H};
-    QAGNN_RETURN_IF(sgemm_tn(x, D, D, extra, D, D, lb + L.wp, 2 * D, lb + L.bp, qkm, 3 * D, s.N, 3 * D, ACT_NONE, st, hm));
+    ProfScope ps(QAGNN_PROF_PROJECTION, f.st);
+    HeadMajorOut hm{f.plan.tiled ? 1 : 0, D, D / s.H, head_dim_padded(D / s.H), s.H};
+    QAGNN_RETURN_IF(sgemm_tn(x, D, D, extra, D, D, lb + L.wp, 2 * D, lb + L.bp, ws + W.qkm, 3 * D, s.N, 3 * D, ACT_NONE, f.st, hm));
   }
-  {  // logits -> per-source softmax -> out-degree rescale -> per-target sum   (:442, :469-484)
-    ProfScope ps(QAGNN_PROF_MESSAGE_PASSING, st);
-    QAGNN_RETURN_IF(zero_alpha_holes(s, prep, pl, alpha_out, st));
-    if (tiled) {
-      QAGNN_RETURN_IF(launch_message_passing_headtile(s, (const int32_t*)prep, pl, qkm, lb + L.keh, lb + L.meh,
-                                                      ws + W.score, ws + W.alpha2, aggr, alpha_out, nullptr, nullptr, st, rg));
-    } else if (use_slice(s)) {
-      QAGNN_RETURN_IF(launch_message_passing_slice(s, (const int32_t*)prep, pl, qkm, lb + L.ke, lb + L.me, ws + W.score, aggr,
-                                                   alpha_out, st));
-    } else {
-      QAGNN_RETURN_IF(launch_message_passing(s, (const int32_t*)prep, pl, qkm, lb + L.ke, lb + L.me, ws + W.score,
-                                             ws + W.alpha, aggr, alpha_out, st));
-    }
-  }
+  QAGNN_RETURN_IF(message_passing(f, lb, aggr, alpha_out, nullptr, nullptr));
   {  // node MLP: Linear -> BatchNorm(eval, folded) -> ReLU -> Linear          (:443, :408)
-    ProfScope ps(QAGNN_PROF_NODE_MLP, st);
-    QAGNN_RETURN_IF(sgemm_tn(aggr, D, D, nullptr, 0, 0, lb + L.w1, D, lb + L.b1, ws + W.hmid, D, s.N, D, ACT_RELU, st));
-    QAGNN_RETURN_IF(sgemm_tn(ws + W.hmid, D, D, nullptr, 0, 0, lb + L.w2, D, lb + L.b2, out, D, s.N, D, final_act, st));
+    ProfScope ps(QAGNN_PROF_NODE_MLP, f.st);
+    QAGNN_RETURN_IF(sgemm_tn(aggr, D, D, nullptr, 0, 0, lb + L.w1, D, lb + L.b1, ws + W.hmid, D, s.N, D, ACT_RELU, f.st));
+    QAGNN_RETURN_IF(sgemm_tn(ws + W.hmid, D, D, nullptr, 0, 0, lb + L.w2, D, lb + L.b2, out, D, s.N, D, final_act, f.st));
   }
   return QAGNN_OK;
 }
 
-// Dense-path selection: wgmma split-bf16 GEMMs when the driver exposes TMA descriptors and the row strides
-// meet TMA's 16-byte rule (D % 8 == 0); else the exact-fp32 FFMA GEMM.  QAGNN_GEMM=ffma forces the latter.
-bool use_tc(const qagnn_shape& s) { return gemm_tc_available() && s.D % 8 == 0; }
-
-// Node MLP on the tensor-core path: the fused one-launch kernel when it takes the width (D <= 208), else mlp.0 and mlp.3 as
-// two GEMMs with the hidden planes in the workspace.  QAGNN_MLP_FUSED=0 forces the two launches (read at every call: tests
-// and A/B runs cover both in one process).
-bool use_mlp_fused(int D) {
-  const char* e = getenv("QAGNN_MLP_FUSED");
-  return !(e && atoi(e) == 0) && mlp_tc_shape_ok(D);
-}
-
-struct Planes {
-  const void* hi;
-  const void* lo;
-  int ld = 0;  // row stride in elements; 0 = D
+struct Planes {  // an operand as bf16 hi / lo planes, row stride ld elements
+  void* hi;
+  void* lo;
+  int ld;
 };
 
-// one GATConvE layer on split-bf16 planes.  x / extra are [N, D] plane pairs; the layer output goes to any of
-// out_f32 (fp32 [N, D]) and out_planes.  passes = 1: every GEMM runs on the hi planes alone (lo planes neither read nor
+// one GATConvE layer on the wgmma GEMMs.  x / extra are [N, D] operand planes; the layer output goes to any of out_f32 (fp32
+// [N, D]) and the planes out_hi / out_lo (row stride out_ldp).  row_class selects the fast-form projection (ForwardPlan::fast):
+// x rows are [x | score_emb] (K = D + D/2, ONE segment), extra is unused, and the type-embedding half of node_feature_extra
+// enters as the bias row of each node's type.  One pass: every GEMM runs on the hi planes alone (lo planes neither read nor
 // written, out_lo ignored); the message passing is the same either way.
-int32_t layer_forward_tc(const qagnn_shape& s, const FoldLayout& L, const WorkLayout& W, int layer, Planes x, Planes extra,
-                         const void* prep, const qagnn_prep_layout& pl, const float* folded, float* out_f32,
-                         void* out_hi, void* out_lo, float* alpha_out, float* aggr_out, float* ws, Act final_act,
-                         bool tiled, cudaStream_t st, const int64_t* type_bias_classes = nullptr, int out_ldp = 0,
-                         int passes = 3, const Ragged& rg = Ragged{}) {
-  const int D = s.D;
-  if (out_ldp == 0) out_ldp = D;
+int32_t layer_forward_tc(const Fwd& f, int layer, Planes x, Planes extra, const int64_t* row_class, float* out_f32, void* out_hi,
+                         void* out_lo, int out_ldp, float* alpha_out, float* aggr_out, Act final_act) {
+  const qagnn_shape& s = f.s;
+  const FoldLayout& L = f.L;
+  const WorkLayout& W = f.W;
+  const int D = s.D, passes = f.plan.passes;
+  cudaStream_t st = f.st;
+  float* ws = f.ws;
   float* const ap_lo = passes == 1 ? nullptr : ws + W.ap_lo;
-  const float* lb = folded + L.layer0 + (size_t)layer * L.layer_stride;
+  const float* lb = f.layer_block(layer);
   float* qkm = ws + W.qkm;
-  const bool fused_split = tiled && (D / s.H) % 2 == 0;  // the tiled kernel emits the bf16 planes of aggr itself
+  const bool fused_split = f.plan.tiled && (D / s.H) % 2 == 0;  // the tiled kernel emits the bf16 planes of aggr itself
   float* aggr = aggr_out ? aggr_out : (fused_split ? nullptr : ws + W.aggr);
   {  // Q | Kx | Mx = [x ‖ extra] @ Wp^T + bp                     (:440, :464-466 node part, :469)
     ProfScope ps(QAGNN_PROF_PROJECTION, st);
-    TcOperand A1{x.hi, x.lo, x.ld ? x.ld : D, D}, A2{extra.hi, extra.lo, D, D};
+    TcOperand A1{x.hi, x.lo, x.ld, D}, A2{extra.hi, extra.lo, extra.ld, D};
     TcOutput o{};
-    if (tiled && type_bias_classes != nullptr) {
-      // fast form (qagnn_mp_forward): x planes are [N, KS] rows of [x | score_emb] (K = D + D/2, ONE segment); the
-      // type-embedding half of node_feature_extra enters as a per-node-type bias row (T distinct rows)
-      const int DP = head_dim_padded(D / s.H), KS = round_up8(D + D / 2);
-      TcOperand Ax{x.hi, x.lo, KS, D + D / 2}, none{nullptr, nullptr, 0, 0};
-      TcOperand Wp{lb + L.wps_hi, lb + L.wps_lo, KS, D + D / 2};
+    if (row_class != nullptr) {  // fast form: T distinct type-embedding rows -> T bias rows
+      const int DP = head_dim_padded(D / s.H);
+      TcOperand Ax{x.hi, x.lo, x.ld, D + D / 2}, none{nullptr, nullptr, 0, 0};
+      TcOperand Wp{lb + L.wps_hi, lb + L.wps_lo, x.ld, D + D / 2};
       o.hm_buf = qkm;
       o.hm = HeadMajorOut{1, D, D / s.H, DP, s.H};
-      o.row_class = type_bias_classes; o.class_stride = 3 * s.H * DP; o.n_class = s.T;
+      o.row_class = row_class; o.class_stride = 3 * s.H * DP; o.n_class = s.T;
       // the resident-weight kernel where its slice fits (split-bf16 only), else the general GEMM
       int32_t rc = passes == 3 ? proj_resident(Ax, Wp, lb + L.tbias, s.N, 3 * s.H * DP, o, st) : QAGNN_ERR_UNSUPPORTED;
       if (rc == QAGNN_ERR_UNSUPPORTED) rc = gemm_tc(Ax, none, Wp, lb + L.tbias, s.N, 3 * s.H * DP, ACT_NONE, o, st, passes);
       QAGNN_RETURN_IF(rc);
-    } else if (tiled) {  // per-head padded weight rows -> the GEMM writes [3][H][N][DP] (pads = exact zeros) itself
+    } else if (f.plan.tiled) {  // per-head padded weight rows -> the GEMM writes [3][H][N][DP] (pads = exact zeros) itself
       const int DP = head_dim_padded(D / s.H);
       TcOperand Wp{lb + L.wph_hi, lb + L.wph_lo, 2 * D, 2 * D};
       o.hm_buf = qkm;
@@ -362,27 +417,13 @@ int32_t layer_forward_tc(const qagnn_shape& s, const FoldLayout& L, const WorkLa
       QAGNN_RETURN_IF(gemm_tc(A1, A2, Wp, lb + L.bp, s.N, 3 * D, ACT_NONE, o, st, passes));
     }
   }
-  {  // logits -> per-source softmax -> out-degree rescale -> per-target sum   (:442, :469-484)
-    ProfScope ps(QAGNN_PROF_MESSAGE_PASSING, st);
-    QAGNN_RETURN_IF(zero_alpha_holes(s, prep, pl, alpha_out, st));
-    if (tiled) {
-      QAGNN_RETURN_IF(launch_message_passing_headtile(s, (const int32_t*)prep, pl, qkm, lb + L.keh, lb + L.meh,
-                                                      ws + W.score, ws + W.alpha2, aggr, alpha_out,
-                                                      fused_split ? ws + W.ap_hi : nullptr, ap_lo, st, rg));
-    } else if (use_slice(s)) {
-      QAGNN_RETURN_IF(launch_message_passing_slice(s, (const int32_t*)prep, pl, qkm, lb + L.ke, lb + L.me, ws + W.score, aggr,
-                                                   alpha_out, st));
-    } else {
-      QAGNN_RETURN_IF(launch_message_passing(s, (const int32_t*)prep, pl, qkm, lb + L.ke, lb + L.me, ws + W.score,
-                                             ws + W.alpha, aggr, alpha_out, st));
-    }
-  }
+  QAGNN_RETURN_IF(message_passing(f, lb, aggr, alpha_out, fused_split ? ws + W.ap_hi : nullptr, ap_lo));
   {  // node MLP: Linear -> BatchNorm(eval, folded) -> ReLU -> Linear          (:443, :408)
     ProfScope ps(QAGNN_PROF_NODE_MLP, st);
     if (!fused_split) QAGNN_RETURN_IF(split_bf16(aggr, D, s.N, D, ws + W.ap_hi, ap_lo, D, st));
     TcOperand A{ws + W.ap_hi, ws + W.ap_lo, D, D}, none{nullptr, nullptr, 0, 0};
     TcOperand W1{lb + L.w1_hi, lb + L.w1_lo, D, D}, W2{lb + L.w2_hi, lb + L.w2_lo, D, D};
-    if (use_mlp_fused(D)) {  // one launch, the hidden layer never leaves registers
+    if (f.plan.mlp_fused) {  // one launch, the hidden layer never leaves registers
       TcOutput o{};
       o.f32 = out_f32; o.ldc = D; o.hi = out_hi; o.lo = out_lo; o.ldp = out_ldp;
       return mlp_tc(A, W1, lb + L.b1, W2, lb + L.b2, s.N, final_act, o, st, passes);
@@ -398,10 +439,13 @@ int32_t layer_forward_tc(const qagnn_shape& s, const FoldLayout& L, const WorkLa
   return QAGNN_OK;
 }
 
-int32_t extra_forward(const qagnn_shape& s, const FoldLayout& L, const WorkLayout& W, const int64_t* node_type,
-                      const float* node_score, const float* folded, float* extra, float* ws, cudaStream_t st,
-                      void* ex_hi = nullptr, void* ex_lo = nullptr) {
-  ProfScope ps(QAGNN_PROF_PRO_EPILOGUE, st);
+// node_feature_extra (:62-73,86) as fp32 `extra` and/or as the split-bf16 planes ex_hi / ex_lo (ex_lo null: hi plane alone)
+int32_t extra_forward(const Fwd& f, const int64_t* node_type, const float* node_score, float* extra, void* ex_hi, void* ex_lo) {
+  ProfScope ps(QAGNN_PROF_PRO_EPILOGUE, f.st);
+  const qagnn_shape& s = f.s;
+  const FoldLayout& L = f.L;
+  const float* folded = f.folded;
+  cudaStream_t st = f.st;
   const int D = s.D, Dh = D / 2;
   if (Dh <= 128 && D % 8 == 0) {
     const size_t smem = ((size_t)Dh * Dh + (size_t)kNfNodes * Dh) * sizeof(float);
@@ -421,13 +465,56 @@ int32_t extra_forward(const qagnn_shape& s, const FoldLayout& L, const WorkLayou
   int64_t g = (n + 255) / 256;
   if (g > kNumSMs * 32) g = kNumSMs * 32;
   node_feature_prologue_kernel<<<(unsigned)g, 256, 0, st>>>(s.N, D, s.T, node_type, node_score, folded + L.type_tab,
-                                                            folded + L.basis, extra, ws + W.sinb);
+                                                            folded + L.basis, extra, f.ws + f.W.sinb);
   QAGNN_CHECK_LAUNCH();
   // extra[:, D/2:] = GELU(emb_score(sinb))                                  (:73)
-  QAGNN_RETURN_IF(sgemm_tn(ws + W.sinb, Dh, Dh, nullptr, 0, 0, folded + L.ws, Dh, folded + L.bs, extra + Dh, D, s.N, Dh,
+  QAGNN_RETURN_IF(sgemm_tn(f.ws + f.W.sinb, Dh, Dh, nullptr, 0, 0, folded + L.ws, Dh, folded + L.bs, extra + Dh, D, s.N, Dh,
                            ACT_GELU, st));
   if (ex_hi != nullptr) QAGNN_RETURN_IF(split_bf16(extra, D, s.N, D, ex_hi, ex_lo, D, st));
   return QAGNN_OK;
+}
+
+// The fast form's score_emb = GELU(emb_score(sin basis)) (:70-73) as columns [D, D + D/2) of the three [N, KS] plane pairs:
+// the sin-basis planes, the emb_score GEMM into pair 0, and a copy into the two activation pairs (layer-invariant: :86)
+int32_t score_emb_planes(const Fwd& f, const float* node_score, void* const* hi, void* const* lo, int KS) {
+  const qagnn_shape& s = f.s;
+  const int D = s.D, Dh = D / 2, KSh = round_up8(Dh);
+  const bool single = f.plan.passes == 1;
+  float* ws = f.ws;
+  const float* fo = f.folded;
+  int64_t g = (s.N * (Dh / 2) + 255) / 256;
+  if (g > kNumSMs * 32) g = kNumSMs * 32;
+  sin_basis_planes_kernel<<<(unsigned)g, 256, 0, f.st>>>(s.N, Dh, KSh, node_score, fo + f.L.basis,
+                                                         (__nv_bfloat16*)(ws + f.W.sb_hi),
+                                                         single ? nullptr : (__nv_bfloat16*)(ws + f.W.sb_lo));
+  QAGNN_CHECK_LAUNCH();
+  const size_t off = (size_t)D * 2;  // bytes to column D of a plane
+  auto at = [&](void* plane) { return (uint2*)((char*)plane + off); };
+  TcOperand A{ws + f.W.sb_hi, ws + f.W.sb_lo, KSh, Dh}, none{nullptr, nullptr, 0, 0}, Wsc{fo + f.L.ws_hi, fo + f.L.ws_lo, KSh, Dh};
+  TcOutput o{};
+  o.hi = at(hi[0]); o.lo = at(lo[0]); o.ldp = KS;
+  QAGNN_RETURN_IF(gemm_tc(A, none, Wsc, fo + f.L.bs, s.N, Dh, ACT_GELU, o, f.st, f.plan.passes));
+  const int w4 = Dh * 2 / 8, ld8 = KS * 2 / 8;  // Dh % 4 == 0 and KS % 8 == 0 (ForwardPlan::fast)
+  int64_t gc = (s.N * w4 + 255) / 256;
+  if (gc > kNumSMs * 16) gc = kNumSMs * 16;
+  copy_plane_columns_kernel<<<(unsigned)gc, 256, 0, f.st>>>(s.N, w4, ld8, at(hi[0]), single ? nullptr : at(lo[0]), at(hi[1]),
+                                                            at(lo[1]), at(hi[2]), at(lo[2]));
+  QAGNN_CHECK_LAUNCH();
+  return QAGNN_OK;
+}
+
+// An [N, D] input as the A-operand planes of the call's GEMMs, row stride ldp: the split-bf16 hi / lo planes of an fp32 input
+// (3 passes), or the hi plane alone (1 pass) - a bf16 input copied (bf16_rn is the identity on it), an fp32 one rounded to
+// nearest even by split_bf16 without its lo plane: autocast's cast, in the same pass that writes the plane
+int32_t input_planes(const Fwd& f, const void* src, void* hi, void* lo, int ldp) {
+  const int64_t N = f.s.N;
+  const int D = f.s.D;
+  if (f.in_bf16) {
+    QAGNN_CHECK_CUDA(cudaMemcpy2DAsync(hi, (size_t)ldp * 2, src, (size_t)D * 2, (size_t)D * 2, (size_t)N,
+                                       cudaMemcpyDeviceToDevice, f.st));
+    return QAGNN_OK;
+  }
+  return split_bf16((const float*)src, D, N, D, hi, f.plan.passes == 1 ? nullptr : lo, ldp, f.st);
 }
 
 __global__ void bf16_to_f32_kernel(int64_t n, const __nv_bfloat16* __restrict__ in, float* __restrict__ out) {
@@ -449,25 +536,96 @@ int32_t convert(int64_t n, const void* in, void* out, bool widen, cudaStream_t s
   return QAGNN_OK;
 }
 
-// bf16 rows [rows, cols] (row stride `ld` elements) copied into a hi plane with row stride `ldp`: a bf16 operand is its own
-// hi plane (bf16_rn is the identity on it)
-int32_t copy_rows_bf16(const void* src, int ld, void* dst, int ldp, int64_t rows, int cols, cudaStream_t st) {
-  if (rows <= 0) return QAGNN_OK;
-  QAGNN_CHECK_CUDA(cudaMemcpy2DAsync(dst, (size_t)ldp * 2, src, (size_t)ld * 2, (size_t)cols * 2, (size_t)rows,
-                                     cudaMemcpyDeviceToDevice, st));
-  return QAGNN_OK;
+// A forward on the FFMA GEMM: `run(in32, out32)` is the fp32 path on n_in (<= 2) [N, D] inputs.  An fp32 call runs it on the
+// caller's buffers.  A bf16 call runs it on the rounded inputs (widened exactly) and rounds its output once; the split-bf16
+// plane buffers, which the FFMA path never touches, stage the fp32 inputs and the output ([hp_hi, ap_hi) spans 4 N*D floats).
+template <class Run>
+int32_t ffma_forward(const Fwd& f, int n_in, const void* const* in, void* out, Run run) {
+  const float* in32[2] = {(const float*)in[0], n_in > 1 ? (const float*)in[1] : nullptr};
+  if (f.plan.passes == 3) return run(in32, (float*)out);
+  const int64_t ND = f.s.N * (int64_t)f.s.D;
+  float* out32 = f.ws + f.W.hp_hi + n_in * ND;
+  for (int i = 0; i < n_in; ++i) {
+    float* x32 = f.ws + f.W.hp_hi + i * ND;
+    if (f.in_bf16) {
+      QAGNN_RETURN_IF(convert(ND, in[i], x32, true, f.st));
+    } else {  // bf16_rn of the fp32 input, back in fp32
+      QAGNN_RETURN_IF(convert(ND, in[i], out32, false, f.st));
+      QAGNN_RETURN_IF(convert(ND, out32, x32, true, f.st));
+    }
+    in32[i] = x32;
+  }
+  QAGNN_RETURN_IF(run(in32, out32));
+  return convert(ND, out32, out, false, f.st);
 }
 
-// The hi plane [rows, cols] (row stride ldp) of a bf16 or fp32 operand (row stride cols): a bf16 operand is copied, an fp32
-// one rounded to nearest even by split_bf16 without its lo plane - autocast's cast, in the same pass that writes the plane
-int32_t hi_plane_of(const void* src, bool src_bf16, void* dst, int ldp, int64_t rows, int cols, cudaStream_t st) {
-  if (src_bf16) return copy_rows_bf16(src, cols, dst, ldp, rows, cols, st);
-  return split_bf16((const float*)src, cols, rows, cols, dst, nullptr, ldp, st);
+// QAGNN_Message_Passing.forward on the FFMA GEMM, fp32 in and out
+int32_t mp_forward_ffma(const Fwd& f, const float* H_in, const int64_t* node_type, const float* node_score, float* out,
+                        float* x_layers_out) {
+  const qagnn_shape& s = f.s;
+  float* extra = f.ws + f.W.extra;
+  QAGNN_RETURN_IF(extra_forward(f, node_type, node_score, extra, nullptr, nullptr));
+  if (f.plan.zero_pads) QAGNN_RETURN_IF(zero_head_pads(s, f.ws + f.W.qkm, f.st));
+  const size_t ND = (size_t)s.N * s.D;
+  const float* x = H_in;
+  for (int l = 0; l < s.k; ++l) {  // mp_helper, :45-50 (dropout is the identity in eval)
+    float* xo = x_layers_out ? x_layers_out + (size_t)l * ND : f.ws + ((l & 1) ? f.W.xb : f.W.xa);
+    QAGNN_RETURN_IF(layer_forward(f, l, x, extra, xo, nullptr, nullptr, ACT_GELU));
+    x = xo;
+  }
+  // output = GELU(Vh(H) + Vx(X))                                             (:92)
+  ProfScope ps(QAGNN_PROF_PRO_EPILOGUE, f.st);
+  return sgemm_tn(H_in, s.D, s.D, x, s.D, s.D, f.folded + f.L.vcat, 2 * s.D, f.folded + f.L.vbias, out, s.D, s.N, s.D, ACT_GELU,
+                  f.st);
 }
 
-// The bf16 entry points on shapes without the wgmma GEMM run the fp32 path on widened inputs: the split-bf16 plane buffers,
-// which that path never touches, hold the fp32 inputs and output there ([hp_hi, ap_hi) spans at least 4 N*D floats).
-float* fp32_staging(const WorkLayout& W, float* ws) { return ws + W.hp_hi; }
+// QAGNN_Message_Passing.forward on the wgmma GEMMs.  The prologue chooses a set of three [N, ld] plane pairs - 0: H_in, 1 and 2:
+// the layer activations, ping-pong - and fills it:
+// * fast form: ld = KS; columns [D, D + D/2) of every pair hold score_emb, the type embedding enters as per-type bias rows;
+// * general form: ld = D; node_feature_extra goes to planes of its own, the projection's second A segment.
+// One layer loop and one Vh|Vx GEMM follow for both.
+int32_t mp_forward_tc(const Fwd& f, const void* H_in, const int64_t* node_type, const float* node_score, void* out,
+                      float* x_layers_out) {
+  const qagnn_shape& s = f.s;
+  const WorkLayout& W = f.W;
+  float* ws = f.ws;
+  const int D = s.D;
+  const bool fast = f.plan.fast;
+  const int ld = fast ? round_up8(D + D / 2) : D;
+  void* hi[3];
+  void* lo[3];
+  for (int i = 0; i < 3; ++i) {
+    hi[i] = ws + (fast ? W.xs_hi[i] : i == 0 ? W.hp_hi : W.xp_hi[i - 1]);
+    lo[i] = ws + (fast ? W.xs_lo[i] : i == 0 ? W.hp_lo : W.xp_lo[i - 1]);
+  }
+  Planes extra{nullptr, nullptr, 0};
+  if (!fast) {  // `extra` is only ever consumed as planes, so the prologue writes those directly (and fp32 only where D/2 > 128)
+    QAGNN_RETURN_IF(extra_forward(f, node_type, node_score, D / 2 <= 128 ? nullptr : ws + W.extra, ws + W.ep_hi,
+                                  f.plan.passes == 1 ? nullptr : ws + W.ep_lo));
+    extra = Planes{ws + W.ep_hi, ws + W.ep_lo, D};
+  }
+  {
+    ProfScope ps(QAGNN_PROF_PRO_EPILOGUE, f.st);
+    if (fast) QAGNN_RETURN_IF(score_emb_planes(f, node_score, hi, lo, ld));
+    QAGNN_RETURN_IF(input_planes(f, H_in, hi[0], lo[0], ld));
+  }
+  const size_t ND = (size_t)s.N * D;
+  int cur = 0;  // the pair holding the layer input
+  for (int l = 0; l < s.k; ++l) {  // mp_helper, :45-50 (dropout is the identity in eval)
+    const int nxt = 1 + (l & 1);
+    float* xo32 = x_layers_out ? x_layers_out + (size_t)l * ND : nullptr;
+    QAGNN_RETURN_IF(layer_forward_tc(f, l, Planes{hi[cur], lo[cur], ld}, extra, fast ? node_type : nullptr, xo32, hi[nxt],
+                                     lo[nxt], ld, nullptr, nullptr, ACT_GELU));
+    cur = nxt;
+  }
+  // output = GELU(Vh(H) + Vx(X)), X = H when k = 0                           (:92)
+  ProfScope ps(QAGNN_PROF_PRO_EPILOGUE, f.st);
+  TcOperand A1{hi[0], lo[0], ld, D}, A2{hi[cur], lo[cur], ld, D}, Wv{f.folded + f.L.vcat_hi, f.folded + f.L.vcat_lo, 2 * D, 2 * D};
+  TcOutput o{};
+  if (f.plan.passes == 1) { o.hi = out; o.ldp = D; }
+  else { o.f32 = (float*)out; o.ldc = D; }
+  return gemm_tc(A1, A2, Wv, f.folded + f.L.vbias, s.N, D, ACT_GELU, o, f.st, f.plan.passes);
+}
 
 }  // namespace
 }  // namespace qagnn
@@ -519,96 +677,44 @@ extern "C" size_t qagnn_forward_workspace_bytes(const qagnn_shape* shape) {
   return align_up(make_work_layout(*shape).total * sizeof(float));
 }
 
-static int32_t gatconve_forward(const qagnn_shape* shape, int32_t layer, const float* x, const float* extra, const void* prep,
-                                const void* folded, float* out, float* alpha_out, float* aggr_out, void* workspace,
-                                size_t workspace_bytes, void* stream, const Ragged& rg) {
-  QAGNN_RETURN_IF(check_shape_fwd(shape));
-  if (!x || !extra || !prep || !folded || !out || !workspace) return QAGNN_ERR_INVALID_ARGUMENT;
-  if (layer < 0 || layer >= shape->k) return QAGNN_ERR_INVALID_ARGUMENT;
-  const FoldLayout L = make_fold_layout(*shape);
-  const WorkLayout W = make_work_layout(*shape);
-  if (workspace_bytes < W.total * sizeof(float)) return QAGNN_ERR_WORKSPACE;
-  qagnn_prep_layout pl;
-  QAGNN_RETURN_IF(qagnn_graph_prep_layout(shape->N, shape->E, &pl));
-  const bool tiled = use_headtile(*shape, rg);
-  cudaStream_t st = (cudaStream_t)stream;
-  float* ws = (float*)workspace;
-  if (tiled && !use_tc(*shape)) QAGNN_RETURN_IF(zero_head_pads(*shape, ws + W.qkm, st));
-  if (use_tc(*shape)) {
-    const int D = shape->D;
-    QAGNN_RETURN_IF(split_bf16(x, D, shape->N, D, ws + W.xp_hi[0], ws + W.xp_lo[0], D, st));
-    QAGNN_RETURN_IF(split_bf16(extra, D, shape->N, D, ws + W.ep_hi, ws + W.ep_lo, D, st));
-    return layer_forward_tc(*shape, L, W, layer, Planes{ws + W.xp_hi[0], ws + W.xp_lo[0]}, Planes{ws + W.ep_hi, ws + W.ep_lo},
-                            prep, pl, (const float*)folded, out, nullptr, nullptr, alpha_out, aggr_out, ws, ACT_NONE, tiled, st,
-                            nullptr, 0, 3, rg);
+// GATConvE.forward, one layer (:411-484): fp32, or a bf16 output (dtype) from fp32 or bf16 x / extra (in_dtype)
+static int32_t gatconve_forward(const qagnn_shape* shape, int32_t dtype, int32_t in_dtype, int32_t layer, const void* x,
+                                const void* extra, const void* prep, const void* folded, void* out, float* alpha_out,
+                                float* aggr_out, void* workspace, size_t workspace_bytes, void* stream, const Ragged& rg) {
+  const bool args_ok = x && extra && prep && folded && out && workspace && shape && layer >= 0 && layer < shape->k;
+  Fwd f;
+  QAGNN_RETURN_IF(setup_forward(shape, dtype, in_dtype, args_ok, prep, folded, workspace, workspace_bytes, stream, rg, f));
+  if (f.plan.tc) {
+    const bool single = f.plan.passes == 1;
+    const int D = f.s.D;
+    float* ws = f.ws;
+    const Planes xp{ws + f.W.xp_hi[0], single ? nullptr : ws + f.W.xp_lo[0], D};
+    const Planes ep{ws + f.W.ep_hi, single ? nullptr : ws + f.W.ep_lo, D};
+    QAGNN_RETURN_IF(input_planes(f, x, xp.hi, xp.lo, D));
+    QAGNN_RETURN_IF(input_planes(f, extra, ep.hi, ep.lo, D));
+    return layer_forward_tc(f, layer, xp, ep, nullptr, single ? nullptr : (float*)out, single ? out : nullptr, nullptr, D,
+                            alpha_out, aggr_out, ACT_NONE);
   }
-  return layer_forward(*shape, L, W, layer, x, extra, prep, pl, (const float*)folded, out, alpha_out, aggr_out, ws,
-                       ACT_NONE, tiled, st, rg);
-}
-
-extern "C" int32_t qagnn_gatconve_forward(const qagnn_shape* shape, int32_t layer, const float* x, const float* extra,
-                                          const void* prep, const void* folded, float* out, float* alpha_out,
-                                          float* aggr_out, void* workspace, size_t workspace_bytes, void* stream) {
-  return gatconve_forward(shape, layer, x, extra, prep, folded, out, alpha_out, aggr_out, workspace, workspace_bytes, stream,
-                          Ragged{});
-}
-
-static int32_t gatconve_forward_typed(const qagnn_shape* shape, int32_t dtype, int32_t in_dtype, int32_t layer, const void* x,
-                                      const void* extra, const void* prep, const void* folded, void* out, float* alpha_out,
-                                      float* aggr_out, void* workspace, size_t workspace_bytes, void* stream, const Ragged& rg) {
-  if (in_dtype != QAGNN_DTYPE_F32 && in_dtype != QAGNN_DTYPE_BF16) return QAGNN_ERR_INVALID_ARGUMENT;
-  if (dtype == QAGNN_DTYPE_F32) {
-    if (in_dtype != QAGNN_DTYPE_F32) return QAGNN_ERR_INVALID_ARGUMENT;
-    return gatconve_forward(shape, layer, (const float*)x, (const float*)extra, prep, folded, (float*)out, alpha_out, aggr_out,
-                            workspace, workspace_bytes, stream, rg);
-  }
-  if (dtype != QAGNN_DTYPE_BF16) return QAGNN_ERR_INVALID_ARGUMENT;
-  const bool in_bf16 = in_dtype == QAGNN_DTYPE_BF16;
-  QAGNN_RETURN_IF(check_shape_fwd(shape));
-  if (!x || !extra || !prep || !folded || !out || !workspace) return QAGNN_ERR_INVALID_ARGUMENT;
-  if (layer < 0 || layer >= shape->k) return QAGNN_ERR_INVALID_ARGUMENT;
-  const FoldLayout L = make_fold_layout(*shape);
-  const WorkLayout W = make_work_layout(*shape);
-  if (workspace_bytes < W.total * sizeof(float)) return QAGNN_ERR_WORKSPACE;
-  qagnn_prep_layout pl;
-  QAGNN_RETURN_IF(qagnn_graph_prep_layout(shape->N, shape->E, &pl));
-  const bool tiled = use_headtile(*shape, rg);
-  cudaStream_t st = (cudaStream_t)stream;
-  float* ws = (float*)workspace;
-  const int D = shape->D;
-  const int64_t ND = shape->N * (int64_t)D;
-  if (use_tc(*shape)) {  // x / extra as hi planes, every GEMM single-pass
-    QAGNN_RETURN_IF(hi_plane_of(x, in_bf16, ws + W.xp_hi[0], D, shape->N, D, st));
-    QAGNN_RETURN_IF(hi_plane_of(extra, in_bf16, ws + W.ep_hi, D, shape->N, D, st));
-    return layer_forward_tc(*shape, L, W, layer, Planes{ws + W.xp_hi[0], nullptr}, Planes{ws + W.ep_hi, nullptr}, prep, pl,
-                            (const float*)folded, nullptr, out, nullptr, alpha_out, aggr_out, ws, ACT_NONE, tiled, st,
-                            nullptr, 0, 1, rg);
-  }
-  // the fp32 path on the rounded inputs (widened exactly), its output rounded once
-  float* x32 = fp32_staging(W, ws);
-  float* ex32 = x32 + ND;
-  float* out32 = ex32 + ND;
-  if (in_bf16) {
-    QAGNN_RETURN_IF(convert(ND, x, x32, true, st));
-    QAGNN_RETURN_IF(convert(ND, extra, ex32, true, st));
-  } else {  // bf16_rn of the fp32 inputs, back in fp32
-    QAGNN_RETURN_IF(convert(ND, x, out32, false, st));
-    QAGNN_RETURN_IF(convert(ND, out32, x32, true, st));
-    QAGNN_RETURN_IF(convert(ND, extra, out32, false, st));
-    QAGNN_RETURN_IF(convert(ND, out32, ex32, true, st));
-  }
-  if (tiled) QAGNN_RETURN_IF(zero_head_pads(*shape, ws + W.qkm, st));
-  QAGNN_RETURN_IF(layer_forward(*shape, L, W, layer, x32, ex32, prep, pl, (const float*)folded, out32, alpha_out, aggr_out, ws,
-                                ACT_NONE, tiled, st, rg));
-  return convert(ND, out32, out, false, st);
+  const void* in[2] = {x, extra};
+  return ffma_forward(f, 2, in, out, [&](const float* const* in32, float* out32) {
+    if (f.plan.zero_pads) QAGNN_RETURN_IF(zero_head_pads(f.s, f.ws + f.W.qkm, f.st));
+    return layer_forward(f, layer, in32[0], in32[1], out32, alpha_out, aggr_out, ACT_NONE);
+  });
 }
 
 extern "C" int32_t qagnn_gatconve_forward_typed(const qagnn_shape* shape, int32_t dtype, int32_t in_dtype, int32_t layer,
                                                 const void* x, const void* extra, const void* prep, const void* folded,
                                                 void* out, float* alpha_out, float* aggr_out, void* workspace,
                                                 size_t workspace_bytes, void* stream) {
-  return gatconve_forward_typed(shape, dtype, in_dtype, layer, x, extra, prep, folded, out, alpha_out, aggr_out, workspace,
-                                workspace_bytes, stream, Ragged{});
+  return gatconve_forward(shape, dtype, in_dtype, layer, x, extra, prep, folded, out, alpha_out, aggr_out, workspace,
+                          workspace_bytes, stream, Ragged{});
+}
+
+extern "C" int32_t qagnn_gatconve_forward(const qagnn_shape* shape, int32_t layer, const float* x, const float* extra,
+                                          const void* prep, const void* folded, float* out, float* alpha_out,
+                                          float* aggr_out, void* workspace, size_t workspace_bytes, void* stream) {
+  return qagnn_gatconve_forward_typed(shape, QAGNN_DTYPE_F32, QAGNN_DTYPE_F32, layer, x, extra, prep, folded, out, alpha_out,
+                                      aggr_out, workspace, workspace_bytes, stream);
 }
 
 // a ragged batch: n_graphs sub-graphs of at most shape->n_per_graph rows at node_ptr, the rest of the N rows a tail
@@ -625,182 +731,54 @@ extern "C" int32_t qagnn_gatconve_forward_ragged(const qagnn_shape* shape, int32
                                                  float* aggr_out, void* workspace, size_t workspace_bytes, void* stream) {
   Ragged rg;
   QAGNN_RETURN_IF(check_ragged(shape, n_graphs, node_ptr, rg));
-  return gatconve_forward_typed(shape, dtype, in_dtype, layer, x, extra, prep, folded, out, alpha_out, aggr_out, workspace,
-                                workspace_bytes, stream, rg);
+  return gatconve_forward(shape, dtype, in_dtype, layer, x, extra, prep, folded, out, alpha_out, aggr_out, workspace,
+                          workspace_bytes, stream, rg);
 }
 
 extern "C" int32_t qagnn_mp_path(const qagnn_shape* shape) {
   QAGNN_RETURN_IF(check_shape_fwd(shape));
-  if (use_headtile(*shape)) return QAGNN_MP_PATH_TILED;
-  return use_slice(*shape) ? QAGNN_MP_PATH_SLICE : QAGNN_MP_PATH_BASIC;
+  const ForwardPlan p = plan_forward(*shape, Ragged{}, 3);
+  if (p.tiled) return QAGNN_MP_PATH_TILED;
+  return p.slice ? QAGNN_MP_PATH_SLICE : QAGNN_MP_PATH_BASIC;
 }
 
 extern "C" int32_t qagnn_node_feature_extra(const qagnn_shape* shape, const int64_t* node_type, const float* node_score,
                                             const void* folded, float* extra_out, void* workspace,
                                             size_t workspace_bytes, void* stream) {
-  QAGNN_RETURN_IF(check_shape_fwd(shape));
-  if (!node_type || !node_score || !folded || !extra_out || !workspace) return QAGNN_ERR_INVALID_ARGUMENT;
-  const FoldLayout L = make_fold_layout(*shape);
-  const WorkLayout W = make_work_layout(*shape);
-  if (workspace_bytes < W.total * sizeof(float)) return QAGNN_ERR_WORKSPACE;
-  return extra_forward(*shape, L, W, node_type, node_score, (const float*)folded, extra_out, (float*)workspace,
-                       (cudaStream_t)stream);
+  const bool args_ok = node_type && node_score && folded && extra_out && workspace;
+  Fwd f;
+  QAGNN_RETURN_IF(setup_forward(shape, QAGNN_DTYPE_F32, QAGNN_DTYPE_F32, args_ok, nullptr, folded, workspace, workspace_bytes,
+                                stream, Ragged{}, f));
+  return extra_forward(f, node_type, node_score, extra_out, nullptr, nullptr);
 }
 
-// QAGNN_Message_Passing.forward; passes = 3: H_in / out fp32 (qagnn_mp_forward), passes = 1: H_in / out bf16 and every
-// GEMM single-pass on the hi planes (qagnn_mp_forward_typed with QAGNN_DTYPE_BF16).
-static int32_t mp_forward(const qagnn_shape& s, int passes, bool h_bf16, const void* H_in_any, const int64_t* node_type,
-                          const float* node_score, const void* prep, const void* folded, void* out_any, float* x_layers_out,
-                          float* ws, cudaStream_t st, const Ragged& rg = Ragged{}) {
-  const FoldLayout L = make_fold_layout(s);
-  const WorkLayout W = make_work_layout(s);
-  qagnn_prep_layout pl;
-  QAGNN_RETURN_IF(qagnn_graph_prep_layout(s.N, s.E, &pl));
-  const bool single = passes == 1;
-  const float* f = (const float*)folded;
-  float* extra = ws + W.extra;
-  const bool tc = use_tc(s);
-  const bool tiled = use_headtile(s, rg);
-  const float* H_in = (const float*)H_in_any;
-  float* out = (float*)out_any;
-  if (single && !tc) {  // the fp32 path on the rounded H (widened exactly), its output rounded once at the end
-    float* h32 = fp32_staging(W, ws);
-    out = h32 + (size_t)s.N * s.D;
-    if (!h_bf16) QAGNN_RETURN_IF(convert((int64_t)s.N * s.D, H_in_any, out, false, st));
-    QAGNN_RETURN_IF(convert((int64_t)s.N * s.D, h_bf16 ? H_in_any : out, h32, true, st));
-    H_in = h32;
-  }
-  // fast form: tensor-core emb_score + type-embedding half of node_feature_extra folded into per-type bias rows
-  // (QAGNN_MP_FASTPROJ=0 keeps the general [x | extra] projection, for A/B runs and tests)
-  const char* efp = getenv("QAGNN_MP_FASTPROJ");
-  const bool fast = tc && tiled && s.k > 0 && (s.D / 2) % 4 == 0 && !(efp && atoi(efp) == 0);
-  if (fast) {
-    const int D = s.D, Dh = D / 2, KSh = round_up8(Dh), KS = round_up8(D + Dh);
-    char* xh[3]; char* xl[3];
-    for (int i = 0; i < 3; ++i) { xh[i] = (char*)(ws + W.xs_hi[i]); xl[i] = (char*)(ws + W.xs_lo[i]); }
-    {
-      ProfScope ps(QAGNN_PROF_PRO_EPILOGUE, st);
-      int64_t g = (s.N * (Dh / 2) + 255) / 256;
-      if (g > kNumSMs * 32) g = kNumSMs * 32;
-      sin_basis_planes_kernel<<<(unsigned)g, 256, 0, st>>>(s.N, Dh, KSh, node_score, f + L.basis, (__nv_bfloat16*)(ws + W.sb_hi),
-                                                           single ? nullptr : (__nv_bfloat16*)(ws + W.sb_lo));
-      QAGNN_CHECK_LAUNCH();
-      // score_emb = GELU(emb_score(sin basis)) -> columns [D, D + D/2) of the H_in planes                   (:73)
-      TcOperand A{ws + W.sb_hi, ws + W.sb_lo, KSh, Dh}, none{nullptr, nullptr, 0, 0}, Wsc{f + L.ws_hi, f + L.ws_lo, KSh, Dh};
-      TcOutput o{};
-      o.hi = xh[0] + (size_t)D * 2; o.lo = xl[0] + (size_t)D * 2; o.ldp = KS;
-      QAGNN_RETURN_IF(gemm_tc(A, none, Wsc, f + L.bs, s.N, Dh, ACT_GELU, o, st, passes));
-      // ... and into the two activation buffers (layer-invariant: modeling_qagnn.py:86)
-      {
-        const int w4 = Dh * 2 / 8, ld8 = KS * 2 / 8;  // Dh % 4 == 0 and KS % 8 == 0 (checked by `fast`)
-        int64_t gc = (s.N * w4 + 255) / 256;
-        if (gc > kNumSMs * 16) gc = kNumSMs * 16;
-        const size_t off = (size_t)D * 2;
-        copy_plane_columns_kernel<<<(unsigned)gc, 256, 0, st>>>(s.N, w4, ld8, (const uint2*)(xh[0] + off),
-                                                              single ? nullptr : (const uint2*)(xl[0] + off),
-                                                              (uint2*)(xh[1] + off), (uint2*)(xl[1] + off), (uint2*)(xh[2] + off),
-                                                              (uint2*)(xl[2] + off));
-        QAGNN_CHECK_LAUNCH();
-      }
-      if (single) QAGNN_RETURN_IF(hi_plane_of(H_in_any, h_bf16, xh[0], KS, s.N, D, st));
-      else QAGNN_RETURN_IF(split_bf16(H_in, D, s.N, D, xh[0], xl[0], KS, st));
-    }
-    const size_t ND = (size_t)s.N * s.D;
-    Planes xin{xh[0], xl[0], KS};
-    const Planes ep{nullptr, nullptr, 0};
-    for (int l = 0; l < s.k; ++l) {  // mp_helper, :45-50 (dropout is the identity in eval)
-      float* xo32 = x_layers_out ? x_layers_out + (size_t)l * ND : nullptr;
-      void* ohi = xh[1 + (l & 1)];
-      void* olo = xl[1 + (l & 1)];
-      QAGNN_RETURN_IF(layer_forward_tc(s, L, W, l, xin, ep, prep, pl, f, xo32, ohi, olo, nullptr, nullptr, ws, ACT_GELU, tiled, st,
-                                       node_type, KS, passes, rg));
-      xin = Planes{ohi, olo, KS};
-    }
-    // output = GELU(Vh(H) + Vx(X))                                           (:92)
-    ProfScope ps(QAGNN_PROF_PRO_EPILOGUE, st);
-    TcOperand A1{xh[0], xl[0], KS, D}, A2{xin.hi, xin.lo, KS, D}, Wv{f + L.vcat_hi, f + L.vcat_lo, 2 * D, 2 * D};
-    TcOutput o{};
-    if (single) { o.hi = out_any; o.ldp = D; }
-    else { o.f32 = out; o.ldc = D; }
-    return gemm_tc(A1, A2, Wv, f + L.vbias, s.N, D, ACT_GELU, o, st, passes);
-  }
-  {
-    // tensor-core path: `extra` is only ever consumed as split-bf16 planes, so the prologue writes those directly
-    QAGNN_RETURN_IF(extra_forward(s, L, W, node_type, node_score, f, tc && s.D / 2 <= 128 ? nullptr : extra, ws, st,
-                                  tc ? ws + W.ep_hi : nullptr, tc && !single ? ws + W.ep_lo : nullptr));
-  }
-  if (tiled && !use_tc(s)) QAGNN_RETURN_IF(zero_head_pads(s, ws + W.qkm, st));
-  const size_t ND = (size_t)s.N * s.D;
-  if (tc) {
-    const int D = s.D;
-    {
-      ProfScope ps(QAGNN_PROF_PRO_EPILOGUE, st);
-      if (single) QAGNN_RETURN_IF(hi_plane_of(H_in_any, h_bf16, ws + W.hp_hi, D, s.N, D, st));
-      else QAGNN_RETURN_IF(split_bf16(H_in, D, s.N, D, ws + W.hp_hi, ws + W.hp_lo, D, st));
-    }
-    Planes xin{ws + W.hp_hi, ws + W.hp_lo};
-    const Planes ep{ws + W.ep_hi, ws + W.ep_lo};
-    for (int l = 0; l < s.k; ++l) {  // mp_helper, :45-50 (dropout is the identity in eval)
-      float* xo32 = x_layers_out ? x_layers_out + (size_t)l * ND : nullptr;
-      void* ohi = ws + W.xp_hi[l & 1];
-      void* olo = ws + W.xp_lo[l & 1];
-      QAGNN_RETURN_IF(layer_forward_tc(s, L, W, l, xin, ep, prep, pl, f, xo32, ohi, olo, nullptr, nullptr, ws, ACT_GELU,
-                                       tiled, st, nullptr, 0, passes, rg));
-      xin = Planes{ohi, olo};
-    }
-    // output = GELU(Vh(H) + Vx(X))                                           (:92)
-    ProfScope ps(QAGNN_PROF_PRO_EPILOGUE, st);
-    TcOperand A1{ws + W.hp_hi, ws + W.hp_lo, D, D}, A2{xin.hi, xin.lo, D, D}, Wv{f + L.vcat_hi, f + L.vcat_lo, 2 * D, 2 * D};
-    TcOutput o{};
-    if (single) { o.hi = out_any; o.ldp = D; }
-    else { o.f32 = out; o.ldc = D; }
-    if (s.k == 0) { A2 = A1; }
-    return gemm_tc(A1, A2, Wv, f + L.vbias, s.N, D, ACT_GELU, o, st, passes);
-  }
-  const float* x = H_in;
-  for (int l = 0; l < s.k; ++l) {  // mp_helper, :45-50 (dropout is the identity in eval)
-    float* xo = x_layers_out ? x_layers_out + (size_t)l * ND : ws + ((l & 1) ? W.xb : W.xa);
-    QAGNN_RETURN_IF(layer_forward(s, L, W, l, x, extra, prep, pl, f, xo, nullptr, nullptr, ws, ACT_GELU, tiled, st, rg));
-    x = xo;
-  }
-  // output = GELU(Vh(H) + Vx(X))                                             (:92)
-  ProfScope ps(QAGNN_PROF_PRO_EPILOGUE, st);
-  QAGNN_RETURN_IF(sgemm_tn(H_in, s.D, s.D, x, s.D, s.D, f + L.vcat, 2 * s.D, f + L.vbias, out, s.D, s.N, s.D, ACT_GELU, st));
-  if (single) return convert((int64_t)s.N * s.D, out, out_any, false, st);
-  return QAGNN_OK;
-}
-
-static int32_t check_mp_forward_args(const qagnn_shape* shape, const void* H_in, const int64_t* node_type,
-                                     const float* node_score, const void* prep, const void* folded, const void* out,
-                                     const void* workspace, size_t workspace_bytes) {
-  QAGNN_RETURN_IF(check_shape_fwd(shape));
-  if (!H_in || !node_type || !node_score || !prep || !folded || !out || !workspace) return QAGNN_ERR_INVALID_ARGUMENT;
-  if (workspace_bytes < make_work_layout(*shape).total * sizeof(float)) return QAGNN_ERR_WORKSPACE;
-  return QAGNN_OK;
-}
-
-extern "C" int32_t qagnn_mp_forward(const qagnn_shape* shape, const float* H_in, const int64_t* node_type,
-                                    const float* node_score, const void* prep, const void* folded, float* out,
-                                    float* x_layers_out, void* workspace, size_t workspace_bytes, void* stream) {
-  QAGNN_RETURN_IF(check_mp_forward_args(shape, H_in, node_type, node_score, prep, folded, out, workspace, workspace_bytes));
-  return mp_forward(*shape, 3, false, H_in, node_type, node_score, prep, folded, out, x_layers_out, (float*)workspace,
-                    (cudaStream_t)stream);
+// QAGNN_Message_Passing.forward (:53-95): fp32, or a bf16 output (dtype) from an fp32 or bf16 H (in_dtype)
+static int32_t mp_forward(const qagnn_shape* shape, int32_t dtype, int32_t in_dtype, const void* H_in, const int64_t* node_type,
+                          const float* node_score, const void* prep, const void* folded, void* out, float* x_layers_out,
+                          void* workspace, size_t workspace_bytes, void* stream, const Ragged& rg) {
+  const bool args_ok = H_in && node_type && node_score && prep && folded && out && workspace;
+  Fwd f;
+  QAGNN_RETURN_IF(setup_forward(shape, dtype, in_dtype, args_ok, prep, folded, workspace, workspace_bytes, stream, rg, f));
+  if (f.plan.tc) return mp_forward_tc(f, H_in, node_type, node_score, out, x_layers_out);
+  const void* in[1] = {H_in};
+  return ffma_forward(f, 1, in, out, [&](const float* const* in32, float* out32) {
+    return mp_forward_ffma(f, in32[0], node_type, node_score, out32, x_layers_out);
+  });
 }
 
 extern "C" int32_t qagnn_mp_forward_typed(const qagnn_shape* shape, int32_t dtype, int32_t in_dtype, const void* H_in,
                                           const int64_t* node_type, const float* node_score, const void* prep,
                                           const void* folded, void* out, float* x_layers_out, void* workspace,
                                           size_t workspace_bytes, void* stream) {
-  if (in_dtype != QAGNN_DTYPE_F32 && in_dtype != QAGNN_DTYPE_BF16) return QAGNN_ERR_INVALID_ARGUMENT;
-  if (dtype == QAGNN_DTYPE_F32) {
-    if (in_dtype != QAGNN_DTYPE_F32) return QAGNN_ERR_INVALID_ARGUMENT;
-    return qagnn_mp_forward(shape, (const float*)H_in, node_type, node_score, prep, folded, (float*)out, x_layers_out,
-                            workspace, workspace_bytes, stream);
-  }
-  if (dtype != QAGNN_DTYPE_BF16) return QAGNN_ERR_INVALID_ARGUMENT;
-  QAGNN_RETURN_IF(check_mp_forward_args(shape, H_in, node_type, node_score, prep, folded, out, workspace, workspace_bytes));
-  return mp_forward(*shape, 1, in_dtype == QAGNN_DTYPE_BF16, H_in, node_type, node_score, prep, folded, out, x_layers_out,
-                    (float*)workspace, (cudaStream_t)stream);
+  return mp_forward(shape, dtype, in_dtype, H_in, node_type, node_score, prep, folded, out, x_layers_out, workspace,
+                    workspace_bytes, stream, Ragged{});
+}
+
+extern "C" int32_t qagnn_mp_forward(const qagnn_shape* shape, const float* H_in, const int64_t* node_type,
+                                    const float* node_score, const void* prep, const void* folded, float* out,
+                                    float* x_layers_out, void* workspace, size_t workspace_bytes, void* stream) {
+  return qagnn_mp_forward_typed(shape, QAGNN_DTYPE_F32, QAGNN_DTYPE_F32, H_in, node_type, node_score, prep, folded, out,
+                                x_layers_out, workspace, workspace_bytes, stream);
 }
 
 extern "C" int32_t qagnn_mp_forward_ragged(const qagnn_shape* shape, int32_t dtype, int32_t in_dtype, int32_t n_graphs,
@@ -809,39 +787,8 @@ extern "C" int32_t qagnn_mp_forward_ragged(const qagnn_shape* shape, int32_t dty
                                            float* x_layers_out, void* workspace, size_t workspace_bytes, void* stream) {
   Ragged rg;
   QAGNN_RETURN_IF(check_ragged(shape, n_graphs, node_ptr, rg));
-  if (in_dtype != QAGNN_DTYPE_F32 && in_dtype != QAGNN_DTYPE_BF16) return QAGNN_ERR_INVALID_ARGUMENT;
-  if (dtype != QAGNN_DTYPE_F32 && dtype != QAGNN_DTYPE_BF16) return QAGNN_ERR_INVALID_ARGUMENT;
-  if (dtype == QAGNN_DTYPE_F32 && in_dtype != QAGNN_DTYPE_F32) return QAGNN_ERR_INVALID_ARGUMENT;
-  QAGNN_RETURN_IF(check_mp_forward_args(shape, H_in, node_type, node_score, prep, folded, out, workspace, workspace_bytes));
-  const bool single = dtype == QAGNN_DTYPE_BF16;
-  return mp_forward(*shape, single ? 1 : 3, in_dtype == QAGNN_DTYPE_BF16, H_in, node_type, node_score, prep, folded, out,
-                    x_layers_out, (float*)workspace, (cudaStream_t)stream, rg);
-}
-
-extern "C" int32_t qagnn_mp_core_forward(const qagnn_shape* shape, const void* prep, const float* qkm, const float* ke,
-                                         const float* me, float* aggr, float* alpha_scaled, float* alpha_out, float* scratch,
-                                         void* stream) {
-  QAGNN_RETURN_IF(check_shape_fwd(shape));
-  if (!prep || !qkm || !ke || !me || !aggr || !alpha_scaled || !scratch) return QAGNN_ERR_INVALID_ARGUMENT;
-  qagnn_prep_layout pl;
-  QAGNN_RETURN_IF(qagnn_graph_prep_layout(shape->N, shape->E, &pl));
-  cudaStream_t st = (cudaStream_t)stream;
-  ProfScope ps(QAGNN_PROF_MESSAGE_PASSING, st);
-  QAGNN_RETURN_IF(zero_alpha_holes(*shape, prep, pl, alpha_out, st));
-  return launch_message_passing(*shape, (const int32_t*)prep, pl, qkm, ke, me, scratch, alpha_scaled, aggr, alpha_out, st);
-}
-
-extern "C" int32_t qagnn_mp_core_backward(const qagnn_shape* shape, const void* prep, const int32_t* combo_order,
-                                          const float* qkm, const float* ke, const float* me, const float* alpha_scaled,
-                                          const float* d_aggr, float* d_qkm, float* d_ke, float* d_me, float* scratch,
-                                          void* stream) {
-  QAGNN_RETURN_IF(check_shape_fwd(shape));
-  if (!prep || !combo_order || !qkm || !ke || !me || !alpha_scaled || !d_aggr || !d_qkm || !d_ke || !d_me || !scratch)
-    return QAGNN_ERR_INVALID_ARGUMENT;
-  qagnn_prep_layout pl;
-  QAGNN_RETURN_IF(qagnn_graph_prep_layout(shape->N, shape->E, &pl));
-  return launch_message_passing_backward(*shape, (const int32_t*)prep, pl, combo_order, qkm, ke, me, alpha_scaled, d_aggr,
-                                         scratch, d_qkm, d_ke, d_me, (cudaStream_t)stream);
+  return mp_forward(shape, dtype, in_dtype, H_in, node_type, node_score, prep, folded, out, x_layers_out, workspace,
+                    workspace_bytes, stream, rg);
 }
 
 extern "C" size_t qagnn_mp_core_scratch_bytes(const qagnn_shape* shape, int32_t dtype) {
@@ -864,6 +811,12 @@ extern "C" int32_t qagnn_mp_core_forward_typed(const qagnn_shape* shape, int32_t
                                       alpha_out, st);
 }
 
+extern "C" int32_t qagnn_mp_core_forward(const qagnn_shape* shape, const void* prep, const float* qkm, const float* ke,
+                                         const float* me, float* aggr, float* alpha_scaled, float* alpha_out, float* scratch,
+                                         void* stream) {
+  return qagnn_mp_core_forward_typed(shape, QAGNN_DTYPE_F32, prep, qkm, ke, me, aggr, alpha_scaled, alpha_out, scratch, stream);
+}
+
 extern "C" int32_t qagnn_mp_core_backward_typed(const qagnn_shape* shape, int32_t dtype, const void* prep,
                                                 const int32_t* combo_order, const void* qkm, const void* ke, const void* me,
                                                 const float* alpha_scaled, const void* d_aggr, void* d_qkm, void* d_ke,
@@ -876,6 +829,14 @@ extern "C" int32_t qagnn_mp_core_backward_typed(const qagnn_shape* shape, int32_
   QAGNN_RETURN_IF(qagnn_graph_prep_layout(shape->N, shape->E, &pl));
   return launch_message_passing_backward_typed(*shape, (const int32_t*)prep, pl, dtype, combo_order, qkm, ke, me, alpha_scaled,
                                                d_aggr, scratch, d_qkm, d_ke, d_me, (cudaStream_t)stream);
+}
+
+extern "C" int32_t qagnn_mp_core_backward(const qagnn_shape* shape, const void* prep, const int32_t* combo_order,
+                                          const float* qkm, const float* ke, const float* me, const float* alpha_scaled,
+                                          const float* d_aggr, float* d_qkm, float* d_ke, float* d_me, float* scratch,
+                                          void* stream) {
+  return qagnn_mp_core_backward_typed(shape, QAGNN_DTYPE_F32, prep, combo_order, qkm, ke, me, alpha_scaled, d_aggr, d_qkm, d_ke,
+                                      d_me, scratch, stream);
 }
 
 extern "C" size_t qagnn_mp_core_backward_det_scratch_bytes(const qagnn_shape* shape, int32_t dtype) {

@@ -210,23 +210,15 @@ int32_t launch_message_passing_headtile(const qagnn_shape& s, const int32_t* pre
                                         cudaStream_t st, const Ragged& rg = Ragged{});
 int32_t zero_head_pads(const qagnn_shape& s, float* qkmh, cudaStream_t st);
 
-int32_t launch_message_passing(const qagnn_shape& s, const int32_t* prep_base, const qagnn_prep_layout& pl,
-                               const float* qkm, const float* ke, const float* me, float* score, float* alpha,
-                               float* aggr, float* alpha_out, cudaStream_t st);
-
 // column-sliced kernels with the edge tables in shared memory, for graphs too large for the per-graph tiles (mp_slice.cu)
 bool slice_supported(const qagnn_shape& s);
 int32_t launch_message_passing_slice(const qagnn_shape& s, const int32_t* prep_base, const qagnn_prep_layout& pl,
                                      const float* qkm, const float* ke, const float* me, float* score, float* aggr,
                                      float* alpha_out, cudaStream_t st);
 
-int32_t launch_message_passing_backward(const qagnn_shape& s, const int32_t* prep_base, const qagnn_prep_layout& pl,
-                                        const int32_t* combo_order, const float* qkm, const float* ke, const float* me,
-                                        const float* alpha_s, const float* d_aggr, float* ds, float* d_qkm, float* d_ke,
-                                        float* d_me, cudaStream_t st);
-
-// The training core on operands stored as `dtype` (QAGNN_DTYPE_*): qkm, ke, me, aggr, d_aggr, d_qkm, d_ke, d_me of that type;
-// score / alpha / alpha_out / alpha_s and the scratch fp32.  QAGNN_DTYPE_F32 runs exactly the two launchers above.
+// The basic CSR message passing (message_passing.cu: the forward's general path and the training core) and its gradient
+// (mp_backward.cu) on operands stored as `dtype` (QAGNN_DTYPE_*): qkm, ke, me, aggr, d_aggr, d_qkm, d_ke, d_me of that type;
+// score / alpha / alpha_out / alpha_s and the scratch fp32.
 int32_t launch_message_passing_typed(const qagnn_shape& s, const int32_t* prep_base, const qagnn_prep_layout& pl,
                                      int32_t dtype, const void* qkm, const void* ke, const void* me, float* score,
                                      float* alpha, void* aggr, float* alpha_out, cudaStream_t st);

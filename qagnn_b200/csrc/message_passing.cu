@@ -228,12 +228,6 @@ int32_t launch_mp(const qagnn_shape& s, const int32_t* prep_base, const qagnn_pr
 
 }  // namespace
 
-int32_t launch_message_passing(const qagnn_shape& s, const int32_t* prep_base, const qagnn_prep_layout& pl,
-                               const float* qkm, const float* ke, const float* me, float* score, float* alpha,
-                               float* aggr, float* alpha_out, cudaStream_t st) {
-  return launch_mp(s, prep_base, pl, qkm, ke, me, score, alpha, aggr, alpha_out, st);
-}
-
 int32_t launch_message_passing_typed(const qagnn_shape& s, const int32_t* prep_base, const qagnn_prep_layout& pl,
                                      int32_t dtype, const void* qkm, const void* ke, const void* me, float* score,
                                      float* alpha, void* aggr, float* alpha_out, cudaStream_t st) {

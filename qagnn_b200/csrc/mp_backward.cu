@@ -500,14 +500,6 @@ size_t mp_core_scratch_bytes(const qagnn_shape& s, int32_t dtype) {
   return sizeof(float) * (mp_core_ds_floats(s) + (dtype == QAGNN_DTYPE_F32 ? 0 : 2 * C * s.D));
 }
 
-int32_t launch_message_passing_backward(const qagnn_shape& s, const int32_t* prep_base, const qagnn_prep_layout& pl,
-                                        const int32_t* combo_order, const float* qkm, const float* ke, const float* me,
-                                        const float* alpha_s, const float* d_aggr, float* ds, float* d_qkm, float* d_ke,
-                                        float* d_me, cudaStream_t st) {
-  return launch_bwd<float>(s, prep_base, pl, combo_order, qkm, ke, me, alpha_s, d_aggr, ds, d_qkm, d_ke, d_me, nullptr, nullptr,
-                           DetTable{}, st);
-}
-
 int32_t launch_message_passing_backward_typed(const qagnn_shape& s, const int32_t* prep_base, const qagnn_prep_layout& pl,
                                               int32_t dtype, const int32_t* combo_order, const void* qkm, const void* ke,
                                               const void* me, const float* alpha_s, const void* d_aggr, float* scratch,
