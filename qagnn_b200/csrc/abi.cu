@@ -260,8 +260,9 @@ struct ForwardPlan {
   bool slice;      // without tiles: the column-sliced kernels (edge tables in shared memory) when the head width allows, else
                    // the basic CSR kernels.  QAGNN_MP_PATH=basic forces the latter.
   bool zero_pads;  // tiled on the FFMA GEMM: its head-major projection never writes the pad columns, so the call zeroes them once
-  bool fast;       // qagnn_mp_forward's fast-form projection (tiled, tc, k > 0, D/2 % 4 == 0): emb_score on the tensor cores
-                   // and the type-embedding half of node_feature_extra folded into per-node-type bias rows.
+  bool fast;       // qagnn_mp_forward's fast-form projection (tiled, tc, k > 0, D/2 % 4 == 0, D/2 >= 8): emb_score on the tensor
+                   // cores (a wgmma GEMM of width D/2, which must be at least 8) and the type-embedding half of
+                   // node_feature_extra folded into per-node-type bias rows.
                    // QAGNN_MP_FASTPROJ=0 keeps the general [x | extra] projection.
   bool mlp_fused;  // node MLP in one launch with the hidden layer in registers (tc, D <= 208), else mlp.0 and mlp.3 as two
                    // GEMMs with the hidden planes in the workspace.  QAGNN_MLP_FUSED=0 forces the two launches.
@@ -279,7 +280,7 @@ ForwardPlan plan_forward(const qagnn_shape& s, const Ragged& rg, int passes) {
   p.tiled = !general && headtile_supported(s, rg);
   p.slice = !p.tiled && !basic && slice_supported(s);
   p.zero_pads = p.tiled && !p.tc;
-  p.fast = p.tc && p.tiled && s.k > 0 && (s.D / 2) % 4 == 0 && !(fastproj && atoi(fastproj) == 0);
+  p.fast = p.tc && p.tiled && s.k > 0 && (s.D / 2) % 4 == 0 && s.D / 2 >= 8 && !(fastproj && atoi(fastproj) == 0);
   p.mlp_fused = p.tc && !(fused && atoi(fused) == 0) && mlp_tc_shape_ok(s.D);
   return p;
 }
