@@ -371,6 +371,19 @@ int32_t qagnn_decoder_tail_ragged(int32_t x_dtype, int32_t B, int32_t n, int32_t
                                   const int64_t *adj_lengths, const float *sent_vecs, const float *wk, const float *bk,
                                   const float *wv, const float *bv, float *concat, float *attn, void *stream);
 
+/* Gradient of qagnn_decoder_tail_ragged, for autograd through the ragged decoder tail.  Given d_concat [B, 2D+S] (fp32) and the
+ * forward's X, qs, attn and weights (node_ptr, adj_lengths as in the forward) it writes d_qs [B, D] (the gradient reaching
+ * w_qs(sent_vecs)), dX [N_rows, D] fp32 (zero on the tail rows and on every row the forward did not pool over; row 0 of each
+ * graph also receives d(Z)), and d_wk / d_wv [D, D], d_bk / d_bv [D], summed over the B graphs.  The d(sent_vecs) columns of
+ * d_concat are the caller's to pass on.  Every sum runs in a fixed order without atomics: two calls give the same bits.
+ * `scratch` holds qagnn_attention_pool_backward_ragged_scratch_bytes(B, n, D, n_head) bytes (0 for an invalid shape). */
+size_t qagnn_attention_pool_backward_ragged_scratch_bytes(int32_t B, int32_t n, int32_t D, int32_t n_head);
+int32_t qagnn_attention_pool_backward_ragged(int32_t x_dtype, int32_t B, int32_t n, int32_t D, int32_t n_head, int32_t S,
+                                             int64_t N_rows, const void *X, const int64_t *node_ptr, const int64_t *adj_lengths,
+                                             const float *qs, const float *wk, const float *bk, const float *wv, const float *attn,
+                                             const float *d_concat, float *dX, float *d_qs, float *d_wk, float *d_bk, float *d_wv,
+                                             float *d_bv, float *scratch, size_t scratch_bytes, void *stream);
+
 /* Launch counters since load (kernels this library enqueued); for bench.py's gpu_launches. */
 int64_t qagnn_launch_count(void);
 

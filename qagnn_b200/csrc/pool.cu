@@ -414,8 +414,242 @@ __global__ void __launch_bounds__(256) decoder_head_ragged_kernel(int n, int D, 
   }
 }
 
+// Gradient of the ragged decoder tail (attention_pool_kernel<XT, true>), with a = attn (saved by the forward), x_i the
+// graph's rows, qk_h = W_k,hᵀ qs_h and xs_h = Σ_i a_hi x_i, given dpooled = d(concat)[:, :D] and dZ = d(concat)[:, D+S:]:
+//   dxs_h = W_v,hᵀ dpooled_h;   g_hi = a_hi (dxs_h·x_i - Σ_i' a_hi' dxs_h·x_i') / sqrt(dk)   (the logit gradient, scaled)
+//   dX_i  = Σ_h (a_hi dxs_h + g_hi qk_h) + [i = 0] dZ;   dqk_h = Σ_i g_hi x_i;   dcst_h = Σ_i g_hi
+//   dqs_h = W_k,h dqk_h + b_k,h dcst_h;   dW_k,h += qs_h ⊗ dqk_h;   dW_v,h += dpooled_h ⊗ xs_h   (summed over graphs)
+// Three launches, every sum in a fixed order and no atomics, so two runs give the same bits: pool_backward_head_kernel (one
+// CTA per (graph, head)) writes the per-(graph, head) vectors to scratch, pool_backward_rows_kernel (one CTA per graph) sums
+// the heads into dX, and pool_backward_weights_kernel (one CTA per weight row) sums the graphs into dW_k, db_k, dW_v, db_v.
+// Scratch (fp32): qk | dxs | xs | dqk [B][nh][D] | g [nh*B][n] (the attn layout) | dcst [B][nh].
+struct PoolBwdScratch {
+  float *qk, *dxs, *xs, *dqk, *g, *dcst;
+  __host__ __device__ PoolBwdScratch(float* s, int B, int n, int D, int nh) {
+    const size_t v = (size_t)B * nh * D;
+    qk = s; dxs = qk + v; xs = dxs + v; dqk = xs + v; g = dqk + v; dcst = g + (size_t)nh * B * n;
+  }
+  static size_t floats(int B, int n, int D, int nh) { return 4 * (size_t)B * nh * D + (size_t)nh * B * n + (size_t)B * nh; }
+};
+
+constexpr int kPoolBwdThreads = 256;
+
+// rows of graph b the forward pooled over: [row0, row0 + nr), the same clamps as attention_pool_kernel<XT, true>
+__device__ __forceinline__ void ragged_graph_rows(int b, int n, const int64_t* node_ptr, const int64_t* adj_lengths,
+                                                  int64_t N_rows, int64_t& row0, int& nr) {
+  row0 = min(max(node_ptr[b], (int64_t)0), N_rows);
+  nr = (int)min(min((int64_t)n, N_rows - row0), max(node_ptr[b + 1] - row0, (int64_t)0));
+  nr = (int)min((int64_t)nr, max((int64_t)0, adj_lengths[b]));
+}
+
+// Sum of one value per lane over a warp, in a fixed order.
+__device__ __forceinline__ float warp_sum(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
+// dynamic smem: qk[D] | dxs[D] | dqk[D] | a[n] | g[n] | red[kPoolBwdThreads / 32]
+template <typename XT>
+__global__ void __launch_bounds__(kPoolBwdThreads) pool_backward_head_kernel(int n, int D, int nh, int S, int64_t N_rows,
+                                                                            const XT* __restrict__ X, const int64_t* __restrict__ node_ptr,
+                                                                            const int64_t* __restrict__ adj_lengths,
+                                                                            const float* __restrict__ qs, const float* __restrict__ wk,
+                                                                            const float* __restrict__ bk, const float* __restrict__ wv,
+                                                                            const float* __restrict__ attn, const float* __restrict__ dconcat,
+                                                                            float* __restrict__ dqs, float* __restrict__ scratch) {
+  extern __shared__ float sm[];
+  const int b = blockIdx.x, h = blockIdx.y, B = gridDim.x, tid = threadIdx.x, dk = D / nh;
+  const int warp = tid >> 5, lane = tid & 31, nwarps = kPoolBwdThreads / 32;
+  float* qk = sm;
+  float* dxs = qk + D;
+  float* dqk = dxs + D;
+  float* a = dqk + D;
+  float* g = a + n;
+  float* red = g + n;
+  PoolBwdScratch sc(scratch, B, n, D, nh);
+  int64_t row0;
+  int nr;
+  ragged_graph_rows(b, n, node_ptr, adj_lengths, N_rows, row0, nr);
+  const XT* Xb = X + (size_t)row0 * D;
+  const float inv_temp = 1.0f / sqrtf((float)dk);
+  const float* qsh = qs + (size_t)b * D + h * dk;
+  const float* dph = dconcat + (size_t)b * (2 * D + S) + h * dk;  // dpooled_h
+  const size_t vo = ((size_t)b * nh + h) * D;
+  for (int i = tid; i < nr; i += kPoolBwdThreads) a[i] = attn[((size_t)h * B + b) * n + i];
+  for (int j = tid; j < D; j += kPoolBwdThreads) {
+    float q = 0.f, d = 0.f;
+    for (int r = 0; r < dk; ++r) {
+      q = fmaf(qsh[r], wk[(size_t)(h * dk + r) * D + j], q);
+      d = fmaf(dph[r], wv[(size_t)(h * dk + r) * D + j], d);
+    }
+    qk[j] = q;
+    dxs[j] = d;
+    sc.qk[vo + j] = q;
+    sc.dxs[vo + j] = d;
+  }
+  __syncthreads();
+  // da_i = dxs·x_i (one warp per node) into g
+  for (int i = warp; i < nr; i += nwarps) {
+    float acc = 0.f;
+    for (int j = lane; j < D; j += 32) acc = fmaf(dxs[j], xval(Xb[(size_t)i * D + j]), acc);
+    acc = warp_sum(acc);
+    if (lane == 0) g[i] = acc;
+  }
+  // xs_h = Σ_i a_i x_i (one thread per column, nodes in order)
+  __syncthreads();
+  for (int j = tid; j < D; j += kPoolBwdThreads) {
+    float acc = 0.f;
+    for (int i = 0; i < nr; ++i) acc = fmaf(a[i], xval(Xb[(size_t)i * D + j]), acc);
+    sc.xs[vo + j] = acc;
+  }
+  if (warp == 0) {
+    float s = 0.f;
+    for (int i = lane; i < nr; i += 32) s = fmaf(a[i], g[i], s);
+    s = warp_sum(s);
+    if (lane == 0) red[0] = s;
+  }
+  __syncthreads();
+  const float sdot = red[0];
+  for (int i = tid; i < n; i += kPoolBwdThreads) {
+    const float gi = i < nr ? a[i] * (g[i] - sdot) * inv_temp : 0.f;
+    if (i < nr) g[i] = gi;
+    sc.g[((size_t)h * B + b) * n + i] = gi;
+  }
+  __syncthreads();
+  for (int j = tid; j < D; j += kPoolBwdThreads) {
+    float acc = 0.f;
+    for (int i = 0; i < nr; ++i) acc = fmaf(g[i], xval(Xb[(size_t)i * D + j]), acc);
+    dqk[j] = acc;
+    sc.dqk[vo + j] = acc;
+  }
+  if (warp == 0) {
+    float s = 0.f;
+    for (int i = lane; i < nr; i += 32) s += g[i];
+    s = warp_sum(s);
+    if (lane == 0) red[1] = s;
+  }
+  __syncthreads();
+  const float dcst = red[1];
+  if (tid == 0) sc.dcst[(size_t)b * nh + h] = dcst;
+  // dqs_h[r] = W_k[h*dk + r, :]·dqk + b_k[h*dk + r] dcst (one warp per row)
+  for (int r = warp; r < dk; r += nwarps) {
+    const float* w = wk + (size_t)(h * dk + r) * D;
+    float acc = 0.f;
+    for (int j = lane; j < D; j += 32) acc = fmaf(w[j], dqk[j], acc);
+    acc = warp_sum(acc);
+    if (lane == 0) dqs[(size_t)b * D + h * dk + r] = fmaf(bk[h * dk + r], dcst, acc);
+  }
+}
+
+// dX rows of graph b: Σ_h (a_hi dxs_h + g_hi qk_h), plus dZ on row 0.  Other rows are left as the caller zeroed them.
+__global__ void __launch_bounds__(kPoolBwdThreads) pool_backward_rows_kernel(int n, int D, int nh, int S, int64_t N_rows,
+                                                                            const int64_t* __restrict__ node_ptr,
+                                                                            const int64_t* __restrict__ adj_lengths,
+                                                                            const float* __restrict__ attn,
+                                                                            const float* __restrict__ dconcat,
+                                                                            const float* __restrict__ scratch, float* __restrict__ dX) {
+  const int b = blockIdx.x, B = gridDim.x;
+  PoolBwdScratch sc(const_cast<float*>(scratch), B, n, D, nh);
+  int64_t row0;
+  int nr;
+  ragged_graph_rows(b, n, node_ptr, adj_lengths, N_rows, row0, nr);
+  const float* dZ = dconcat + (size_t)b * (2 * D + S) + D + S;
+  for (int idx = threadIdx.x; idx < nr * D; idx += kPoolBwdThreads) {
+    const int i = idx / D, j = idx - i * D;
+    float acc = i == 0 ? dZ[j] : 0.f;
+    for (int h = 0; h < nh; ++h) {
+      const size_t vo = ((size_t)b * nh + h) * D + j, ao = ((size_t)h * B + b) * n + i;
+      acc = fmaf(attn[ao], sc.dxs[vo], acc);
+      acc = fmaf(sc.g[ao], sc.qk[vo], acc);
+    }
+    dX[(size_t)(row0 + i) * D + j] = acc;
+  }
+}
+
+// Row r of dW_k / dW_v (head h = r / dk) and db_k[r] / db_v[r]: sums over the graphs in order.
+__global__ void __launch_bounds__(kPoolBwdThreads) pool_backward_weights_kernel(int B, int n, int D, int nh, int S,
+                                                                               const float* __restrict__ qs,
+                                                                               const float* __restrict__ dconcat,
+                                                                               const float* __restrict__ scratch,
+                                                                               float* __restrict__ dwk, float* __restrict__ dbk,
+                                                                               float* __restrict__ dwv, float* __restrict__ dbv) {
+  const int r = blockIdx.x, h = r / (D / nh);
+  PoolBwdScratch sc(const_cast<float*>(scratch), B, n, D, nh);
+  const size_t ld = 2 * (size_t)D + S;
+  for (int j = threadIdx.x; j < D; j += kPoolBwdThreads) {
+    float ak = 0.f, av = 0.f;
+    for (int b = 0; b < B; ++b) {
+      const size_t vo = ((size_t)b * nh + h) * D + j;
+      ak = fmaf(qs[(size_t)b * D + r], sc.dqk[vo], ak);
+      av = fmaf(dconcat[b * ld + r], sc.xs[vo], av);
+    }
+    dwk[(size_t)r * D + j] = ak;
+    dwv[(size_t)r * D + j] = av;
+  }
+  if (threadIdx.x == 0) {
+    float ak = 0.f, av = 0.f;
+    for (int b = 0; b < B; ++b) {
+      ak = fmaf(qs[(size_t)b * D + r], sc.dcst[(size_t)b * nh + h], ak);
+      av += dconcat[b * ld + r];
+    }
+    dbk[r] = ak;
+    dbv[r] = av;
+  }
+}
+
+inline size_t pool_backward_smem_bytes(int n, int D) {
+  return ((size_t)3 * D + 2 * (size_t)n + kPoolBwdThreads / 32) * sizeof(float);
+}
+
+template <typename XT>
+int32_t pool_backward_ragged(int32_t B, int32_t n, int32_t D, int32_t n_head, int32_t S, int64_t N_rows, const XT* X,
+                             const int64_t* node_ptr, const int64_t* adj_lengths, const float* qs, const float* wk,
+                             const float* bk, const float* wv, const float* attn, const float* dconcat, float* dX, float* dqs,
+                             float* dwk, float* dbk, float* dwv, float* dbv, float* scratch, size_t scratch_bytes,
+                             cudaStream_t st) {
+  if (B <= 0 || n <= 0 || D <= 0 || n_head <= 0 || D % n_head != 0 || S < 0 || N_rows <= 0) return QAGNN_ERR_INVALID_ARGUMENT;
+  if (n_head > 8) return QAGNN_ERR_UNSUPPORTED;
+  if (!X || !node_ptr || !adj_lengths || !qs || !wk || !bk || !wv || !attn || !dconcat || !dX || !dqs || !dwk || !dbk || !dwv ||
+      !dbv || !scratch)
+    return QAGNN_ERR_INVALID_ARGUMENT;
+  if (scratch_bytes < PoolBwdScratch::floats(B, n, D, n_head) * sizeof(float)) return QAGNN_ERR_WORKSPACE;
+  const size_t smem = pool_backward_smem_bytes(n, D);
+  if (smem > 48 * 1024) return QAGNN_ERR_UNSUPPORTED;
+  QAGNN_CHECK_CUDA(cudaMemsetAsync(dX, 0, (size_t)N_rows * D * sizeof(float), st));
+  pool_backward_head_kernel<XT><<<dim3(B, n_head), kPoolBwdThreads, smem, st>>>(n, D, n_head, S, N_rows, X, node_ptr, adj_lengths,
+                                                                                qs, wk, bk, wv, attn, dconcat, dqs, scratch);
+  QAGNN_CHECK_LAUNCH();
+  pool_backward_rows_kernel<<<B, kPoolBwdThreads, 0, st>>>(n, D, n_head, S, N_rows, node_ptr, adj_lengths, attn, dconcat,
+                                                           scratch, dX);
+  QAGNN_CHECK_LAUNCH();
+  pool_backward_weights_kernel<<<D, kPoolBwdThreads, 0, st>>>(B, n, D, n_head, S, qs, dconcat, scratch, dwk, dbk, dwv, dbv);
+  QAGNN_CHECK_LAUNCH();
+  return QAGNN_OK;
+}
+
 }  // namespace
 }  // namespace qagnn
+
+extern "C" size_t qagnn_attention_pool_backward_ragged_scratch_bytes(int32_t B, int32_t n, int32_t D, int32_t n_head) {
+  if (B <= 0 || n <= 0 || D <= 0 || n_head <= 0 || D % n_head != 0) return 0;
+  return qagnn::PoolBwdScratch::floats(B, n, D, n_head) * sizeof(float);
+}
+
+extern "C" int32_t qagnn_attention_pool_backward_ragged(int32_t x_dtype, int32_t B, int32_t n, int32_t D, int32_t n_head,
+                                                        int32_t S, int64_t N_rows, const void* X, const int64_t* node_ptr,
+                                                        const int64_t* adj_lengths, const float* qs, const float* wk,
+                                                        const float* bk, const float* wv, const float* attn,
+                                                        const float* d_concat, float* dX, float* d_qs, float* d_wk, float* d_bk,
+                                                        float* d_wv, float* d_bv, float* scratch, size_t scratch_bytes,
+                                                        void* stream) {
+  if (x_dtype == QAGNN_DTYPE_F32)
+    return pool_backward_ragged(B, n, D, n_head, S, N_rows, (const float*)X, node_ptr, adj_lengths, qs, wk, bk, wv, attn, d_concat,
+                                dX, d_qs, d_wk, d_bk, d_wv, d_bv, scratch, scratch_bytes, (cudaStream_t)stream);
+  if (x_dtype != QAGNN_DTYPE_BF16) return QAGNN_ERR_INVALID_ARGUMENT;
+  return pool_backward_ragged(B, n, D, n_head, S, N_rows, (const __nv_bfloat16*)X, node_ptr, adj_lengths, qs, wk, bk, wv, attn,
+                              d_concat, dX, d_qs, d_wk, d_bk, d_wv, d_bv, scratch, scratch_bytes, (cudaStream_t)stream);
+}
 
 extern "C" int32_t qagnn_decoder_head_ragged(int32_t B, int32_t n, int32_t D, int64_t N_rows, const int64_t* concept_ids,
                                              int64_t n_concept, const float* table, const float* ctx, const float* node_scores,

@@ -120,28 +120,17 @@ class MultiheadAttPoolLayer(nn.Module):
     def pool_concat_ragged(self, q, k, node_ptr, node_type, adj_lengths, n):
         """pool_concat on a ragged batch (qagnn_decoder_tail_ragged): k [N_cap, D] and node_type [N_cap] are packed rows, graph b's
         from node_ptr[b] (device int64 [b + 1]); returns (concat [b, 2D + S], attn [n_head*b, n]) with attn exactly 0 at
-        positions >= adj_lengths[b].  Raises where pool_concat would return None: there is no padded fallback."""
+        positions >= adj_lengths[b].  Raises where pool_concat would return None: there is no padded fallback.
+        Differentiable in q, k and the w_qs / w_ks / w_vs parameters (qagnn_attention_pool_backward_ragged); attn is not."""
         from . import _lib
-        if self.training or not k.is_cuda or k.dtype not in _POOL_X_DTYPES:
-            raise ValueError("pool_concat_ragged: eval mode and a CUDA fp32 / bf16 k only")
-        lib = _lib.load()
-        N_cap, D = k.shape
-        b, S = q.size(0), q.size(1)
-        qc = _lib.f32c(q, "q")
-        qs = self.w_qs(qc).detach().float().contiguous()
-        kc = k.detach().contiguous()
-        concat = torch.empty(b, 2 * D + S, dtype=torch.float32, device=k.device)
-        attn = torch.empty(self.n_head * b, n, dtype=torch.float32, device=k.device)
-        with torch.cuda.device(k.device):
-            st = lib.qagnn_decoder_tail_ragged(_lib.DTYPE_CODES[kc.dtype], b, n, D, self.n_head, S, N_cap, _lib.ptr(kc),
-                                               _lib.ptr(_lib.i64c(node_ptr, "node_ptr")), _lib.ptr(qs),
-                                               _lib.ptr(_lib.i64c(node_type, "node_type")),
-                                               _lib.ptr(_lib.i64c(adj_lengths, "adj_lengths")), _lib.ptr(qc),
-                                               _lib.ptr(self.w_ks.weight.detach()), _lib.ptr(self.w_ks.bias.detach()),
-                                               _lib.ptr(self.w_vs.weight.detach()), _lib.ptr(self.w_vs.bias.detach()),
-                                               _lib.ptr(concat), _lib.ptr(attn), _lib.stream_ptr(k.device))
-        _lib.check(st, "qagnn_decoder_tail_ragged")
-        return concat, attn
+        if self.training or not k.is_cuda or k.dtype not in _POOL_X_DTYPES + (torch.float16,):
+            raise ValueError("pool_concat_ragged: eval mode and a CUDA fp32 / bf16 / fp16 k only")
+        if k.dtype == torch.float16:  # only the autograd decoder under fp16 autocast gives one: widened exactly
+            k = k.float()
+        _lib.f32c(q, "q")  # raises unless q is CUDA fp32: the kernel copies it into concat
+        qs = self.w_qs(q).float()
+        return _RaggedPoolConcat.apply(qs, k, q, self.w_ks.weight, self.w_ks.bias, self.w_vs.weight, self.w_vs.bias,
+                                       (node_ptr, node_type, adj_lengths, n, self.n_head))
 
     def forward(self, q, k, mask=None):
         b, l, _ = k.shape
@@ -177,6 +166,60 @@ class MultiheadAttPoolLayer(nn.Module):
         attn = self.attn_dropout(torch.softmax(logits, dim=2))
         pooled = torch.einsum("hbl,blhd->bhd", attn, vs).reshape(b, nh * dv)
         return self.dropout(pooled), attn.reshape(nh * b, l)
+
+
+class _RaggedPoolConcat(torch.autograd.Function):
+    """concat, attn = the ragged decoder tail (qagnn_decoder_tail_ragged) of qs = w_qs(q); its backward is
+    qagnn_attention_pool_backward_ragged, whose sums run in a fixed order, so the gradients are the same bits on every run."""
+
+    @staticmethod
+    def forward(ctx, qs, k, q, wk, bk, wv, bv, batch):
+        from . import _lib
+        lib = _lib.load()
+        node_ptr, node_type, adj_lengths, n, nh = batch
+        N_cap, D = k.shape
+        b, S = q.size(0), q.size(1)
+        qc, qsc = _lib.f32c(q, "q"), _lib.f32c(qs, "qs")
+        kc = k.detach().contiguous()
+        node_ptr, adj_lengths = _lib.i64c(node_ptr, "node_ptr"), _lib.i64c(adj_lengths, "adj_lengths")
+        wk, bk, wv, bv = (_lib.f32c(t, "pooler weight") for t in (wk, bk, wv, bv))
+        concat = torch.empty(b, 2 * D + S, dtype=torch.float32, device=k.device)
+        attn = torch.empty(nh * b, n, dtype=torch.float32, device=k.device)
+        with torch.cuda.device(k.device):
+            st = lib.qagnn_decoder_tail_ragged(_lib.DTYPE_CODES[kc.dtype], b, n, D, nh, S, N_cap, _lib.ptr(kc), _lib.ptr(node_ptr),
+                                               _lib.ptr(qsc), _lib.ptr(_lib.i64c(node_type, "node_type")), _lib.ptr(adj_lengths),
+                                               _lib.ptr(qc), _lib.ptr(wk), _lib.ptr(bk), _lib.ptr(wv), _lib.ptr(bv),
+                                               _lib.ptr(concat), _lib.ptr(attn), _lib.stream_ptr(k.device))
+        _lib.check(st, "qagnn_decoder_tail_ragged")
+        if any(ctx.needs_input_grad):
+            ctx.save_for_backward(qsc, kc, wk, bk, wv, attn, node_ptr, adj_lengths)
+            ctx.dims = (b, n, D, nh, S, N_cap)
+        ctx.mark_non_differentiable(attn)
+        return concat, attn
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, d_concat, _d_attn):
+        from . import _lib
+        lib = _lib.load()
+        qs, k, wk, bk, wv, attn, node_ptr, adj_lengths = ctx.saved_tensors
+        b, n, D, nh, S, N_cap = ctx.dims
+        dev = k.device
+        g = d_concat.float().contiguous()
+        dk = torch.empty(N_cap, D, dtype=torch.float32, device=dev)
+        dqs = torch.empty(b, D, dtype=torch.float32, device=dev)
+        dwk, dwv = torch.empty(D, D, dtype=torch.float32, device=dev), torch.empty(D, D, dtype=torch.float32, device=dev)
+        dbk, dbv = torch.empty(D, dtype=torch.float32, device=dev), torch.empty(D, dtype=torch.float32, device=dev)
+        nbytes = lib.qagnn_attention_pool_backward_ragged_scratch_bytes(b, n, D, nh)
+        scratch = torch.empty(max(nbytes // 4, 1), dtype=torch.float32, device=dev)
+        with torch.cuda.device(dev):
+            st = lib.qagnn_attention_pool_backward_ragged(_lib.DTYPE_CODES[k.dtype], b, n, D, nh, S, N_cap, _lib.ptr(k),
+                                                          _lib.ptr(node_ptr), _lib.ptr(adj_lengths), _lib.ptr(qs), _lib.ptr(wk),
+                                                          _lib.ptr(bk), _lib.ptr(wv), _lib.ptr(attn), _lib.ptr(g), _lib.ptr(dk),
+                                                          _lib.ptr(dqs), _lib.ptr(dwk), _lib.ptr(dbk), _lib.ptr(dwv), _lib.ptr(dbv),
+                                                          _lib.ptr(scratch), nbytes, _lib.stream_ptr(dev))
+        _lib.check(st, "qagnn_attention_pool_backward_ragged")
+        return dqs, dk.to(k.dtype), g[:, D:D + S], dwk, dbk, dwv, dbv, None
 
 
 class CustomizedEmbedding(nn.Module):

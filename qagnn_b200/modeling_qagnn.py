@@ -14,7 +14,8 @@ own parameters and device buffers (PyTorch = memory + streams).
 Modes: `.eval()` = the fused inference forward (dropout = identity, BatchNorm running statistics folded into the
 weights) — the reference's `evaluate_accuracy` path (qagnn.py:30-38); `.train()` = dropout, BatchNorm batch statistics
 and autograd through the CUDA message-passing forward / backward kernels (qagnn_b200/training.py; qagnn.py:249-278).
-CPU tensors raise: there is no CPU fallback.
+An `.eval()` call whose inputs require grad (under grad mode) takes that autograd path with eval semantics instead, so
+`backward()` reaches every parameter as in the reference.  CPU tensors raise: there is no CPU fallback.
 """
 import ctypes as C
 
@@ -37,17 +38,11 @@ def _version_key(tensors):
     return tuple((t.data_ptr(), t._version, tuple(t.shape)) for t in tensors)
 
 
-_warned_grad = set()
-
-
-def _warn_if_grad_wanted(what, *tensors):
-    """The eval-mode forward runs outside autograd (its outputs carry no grad_fn).  Say so once if a caller seems to
-    expect gradients; `.train()` selects the differentiable path (qagnn_b200/training.py)."""
-    if torch.is_grad_enabled() and what not in _warned_grad and any(t is not None and t.requires_grad for t in tensors):
-        import warnings
-        _warned_grad.add(what)
-        warnings.warn(f"qagnn_b200.{what}: eval-mode forward is not differentiable (inputs require grad but the output "
-                      f"has no grad_fn); call .train() for the autograd path")
+def _wants_autograd(module, *tensors):
+    """The differentiable path (qagnn_b200/training.py) runs in .train(), and in .eval() when grad mode is on and an input
+    requires grad (the rule MultiheadAttPoolLayer.forward applies); every other eval call runs the fused kernels, which
+    are outside autograd."""
+    return module.training or (torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in tensors))
 
 
 class _DeviceBlob:
@@ -241,11 +236,12 @@ def graph_prep(A, node_type, n, n_ntype, n_etype, validate):
     return GraphPrep(ei, et, nt, n_ntype, n_etype, 0, validate)
 
 
-def _ragged_eval_only(module, what, *tensors):
-    """A ragged batch runs the eval forward only: the reference's training BatchNorm statistics include the padded rows."""
-    if module.training or (torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in tensors)):
-        raise ValueError(f"{what}: a ragged batch runs in .eval() without gradients only; training keeps the padded layout "
-                         "because BatchNorm batch statistics include the padded rows")
+def _refuse_ragged_training(module, what):
+    """A ragged batch runs in .eval() only, with or without gradients: the reference's training BatchNorm statistics include
+    the padded rows, which a ragged batch does not have.  In eval a padding row is inert, so nothing else differs."""
+    if module.training:
+        raise ValueError(f"{what}: a ragged batch runs in .eval() only (gradients included); training keeps the padded "
+                         "layout because BatchNorm batch statistics include the padded rows")
 
 
 def _edge_encoder_params(enc):
@@ -361,17 +357,16 @@ class GATConvE(nn.Module):
         Returns out [N, emb_dim], or (out, (edge_index' [2,E+N], alpha [E+N, heads])) with
         return_attention_weights=True (alpha = softmax before the out-degree rescale, :473).  edge_index may be a
         qagnn_b200.data.PackedAdj (edge_type is then ignored), also one packed at an edge capacity: E is then its real
-        edge count.  A ragged PackedAdj (eval only) takes x / node_feature_extra [N_cap, emb_dim] and node_type [N_cap]."""
+        edge count.  A ragged PackedAdj (eval only) takes x / node_feature_extra [N_cap, emb_dim] and node_type [N_cap].
+        In .train(), or in .eval() with inputs that require grad, the output is differentiable (qagnn_b200/training.py)."""
         if getattr(edge_index, "ragged", False):
-            _ragged_eval_only(self, "GATConvE", x, node_feature_extra)
-        if self.training:  # dropout-free layer, BatchNorm batch statistics, autograd through the CUDA message passing
+            _refuse_ragged_training(self, "GATConvE")
+        if _wants_autograd(self, x, node_feature_extra):  # autograd through the CUDA message passing, this module's mode
             from . import training as TR
             if prep is None:
                 prep = self._prep(edge_index, edge_type, node_type)
-            tab = TR.edge_table_train(self.edge_encoder, TR.combo_onehot_table(self.n_ntype, self.n_etype, x.device),
-                                      prep.combo_count(), 1)
-            return TR.gatconve_train(self, x, node_feature_extra, node_type, prep, tab, return_attention_weights)
-        _warn_if_grad_wanted("GATConvE", x, node_feature_extra)
+            tab = TR.edge_table(self.edge_encoder, TR.combo_onehot_table(self.n_ntype, self.n_etype, x.device), prep, 1)
+            return TR.gatconve_autograd(self, x, node_feature_extra, node_type, prep, tab, return_attention_weights)
         lib = _lib.load()
         # under bf16 autocast: bf16 in and out, single-pass bf16 GEMMs (include/qagnn_b200.h, qagnn_gatconve_forward_typed)
         xc, dt = _lib.eval_dtype(x, "x")
@@ -510,21 +505,22 @@ class QAGNN_Message_Passing(nn.Module):
 
         With A a ragged qagnn_b200.data.PackedAdj (eval only): H [N_cap, d_node], node_type [N_cap], node_score [N_cap, 1],
         one row per node of the batch (rows past A.node_ptr[-1] unused); returns [N_cap, d_node].
+
+        In .train(), or in .eval() with H or node_score requiring grad, the output is differentiable (qagnn_b200/training.py).
         """
         ragged = getattr(A, "ragged", False)
         if ragged:
-            _ragged_eval_only(self, "QAGNN_Message_Passing", H, node_score)
+            _refuse_ragged_training(self, "QAGNN_Message_Passing")
         for status in self._replayed:  # never waits for the GPU: a replay whose copy has not landed is looked at later
             status.check("QAGNN_Message_Passing")
         self._replayed = [s for s in self._replayed if s.pending is not None]
-        if self.training:  # dropout, BatchNorm batch statistics, autograd through the CUDA message passing (training.py)
+        if _wants_autograd(self, H, node_score):  # autograd through the CUDA message passing, this module's mode (training.py)
             from . import training as TR
             if prep is None:  # a PackedAdj (possibly at an edge capacity) gets the packed prep, a plain pair the general one
                 n = H.size(1) if getattr(A, "graph_ptr_dev", None) is not None else 0
                 prep = graph_prep(A, node_type, n, self.n_ntype, self.n_etype, self.check_indices)
             self._last_prep = prep
-            return TR.mp_forward_train(self, H, A, node_type, node_score, prep)
-        _warn_if_grad_wanted("QAGNN_Message_Passing", H, node_score)
+            return TR.mp_forward_autograd(self, H, A, node_type, node_score, prep)
         if self.use_cuda_graph and prep is None and not return_layers:
             return self._graphed_forward(H, A, node_type, node_score)
         lib = _lib.load()
@@ -664,14 +660,7 @@ class QAGNN(nn.Module):
             _lib.check(st, "qagnn_decoder_head")
             s = s.unsqueeze(2)
         else:
-            gnn_input0 = self.activation(self.svec2nvec(sent_vecs)).unsqueeze(1)
-            gnn_input1 = self.concept_emb(concept_ids[:, 1:] - 1, emb_data).to(node_type_ids.device)
-            gnn_input = self.dropout_e(torch.cat([gnn_input0, gnn_input1], dim=1))
-            valid = (pos < adj_lengths.unsqueeze(1)).float()
-            s = -node_scores
-            s = (s - s[:, 0:1, :]).squeeze(2) * valid
-            mean_norm = s.abs().sum(dim=1) / adj_lengths
-            s = (s / (mean_norm.unsqueeze(1) + 1e-05)).unsqueeze(2)
+            gnn_input, s = self._head(sent_vecs, concept_ids, node_type_ids, node_scores, adj_lengths, emb_data)
 
         gnn_output = self.gnn(gnn_input, adj, node_type_ids, s)
         fused = self.pooler.pool_concat(sent_vecs, gnn_output, node_type_ids, adj_lengths) if not self.training else None
@@ -688,41 +677,75 @@ class QAGNN(nn.Module):
         concat = self.dropout_fc(torch.cat((graph_vecs, sent_vecs, Z_vecs), 1))
         return concat, pool_attn
 
+    def _head(self, sent_vecs, concept_ids, node_type_ids, node_scores, adj_lengths, emb_data):
+        """The input assembly in PyTorch ops (modeling_qagnn.py:153-167): (gnn_input [B, n, D], normalised scores [B, n, 1])."""
+        n = node_scores.size(1)
+        gnn_input0 = self.activation(self.svec2nvec(sent_vecs)).unsqueeze(1)
+        gnn_input1 = self.concept_emb(concept_ids[:, 1:] - 1, emb_data).to(node_type_ids.device)
+        gnn_input = self.dropout_e(torch.cat([gnn_input0, gnn_input1], dim=1))
+        valid = (torch.arange(n, device=node_scores.device) < adj_lengths.unsqueeze(1)).float()
+        s = -node_scores
+        s = (s - s[:, 0:1, :]).squeeze(2) * valid
+        mean_norm = s.abs().sum(dim=1) / adj_lengths
+        return gnn_input, (s / (mean_norm.unsqueeze(1) + 1e-05)).unsqueeze(2)
+
     def _pooled_features_ragged(self, sent_vecs, concept_ids, node_type_ids, node_scores, adj_lengths, adj, emb_data,
                                 cache_output):
         """pooled_features on a ragged PackedAdj (eval): the head writes only the valid positions of the padded [B, n] inputs
         as packed rows (qagnn_decoder_head_ragged), the message passing runs on adj.node_capacity rows and the tail pools each
-        graph over its own rows (qagnn_decoder_tail_ragged); `pool_attn` keeps the padded [n_head*B, n] layout."""
-        _ragged_eval_only(self, "QAGNN", sent_vecs, node_scores)
+        graph over its own rows (qagnn_decoder_tail_ragged); `pool_attn` keeps the padded [n_head*B, n] layout.
+        Under grad mode the head is the PyTorch one (as in the padded layout), its rows gathered into the packed layout, so
+        autograd scatters dL/d(packed rows) back to the padded positions; the padded batch's gradients result."""
+        _refuse_ragged_training(self, "QAGNN")
         if (emb_data is not None or not node_scores.is_cuda or self.concept_emb.use_contextualized or self.concept_dim % 4 != 0
                 or concept_ids.device != node_scores.device or sent_vecs.dtype != torch.float32):
             raise ValueError("QAGNN: a ragged batch needs the fused decoder head (CUDA inputs, fp32 sent_vecs, no contextualized "
                              "embeddings, concept_dim % 4 == 0)")
-        lib = _lib.load()
         B_, n = concept_ids.shape
         N_cap = adj.node_capacity
         dev = node_scores.device
-        table = self.concept_emb.projected_table()
-        ctx = self.activation(self.svec2nvec(sent_vecs)).float().contiguous()
         node_ptr = _lib.i64c(adj.node_ptr_dev, "node_ptr")
         if node_ptr.numel() != B_ + 1 or N_cap <= 0:
             raise ValueError("ragged PackedAdj: node_ptr must have one entry per graph plus one and node_capacity be set")
-        gnn_input = torch.empty(N_cap, self.concept_dim, dtype=torch.float32, device=dev)
-        s = torch.empty(N_cap, dtype=torch.float32, device=dev)
-        nt = torch.empty(N_cap, dtype=torch.int64, device=dev)
         al = _lib.i64c(adj_lengths, "adj_lengths")
-        with torch.cuda.device(dev):
-            st = lib.qagnn_decoder_head_ragged(B_, n, self.concept_dim, N_cap, _lib.ptr(_lib.i64c(concept_ids, "concept_ids")),
-                                               table.size(0), _lib.ptr(table), _lib.ptr(ctx),
-                                               _lib.ptr(_lib.f32c(node_scores.reshape(B_, n), "node_scores")), _lib.ptr(al),
-                                               _lib.ptr(_lib.i64c(node_type_ids, "node_type_ids")), _lib.ptr(node_ptr),
-                                               _lib.ptr(gnn_input), _lib.ptr(s), _lib.ptr(nt), _lib.stream_ptr(dev))
-        _lib.check(st, "qagnn_decoder_head_ragged")
-        gnn_output = self.gnn(gnn_input, adj, nt, s.unsqueeze(1))
+        if torch.is_grad_enabled():
+            gnn_input, s, nt = self._head_ragged(sent_vecs, concept_ids, node_type_ids, node_scores, al, node_ptr, N_cap)
+        else:
+            lib = _lib.load()
+            table = self.concept_emb.projected_table()
+            ctx = self.activation(self.svec2nvec(sent_vecs)).float().contiguous()
+            gnn_input = torch.empty(N_cap, self.concept_dim, dtype=torch.float32, device=dev)
+            s = torch.empty(N_cap, 1, dtype=torch.float32, device=dev)
+            nt = torch.empty(N_cap, dtype=torch.int64, device=dev)
+            with torch.cuda.device(dev):
+                st = lib.qagnn_decoder_head_ragged(B_, n, self.concept_dim, N_cap, _lib.ptr(_lib.i64c(concept_ids, "concept_ids")),
+                                                   table.size(0), _lib.ptr(table), _lib.ptr(ctx),
+                                                   _lib.ptr(_lib.f32c(node_scores.reshape(B_, n), "node_scores")), _lib.ptr(al),
+                                                   _lib.ptr(_lib.i64c(node_type_ids, "node_type_ids")), _lib.ptr(node_ptr),
+                                                   _lib.ptr(gnn_input), _lib.ptr(s), _lib.ptr(nt), _lib.stream_ptr(dev))
+            _lib.check(st, "qagnn_decoder_head_ragged")
+        gnn_output = self.gnn(gnn_input, adj, nt, s)
         concat, pool_attn = self.pooler.pool_concat_ragged(sent_vecs, gnn_output, node_ptr, nt, adj_lengths, n)
         if cache_output:
             self.concept_ids, self.adj, self.pool_attn = concept_ids, adj, pool_attn
         return concat, pool_attn
+
+    def _head_ragged(self, sent_vecs, concept_ids, node_type_ids, node_scores, adj_lengths, node_ptr, N_cap):
+        """(gnn_input [N_cap, D], scores [N_cap, 1], node types [N_cap]): the PyTorch head's values at the rows
+        qagnn_decoder_head_ragged writes.  Packed row r of graph b = position r - node_ptr[b] < adj_lengths[b]; the tail rows
+        get zeros, score 0 and type 2.  A gather, so its gradient is a scatter to exactly one padded position per row."""
+        B_, n = concept_ids.shape
+        gnn_input, s = self._head(sent_vecs, concept_ids, node_type_ids, node_scores, adj_lengths, None)
+        r = torch.arange(N_cap, device=node_ptr.device)
+        g = (torch.searchsorted(node_ptr, r, right=True) - 1).clamp_(0, B_ - 1)
+        i = r - node_ptr[g]
+        valid = (r < node_ptr[-1]) & (i < adj_lengths[g].clamp(max=n))
+        src = torch.where(valid, g * n + i, 0)
+        v = valid.unsqueeze(1)
+        gnn_input = torch.where(v, gnn_input.reshape(B_ * n, -1)[src], 0)
+        s = torch.where(v, s.reshape(B_ * n, 1)[src], 0)
+        nt = torch.where(valid, node_type_ids.reshape(-1)[src], 2)
+        return gnn_input, s, nt
 
     def forward(self, sent_vecs, concept_ids, node_type_ids, node_scores, adj_lengths, adj, emb_data=None,
                 cache_output=False):

@@ -1,9 +1,11 @@
-"""Training-mode forward + backward of the QA-GNN message-passing path (SURVEY.md §8f #3).
+"""Differentiable forward + backward of the QA-GNN message-passing path (SURVEY.md §8f #3).
 
 What the reference does in `qagnn.py:249-278` (`model.train()`, `loss.backward()`) for this path:
 dropout after every layer (`modeling_qagnn.py:49,93`), BatchNorm batch statistics in the shared
 `edge_encoder` (`:30`) and in every layer's `mlp` (`:408`), and autograd through
-`GATConvE.message` / `propagate` (`:442,455-484`).
+`GATConvE.message` / `propagate` (`:442,455-484`).  The same functions serve an eval-mode module whose caller wants
+gradients (fine-tuning the encoder under a frozen decoder, attributions): the modules' own mode then picks the reference's
+eval semantics, dropout the identity and every BatchNorm on its running statistics, and no buffer is written.
 
 Split here:
   * the graph part — logits, per-source softmax, out-degree rescale, per-target sum and ITS GRADIENT — runs in the
@@ -68,6 +70,14 @@ def edge_table_train(enc, onehot_tab, combo_count, k_calls):
             bn.running_var.mul_(keep).add_(unbiased * (1.0 - keep))
             bn.num_batches_tracked += k_calls
     return lin3(F.relu(y))
+
+
+def edge_table(enc, onehot_tab, prep, k_calls):
+    """tab[c] = edge_encoder(onehot(c)) [C, D] in the encoder's own mode: edge_table_train in .train(); in .eval() the module
+    itself, whose BatchNorm uses its running statistics, so no combo histogram is needed and no buffer changes."""
+    if enc.training:
+        return edge_table_train(enc, onehot_tab, prep.combo_count(), k_calls)
+    return enc(onehot_tab)
 
 
 def _core_dtype(*ts):
@@ -166,8 +176,10 @@ class _MPCore(torch.autograd.Function):
         return d_qkm, d_ke, d_me, None, None, None
 
 
-def gatconve_train(layer, x, extra, node_type, prep, tab, return_attention_weights=False):
-    """GATConvE.forward in training mode (modeling_qagnn.py:411-452) given the edge table `tab` [C, D]."""
+def gatconve_autograd(layer, x, extra, node_type, prep, tab, return_attention_weights=False):
+    """Differentiable GATConvE.forward (modeling_qagnn.py:411-452) given the edge table `tab` [C, D]; `layer.mlp`'s BatchNorm
+    takes batch or running statistics by its mode.  Row-local apart from the message passing, so a ragged prep needs nothing
+    more: x / extra are its [N_cap, D] packed rows."""
     D, H = layer.emb_dim, layer.head_count
     d = D // H
     x2 = torch.cat([x, extra], dim=1)                                        # :440
@@ -180,15 +192,16 @@ def gatconve_train(layer, x, extra, node_type, prep, tab, return_attention_weigh
     qkm = torch.cat([q, kx, mx], dim=1)
     aggr, alpha = _MPCore.apply(qkm, ke, me, prep, (x.size(0), prep.E, D, H, layer.n_ntype, layer.n_etype),
                                 return_attention_weights)
-    out = layer.mlp(aggr)                                                    # :443 (BatchNorm batch statistics)
+    out = layer.mlp(aggr)                                                    # :443
     if return_attention_weights:
         return out, (prep.edge_index_prime(), prep.compact_edges(alpha))
     return out
 
 
-def mp_forward_train(mod, H, A, node_type, node_score, prep):
-    """QAGNN_Message_Passing.forward in training mode (modeling_qagnn.py:53-95)."""
-    B, n, D = H.shape
+def mp_forward_autograd(mod, H, A, node_type, node_score, prep):
+    """Differentiable QAGNN_Message_Passing.forward (modeling_qagnn.py:53-95) with the module's dropout and BatchNorm
+    semantics.  H is [B, n, D], or a ragged batch's [N_cap, D] rows: every step around the message passing is row-local."""
+    D = H.size(-1)
     nt = node_type.reshape(-1)
     T_ = F.one_hot(nt, mod.n_ntype).to(H.dtype)
     type_emb = mod.activation(mod.emb_node_type(T_))                         # :65-66
@@ -196,11 +209,10 @@ def mp_forward_train(mod, H, A, node_type, node_score, prep):
     Bs = torch.sin(js.view(1, -1) * node_score.reshape(-1, 1))               # :70-72
     score_emb = mod.activation(mod.emb_score(Bs))                            # :73
     extra = torch.cat([type_emb, score_emb], dim=1)                          # :86
-    tab = edge_table_train(mod.edge_encoder, combo_onehot_table(mod.n_ntype, mod.n_etype, H.device), prep.combo_count(),
-                           max(mod.k, 1))
+    tab = edge_table(mod.edge_encoder, combo_onehot_table(mod.n_ntype, mod.n_etype, H.device), prep, max(mod.k, 1))
     X = H.reshape(-1, D)
     for layer in mod.gnn_layers:                                             # mp_helper :45-50
-        X = mod.activation(gatconve_train(layer, X, extra, nt, prep, tab))
-        X = F.dropout(X, mod.dropout_rate, training=True)
-    out = mod.activation(mod.Vh(H) + mod.Vx(X.view(B, n, D)))                # :92
+        X = mod.activation(gatconve_autograd(layer, X, extra, nt, prep, tab))
+        X = F.dropout(X, mod.dropout_rate, training=mod.training)
+    out = mod.activation(mod.Vh(H) + mod.Vx(X.view(H.shape)))                # :92
     return mod.dropout(out)                                                  # :93
