@@ -45,7 +45,7 @@
 extern "C" {
 #endif
 
-#define QAGNN_ABI_VERSION 3 /* 3: + training core, packed graph prep, decoder head / tail (round 2); ragged eval entry points */
+#define QAGNN_ABI_VERSION 3 /* 3: + training core, packed graph prep, decoder head / tail (round 2); ragged eval entry points; batch assembly */
 
 enum {
   QAGNN_OK = 0,
@@ -383,6 +383,21 @@ int32_t qagnn_attention_pool_backward_ragged(int32_t x_dtype, int32_t B, int32_t
                                              const float *qs, const float *wk, const float *bk, const float *wv, const float *attn,
                                              const float *d_concat, float *dX, float *d_qs, float *d_wk, float *d_bk, float *d_wv,
                                              float *d_bv, float *scratch, size_t scratch_bytes, void *stream);
+
+/* Batch assembly from a split held on the device (qagnn_b200.data.DeviceSplit): the packed adjacency of the B = bs * num_choice
+ * sub-graphs of the questions question_ids (device int64 [bs]), equal to FlatAdjCache.pack of the same ids bit for bit.  The split
+ * is the FlatAdjCache layout of G sub-graphs: local ids src / tgt int32 [E_split], etype int16 [E_split], graph_ptr int64 [G + 1]
+ * and, for a ragged batch, adj_lengths int64 [G]; graph g is choice g % num_choice of question g / num_choice.  Outputs:
+ *   edges int64 [3, K]: row 0 src + base, row 1 tgt + base, row 2 etype; columns [graph_ptr_out[B], K) are zero;
+ *   graph_ptr_out int64 [B + 1]: the first edge of every graph;
+ *   node_ptr_out int64 [B + 1] (N_cap >= 0 only): the exclusive cumsum of the graphs' adj_lengths;
+ * with base = b * n_nodes for a padded batch (N_cap = -1) and node_ptr_out[b] for a ragged one.  No host synchronisation and no
+ * atomics.  The caller checks the ids and capacities first; the kernels clamp ids to [0, G / num_choice), graph_ptr_out to K and
+ * node_ptr_out to N_cap, so a bad id or count never writes past K, N_cap or B + 1 entries.  Two launches (one when K = 0). */
+int32_t qagnn_assemble_batch(const int32_t *src, const int32_t *tgt, const int16_t *etype, const int64_t *graph_ptr,
+                             const int64_t *adj_lengths, int64_t G, int32_t num_choice, int32_t n_nodes,
+                             const int64_t *question_ids, int32_t bs, int64_t K, int64_t N_cap, int64_t *edges,
+                             int64_t *graph_ptr_out, int64_t *node_ptr_out, void *stream);
 
 /* Launch counters since load (kernels this library enqueued); for bench.py's gpu_launches. */
 int64_t qagnn_launch_count(void);

@@ -381,6 +381,145 @@ def load_flat_adj_cache(adj_pk_path, max_node_num, num_choice, args=None):
     return cids, ntypes, scores, lens, flat
 
 
+class DeviceSplit:
+    """A whole split on one GPU: the FlatAdjCache adjacency and the loader's decoder tensors, uploaded and validated once, so
+    a batch's only per-call input is its question ids.  `batch(question_ids, K[, node_capacity=N_cap])` gives on the device
+    what `flat.pack(question_ids, edge_capacity=K[, adj_lengths=..., node_capacity=N_cap]).to(device)` and the host-sliced
+    node arrays give, bit for bit: the adjacency from qagnn_assemble_batch (include/qagnn_b200.h), the node rows from
+    index_select.  Nothing reads the device: the batch checks and the PackedAdj's host fields come from host copies of the
+    per-graph edge counts and adj_lengths.
+
+    Held as: src / tgt int32 and etype int16 [E_split], graph_ptr int64 [G + 1], adj_lengths int64 [G], concept_ids and
+    node_type_ids int64 [G, n], node_scores fp32 [G, n, 1], with G = Q * num_choice sub-graphs.  At the loader's density
+    (~584 edges per graph) a split of 50 k graphs takes about 0.3 GB of adjacency and 0.2 GB of node arrays."""
+
+    def __init__(self, flat, concept_ids, node_type_ids, node_scores, adj_lengths, device, n_ntype, n_etype):
+        """What load_flat_adj_cache returns (concept_ids / node_type_ids [Q, nc, n], node_scores [Q, nc, n, 1], adj_lengths
+        [Q, nc], flat a FlatAdjCache), uploaded to `device`.  Raises IndexError naming the first offending question when an
+        edge's local ids leave [0, adj_length) of its graph, an etype leaves [0, n_etype), a node type leaves [0, n_ntype) or
+        an adj_length leaves [1, n]."""
+        self.device = torch.device(device)
+        self.num_choice, self.n_nodes = flat.num_choice, flat.n_nodes
+        nc, n = self.num_choice, self.n_nodes
+        G = flat.n_graphs()
+        self.n_questions = G // nc
+        self.counts = np.diff(np.asarray(flat.graph_ptr, dtype=np.int64))  # host copies: every batch is checked from these
+        self.lens = torch.as_tensor(adj_lengths).to("cpu", torch.long).reshape(-1)
+        shapes = {"concept_ids": concept_ids.reshape(-1, n), "node_type_ids": node_type_ids.reshape(-1, n),
+                  "node_scores": node_scores.reshape(-1, n, 1), "adj_lengths": self.lens}
+        for name, t in shapes.items():
+            if t.size(0) != G:
+                raise ValueError(f"DeviceSplit: {name} has {t.size(0)} graphs, the adjacency {G}")
+        dev = self.device
+        self.src = torch.from_numpy(np.ascontiguousarray(flat.src, dtype=np.int32)).to(dev)
+        self.tgt = torch.from_numpy(np.ascontiguousarray(flat.tgt, dtype=np.int32)).to(dev)
+        self.etype = torch.from_numpy(np.ascontiguousarray(flat.etype, dtype=np.int16)).to(dev)
+        self.graph_ptr = torch.from_numpy(np.ascontiguousarray(flat.graph_ptr, dtype=np.int64)).to(dev)
+        self.adj_lengths = self.lens.to(dev)
+        self.concept_ids = shapes["concept_ids"].to(dev, torch.long).contiguous()
+        self.node_type_ids = shapes["node_type_ids"].to(dev, torch.long).contiguous()
+        self.node_scores = shapes["node_scores"].to(dev, torch.float32).contiguous()
+        self._validate(int(n_ntype), int(n_etype))
+
+    def _validate(self, T, R):
+        """The split's indices, checked once on the device (one synchronisation per check)."""
+        nc, n, dev = self.num_choice, self.n_nodes, self.device
+        G = self.lens.numel()
+        edge_graph = torch.repeat_interleave(torch.arange(G, device=dev), torch.from_numpy(self.counts).to(dev))
+        rows = self.adj_lengths[edge_graph]
+        checks = (("an adj_length outside [1, %d]" % n, (self.adj_lengths < 1) | (self.adj_lengths > n), None),
+                  ("an edge outside its graph's rows [0, adj_length)",
+                   (self.src < 0) | (self.src >= rows) | (self.tgt < 0) | (self.tgt >= rows), edge_graph),
+                  ("an edge type outside [0, %d)" % R, (self.etype < 0) | (self.etype >= R), edge_graph),
+                  ("a node type outside [0, %d)" % T, ((self.node_type_ids < 0) | (self.node_type_ids >= T)).any(1), None))
+        for what, bad, graph_of in checks:
+            idx = torch.nonzero(bad)
+            if idx.numel():
+                g = int(idx[0, 0]) if graph_of is None else int(graph_of[idx[0, 0]])
+                raise IndexError(f"DeviceSplit: question {g // nc} (graph {g}) has {what}")
+
+    def check(self, question_ids, edge_capacity, node_capacity=None):
+        """The host checks of one batch, O(bs * num_choice), with FlatAdjCache.pack's exceptions: IndexError for a question id
+        outside [0, Q), ValueError for more than `edge_capacity` edges or (ragged) more than `node_capacity` rows.  Returns
+        (question ids int64 [bs], graph_ptr [B + 1], node_ptr [B + 1] or None, K, N_cap or -1), all on the host."""
+        q = np.asarray(question_ids, dtype=np.int64).reshape(-1)
+        if q.size == 0:
+            raise ValueError("DeviceSplit: an empty batch")
+        lo, hi = int(q.min()), int(q.max())
+        if lo < 0 or hi >= self.n_questions:
+            raise IndexError(f"DeviceSplit: question id {lo if lo < 0 else hi} is outside [0, {self.n_questions})")
+        gids = (q[:, None] * self.num_choice + np.arange(self.num_choice)[None, :]).reshape(-1)
+        ptr = np.zeros(len(gids) + 1, dtype=np.int64)
+        np.cumsum(self.counts[gids], out=ptr[1:])
+        K = _capacity(int(ptr[-1]), edge_capacity)
+        node_ptr, n_cap = None, -1
+        if node_capacity is not None:
+            node_ptr = node_ptr_of(self.lens[torch.from_numpy(gids)], self.n_nodes, len(gids))
+            n_cap = _node_capacity(int(node_ptr[-1]), node_capacity)
+        return q, torch.from_numpy(ptr), node_ptr, K, n_cap
+
+    def buffers(self, batch_size, edge_capacity, node_capacity=None):
+        """Device buffers for batches of `batch_size` questions at edge capacity K (and node capacity N_cap): the `out` of
+        assemble() / batch(), which a captured step fills in every replay."""
+        B, n, dev = int(batch_size) * self.num_choice, self.n_nodes, self.device
+        out = {"concept_ids": torch.empty(B, n, dtype=torch.long, device=dev),
+               "node_type_ids": torch.empty(B, n, dtype=torch.long, device=dev),
+               "node_scores": torch.empty(B, n, 1, dtype=torch.float32, device=dev),
+               "adj_lengths": torch.empty(B, dtype=torch.long, device=dev),
+               "edges": torch.empty(3, int(edge_capacity), dtype=torch.long, device=dev),
+               "graph_ptr": torch.empty(B + 1, dtype=torch.long, device=dev)}
+        if node_capacity is not None:
+            out["node_ptr"] = torch.empty(B + 1, dtype=torch.long, device=dev)
+        return out
+
+    def assemble(self, qids, edge_capacity, node_capacity=-1, out=None):
+        """The device half of batch(): enqueues the batch of the question ids `qids` (device int64 [bs], already checked)
+        without a host synchronisation.  Returns `out` (buffers()) filled; N_cap = -1 assembles a padded batch."""
+        from . import _lib
+        bs, K, N_cap = qids.numel(), int(edge_capacity), int(node_capacity)
+        if out is None:
+            out = self.buffers(bs, K, None if N_cap < 0 else N_cap)
+        dev = self.device
+        lib = _lib.load()
+        with torch.cuda.device(dev):
+            st = lib.qagnn_assemble_batch(_lib.ptr(self.src), _lib.ptr(self.tgt), _lib.ptr(self.etype), _lib.ptr(self.graph_ptr),
+                                          _lib.ptr(self.adj_lengths), self.lens.numel(), self.num_choice, self.n_nodes,
+                                          _lib.ptr(qids), bs, K, N_cap, _lib.ptr(out["edges"]), _lib.ptr(out["graph_ptr"]),
+                                          _lib.ptr(out.get("node_ptr")) if N_cap >= 0 else None, _lib.stream_ptr(dev))
+        _lib.check(st, "qagnn_assemble_batch")
+        # the rows of every choice of every question; ids are clamped as the kernel clamps them, so nothing reads out of range
+        gids = (qids.clamp(0, self.n_questions - 1).unsqueeze(1) * self.num_choice
+                + torch.arange(self.num_choice, device=dev).unsqueeze(0)).reshape(-1)
+        torch.index_select(self.concept_ids, 0, gids, out=out["concept_ids"])
+        torch.index_select(self.node_type_ids, 0, gids, out=out["node_type_ids"])
+        torch.index_select(self.node_scores, 0, gids, out=out["node_scores"])
+        torch.index_select(self.adj_lengths, 0, gids, out=out["adj_lengths"])
+        return out
+
+    def packed_adj(self, out, max_edges, edge_capacity, node_capacity=-1, graph_ptr=None, n_edges=-1, node_ptr=None):
+        """The PackedAdj over the buffers `out` (views, no copy); the host fields are the caller's (None / -1 when unknown)."""
+        e = out["edges"]
+        ragged = int(node_capacity) >= 0
+        return PackedAdj(e[:2], e[2], graph_ptr, self.n_nodes, e, out["graph_ptr"], int(max_edges), int(n_edges),
+                         int(edge_capacity), node_ptr, out["node_ptr"] if ragged else None, int(node_capacity))
+
+    def batch(self, question_ids, edge_capacity, node_capacity=None, out=None):
+        """(concept_ids [B, n], node_type_ids [B, n], node_scores [B, n, 1], adj_lengths [B], PackedAdj) on the device for the
+        questions `question_ids` (host ids, all their choices in order, B = bs * num_choice): the PackedAdj equals
+        `flat.pack(question_ids, edge_capacity=K, ...).to(device)` (ragged at `node_capacity` N_cap when given), with
+        graph_ptr_dev, node_ptr_dev, the batch's max_edges and both capacities set.  Checked on the host first (check()), so a
+        bad batch raises before anything is enqueued.  `out` (buffers()) names static buffers to fill."""
+        q, ptr, node_ptr, K, n_cap = self.check(question_ids, edge_capacity, node_capacity)
+        if out is not None and out["edges"].size(1) != K:
+            raise ValueError(f"DeviceSplit: the buffers hold {out['edges'].size(1)} edge columns, the batch needs {K}")
+        qh = torch.from_numpy(q)
+        qd = (qh.pin_memory() if self.device.type == "cuda" else qh).to(self.device, non_blocking=True)
+        out = self.assemble(qd, K, n_cap, out)
+        me = int((ptr[1:] - ptr[:-1]).max()) if ptr.numel() > 1 else 0
+        adj = self.packed_adj(out, me, K, n_cap, ptr, int(ptr[-1]), node_ptr)
+        return out["concept_ids"], out["node_type_ids"], out["node_scores"], out["adj_lengths"], adj
+
+
 class PackedAdjBatchGenerator:
     """Drop-in for the reference's MultiGPUSparseAdjDataBatchGenerator (utils/data_utils.py:17-76): same constructor, same
     batch tuple  (qids, labels, *tensors0, *lists0, *tensors1, *lists1, edge_index, edge_type),  same partial-batch

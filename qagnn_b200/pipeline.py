@@ -15,6 +15,9 @@ batch still pays its own H2D and D2H; they just stop serialising with the kernel
 
 `TrainStep` is the training counterpart of DecoderStep: QAGNN.forward in .train() and its backward as two CUDA graphs,
 behind one autograd node, for the micro-steps of qagnn.py:252-278.
+
+`SplitEvalStep` evaluates a split held on the GPU (qagnn_b200.data.DeviceSplit): one CUDA graph assembles a batch from its
+question ids and runs QAGNN.forward in .eval() on it, so nothing of the batch is packed or uploaded on the host.
 """
 import contextlib
 
@@ -415,6 +418,109 @@ class TrainStep:
         # the replay changed the running statistics behind autograd's back: the eval path's folded weights key on versions
         torch.autograd.graph.increment_version(self._bn_buffers)
         return out
+
+
+class SplitEvalStep:
+    """Evaluation of a split held on the GPU (qagnn_b200.data.DeviceSplit) as one CUDA graph per step: batch assembly from the
+    question ids (qagnn_assemble_batch), the node-row gathers and `decoder(...)` itself under no_grad, i.e. QAGNN.forward in
+    .eval() (head kernel -> message passing -> pooling tail -> fc).  A call's only inputs are the question ids and sent_vecs:
+
+        step = SplitEvalStep(model.decoder.eval(), split, bs, edge_capacity=K, max_edges=M)
+        logits, pool_attn = step(qids, sent_vecs)      # static buffers, overwritten by the next call
+
+    Each call checks the batch on the host (DeviceSplit.check: IndexError / ValueError before anything is enqueued), copies
+    the ids and sent_vecs (as fp32, which both decoder heads read) into static buffers and replays the graph.  The results
+    equal `decoder(sent_vecs.float(), *split.batch(qids, K, node_capacity))` under the same autocast, bit for bit.
+    `node_capacity` N_cap (data.split_node_capacity) makes the step ragged; `max_edges` bounds one sub-graph's edges over the
+    split (FlatAdjCache.max_graph_edges()).  `autocast_dtype` is None or torch.bfloat16, as for DecoderStep.  One GPU.
+
+    The graph bakes in the folded weights and the projected concept table.  A call whose decoder changed since capture (an
+    optimiser step, load_state_dict, .to(): the parameter and buffer versions, the folded weights' and the projected table's
+    cache keys) captures again first, so results are never computed from stale weights; in-place `.data` edits need
+    `decoder.gnn.invalidate()` / `decoder.concept_emb.invalidate_table()` as for eager calls.  The first call captures, on its own
+    batch; a capture raises ValueError when the packed graph prep refuses the split's sub-graphs.  Every call needs exactly
+    `batch_size` questions: run a final partial batch eagerly through split.batch + decoder, or with a step of its size."""
+
+    def __init__(self, decoder, split, batch_size, *, edge_capacity, max_edges, node_capacity=None, autocast_dtype=None,
+                 use_cuda_graph=True):
+        if autocast_dtype not in (None, torch.bfloat16):
+            raise ValueError("autocast_dtype must be None or torch.bfloat16")
+        if decoder.training:
+            raise ValueError("SplitEvalStep runs the eval forward: call decoder.eval() first")
+        self.decoder, self.split, self.autocast_dtype = decoder, split, autocast_dtype
+        self.batch_size, self.edge_capacity, self.max_edges = int(batch_size), int(edge_capacity), int(max_edges)
+        self.node_capacity = node_capacity
+        self._n_cap = -1 if node_capacity is None else int(node_capacity)
+        dev = split.device
+        B = self.batch_size * split.num_choice
+        self._qids = torch.zeros(self.batch_size, dtype=torch.int64, device=dev)
+        self._sv = torch.zeros(B, decoder.svec2nvec.in_features, dtype=torch.float32, device=dev)
+        self._out = split.buffers(self.batch_size, self.edge_capacity, node_capacity)
+        self._adj = split.packed_adj(self._out, self.max_edges, self.edge_capacity, self._n_cap)
+        self.use_cuda_graph = use_cuda_graph
+        self.graph, self._status, self._key, self.captures = None, None, None, 0
+        self.logits = self.pool_attn = None
+        self.mode = "eager"
+
+    def _autocast(self):
+        if self.autocast_dtype is None:
+            return contextlib.nullcontext()
+        return torch.autocast("cuda", dtype=self.autocast_dtype, cache_enabled=False)
+
+    def _weights_key(self):
+        """What the decoder's caches key on: parameter and buffer versions, the folded weights' key and the projected table's."""
+        from .modeling_qagnn import _version_key
+        dec = self.decoder
+        return (_version_key(list(dec.parameters()) + list(dec.buffers())), dec.gnn._folded.key,
+                getattr(dec.concept_emb, "_ptab_key", None))
+
+    def _load(self, question_ids, sent_vecs):
+        q = self.split.check(question_ids, self.edge_capacity, self.node_capacity)[0]
+        if q.size != self.batch_size:
+            raise ValueError(f"SplitEvalStep: {q.size} questions, the step was built for {self.batch_size}; run a partial "
+                             "batch through split.batch + decoder")
+        if tuple(sent_vecs.shape) != tuple(self._sv.shape):
+            raise ValueError(f"SplitEvalStep: sent_vecs is {tuple(sent_vecs.shape)}, the step was built for {tuple(self._sv.shape)}")
+        # a pinned block from the caching host allocator per call: it is not reused before this copy has run
+        self._qids.copy_(torch.from_numpy(q).pin_memory(), non_blocking=True)
+        if self._sv.data_ptr() != sent_vecs.data_ptr():
+            self._sv.copy_(sent_vecs)
+
+    @torch.no_grad()
+    def _body(self):
+        with self._autocast():
+            out = self.split.assemble(self._qids, self.edge_capacity, self._n_cap, self._out)
+            return self.decoder(self._sv, out["concept_ids"], out["node_type_ids"], out["node_scores"], out["adj_lengths"],
+                                self._adj)
+
+    def _capture(self):
+        self.graph = self._status = None  # frees the previous capture's pool before the next one is made
+        gnn = self.decoder.gnn
+        self.split.assemble(self._qids, self.edge_capacity, self._n_cap, self._out)  # capture_guard validates this batch
+        self.graph, (self.logits, self.pool_attn), self._status = capture(gnn, self._adj, self._out["node_type_ids"],
+                                                                          "SplitEvalStep", self._body)
+        self._keep = (gnn._ws.buf, gnn._folded.blob, gnn._last_prep, getattr(self.decoder.concept_emb, "_ptab", None))
+        self._key = self._weights_key()
+        self.captures += 1
+        self.mode = "one CUDA graph (assembly + gathers + head + prep + k layers + pooling + fc)"
+
+    def __call__(self, question_ids, sent_vecs):
+        """(logits [bs*nc, 1], pool_attn) of the questions `question_ids` (host ids, bs of them) with their sent_vecs
+        [bs*nc, S] (device); static buffers that the next call overwrites."""
+        if self.decoder.training:
+            raise RuntimeError("SplitEvalStep runs the eval forward: call decoder.eval() first")
+        if self._status is not None:
+            self._status.check("SplitEvalStep")
+        self._load(question_ids, sent_vecs)
+        if not self.use_cuda_graph:
+            self.logits, self.pool_attn = self._body()
+            return self.logits, self.pool_attn
+        if self.graph is None or self._weights_key() != self._key:
+            self._capture()  # on the batch just loaded, which the host checks accepted
+        self.graph.replay()
+        if self._status is not None:
+            self._status.replayed()
+        return self.logits, self.pool_attn
 
 
 def packed_host_batch(adj, H, node_type, node_score, sent_vecs, adj_lengths):
