@@ -38,7 +38,8 @@ def fingerprint(*tensors):
 
 
 # ---------------------------------------------------------------------------------------------
-# case table (shared with the tests through the saved 'case' dict)
+# case table (shared with the tests through the saved 'case' dict).  A case without n_ntype / n_etype is minted at the
+# reference's (4, 38); the fixture records the pair it was minted at either way.
 # ---------------------------------------------------------------------------------------------
 MP_CASES = [
     # name, B, n, e/graph, D, k, regime, realistic, seed
@@ -49,6 +50,8 @@ MP_CASES = [
     dict(name="cfg2small_realistic", B=5, n=200, e=1000, D=200, k=5, regime="peaky", realistic=True, seed=3),
     dict(name="tiny_realistic_d100", B=6, n=24, e=60, D=100, k=3, regime="peaky", realistic=True, seed=4),
     dict(name="no_edges", B=3, n=10, e=0, D=64, k=2, regime="peaky", realistic=False, seed=5),
+    # six node types and five relations (C = R*T*T + T = 186): node types come from all of [0, T)
+    dict(name="mp_t6_r5", B=3, n=40, e=150, D=64, k=2, regime="peaky", realistic=False, seed=6, n_ntype=6, n_etype=5),
 ]
 
 # single-layer GATConvE cases (hand-built graphs and non-default head counts)
@@ -60,6 +63,10 @@ LAYER_CASES = [
     dict(name="layer_src_only_tgt_only", N=9, E=0, D=64, H=4, regime="peaky", seed=14, kind="bipartite"),
     dict(name="layer_hub", N=300, E=0, D=64, H=4, regime="peaky", seed=15, kind="hub"),
     dict(name="layer_single_node", N=1, E=0, D=64, H=4, regime="peaky", seed=16, kind="random"),
+    # other (node type, relation) counts T, R: the combo count C = R*T*T + T sizes every edge table
+    dict(name="layer_t1_r5", N=120, E=600, D=64, H=4, regime="peaky", seed=17, kind="random", n_ntype=1, n_etype=5),
+    dict(name="layer_t7_r3", N=120, E=600, D=64, H=4, regime="peaky", seed=18, kind="random", n_ntype=7, n_etype=3),
+    dict(name="layer_t16_r23", N=120, E=600, D=64, H=4, regime="peaky", seed=19, kind="random", n_ntype=16, n_etype=23),
 ]
 
 
@@ -104,7 +111,7 @@ def layer_state_dict(case, n_ntype=4, n_etype=38):
 
 @torch.no_grad()
 def mint_mp_case(ref, case, n_ntype=4, n_etype=38):
-    inp = O.synth_graph_batch(case["B"], case["n"], case["e"], case["D"], n_etype, case["seed"], case["realistic"])
+    inp = O.synth_graph_batch(case["B"], case["n"], case["e"], case["D"], n_etype, case["seed"], case["realistic"], n_ntype)
     sd = O.random_state_dict(case["k"], case["D"], n_ntype, n_etype, case["regime"], case["seed"])
     mod = ref.QAGNN_Message_Passing(None, k=case["k"], n_ntype=n_ntype, n_etype=n_etype, input_size=case["D"],
                                     hidden_size=case["D"], output_size=case["D"], dropout=0.2)
@@ -317,32 +324,44 @@ def all_cases():
             [(mint_decoder_case, c) for c in DEC_CASES])
 
 
+def mint_case(ref, mint, case):
+    """One fixture, at the case's own (n_ntype, n_etype) or the reference's (4, 38)."""
+    return mint(ref, case, case.get("n_ntype", 4), case.get("n_etype", 38))
+
+
 def check(names=None):
     """Re-mints every fixture (or those in `names`) from the reference in memory and returns {name: max |diff|} against the
-    committed file — nothing is written.  0.0 everywhere = the fixtures are what the reference's own modules produce here."""
+    committed file — nothing is written.  0.0 everywhere = the fixtures are what the reference's own modules produce here.
+    A case whose file is not in the tree maps to None."""
     torch.set_num_threads(8)
     ref = load_reference()
     out = {}
     for mint, case in all_cases():
         if names is not None and case["name"] not in names:
             continue
-        have = torch.load(os.path.join(GOLDEN_DIR, case["name"] + ".pt"), weights_only=False)
-        out[case["name"]] = _max_diff(mint(ref, case), have, case["name"])
+        path = os.path.join(GOLDEN_DIR, case["name"] + ".pt")
+        if not os.path.exists(path):  # nothing committed to compare with (tests/test_oracle_golden.py requires every file)
+            out[case["name"]] = None
+            continue
+        have = torch.load(path, weights_only=False)
+        out[case["name"]] = _max_diff(mint_case(ref, mint, case), have, case["name"])
     return out
 
 
 def fuzz_cases(count):
     """The random small cases of --fuzz, deterministic: 1-4 graphs, 1-30 nodes, 0-80 edges, D 16-100, k 1-3, 6 / 17 / 38
-    edge types, both weight regimes."""
+    edge types, 1 / 3 / 4 / 6 node types, both weight regimes."""
     g = torch.Generator().manual_seed(12345)
     ri = lambda lo, hi: int(torch.randint(lo, hi + 1, (1,), generator=g))  # noqa: E731
     cases = []
     for i in range(count):
         n = ri(1, 30)
         R = (38, 38, 6, 17)[ri(0, 3)]
+        T = (1, 3, 4, 6)[ri(0, 3)]
         case = dict(name=f"fuzz{i}", B=ri(1, 4), n=n, e=ri(0, 80), D=(16, 32, 64, 100)[ri(0, 3)], k=ri(1, 3),
-                    regime=("prod", "peaky")[ri(0, 1)], realistic=bool(ri(0, 1)) and n >= 8 and R >= 6, seed=100 + i)
-        cases.append(dict(case, n_etype=R))
+                    regime=("prod", "peaky")[ri(0, 1)], realistic=bool(ri(0, 1)) and n >= 8 and R >= 6 and T >= 4,
+                    seed=100 + i)
+        cases.append(dict(case, n_ntype=T, n_etype=R))
     return cases
 
 
@@ -355,10 +374,11 @@ def fuzz_compared(out, extra, layers, keep):
 
 
 def oracle_fuzz_outputs(case):
-    inp = O.synth_graph_batch(case["B"], case["n"], case["e"], case["D"], case["n_etype"], case["seed"], case["realistic"])
-    sd = O.random_state_dict(case["k"], case["D"], 4, case["n_etype"], case["regime"], case["seed"])
+    T, R = case.get("n_ntype", 4), case["n_etype"]  # fuzz files minted before T varied hold 4-type cases without the key
+    inp = O.synth_graph_batch(case["B"], case["n"], case["e"], case["D"], R, case["seed"], case["realistic"], T)
+    sd = O.random_state_dict(case["k"], case["D"], T, R, case["regime"], case["seed"])
     return O.message_passing_forward(sd, inp["H"], inp["edge_index"], inp["edge_type"], inp["node_type"], inp["node_score"],
-                                     case["k"], 4, case["n_etype"], return_layers=True)
+                                     case["k"], T, R, return_layers=True)
 
 
 def fuzz(count, tol_abs=2e-6, tol_rel=2e-5):
@@ -369,7 +389,7 @@ def fuzz(count, tol_abs=2e-6, tol_rel=2e-5):
     ref = load_reference()
     results = []
     for case in fuzz_cases(count):
-        fx = mint_mp_case(ref, case, 4, case["n_etype"])
+        fx = mint_mp_case(ref, case, case["n_ntype"], case["n_etype"])
         out, extra, layers = oracle_fuzz_outputs(case)
         keep = sorted(fx["layers"])
         got = dict(fuzz_compared(out, extra, layers, keep))
@@ -385,7 +405,7 @@ def mint_fuzz_samples(ref, count=24):
     cases, entries, index, value = [], [], [], []
     off = 0
     for ci, case in enumerate(fuzz_cases(count)):
-        fx = mint_mp_case(ref, case, 4, case["n_etype"])
+        fx = mint_mp_case(ref, case, case["n_ntype"], case["n_etype"])
         keep = sorted(fx["layers"])
         cases.append(dict(case, keep=keep))
         for name, t in fuzz_compared(fx["out"], fx["extra"], fx["layers"], keep):
@@ -467,6 +487,9 @@ def main():
     if "--check" in sys.argv[1:]:
         worst = 0.0
         for name, diff in check().items():
+            if diff is None:
+                print(f"{name}: no committed fixture")
+                continue
             print(f"{name}: max |re-minted - committed| = {diff:.3g}")
             worst = max(worst, diff)
         sys.exit(0 if worst == 0.0 else 1)
@@ -474,7 +497,7 @@ def main():
     ref = load_reference()
     os.makedirs(GOLDEN_DIR, exist_ok=True)
     for mint, case in all_cases():
-        fx = mint(ref, case)
+        fx = mint_case(ref, mint, case)
         torch.save(fx, os.path.join(GOLDEN_DIR, case["name"] + ".pt"))
         print("minted", case["name"], fx.get("kind"))
     os.makedirs(REF_DATA_DIR, exist_ok=True)

@@ -302,20 +302,24 @@ def graph_prep_oracle(edge_index, edge_type, node_type, n_ntype, n_etype):
 # ----------------------------------------------------------------------------------------------
 # Deterministic synthetic inputs (SURVEY.md §8d); shared by tests, goldens and bench
 # ----------------------------------------------------------------------------------------------
-def synth_graph_batch(B, n, e_per_graph, D, n_etype=38, seed=0, realistic=False):
+def synth_graph_batch(B, n, e_per_graph, D, n_etype=38, seed=0, realistic=False, n_ntype=4):
     """cfg-1/cfg-2 style batch: x, extra-free inputs for QAGNN_Message_Passing.
 
     Plain variant: edge endpoints ~ U{0..n-1}^2 (+g*n), duplicates and i->i allowed; edge_type
-    ~ U{0..R-1}; node_type ~ U{0,1,2} with node 0 of each graph = 3; H ~ N(0,1)*0.5; scores N(0,1).
-    Realistic variant: adj_lengths ~ U{8..n}, min(e/2, 2.5*len) forward edges among the valid nodes +
-    the exact inverse half with type + R/2, context node 0 linked to the q/a nodes with types 0/1,
-    padded nodes isolated (self loop only).
+    ~ U{0..R-1}; node_type ~ U{0..T-2} with node 0 of each graph = T-1 (T = n_ntype; every node is
+    type 0 at T = 1); H ~ N(0,1)*0.5; scores N(0,1).
+    Realistic variant (T >= 4: it uses the loader's types 0, 1, 2 and 3): adj_lengths ~ U{8..n},
+    min(e/2, 2.5*len) forward edges among the valid nodes + the exact inverse half with type + R/2,
+    context node 0 linked to the q/a nodes with types 0/1, padded nodes isolated (self loop only).
+    At the default T = 4 the draws are those of the loader's four types.
     """
+    if n_ntype < 1 or (realistic and n_ntype < 4):
+        raise ValueError(f"synth_graph_batch: n_ntype = {n_ntype} (the realistic variant needs at least 4 node types)")
     g = torch.Generator().manual_seed(seed)
     H = torch.randn(B, n, D, generator=g) * 0.5
     node_score = torch.randn(B, n, 1, generator=g)
-    node_type = torch.randint(0, 3, (B, n), generator=g)
-    node_type[:, 0] = 3
+    node_type = torch.randint(0, max(n_ntype - 1, 1), (B, n), generator=g)
+    node_type[:, 0] = n_ntype - 1
     if not realistic:
         ei = torch.randint(0, n, (B, 2, e_per_graph), generator=g)
         ei = ei + (torch.arange(B) * n).view(B, 1, 1)

@@ -85,6 +85,16 @@ def _capacity(total, edge_capacity):
     return int(edge_capacity)
 
 
+def _etype_int16(etype, what):
+    """`etype` as int16, the width the flat cache and DeviceSplit store edge types in.  numpy's cast wraps (65541 -> 5), and
+    a wrapped type is a valid but wrong relation, so a value outside int16 raises instead."""
+    et = np.asarray(etype)
+    if et.size and (int(et.min()) < -(1 << 15) or int(et.max()) >= 1 << 15):
+        bad = int(et.max()) if int(et.max()) >= 1 << 15 else int(et.min())
+        raise ValueError(f"{what}: edge type {bad} does not fit the int16 edge types of the flat adjacency")
+    return np.ascontiguousarray(et, dtype=np.int16)
+
+
 def node_ptr_of(adj_lengths, n_nodes, n_graphs):
     """node_ptr int64 [n_graphs + 1] = the exclusive cumsum of a batch's adj_lengths (any shape, one entry per graph); raises
     ValueError for a length outside [1, n_nodes]."""
@@ -290,7 +300,8 @@ class FlatAdjCache:
             et = torch.cat(flat_et, dim=0).numpy()
         else:
             ei, et = np.zeros((2, 0), np.int64), np.zeros((0,), np.int64)
-        return cls(ei[0].astype(np.int32), ei[1].astype(np.int32), et.astype(np.int16), ptr, len(edge_index_nested[0]), n_nodes)
+        return cls(ei[0].astype(np.int32), ei[1].astype(np.int32), _etype_int16(et, "FlatAdjCache"), ptr,
+                   len(edge_index_nested[0]), n_nodes)
 
     def save(self, path):
         np.savez(path, src=self.src, tgt=self.tgt, etype=self.etype, graph_ptr=self.graph_ptr,
@@ -413,7 +424,9 @@ class DeviceSplit:
         dev = self.device
         self.src = torch.from_numpy(np.ascontiguousarray(flat.src, dtype=np.int32)).to(dev)
         self.tgt = torch.from_numpy(np.ascontiguousarray(flat.tgt, dtype=np.int32)).to(dev)
-        self.etype = torch.from_numpy(np.ascontiguousarray(flat.etype, dtype=np.int16)).to(dev)
+        if int(n_etype) > 1 << 15:  # the largest type, n_etype - 1, must fit the int16 edge types
+            raise ValueError(f"DeviceSplit: n_etype = {int(n_etype)} does not fit the int16 edge types of the flat adjacency")
+        self.etype = torch.from_numpy(_etype_int16(flat.etype, "DeviceSplit")).to(dev)
         self.graph_ptr = torch.from_numpy(np.ascontiguousarray(flat.graph_ptr, dtype=np.int64)).to(dev)
         self.adj_lengths = self.lens.to(dev)
         self.concept_ids = shapes["concept_ids"].to(dev, torch.long).contiguous()
@@ -427,10 +440,12 @@ class DeviceSplit:
         G = self.lens.numel()
         edge_graph = torch.repeat_interleave(torch.arange(G, device=dev), torch.from_numpy(self.counts).to(dev))
         rows = self.adj_lengths[edge_graph]
+        # int16 etype against R = 2^15 would cast R to int16 (-32768) and flag every edge; no int16 reaches 2^15 anyway
+        etype_high = self.etype >= R if R < 1 << 15 else torch.zeros_like(self.etype, dtype=torch.bool)
         checks = (("an adj_length outside [1, %d]" % n, (self.adj_lengths < 1) | (self.adj_lengths > n), None),
                   ("an edge outside its graph's rows [0, adj_length)",
                    (self.src < 0) | (self.src >= rows) | (self.tgt < 0) | (self.tgt >= rows), edge_graph),
-                  ("an edge type outside [0, %d)" % R, (self.etype < 0) | (self.etype >= R), edge_graph),
+                  ("an edge type outside [0, %d)" % R, (self.etype < 0) | etype_high, edge_graph),
                   ("a node type outside [0, %d)" % T, ((self.node_type_ids < 0) | (self.node_type_ids >= T)).any(1), None))
         for what, bad, graph_of in checks:
             idx = torch.nonzero(bad)

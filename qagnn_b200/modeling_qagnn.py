@@ -210,8 +210,11 @@ def graph_prep(A, node_type, n, n_ntype, n_etype, validate):
                              node_ptr=A.node_ptr_dev)
         except _lib.QagnnError as e:
             if e.status == -5:  # QAGNN_ERR_UNSUPPORTED
-                raise ValueError(f"ragged batch: graphs of {A.n_nodes} nodes and {A.max_edges} edges do not fit the one-CTA "
-                                 "graph prep; run this batch padded") from e
+                combos = n_etype * n_ntype * n_ntype + n_ntype
+                why = (f"{combos} edge-feature combos (n_etype * n_ntype^2 + n_ntype) exceed the 65536 that the one-CTA "
+                       "graph prep's 16-bit combo ids hold" if combos > 65536 else
+                       f"graphs of {A.n_nodes} nodes and {A.max_edges} edges do not fit the one-CTA graph prep")
+                raise ValueError(f"ragged batch: {why}; run this batch padded") from e
             raise
     if gp is not None:
         if n > 0 and A.n_nodes == n and A.max_edges >= 0:

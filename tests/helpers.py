@@ -43,7 +43,7 @@ def assert_close(got, ref, what="", atol=ATOL, rtol=RTOL):
 
 def regen_mp_inputs(fx):
     c = fx["case"]
-    inp = O.synth_graph_batch(c["B"], c["n"], c["e"], c["D"], fx["n_etype"], c["seed"], c["realistic"])
+    inp = O.synth_graph_batch(c["B"], c["n"], c["e"], c["D"], fx["n_etype"], c["seed"], c["realistic"], fx["n_ntype"])
     sd = O.random_state_dict(c["k"], c["D"], fx["n_ntype"], fx["n_etype"], c["regime"], c["seed"])
     fp = MG.fingerprint(inp["H"], inp["edge_index"], inp["edge_type"], inp["node_type"], inp["node_score"])
     assert fp == fx["input_fp"], "regenerated inputs differ from the ones the golden was minted on"

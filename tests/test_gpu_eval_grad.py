@@ -70,16 +70,18 @@ def test_gatconve_eval_gradients_match_fp64_autograd(name, heads):
     x, extra, nt, ei, et, sd = Hh.regen_layer_inputs(fx)
     sd = _set_running_stats(dict(sd), seed=heads)
     D = x.size(1)
+    T_, R_ = fx["n_ntype"], fx["n_etype"]
     pre = "gnn_layers.0."
     s64 = _leaves64(sd)
     x64, e64 = x.double().requires_grad_(True), extra.double().requires_grad_(True)
-    ref_out, _, ref_alpha, _ = O.gatconve_forward(s64, "gnn_layers.0", x64, ei, et, nt, e64, T, R, head_count=heads,
+    ref_out, _, ref_alpha, _ = O.gatconve_forward(s64, "gnn_layers.0", x64, ei, et, nt, e64, T_, R_, head_count=heads,
                                                   dtype=torch.float64)
     G = torch.randn(ref_out.shape, generator=torch.Generator().manual_seed(7), dtype=torch.float64)
     (ref_out * G).sum().backward()
 
-    enc = torch.nn.Sequential(torch.nn.Linear(R + 1 + 2 * T, D), torch.nn.BatchNorm1d(D), torch.nn.ReLU(), torch.nn.Linear(D, D))
-    layer = qagnn_b200.GATConvE(None, D, T, R, enc, head_count=heads)
+    enc = torch.nn.Sequential(torch.nn.Linear(R_ + 1 + 2 * T_, D), torch.nn.BatchNorm1d(D), torch.nn.ReLU(),
+                              torch.nn.Linear(D, D))
+    layer = qagnn_b200.GATConvE(None, D, T_, R_, enc, head_count=heads)
     layer.load_state_dict({k[len(pre):]: v for k, v in sd.items() if k.startswith(pre)})
     layer = layer.to(DEV).eval()
     before = _bn_buffers(layer)
@@ -101,7 +103,7 @@ def test_gatconve_eval_gradients_match_fp64_autograd(name, heads):
 # ---- QAGNN_Message_Passing against fp64 autograd ------------------------------------------------------------------------
 def _mp_module(fx, sd, dropout=0.2):
     c = fx["case"]
-    mod = qagnn_b200.QAGNN_Message_Passing(None, c["k"], T, R, c["D"], c["D"], c["D"], dropout=dropout)
+    mod = qagnn_b200.QAGNN_Message_Passing(None, c["k"], fx["n_ntype"], fx["n_etype"], c["D"], c["D"], c["D"], dropout=dropout)
     mod.load_state_dict(sd, strict=True)
     return mod.to(DEV).eval()
 
@@ -115,8 +117,8 @@ def test_message_passing_eval_gradients_match_fp64_autograd(name):
     s64 = _leaves64(sd)
     H64 = inp["H"].double().requires_grad_(True)
     sc64 = inp["node_score"].double().requires_grad_(True)
-    ref = O.message_passing_forward(s64, H64, inp["edge_index"], inp["edge_type"], inp["node_type"], sc64, c["k"], T, R,
-                                    dtype=torch.float64)
+    ref = O.message_passing_forward(s64, H64, inp["edge_index"], inp["edge_type"], inp["node_type"], sc64, c["k"],
+                                    fx["n_ntype"], fx["n_etype"], dtype=torch.float64)
     G = torch.randn(ref.shape, generator=torch.Generator().manual_seed(3), dtype=torch.float64)
     (ref * G).sum().backward()
 
@@ -185,7 +187,7 @@ def _decoder(name):
     fx = Hh.load_golden(name)
     c = fx["case"]
     inp, sent_vecs, concept_ids = MG.build_decoder_inputs(c, fx["n_etype"])
-    dec = qagnn_b200.QAGNN(None, c["k"], T, R, c["sent_dim"], c["n_concept"], c["D"], c["concept_in_dim"], c["n_head"], c["D"],
+    dec = qagnn_b200.QAGNN(None, c["k"], fx["n_ntype"], fx["n_etype"], c["sent_dim"], c["n_concept"], c["D"], c["concept_in_dim"], c["n_head"], c["D"],
                            c["n_fc_layer"], 0.3, 0.3, 0.3)
     sd = _set_running_stats({k: v.clone() for k, v in fx["state_dict"].items()}, seed=c["seed"])
     dec.load_state_dict(sd, strict=True)

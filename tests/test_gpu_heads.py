@@ -43,19 +43,26 @@ def mp_core_ref(qkm, ke, me, src, tgt, combo, H):
     return torch.zeros(N, H, d, dtype=s.dtype).index_add(0, tgt, msg).reshape(N, D), alpha
 
 
-def _edges(edge_index, edge_type, node_type):
+def _edges(edge_index, edge_type, node_type, T, R):
     p = O.graph_prep_oracle(edge_index, edge_type, node_type, T, R)
     return tuple(torch.from_numpy(p[k]) for k in ("src", "tgt", "combo"))
 
 
-def _combo_onehots(dtype):
-    """[C, R+1+2T] one-hot edge features in graph prep's combo numbering."""
-    c = torch.arange(NC)
+def combo_parts(c, T, R):
+    """(edge type, source type, target type) of combo ids c in graph prep's numbering; a self loop's edge type is R."""
     real = c < R * T * T
     et = torch.where(real, c // (T * T), torch.full_like(c, R))
     ts = torch.where(real, (c // T) % T, c - R * T * T)
     tt = torch.where(real, c % T, c - R * T * T)
-    tab = torch.zeros(NC, R + 1 + 2 * T, dtype=dtype)
+    return et, ts, tt
+
+
+def _combo_onehots(dtype, T, R):
+    """[C, R+1+2T] one-hot edge features in graph prep's combo numbering."""
+    C_ = R * T * T + T
+    c = torch.arange(C_)
+    et, ts, tt = combo_parts(c, T, R)
+    tab = torch.zeros(C_, R + 1 + 2 * T, dtype=dtype)
     tab[c, et] = 1
     tab[c, R + 1 + ts] = 1
     tab[c, R + 1 + T + tt] = 1
@@ -70,7 +77,7 @@ def _projections(sd, prefix, x, extra, H, dtype):
     wk, wm = W("linear_key.weight"), W("linear_msg.weight")
     q = (x2 @ W("linear_query.weight").t() + W("linear_query.bias")) / (D // H) ** 0.5
     qkm = torch.cat([q, x2 @ wk[:, :2 * D].t(), x2 @ wm[:, :2 * D].t()], 1)
-    tab = O.mlp_lin_bn_relu_lin(_combo_onehots(dtype), sd, prefix + ".edge_encoder")
+    tab = O.mlp_lin_bn_relu_lin(_combo_onehots(dtype, T, R), sd, prefix + ".edge_encoder")
     return qkm, tab @ wk[:, 2 * D:].t() + W("linear_key.bias"), tab @ wm[:, 2 * D:].t() + W("linear_msg.bias")
 
 
@@ -85,7 +92,7 @@ def test_mp_core_reference_equals_the_oracle(H, D, seed):
     _, _, alpha_o, aggr_o = O.gatconve_forward(sd, "gnn_layers.0", x, b["edge_index"], b["edge_type"], nt, extra, T, R,
                                                head_count=H, dtype=F64)
     qkm, ke, me = _projections(sd, "gnn_layers.0", x, extra, H, F64)
-    aggr, alpha = mp_core_ref(qkm, ke, me, *_edges(b["edge_index"], b["edge_type"], nt), H)
+    aggr, alpha = mp_core_ref(qkm, ke, me, *_edges(b["edge_index"], b["edge_type"], nt, T, R), H)
     assert torch.allclose(alpha, alpha_o, rtol=0, atol=1e-10)
     assert torch.allclose(aggr, aggr_o, rtol=1e-10, atol=1e-10)
 
@@ -174,7 +181,7 @@ def _core_case(H, D, kind):
     grads = torch.autograd.grad(aggr, leaves, G.to(DEV), retain_graph=True)
     grads2 = torch.autograd.grad(aggr, leaves, G.to(DEV))
     ref_leaves = [t.double().requires_grad_(True) for t in (qkm, ke, me)]
-    edges = _edges(ei, et, nt)
+    edges = _edges(ei, et, nt, T, R)
     raggr, ralpha = mp_core_ref(*ref_leaves, *edges, H)
     rgrads = torch.autograd.grad(raggr, ref_leaves, G.double())
     cpu = lambda ts: [t.detach().cpu() for t in ts]  # noqa: E731
@@ -242,7 +249,7 @@ def test_core_tolerance_rejects_a_missing_edge_and_swapped_heads():
     qkm, ke, me, G, ei, et, nt = case["inputs"]
     # the reference of the same graph without its first edge
     leaves = [t.double().requires_grad_(True) for t in (qkm, ke, me)]
-    paggr, _ = mp_core_ref(*leaves, *_edges(ei[:, 1:], et[1:], nt), H)
+    paggr, _ = mp_core_ref(*leaves, *_edges(ei[:, 1:], et[1:], nt, T, R), H)
     pd_qkm, pd_ke, pd_me = torch.autograd.grad(paggr, leaves, G.double())
     for name, g_, r_ in (("aggr", aggr, paggr), ("d_qkm", d_qkm, pd_qkm), ("d_ke", d_ke, pd_ke), ("d_me", d_me, pd_me)):
         assert _excess(g_, r_.detach()) > 0, f"{name}: a reference missing one edge passes the tolerance"

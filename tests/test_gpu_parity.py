@@ -1,5 +1,7 @@
 """Parity of the CUDA path (through the C ABI) against the goldens minted from the reference and
 against the CPU oracle.  Needs a GPU: run with -m gpu."""
+import copy
+
 import numpy as np
 import pytest
 import torch
@@ -521,6 +523,8 @@ def test_decoder_step_graph_matches_module_composition():
     torch.manual_seed(4)
     pooler = MultiheadAttPoolLayer(2, S, D).eval().to(DEV)
     fc = MLP(D + S + D, D, 1, 0, 0.2, layer_norm=True).eval().to(DEV)
+    # the reference's answer MLP is a CPU copy: moving `fc` itself would free the weights the captured graph reads
+    fc_ref = copy.deepcopy(fc).cpu()
 
     def batch(seed):
         inp = O.synth_graph_batch(B, n, e, D, 38, seed, realistic=True)
@@ -545,8 +549,7 @@ def test_decoder_step_graph_matches_module_composition():
             mask[mask.all(1), 0] = 0
             psd = {"pooler." + k_: v.cpu() for k_, v in pooler.state_dict().items()}
             gv, ref_attn = O.multihead_att_pool(psd, "pooler", ninp["sent_vecs"], ref_out, mask, 2)
-            ref_logits = fc.cpu()(torch.cat((gv, ninp["sent_vecs"], ref_out[:, 0]), 1))
-            fc.to(DEV)
+            ref_logits = fc_ref(torch.cat((gv, ninp["sent_vecs"], ref_out[:, 0]), 1))
         Hh.assert_close(gout, ref_out, f"gnn_out seed {seed}")
         Hh.assert_close(attn, ref_attn, f"pool_attn seed {seed}", atol=2e-5)
         Hh.assert_close(logits, ref_logits, f"logits seed {seed}")

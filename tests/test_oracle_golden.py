@@ -96,10 +96,10 @@ def test_committed_goldens_are_what_the_reference_produces_here():
 
 
 def test_oracle_equals_the_reference_on_uncommitted_random_cases():
-    """24 random small cases (1-4 graphs, 1-30 nodes, 0-80 edges, D 16-100, k 1-3, 6 / 17 / 38 edge types, both weight
-    regimes) that are not fixtures: the oracle against the reference's own QAGNN_Message_Passing, fp32, 2e-6 + 2e-5 rel, on a
-    seeded sample of every compared tensor stored by `python -m oracle.make_goldens` (tests/golden/ref/fuzz24.pt) — widens
-    the pinned region beyond the committed fixtures."""
+    """24 random small cases (1-4 graphs, 1-30 nodes, 0-80 edges, D 16-100, k 1-3, 6 / 17 / 38 edge types, 1 / 3 / 4 / 6 node
+    types, both weight regimes) that are not fixtures: the oracle against the reference's own QAGNN_Message_Passing, fp32,
+    2e-6 + 2e-5 rel, on a seeded sample of every compared tensor stored by `python -m oracle.make_goldens`
+    (tests/golden/ref/fuzz24.pt) — widens the pinned region beyond the committed fixtures."""
     from oracle import make_goldens as MG
     fz = torch.load(MG.FUZZ_FILE, weights_only=False)
     assert len(fz["cases"]) == 24 and [c["name"] for c in fz["cases"]] == [c["name"] for c in MG.fuzz_cases(24)]
@@ -113,3 +113,12 @@ def test_oracle_equals_the_reference_on_uncommitted_random_cases():
         assert tuple(t.shape) == shape, (fz["cases"][ci]["name"], name)
         Hh.assert_close(t.reshape(-1)[fz["index"][off:off + cnt].long()], fz["value"][off:off + cnt],
                         f"{fz['cases'][ci]['name']} {name}", **TIGHT)
+
+
+def test_every_golden_case_has_its_committed_fixture():
+    """`make_goldens --check` reports a case whose fixture is not in the tree without comparing it: every case of the table
+    must have its file here."""
+    import os
+    from oracle import make_goldens as MG
+    missing = [c["name"] for _, c in MG.all_cases() if not os.path.exists(os.path.join(MG.GOLDEN_DIR, c["name"] + ".pt"))]
+    assert not missing, f"cases without a committed fixture: {missing}"
