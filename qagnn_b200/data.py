@@ -401,14 +401,18 @@ class DeviceSplit:
     per-graph edge counts and adj_lengths.
 
     Held as: src / tgt int32 and etype int16 [E_split], graph_ptr int64 [G + 1], adj_lengths int64 [G], concept_ids and
-    node_type_ids int64 [G, n], node_scores fp32 [G, n, 1], with G = Q * num_choice sub-graphs.  At the loader's density
+    node_type_ids int64 [G, n], node_scores fp32 [G, n, 1], with G = Q * num_choice sub-graphs, and labels int64 [Q] when given.  At the loader's density
     (~584 edges per graph) a split of 50 k graphs takes about 0.3 GB of adjacency and 0.2 GB of node arrays."""
 
-    def __init__(self, flat, concept_ids, node_type_ids, node_scores, adj_lengths, device, n_ntype, n_etype):
+    def __init__(self, flat, concept_ids, node_type_ids, node_scores, adj_lengths, device, n_ntype, n_etype, *, labels=None):
         """What load_flat_adj_cache returns (concept_ids / node_type_ids [Q, nc, n], node_scores [Q, nc, n, 1], adj_lengths
         [Q, nc], flat a FlatAdjCache), uploaded to `device`.  Raises IndexError naming the first offending question when an
         edge's local ids leave [0, adj_length) of its graph, an etype leaves [0, n_etype), a node type leaves [0, n_ntype) or
-        an adj_length leaves [1, n]."""
+        an adj_length leaves [1, n].
+
+        `labels` (optional, integer [Q]: the loader's answer index per question, e.g. LM_QAGNN_DataLoader.train_labels) is
+        uploaded as `self.labels` (int64) for pipeline.SplitTrainStep; a label outside [0, num_choice) raises IndexError naming
+        its question, another shape or a non-integer dtype ValueError.  Without it `self.labels` is None."""
         self.device = torch.device(device)
         self.num_choice, self.n_nodes = flat.num_choice, flat.n_nodes
         nc, n = self.num_choice, self.n_nodes
@@ -421,6 +425,12 @@ class DeviceSplit:
         for name, t in shapes.items():
             if t.size(0) != G:
                 raise ValueError(f"DeviceSplit: {name} has {t.size(0)} graphs, the adjacency {G}")
+        if labels is not None:
+            labels = torch.as_tensor(labels)
+            if tuple(labels.shape) != (self.n_questions,) or labels.is_floating_point() or labels.is_complex() \
+                    or labels.dtype == torch.bool:
+                raise ValueError(f"DeviceSplit: labels must be integer [{self.n_questions}] (one per question), got "
+                                 f"{tuple(labels.shape)} {labels.dtype}")
         dev = self.device
         self.src = torch.from_numpy(np.ascontiguousarray(flat.src, dtype=np.int32)).to(dev)
         self.tgt = torch.from_numpy(np.ascontiguousarray(flat.tgt, dtype=np.int32)).to(dev)
@@ -432,6 +442,7 @@ class DeviceSplit:
         self.concept_ids = shapes["concept_ids"].to(dev, torch.long).contiguous()
         self.node_type_ids = shapes["node_type_ids"].to(dev, torch.long).contiguous()
         self.node_scores = shapes["node_scores"].to(dev, torch.float32).contiguous()
+        self.labels = None if labels is None else labels.to(dev, torch.long).contiguous()
         self._validate(int(n_ntype), int(n_etype))
 
     def _validate(self, T, R):
@@ -452,6 +463,11 @@ class DeviceSplit:
             if idx.numel():
                 g = int(idx[0, 0]) if graph_of is None else int(graph_of[idx[0, 0]])
                 raise IndexError(f"DeviceSplit: question {g // nc} (graph {g}) has {what}")
+        if self.labels is not None:  # the captured cross entropy must never see a target outside [0, nc)
+            idx = torch.nonzero((self.labels < 0) | (self.labels >= nc))
+            if idx.numel():
+                q = int(idx[0, 0])
+                raise IndexError(f"DeviceSplit: question {q} has label {int(self.labels[q])}, outside [0, {nc})")
 
     def check(self, question_ids, edge_capacity, node_capacity=None):
         """The host checks of one batch, O(bs * num_choice), with FlatAdjCache.pack's exceptions: IndexError for a question id

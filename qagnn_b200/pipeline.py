@@ -18,6 +18,9 @@ behind one autograd node, for the micro-steps of qagnn.py:252-278.
 
 `SplitEvalStep` evaluates a split held on the GPU (qagnn_b200.data.DeviceSplit): one CUDA graph assembles a batch from its
 question ids and runs QAGNN.forward in .eval() on it, so nothing of the batch is packed or uploaded on the host.
+
+`SplitTrainStep` trains from such a split: its forward graph assembles the micro-batch, gathers its labels and takes the
+cross-entropy loss; its backward graph adds the parameter gradients into `.grad` itself.
 """
 import contextlib
 
@@ -226,6 +229,97 @@ class DecoderStep:
         return self.logits, self.pool_attn, self.gnn_out
 
 
+class _TrainingGraphs:
+    """What TrainStep and SplitTrainStep share: the training forward and its backward captured as two CUDA graphs in one
+    pool, after capture_guard's validation and warm-up, and the checks before and bookkeeping after every replay."""
+
+    what = None  # the class name in messages
+
+    def _init_training(self, decoder, autocast_dtype):
+        if autocast_dtype not in (None, torch.float16, torch.bfloat16):
+            raise ValueError("autocast_dtype must be None, torch.float16 or torch.bfloat16")
+        if not decoder.training:
+            raise ValueError(f"{self.what} captures the training forward: call decoder.train() first")
+        self.decoder, self.autocast_dtype = decoder, autocast_dtype
+        self.deterministic = torch.are_deterministic_algorithms_enabled()
+        self._fwd = self._status = None
+        self.mode = "eager"
+
+    def _autocast(self):
+        if self.autocast_dtype is None:
+            return contextlib.nullcontext()
+        return torch.autocast("cuda", dtype=self.autocast_dtype, cache_enabled=False)
+
+    def _addresses(self):
+        return tuple(t.data_ptr() for t in self._params + self._buffers)
+
+    def _capture_graphs(self, adj, node_type, forward, backward, owned=()):
+        """Captures `forward()` -> (y, ...) and `backward(y, dy)` as two CUDA graphs in one pool, on the batch (adj,
+        node_type) already in the static buffers.  capture_guard first validates that batch and runs forward + backward twice
+        (dy = 1) on a side stream; `forward` records graph prep's status word into self._status when that is set.  The
+        warm-up really runs: the decoder's buffers, the .grad of its trainable parameters (self._params), the tensors `owned`
+        and the CUDA RNG state are put back afterwards.  Returns (forward's outputs, the static dy buffer, backward's result)."""
+        dec = self.decoder
+        dev = node_type.device
+        self._params = [p for p in dec.parameters() if p.requires_grad]
+        self._buffers = list(dec.buffers())
+
+        def warmup():  # also builds the cached tables of the training path
+            out = forward()
+            backward(out[0], torch.ones_like(out[0]))
+
+        saved = [b.detach().clone() for b in self._buffers + list(owned)]
+        grads = [None if p.grad is None else p.grad.detach().clone() for p in self._params]
+        rng = torch.cuda.get_rng_state(dev)
+        try:
+            with capture_guard(dec.gnn, adj, node_type, self.what, warmup) as status:
+                self._status = status
+                pool = torch.cuda.graph_pool_handle()
+                fwd, bwd = torch.cuda.CUDAGraph(), torch.cuda.CUDAGraph()
+                with torch.cuda.graph(fwd, pool=pool):
+                    out = forward()
+                dy = torch.empty_like(out[0])
+                with torch.cuda.graph(bwd, pool=pool):
+                    res = backward(out[0], dy)
+            self._fwd, self._bwd = fwd, bwd
+            self._bn_buffers = [b for m in dec.modules() if isinstance(m, torch.nn.modules.batchnorm._BatchNorm)
+                                for b in (m.running_mean, m.running_var, m.num_batches_tracked) if b is not None]
+            self._ptrs = self._addresses()
+            self.mode = "two CUDA graphs (forward + backward)"
+            return out, dy, res
+        except BaseException:
+            self._status = None
+            raise
+        finally:
+            with torch.no_grad():
+                for b, s in zip(self._buffers + list(owned), saved):
+                    b.copy_(s)
+            for p, g in zip(self._params, grads):
+                p.grad = g
+            torch.cuda.set_rng_state(rng, dev)
+
+    def _check_replay(self):
+        """Before a replay: RuntimeError when the graphs no longer fit the decoder, IndexError when an earlier replay's graph
+        prep flagged its batch."""
+        what = self.what
+        if not self.decoder.training:
+            raise RuntimeError(f"{what} replays the training forward: call decoder.train() first")
+        if self._addresses() != self._ptrs:
+            raise RuntimeError(f"{what}: the decoder's parameters or buffers moved since capture (.to() / .cuda() / "
+                               f".half()?); the graphs would read the old addresses. Build a new {what}.")
+        if torch.are_deterministic_algorithms_enabled() != self.deterministic:
+            raise RuntimeError(f"{what} was captured with torch.use_deterministic_algorithms({self.deterministic}) and "
+                               f"its backward graph holds that mode's kernels; the flag changed since. Build a new {what}.")
+        if self._status is not None:
+            self._status.check(what)
+
+    def _replayed(self):
+        if self._status is not None:
+            self._status.replayed()
+        # the replay changed the running statistics behind autograd's back: the eval path's folded weights key on versions
+        torch.autograd.graph.increment_version(self._bn_buffers)
+
+
 class _TrainReplay(torch.autograd.Function):
     """The captured forward and backward of a TrainStep as one autograd node.  Gradient accumulation into `.grad` stays in
     autograd, outside the graphs.  The backward hands out the static gradient buffers themselves: autograd then copies
@@ -251,7 +345,7 @@ class _TrainReplay(torch.autograd.Function):
         return (None,) + tuple(g if need else None for g, need in zip(step._grads, ctx.needs_input_grad[1:]))
 
 
-class TrainStep:
+class TrainStep(_TrainingGraphs):
     """QAGNN.forward in .train() and its backward, each replayed as one CUDA graph: the training counterpart of DecoderStep
     for the loop body of qagnn.py:252-278, on packed batches at a fixed edge capacity K
     (qagnn_b200.data.PackedAdjBatchGenerator(..., edge_capacity=K)):
@@ -282,18 +376,15 @@ class TrainStep:
     give the same gradients bit for bit.  `deterministic` records that mode; a graph call after the flag changed raises
     RuntimeError (build a new TrainStep)."""
 
+    what = "TrainStep"
+
     def __init__(self, decoder, sent_vecs, concept_ids, node_type_ids, node_scores, adj_lengths, packed_adj, *, max_edges,
                  edge_capacity=None, autocast_dtype=None, use_cuda_graph=True):
         """The example batch (device tensors with the shapes of every later batch, valid indices, `packed_adj` a PackedAdj)
         sizes the static buffers and is what warm-up and capture run on.  `edge_capacity` K defaults to the width of
         packed_adj's edge buffer; `max_edges` bounds the edges of one sub-graph over the whole split
         (FlatAdjCache.max_graph_edges())."""
-        if autocast_dtype not in (None, torch.float16, torch.bfloat16):
-            raise ValueError("autocast_dtype must be None, torch.float16 or torch.bfloat16")
-        if not decoder.training:
-            raise ValueError("TrainStep captures the training forward: call decoder.train() first")
-        self.decoder, self.autocast_dtype = decoder, autocast_dtype
-        self.deterministic = torch.are_deterministic_algorithms_enabled()
+        self._init_training(decoder, autocast_dtype)
         dev = node_type_ids.device
         B, n = node_type_ids.shape
         K = int(edge_capacity) if edge_capacity is not None else packed_adj.edge_index.size(1)
@@ -306,15 +397,8 @@ class TrainStep:
         from .data import PackedAdj
         self._adj = PackedAdj(self._edges[:2], self._edges[2], None, n, self._edges, self._gp, self.max_edges, -1, K)
         self._copy_batch(sent_vecs, concept_ids, node_type_ids, node_scores, adj_lengths, packed_adj)
-        self._fwd = self._status = None
-        self.mode = "eager"
         if use_cuda_graph:
             self._capture()
-
-    def _autocast(self):
-        if self.autocast_dtype is None:
-            return contextlib.nullcontext()
-        return torch.autocast("cuda", dtype=self.autocast_dtype, cache_enabled=False)
 
     def _copy_batch(self, sent_vecs, concept_ids, node_type_ids, node_scores, adj_lengths, adj):
         for name, t, static in (("sent_vecs", sent_vecs, self._sv), ("concept_ids", concept_ids, self._cid),
@@ -348,75 +432,27 @@ class TrainStep:
             self._status.record(self.decoder.gnn._last_prep.status_word())
         return logits, pool_attn
 
-    def _addresses(self):
-        return tuple(t.data_ptr() for t in self._params + self._buffers)
-
     def _capture(self):
-        dec, gnn = self.decoder, self.decoder.gnn
-        dev = self._nt.device
-        self._params = [p for p in dec.parameters() if p.requires_grad]
-        self._buffers = list(dec.buffers())
-        inputs = [self._sv, self._ns] + self._params
-
-        def warmup():  # also builds the cached tables of the training path
+        def forward():
             with self._autocast():
-                logits, _ = self._forward(self._sv, self._ns)
-            torch.autograd.grad(logits, inputs, torch.ones_like(logits), allow_unused=True)
+                return self._forward(self._sv, self._ns)
 
-        # the warm-up iterations really run: BatchNorm statistics, RNG offsets and .grad are put back afterwards
-        buffers = [b.detach().clone() for b in self._buffers]
-        grads = [None if p.grad is None else p.grad.detach().clone() for p in self._params]
-        rng = torch.cuda.get_rng_state(dev)
-        try:
-            with capture_guard(gnn, self._adj, self._nt, "TrainStep", warmup) as status:
-                self._status = status  # _forward records graph prep's status word into it
-                pool = torch.cuda.graph_pool_handle()
-                fwd, bwd = torch.cuda.CUDAGraph(), torch.cuda.CUDAGraph()
-                with torch.cuda.graph(fwd, pool=pool):
-                    with self._autocast():
-                        logits, pool_attn = self._forward(self._sv, self._ns)
-                self._g_logits = torch.empty_like(logits)
-                with torch.cuda.graph(bwd, pool=pool):
-                    self._grads = torch.autograd.grad(logits, inputs, self._g_logits, allow_unused=True)
-            self._logits, self._pool_attn = logits.detach(), pool_attn.detach()
-            self._fwd, self._bwd = fwd, bwd
-            self._bn_buffers = [b for m in dec.modules() if isinstance(m, torch.nn.modules.batchnorm._BatchNorm)
-                                for b in (m.running_mean, m.running_var, m.num_batches_tracked) if b is not None]
-            self._ptrs = self._addresses()
-            self.mode = "two CUDA graphs (forward + backward)"
-        except BaseException:
-            self._status = None
-            raise
-        finally:
-            with torch.no_grad():
-                for b, s in zip(self._buffers, buffers):
-                    b.copy_(s)
-            for p, g in zip(self._params, grads):
-                p.grad = g
-            torch.cuda.set_rng_state(rng, dev)
+        def backward(logits, d_logits):
+            return torch.autograd.grad(logits, [self._sv, self._ns] + self._params, d_logits, allow_unused=True)
+
+        (logits, pool_attn), self._g_logits, self._grads = self._capture_graphs(self._adj, self._nt, forward, backward)
+        self._logits, self._pool_attn = logits.detach(), pool_attn.detach()
 
     def __call__(self, sent_vecs, concept_ids, node_type_ids, node_scores, adj_lengths, packed_adj):
         """Returns (logits [B, 1], pool_attn) of one micro-batch; `.backward()` through logits replays the backward graph."""
         if self._fwd is not None:
-            if not self.decoder.training:
-                raise RuntimeError("TrainStep replays the training forward: call decoder.train() first")
-            if self._addresses() != self._ptrs:
-                raise RuntimeError("TrainStep: the decoder's parameters or buffers moved since capture (.to() / .cuda() / "
-                                   ".half()?); the graphs would read the old addresses. Build a new TrainStep.")
-            if torch.are_deterministic_algorithms_enabled() != self.deterministic:
-                raise RuntimeError(f"TrainStep was captured with torch.use_deterministic_algorithms({self.deterministic}) and "
-                                   "its backward graph holds that mode's kernels; the flag changed since. Build a new TrainStep.")
-            if self._status is not None:
-                self._status.check("TrainStep")
+            self._check_replay()
         self._copy_batch(sent_vecs, concept_ids, node_type_ids, node_scores, adj_lengths, packed_adj)
         with self._autocast():
             if self._fwd is None:
                 return self._forward(sent_vecs, node_scores)
             out = _TrainReplay.apply(self, sent_vecs, node_scores, *self._params)
-        if self._status is not None:
-            self._status.replayed()
-        # the replay changed the running statistics behind autograd's back: the eval path's folded weights key on versions
-        torch.autograd.graph.increment_version(self._bn_buffers)
+        self._replayed()
         return out
 
 
@@ -521,6 +557,168 @@ class SplitEvalStep:
         if self._status is not None:
             self._status.replayed()
         return self.logits, self.pool_attn
+
+
+class _SplitTrainReplay(torch.autograd.Function):
+    """The captured forward and backward of a SplitTrainStep as one autograd node.  Its inputs are a zero-element anchor that
+    always requires grad, so the node exists when sent_vecs does not (a frozen encoder), and sent_vecs.  The parameters are
+    not inputs: the backward graph adds their gradients into the step-owned `.grad` buffers."""
+
+    @staticmethod
+    def forward(ctx, step, anchor, sent_vecs):
+        if step._sv.data_ptr() != sent_vecs.data_ptr():
+            step._sv.copy_(sent_vecs)
+        step._fwd.replay()
+        ctx.step, ctx.call = step, step.calls
+        return step._loss.detach()
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, d_loss):
+        step = ctx.step
+        if ctx.call != step.calls:
+            raise RuntimeError("SplitTrainStep: backward through the loss of an earlier call; the next call's forward replay "
+                               "has overwritten its activations. Run each call's backward before the next call.")
+        step._own_grads()
+        step._d_loss.copy_(d_loss)
+        step._bwd.replay()
+        return None, None, step._g_sv if ctx.needs_input_grad[2] else None
+
+
+class SplitTrainStep(_TrainingGraphs):
+    """A training micro-step on a split held on the GPU (qagnn_b200.data.DeviceSplit built with `labels`) as two CUDA graphs:
+    the loop body of qagnn.py:252-278 with `--loss cross_entropy`, whose only per-call inputs are the question ids and
+    sent_vecs:
+
+        step = SplitTrainStep(model.decoder.train(), split, mbs, edge_capacity=K, max_edges=M, autocast_dtype=torch.float16)
+        loss = step(qids, sent_vecs) * len(qids) / bs     # qids: mbs host ids; the micro-batch's mean cross entropy, fp32
+        scaler.scale(loss).backward()                     # replays the backward graph
+
+    The forward graph holds split.assemble (qagnn_assemble_batch and the node-row gathers), the gather of the micro-batch's
+    labels, `decoder(...)` in .train() on the padded batch and F.cross_entropy(logits.view(-1, num_choice), labels), under
+    torch.autocast(autocast_dtype, cache_enabled=False) (None, torch.float16 or torch.bfloat16).  The results equal
+    `decoder(sent_vecs, *split.batch(qids, K))` and that cross entropy under the same autocast.  A call checks the ids on the
+    host (DeviceSplit.check: IndexError / ValueError before anything is enqueued), uploads them (8 bytes per question),
+    copies sent_vecs into a static buffer (shape and dtype fixed by the first call, else ValueError) and replays the forward
+    graph.  It returns the loss as a 0-dim fp32 tensor; `logits` [mbs*nc, 1] and `pool_attn` are static buffers for logging.
+    The next call overwrites all three, so each call's backward must run before the next call (else RuntimeError).
+
+    The backward graph is torch.autograd.grad of the loss, seeded with the scalar autograd hands the step's node (the loss
+    weight times the GradScaler scale, read on the device), followed by one torch._foreach_add_ of the parameter gradients
+    into step-owned buffers.  Before every backward replay each trainable parameter's `.grad` becomes its buffer: zeroed
+    when `.grad` was None (zero_grad()), loaded from `.grad` when that was another tensor (zero_grad(set_to_none=False), an
+    assignment).  So `.grad` holds what eager accumulation would, and GradScaler.unscale_, clip_grad_norm_ and the optimiser
+    use it unchanged.  There is no AccumulateGrad node for the decoder's parameters: hooks registered on them
+    (register_hook, register_post_accumulate_grad_hook) do not fire on replays (register_hook fires during the first
+    call's capture, whose warm-up runs autograd.grad and discards the result).  dL/dsent_vecs flows on into the encoder when
+    sent_vecs requires grad; with a frozen encoder backward() still accumulates the decoder's gradients.  A parameter the
+    loss does not reach keeps `.grad` None, as in eager mode.
+
+    The first call captures, on its own batch: the warm-up that precedes the capture restores BatchNorm buffers, `.grad` and
+    the CUDA RNG state.  Dropout draws a new mask on every replay and BatchNorm running statistics advance on every replay.
+    Optimiser steps and load_state_dict keep the parameters' addresses, so the graphs stay valid; a call raises RuntimeError
+    after `.to()` / `.cuda()`, after torch.use_deterministic_algorithms changed, after a change in which decoder parameters
+    require grad, and in .eval() (build a new SplitTrainStep).  Every call needs exactly `batch_size` questions: run a final
+    partial micro-batch eagerly through split.batch + decoder + F.cross_entropy.  Padded batches on one GPU only."""
+
+    what = "SplitTrainStep"
+
+    def __init__(self, decoder, split, batch_size, *, edge_capacity, max_edges, autocast_dtype=None):
+        """`edge_capacity` K bounds the edges of every micro-batch (FlatAdjCache.max_batch_edges(batch_size)), `max_edges` M
+        those of one sub-graph over the split (FlatAdjCache.max_graph_edges()): one capture then serves every micro-batch."""
+        self._init_training(decoder, autocast_dtype)
+        if split.labels is None:
+            raise ValueError("SplitTrainStep: the split has no labels; build the DeviceSplit with labels=")
+        self.split, self.batch_size = split, int(batch_size)
+        self.edge_capacity, self.max_edges = int(edge_capacity), int(max_edges)
+        largest = int(split.counts.max()) if split.counts.size else 0
+        if self.max_edges < largest:
+            raise ValueError(f"SplitTrainStep: max_edges = {self.max_edges}, the split has a sub-graph of {largest} edges")
+        dev = split.device
+        self._qids = torch.zeros(self.batch_size, dtype=torch.int64, device=dev)
+        self._labels = torch.zeros(self.batch_size, dtype=torch.int64, device=dev)
+        self._out = split.buffers(self.batch_size, self.edge_capacity)
+        self._adj = split.packed_adj(self._out, self.max_edges, self.edge_capacity)
+        self._anchor = torch.empty(0, device=dev, requires_grad=True)
+        self._sv = None  # sized by the first call
+        self.logits = self.pool_attn = None
+        self.calls = self.captures = 0
+
+    def _forward(self):
+        nc = self.split.num_choice
+        with self._autocast():
+            out = self.split.assemble(self._qids, self.edge_capacity, -1, self._out)
+            torch.index_select(self.split.labels, 0, self._qids, out=self._labels)
+            logits, pool_attn = self.decoder(self._sv, out["concept_ids"], out["node_type_ids"], out["node_scores"],
+                                             out["adj_lengths"], self._adj)
+            loss = torch.nn.functional.cross_entropy(logits.view(-1, nc), self._labels)
+        if self._status is not None:
+            self._status.record(self.decoder.gnn._last_prep.status_word())
+        return loss, logits, pool_attn
+
+    def _capture(self):
+        bufs = [torch.zeros_like(p) for p in self.decoder.parameters() if p.requires_grad]
+        used = []
+
+        def backward(loss, d_loss):
+            grads = torch.autograd.grad(loss, [self._sv] + self._params, d_loss, allow_unused=True)
+            used[:] = [i for i, g in enumerate(grads[1:]) if g is not None]
+            torch._foreach_add_([bufs[i] for i in used], [grads[1 + i] for i in used])
+            return grads[0]
+
+        self.split.assemble(self._qids, self.edge_capacity, -1, self._out)  # capture_guard validates this batch
+        (self._loss, logits, pool_attn), self._d_loss, self._g_sv = self._capture_graphs(
+            self._adj, self._out["node_type_ids"], self._forward, backward, owned=bufs)
+        self.logits, self.pool_attn = logits.detach(), pool_attn.detach()
+        self._owned = [(self._params[i], bufs[i]) for i in used]
+        self._requires_grad = [p.requires_grad for p in self.decoder.parameters()]
+        self.captures += 1
+
+    def _own_grads(self):
+        """Makes every accumulated parameter's .grad the step's buffer, holding what .grad held (None counts as zeros)."""
+        fresh = [b for p, b in self._owned if p.grad is None]
+        if fresh:
+            torch._foreach_zero_(fresh)
+        for p, b in self._owned:
+            if p.grad is not b:
+                if p.grad is not None:
+                    b.copy_(p.grad)
+                p.grad = b
+
+    def __call__(self, question_ids, sent_vecs):
+        """The mean cross-entropy loss (0-dim fp32) of the questions `question_ids` (host ids, batch_size of them) with their
+        sent_vecs [batch_size*nc, S] (device); `.backward()` replays the backward graph."""
+        if not self.decoder.training:
+            raise RuntimeError("SplitTrainStep replays the training forward: call decoder.train() first")
+        if self._fwd is not None:
+            self._check_replay()
+            if [p.requires_grad for p in self.decoder.parameters()] != self._requires_grad:
+                raise RuntimeError("SplitTrainStep: which decoder parameters require grad changed since capture; the "
+                                   "backward graph accumulates the old set. Build a new SplitTrainStep.")
+        q = self.split.check(question_ids, self.edge_capacity)[0]
+        if q.size != self.batch_size:
+            raise ValueError(f"SplitTrainStep: {q.size} questions, the step was built for {self.batch_size}; run a partial "
+                             "micro-batch through split.batch + decoder")
+        want = (self.batch_size * self.split.num_choice, self.decoder.svec2nvec.in_features)
+        if self._sv is None and (tuple(sent_vecs.shape) != want or not sent_vecs.is_floating_point()):
+            raise ValueError(f"SplitTrainStep: sent_vecs is {tuple(sent_vecs.shape)} {sent_vecs.dtype}, the step needs "
+                             f"floating-point {want}")
+        if self._sv is not None and (sent_vecs.shape != self._sv.shape or sent_vecs.dtype != self._sv.dtype):
+            raise ValueError(f"SplitTrainStep: sent_vecs is {tuple(sent_vecs.shape)} {sent_vecs.dtype}, the step was built "
+                             f"for {tuple(self._sv.shape)} {self._sv.dtype}")
+        # a pinned block from the caching host allocator per call: it is not reused before this copy has run
+        self._qids.copy_(torch.from_numpy(q).pin_memory(), non_blocking=True)
+        if self._fwd is None:
+            self._sv = sent_vecs.detach().clone().requires_grad_(True)
+            try:
+                self._capture()  # on the micro-batch just loaded, which the host checks accepted
+            except BaseException:
+                self._sv = None
+                raise
+        self.calls += 1
+        loss = _SplitTrainReplay.apply(self, self._anchor, sent_vecs)
+        self._replayed()
+        return loss
 
 
 def packed_host_batch(adj, H, node_type, node_score, sent_vecs, adj_lengths):
