@@ -20,13 +20,14 @@ behind one autograd node, for the micro-steps of qagnn.py:252-278.
 question ids and runs QAGNN.forward in .eval() on it, so nothing of the batch is packed or uploaded on the host.
 
 `SplitTrainStep` trains from such a split: its forward graph assembles the micro-batch, gathers its labels and takes the
-cross-entropy loss; its backward graph adds the parameter gradients into `.grad` itself.
+cross-entropy or margin-rank loss; its backward graph adds the parameter gradients into `.grad` itself.
 """
 import contextlib
 
 import torch
 
 from . import distributed as _dist
+from .training import answer_loss, check_answer_loss
 
 
 class StatusWord:
@@ -475,7 +476,15 @@ class SplitEvalStep:
     cache keys) captures again first, so results are never computed from stale weights; in-place `.data` edits need
     `decoder.gnn.invalidate()` / `decoder.concept_emb.invalidate_table()` as for eager calls.  The first call captures, on its own
     batch; a capture raises ValueError when the packed graph prep refuses the split's sub-graphs.  Every call needs exactly
-    `batch_size` questions: run a final partial batch eagerly through split.batch + decoder, or with a step of its size."""
+    `batch_size` questions: run a final partial batch eagerly through split.batch + decoder, or with a step of its size.
+
+    A split built with `labels` is also scored, as evaluate_accuracy and the test loop of qagnn.py:30-38,298-310 score it,
+    inside the graph: pred = logits.view(bs, nc).argmax(1) (the first maximal choice on ties), `(pred == label).sum()` added
+    into `n_correct` and bs into `n_scored` (0-dim int64), and pred written into `predictions` (int64 [Q], -1 for a question
+    not scored since the last reset).  A question that appears more than once in a batch counts once per appearance and keeps
+    its last appearance's prediction.  These device tensors are allocated once and keep accumulating across recaptures;
+    `accuracy()` reads them once, `reset_scores()` starts over, and `score(question_ids, logits)` scores a final partial batch
+    run through split.batch + decoder with the same ops.  A split without labels is not scored."""
 
     def __init__(self, decoder, split, batch_size, *, edge_capacity, max_edges, node_capacity=None, autocast_dtype=None,
                  use_cuda_graph=True):
@@ -497,6 +506,13 @@ class SplitEvalStep:
         self.graph, self._status, self._key, self.captures = None, None, None, 0
         self.logits = self.pool_attn = None
         self.mode = "eager"
+        self.n_correct = self.n_scored = self.predictions = None
+        if split.labels is not None:
+            self.n_correct = torch.zeros((), dtype=torch.int64, device=dev)
+            self.n_scored = torch.zeros((), dtype=torch.int64, device=dev)
+            # one slot past the split takes the predictions of earlier appearances of a repeated id, which nobody reads
+            self._pred_slots = torch.full((split.n_questions + 1,), -1, dtype=torch.int64, device=dev)
+            self.predictions = self._pred_slots[:-1]
 
     def _autocast(self):
         if self.autocast_dtype is None:
@@ -526,15 +542,38 @@ class SplitEvalStep:
     def _body(self):
         with self._autocast():
             out = self.split.assemble(self._qids, self.edge_capacity, self._n_cap, self._out)
-            return self.decoder(self._sv, out["concept_ids"], out["node_type_ids"], out["node_scores"], out["adj_lengths"],
-                                self._adj)
+            logits, pool_attn = self.decoder(self._sv, out["concept_ids"], out["node_type_ids"], out["node_scores"],
+                                             out["adj_lengths"], self._adj)
+        if self.n_correct is not None:
+            self._score(self._qids, logits)
+        return logits, pool_attn
+
+    @torch.no_grad()
+    def _score(self, qids, logits):
+        """Enqueues the scoring of the questions `qids` (device int64 [bs], checked) from their logits; no host read."""
+        bs = qids.numel()
+        pred = logits.reshape(bs, self.split.num_choice).argmax(1)
+        self.n_correct.add_((pred == torch.index_select(self.split.labels, 0, qids)).sum())
+        self.n_scored.add_(bs)
+        # each id is written by its last appearance only (the others go to the spare slot), so no two writes race
+        pos = torch.arange(bs, device=qids.device)
+        again_later = ((qids[:, None] == qids[None, :]) & (pos[:, None] < pos[None, :])).any(1)
+        slot = torch.where(again_later, self.split.n_questions, qids)
+        self._pred_slots.index_copy_(0, slot, pred)
 
     def _capture(self):
         self.graph = self._status = None  # frees the previous capture's pool before the next one is made
         gnn = self.decoder.gnn
         self.split.assemble(self._qids, self.edge_capacity, self._n_cap, self._out)  # capture_guard validates this batch
-        self.graph, (self.logits, self.pool_attn), self._status = capture(gnn, self._adj, self._out["node_type_ids"],
-                                                                          "SplitEvalStep", self._body)
+        # capture_guard's warm-up really runs the body twice: keep it out of the scores
+        scores = [] if self.n_correct is None else [self.n_correct, self.n_scored, self._pred_slots]
+        saved = [t.clone() for t in scores]
+        try:
+            self.graph, (self.logits, self.pool_attn), self._status = capture(gnn, self._adj, self._out["node_type_ids"],
+                                                                              "SplitEvalStep", self._body)
+        finally:
+            for t, v in zip(scores, saved):
+                t.copy_(v)
         self._keep = (gnn._ws.buf, gnn._folded.blob, gnn._last_prep, getattr(self.decoder.concept_emb, "_ptab", None))
         self._key = self._weights_key()
         self.captures += 1
@@ -557,6 +596,36 @@ class SplitEvalStep:
         if self._status is not None:
             self._status.replayed()
         return self.logits, self.pool_attn
+
+    def _require_labels(self):
+        if self.n_correct is None:
+            raise ValueError("SplitEvalStep: the split has no labels, so nothing is scored; build the DeviceSplit with labels=")
+
+    def score(self, question_ids, logits):
+        """Scores the questions `question_ids` (host ids, any number) from their logits [bs*nc, 1] or [bs, nc] (device), e.g.
+        a final partial batch run through split.batch + decoder; the same ops the graph runs, enqueued on the current stream."""
+        self._require_labels()
+        q = self.split.check(question_ids, None)[0]
+        if logits.numel() != q.size * self.split.num_choice:
+            raise ValueError(f"SplitEvalStep.score: {logits.numel()} logits for {q.size} questions of "
+                             f"{self.split.num_choice} choices")
+        qids = torch.from_numpy(q).pin_memory().to(self.split.device, non_blocking=True)
+        self._score(qids, logits)
+
+    def accuracy(self):
+        """n_correct / n_scored as a float: the one host read of the scores."""
+        self._require_labels()
+        correct, scored = torch.stack((self.n_correct, self.n_scored)).tolist()
+        if scored == 0:
+            raise ValueError("SplitEvalStep: no question was scored since the last reset")
+        return correct / scored
+
+    def reset_scores(self):
+        """Zeroes n_correct and n_scored and sets every prediction to -1 (enqueued on the current stream)."""
+        self._require_labels()
+        self.n_correct.zero_()
+        self.n_scored.zero_()
+        self._pred_slots.fill_(-1)
 
 
 class _SplitTrainReplay(torch.autograd.Function):
@@ -587,20 +656,23 @@ class _SplitTrainReplay(torch.autograd.Function):
 
 class SplitTrainStep(_TrainingGraphs):
     """A training micro-step on a split held on the GPU (qagnn_b200.data.DeviceSplit built with `labels`) as two CUDA graphs:
-    the loop body of qagnn.py:252-278 with `--loss cross_entropy`, whose only per-call inputs are the question ids and
-    sent_vecs:
+    the loop body of qagnn.py:252-278 with `--loss cross_entropy` or `--loss margin_rank`, whose only per-call inputs are the
+    question ids and sent_vecs:
 
-        step = SplitTrainStep(model.decoder.train(), split, mbs, edge_capacity=K, max_edges=M, autocast_dtype=torch.float16)
-        loss = step(qids, sent_vecs) * len(qids) / bs     # qids: mbs host ids; the micro-batch's mean cross entropy, fp32
+        step = SplitTrainStep(model.decoder.train(), split, mbs, edge_capacity=K, max_edges=M, autocast_dtype=torch.float16,
+                              loss=args.loss)
+        loss = step(qids, sent_vecs) * len(qids) / bs     # qids: mbs host ids; the micro-batch's mean loss, fp32
         scaler.scale(loss).backward()                     # replays the backward graph
 
     The forward graph holds split.assemble (qagnn_assemble_batch and the node-row gathers), the gather of the micro-batch's
-    labels, `decoder(...)` in .train() on the padded batch and F.cross_entropy(logits.view(-1, num_choice), labels), under
-    torch.autocast(autocast_dtype, cache_enabled=False) (None, torch.float16 or torch.bfloat16).  The results equal
-    `decoder(sent_vecs, *split.batch(qids, K))` and that cross entropy under the same autocast.  A call checks the ids on the
-    host (DeviceSplit.check: IndexError / ValueError before anything is enqueued), uploads them (8 bytes per question),
-    copies sent_vecs into a static buffer (shape and dtype fixed by the first call, else ValueError) and replays the forward
-    graph.  It returns the loss as a 0-dim fp32 tensor; `logits` [mbs*nc, 1] and `pool_attn` are static buffers for logging.
+    labels, `decoder(...)` in .train() on the padded batch and training.answer_loss(logits, labels, num_choice, loss), under
+    torch.autocast(autocast_dtype, cache_enabled=False) (None, torch.float16 or torch.bfloat16).  `loss` is "cross_entropy"
+    (F.cross_entropy(logits.view(-1, num_choice), labels)) or "margin_rank" (the reference's margin-rank loss, with gathers
+    where the reference selects with boolean masks); any other name, or "margin_rank" with one choice, raises ValueError at
+    construction.  The results equal `decoder(sent_vecs, *split.batch(qids, K))` and the reference's loss under the same
+    autocast.  A call checks the ids on the host (DeviceSplit.check: IndexError / ValueError before anything is enqueued),
+    uploads them (8 bytes per question), copies sent_vecs into a static buffer (shape and dtype fixed by the first call, else
+    ValueError) and replays the forward graph.  It returns the loss as a 0-dim fp32 tensor; `logits` [mbs*nc, 1] and `pool_attn` are static buffers for logging.
     The next call overwrites all three, so each call's backward must run before the next call (else RuntimeError).
 
     The backward graph is torch.autograd.grad of the loss, seeded with the scalar autograd hands the step's node (the loss
@@ -619,16 +691,18 @@ class SplitTrainStep(_TrainingGraphs):
     Optimiser steps and load_state_dict keep the parameters' addresses, so the graphs stay valid; a call raises RuntimeError
     after `.to()` / `.cuda()`, after torch.use_deterministic_algorithms changed, after a change in which decoder parameters
     require grad, and in .eval() (build a new SplitTrainStep).  Every call needs exactly `batch_size` questions: run a final
-    partial micro-batch eagerly through split.batch + decoder + F.cross_entropy.  Padded batches on one GPU only."""
+    partial micro-batch eagerly through split.batch + decoder + training.answer_loss.  Padded batches on one GPU only."""
 
     what = "SplitTrainStep"
 
-    def __init__(self, decoder, split, batch_size, *, edge_capacity, max_edges, autocast_dtype=None):
+    def __init__(self, decoder, split, batch_size, *, edge_capacity, max_edges, autocast_dtype=None, loss="cross_entropy"):
         """`edge_capacity` K bounds the edges of every micro-batch (FlatAdjCache.max_batch_edges(batch_size)), `max_edges` M
         those of one sub-graph over the split (FlatAdjCache.max_graph_edges()): one capture then serves every micro-batch."""
         self._init_training(decoder, autocast_dtype)
         if split.labels is None:
             raise ValueError("SplitTrainStep: the split has no labels; build the DeviceSplit with labels=")
+        check_answer_loss(loss, split.num_choice)
+        self.loss = loss
         self.split, self.batch_size = split, int(batch_size)
         self.edge_capacity, self.max_edges = int(edge_capacity), int(max_edges)
         largest = int(split.counts.max()) if split.counts.size else 0
@@ -651,7 +725,7 @@ class SplitTrainStep(_TrainingGraphs):
             torch.index_select(self.split.labels, 0, self._qids, out=self._labels)
             logits, pool_attn = self.decoder(self._sv, out["concept_ids"], out["node_type_ids"], out["node_scores"],
                                              out["adj_lengths"], self._adj)
-            loss = torch.nn.functional.cross_entropy(logits.view(-1, nc), self._labels)
+            loss = answer_loss(logits, self._labels, nc, self.loss)
         if self._status is not None:
             self._status.record(self.decoder.gnn._last_prep.status_word())
         return loss, logits, pool_attn
@@ -686,7 +760,7 @@ class SplitTrainStep(_TrainingGraphs):
                 p.grad = b
 
     def __call__(self, question_ids, sent_vecs):
-        """The mean cross-entropy loss (0-dim fp32) of the questions `question_ids` (host ids, batch_size of them) with their
+        """The mean loss (0-dim fp32) of the questions `question_ids` (host ids, batch_size of them) with their
         sent_vecs [batch_size*nc, S] (device); `.backward()` replays the backward graph."""
         if not self.decoder.training:
             raise RuntimeError("SplitTrainStep replays the training forward: call decoder.train() first")

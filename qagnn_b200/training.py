@@ -80,6 +80,39 @@ def edge_table(enc, onehot_tab, prep, k_calls):
     return enc(onehot_tab)
 
 
+ANSWER_LOSSES = ("cross_entropy", "margin_rank")
+
+
+def check_answer_loss(loss, num_choice):
+    """ValueError unless answer_loss accepts (loss, num_choice)."""
+    if loss not in ANSWER_LOSSES:
+        raise ValueError(f"qagnn_b200: loss must be one of {ANSWER_LOSSES}, got {loss!r}")
+    if loss == "margin_rank" and int(num_choice) < 2:  # the reference would take the mean of no pairs (NaN)
+        raise ValueError(f"qagnn_b200: the margin-rank loss needs at least 2 choices, got num_choice = {int(num_choice)}")
+
+
+def answer_loss(logits, labels, num_choice, loss="cross_entropy"):
+    """The answer loss of qagnn.py:208-224 (`--loss cross_entropy` or `--loss margin_rank`) as a 0-dim tensor, from logits
+    [bs * nc, 1] or [bs, nc] and labels int64 [bs] on the same device.  Static shapes, no host read and no data-dependent op,
+    so it can be captured in a CUDA graph.
+
+    "cross_entropy" is F.cross_entropy(logits.view(-1, nc), labels).  "margin_rank" pairs every question's correct logit
+    with each of its nc - 1 wrong ones in the order the reference's boolean masks give (row-major, wrong choices in choice
+    order), selected with gathers instead of masks, and calls the op nn.MarginRankingLoss(margin=0.1) calls on them.  Same
+    op, same values, same order: the loss and its gradients equal the reference's bit for bit, under autocast too."""
+    check_answer_loss(loss, num_choice)
+    nc = int(num_choice)
+    logits2d = logits.view(-1, nc)
+    if loss == "cross_entropy":
+        return F.cross_entropy(logits2d, labels)
+    lab = labels.view(-1, 1)
+    correct = logits2d.gather(1, lab).expand(-1, nc - 1).reshape(-1)
+    j = torch.arange(nc - 1, device=logits.device)
+    wrong = logits2d.gather(1, j + (j >= lab)).reshape(-1)  # choice j, or j + 1 from the correct one on
+    y = wrong.new_ones((wrong.size(0),))
+    return F.margin_ranking_loss(correct, wrong, y, margin=0.1)
+
+
 def _core_dtype(*ts):
     """Storage dtype of one core call: the widest dtype of its operands (fp16 with bf16 widens to fp32).  Under autocast,
     operands of another floating dtype (fp64) are cast to fp32, as torch.amp.custom_fwd(cast_inputs=torch.float32) casts."""

@@ -9,6 +9,10 @@ synchronise, alternated over --reps repetitions:
 
   host_padded / host_ragged          flat.pack (pinned) + node rows sliced on the host, uploaded, eager decoder(...)
   resident_padded / resident_ragged  SplitEvalStep(question ids, sent_vecs): one CUDA graph per batch
+  resident_*_item                    the same step on a split without labels, scored as evaluate_accuracy (qagnn.py:30-38)
+                                     scores: argmax, compare with the batch's labels (on the device) and .item() per batch
+  resident_*_scored                  a step on the same split built with labels: scored inside its graph, reset_scores()
+                                     before the split and accuracy() (one read) after it
 
 It also reports the host pack time alone (per batch), the assembly kernel alone (qagnn_assemble_batch: CUDA events around a
 CUDA graph of 200 calls, so that the host's enqueue is not what is timed), max |d logits| and |d pool_attn| between every route
@@ -76,8 +80,14 @@ def main():
     svs = [torch.randn(B, SENT_DIM, device=dev, generator=g) * 0.5 for _ in batches]
 
     split = Dt.DeviceSplit(flat, cids, ntypes, scores, lens, dev, T, R)
+    labels = torch.from_numpy(np.random.default_rng(args.seed).integers(0, NC, bs * nb))
+    labelled = Dt.DeviceSplit(flat, cids, ntypes, scores, lens, dev, T, R, labels=labels)
+    batch_labels = [labels[q].to(dev) for q in batches]  # what the reference's loader hands evaluate_accuracy per batch
     caps = {"padded": None, "ragged": N_cap}
     steps = {name: SplitEvalStep(dec, split, bs, edge_capacity=K, max_edges=M, node_capacity=nc_) for name, nc_ in caps.items()}
+    scored = {name: SplitEvalStep(dec, labelled, bs, edge_capacity=K, max_edges=M, node_capacity=nc_)
+              for name, nc_ in caps.items()}
+    accuracy = {}
 
     def up(t):
         return t.contiguous().pin_memory().to(dev, non_blocking=True)
@@ -102,10 +112,34 @@ def main():
                 out.append((logits.clone(), attn.clone()))
         return out
 
+    def item_route(layout, keep=False):
+        out, n_correct = [], 0
+        for q, sv, lab in zip(batches, svs, batch_labels):
+            logits, attn = steps[layout](q, sv)
+            n_correct += (logits.view(bs, NC).argmax(1) == lab).sum().item()
+            if keep:
+                out.append((logits.clone(), attn.clone()))
+        accuracy[f"resident_{layout}_item"] = n_correct / (bs * nb)
+        return out
+
+    def scored_route(layout, keep=False):
+        out, step = [], scored[layout]
+        step.reset_scores()
+        for q, sv in zip(batches, svs):
+            logits, attn = step(q, sv)
+            if keep:
+                out.append((logits.clone(), attn.clone()))
+        accuracy[f"resident_{layout}_scored"] = step.accuracy()
+        return out
+
     routes = {f"host_{l}": (lambda l=l, keep=False: host_route(l, keep)) for l in caps}
     routes.update({f"resident_{l}": (lambda l=l, keep=False: resident_route(l, keep)) for l in caps})
+    routes.update({f"resident_{l}_item": (lambda l=l, keep=False: item_route(l, keep)) for l in caps})
+    routes.update({f"resident_{l}_scored": (lambda l=l, keep=False: scored_route(l, keep)) for l in caps})
     results = {name: fn(keep=True) for name, fn in routes.items()}  # also warms every route up (and captures the steps)
     torch.cuda.synchronize()
+    if len(set(accuracy.values())) != 1:
+        raise SystemExit(f"bench_resident_split.py: the scoring routes disagree: {accuracy}")
     ref = results["host_padded"]
     deltas = {name: {"max_abs_d_logits": max((a[0] - b[0]).abs().max().item() for a, b in zip(res, ref)),
                      "max_abs_d_pool_attn": max((a[1] - b[1]).abs().max().item() for a, b in zip(res, ref))}
@@ -169,7 +203,8 @@ def main():
            "D": D, "k": K_LAYERS, "sent_dim": SENT_DIM, "edge_capacity": K, "node_capacity": N_cap,
            "split_edges": int(flat.graph_ptr[-1]), "routes": {name: stats(ts) for name, ts in times.items()},
            "host_pack": pack_ms, "assemble_kernel_us": kernel_us, "vs_host_padded": deltas,
-           "captures": {name: s.captures for name, s in steps.items()}}
+           "captures": {name: s.captures for name, s in steps.items()},
+           "captures_scored": {name: s.captures for name, s in scored.items()}, "accuracy": accuracy}
     res["speedup"] = {l: res["routes"][f"host_{l}"]["ms_per_batch"] / res["routes"][f"resident_{l}"]["ms_per_batch"] for l in caps}
     line = json.dumps(res)
     print(line)
