@@ -399,6 +399,24 @@ int32_t qagnn_assemble_batch(const int32_t *src, const int32_t *tgt, const int16
                              const int64_t *question_ids, int32_t bs, int64_t K, int64_t N_cap, int64_t *edges,
                              int64_t *graph_ptr_out, int64_t *node_ptr_out, void *stream);
 
+/* One step of the reference's RAdam (utils/optimization_utils.py) over n_tensors fp32 tensors of the current device, in one
+ * launch per 512 tensors or 16 distinct groups (qagnn_b200.optim.RAdam).  Tensor i: contiguous params[i], grads[i], exp_avgs[i],
+ * exp_avg_sqs[i] of numels[i] elements, its int64 device step counter steps[i], and its group group_index[i] < n_groups.  The
+ * per-group host arrays lr, weight_decay, beta1, beta2, eps and degenerated_to_sgd hold the Python values; each scalar the
+ * update uses is rounded to fp32 as torch rounds it.  step_tables[g] is a device fp64 [table_len, 2] table of (1.0 when
+ * rho_t >= 5 else 0.0, step size) for t = row, built with the reference's formula for the group's betas; the device step after
+ * the increment indexes it, so table_len must exceed every step counter.  found_inf (optional, device fp32): nonzero leaves
+ * every tensor and step as it is.  grad_scale (optional, device fp32): the gradients are first multiplied by
+ * (float)(1.0 / (double)*grad_scale), as GradScaler.unscale_ does, and written back.  counter: a device int32 that is zero
+ * between calls (the kernel resets it).  Every element is the eager torch op sequence's result bit for bit; no host
+ * synchronisation. */
+int32_t qagnn_radam_step(int32_t n_tensors, void *const *params, void *const *grads, void *const *exp_avgs,
+                         void *const *exp_avg_sqs, void *const *steps, const int64_t *numels, const int32_t *group_index,
+                         int32_t n_groups, const double *lr, const double *weight_decay, const double *beta1,
+                         const double *beta2, const double *eps, const int32_t *degenerated_to_sgd,
+                         void *const *step_tables, int64_t table_len, const float *found_inf, const float *grad_scale,
+                         int32_t *counter, void *stream);
+
 /* Launch counters since load (kernels this library enqueued); for bench.py's gpu_launches. */
 int64_t qagnn_launch_count(void);
 

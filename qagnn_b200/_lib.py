@@ -103,6 +103,8 @@ EXPORTS = {
                                                          C.c_int64] + [_P] * 16 + [C.c_size_t, _P]),
     "qagnn_assemble_batch": (C.c_int32, [_P, _P, _P, _P, _P, C.c_int64, C.c_int32, C.c_int32, _P, C.c_int32, C.c_int64,
                                          C.c_int64, _P, _P, _P, _P]),
+    "qagnn_radam_step": (C.c_int32, [C.c_int32, _P, _P, _P, _P, _P, _P, _P, C.c_int32, _P, _P, _P, _P, _P, _P, _P, C.c_int64,
+                                     _P, _P, _P, _P]),
     "qagnn_launch_count": (C.c_int64, []),
     "qagnn_profile_enable": (C.c_int32, [C.c_int32]),
     "qagnn_profile_read": (C.c_int32, [C.POINTER(C.c_double), C.POINTER(C.c_int64)]),
