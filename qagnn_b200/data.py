@@ -8,7 +8,7 @@ tensors, so a batch needs two H2D copies.  The nested-list format keeps working 
 """
 import os
 import pickle
-from dataclasses import dataclass
+from dataclasses import dataclass, replace
 
 import numpy as np
 import torch
@@ -58,11 +58,10 @@ class PackedAdj:
         me = self.max_edges if self.max_edges >= 0 else (int((self.graph_ptr[1:] - self.graph_ptr[:-1]).max()) if self.graph_ptr.numel() > 1 else 0)
         if self.buf is not None:
             b = self.buf.to(device, non_blocking=non_blocking)
-            return PackedAdj(b[:2], b[2], self.graph_ptr, self.n_nodes, b, gpd, me, self.n_edges, self.edge_capacity,
-                             self.node_ptr, npd, self.node_capacity)
-        return PackedAdj(self.edge_index.to(device, non_blocking=non_blocking),
-                         self.edge_type.to(device, non_blocking=non_blocking), self.graph_ptr, self.n_nodes, None, gpd, me,
-                         self.n_edges, self.edge_capacity, self.node_ptr, npd, self.node_capacity)
+            return replace(self, edge_index=b[:2], edge_type=b[2], buf=b, graph_ptr_dev=gpd, max_edges=me, node_ptr_dev=npd)
+        return replace(self, edge_index=self.edge_index.to(device, non_blocking=non_blocking),
+                       edge_type=self.edge_type.to(device, non_blocking=non_blocking), graph_ptr_dev=gpd, max_edges=me,
+                       node_ptr_dev=npd)
 
     # LM_QAGNN.forward slices inputs positionally and calls .size() only on tensors before the last two; everywhere an
     # (edge_index, edge_type) pair is expected a PackedAdj unpacks / indexes as that pair
@@ -531,8 +530,10 @@ class DeviceSplit:
         """The PackedAdj over the buffers `out` (views, no copy); the host fields are the caller's (None / -1 when unknown)."""
         e = out["edges"]
         ragged = int(node_capacity) >= 0
-        return PackedAdj(e[:2], e[2], graph_ptr, self.n_nodes, e, out["graph_ptr"], int(max_edges), int(n_edges),
-                         int(edge_capacity), node_ptr, out["node_ptr"] if ragged else None, int(node_capacity))
+        return PackedAdj(edge_index=e[:2], edge_type=e[2], graph_ptr=graph_ptr, n_nodes=self.n_nodes, buf=e,
+                         graph_ptr_dev=out["graph_ptr"], max_edges=int(max_edges), n_edges=int(n_edges),
+                         edge_capacity=int(edge_capacity), node_ptr=node_ptr,
+                         node_ptr_dev=out["node_ptr"] if ragged else None, node_capacity=int(node_capacity))
 
     def batch(self, question_ids, edge_capacity, node_capacity=None, out=None):
         """(concept_ids [B, n], node_type_ids [B, n], node_scores [B, n, 1], adj_lengths [B], PackedAdj) on the device for the

@@ -584,19 +584,34 @@ class QAGNN_Message_Passing(nn.Module):
         entry = self._graphs.get(key)
         if entry is None:
             from .pipeline import capture
-            graph, out, status = capture(self, A, node_type, "QAGNN_Message_Passing",
-                                         lambda: self.forward(H, A, node_type, node_score))
+            captured = capture(self, A, node_type, "QAGNN_Message_Passing", lambda: self.forward(H, A, node_type, node_score))
             if len(self._graphs) >= 8:
                 self._graphs.pop(next(iter(self._graphs)))
-            # the entry keeps alive everything whose address the graph baked in: inputs, workspace, folded blob, prep
-            entry = self._graphs[key] = (graph, out, status, tensors, self._ws.buf, self._folded.blob, self._last_prep)
+            # the entry keeps alive everything whose address the graph baked in: the inputs and what capture() kept
+            entry = self._graphs[key] = captured + (tensors,)
         graph, out, status = entry[:3]
         graph.replay()
-        if status is not None:
-            status.replayed()
-            if status not in self._replayed:
-                self._replayed.append(status)
+        status.replayed()
+        if status not in self._replayed:
+            self._replayed.append(status)
         return out
+
+
+def decoder_tail(pooler, sent_vecs, gnn_output, node_type_ids, adj_lengths, fused=True, dropout=None):
+    """The decoder tail of a padded batch (modeling_qagnn.py:172-187): (cat(graph_vecs, sent_vecs, Z) [B, 2D + S], pool_attn).
+    With `fused` it first tries pooler.pool_concat, mask + pooling + cat in one kernel, which runs in eval only, where
+    dropout is the identity.  When that is off or refuses the shape: the pool mask, pooler(...) and torch.cat, with
+    `dropout` (if given) applied to the concat."""
+    if fused:
+        out = pooler.pool_concat(sent_vecs, gnn_output, node_type_ids, adj_lengths)
+        if out is not None:
+            return out
+    pos = torch.arange(gnn_output.size(1), device=gnn_output.device)
+    mask = (pos >= adj_lengths.unsqueeze(1)) | (node_type_ids == 3)
+    mask[:, 0] = mask[:, 0] & ~mask.all(1)  # a fully masked row keeps node 0 (:176; written without a host sync)
+    graph_vecs, pool_attn = pooler(sent_vecs, gnn_output, mask)
+    concat = torch.cat((graph_vecs, sent_vecs, gnn_output[:, 0]), 1)
+    return (concat if dropout is None else dropout(concat)), pool_attn
 
 
 class QAGNN(nn.Module):
@@ -639,7 +654,6 @@ class QAGNN(nn.Module):
             return self._pooled_features_ragged(sent_vecs, concept_ids, node_type_ids, node_scores, adj_lengths, adj, emb_data,
                                                 cache_output)
         n = node_scores.size(1)
-        pos = torch.arange(n, device=node_scores.device)
         fused_head = (not self.training and not torch.is_grad_enabled() and emb_data is None and node_scores.is_cuda
                       and not self.concept_emb.use_contextualized and self.concept_dim % 4 == 0
                       and concept_ids.device == node_scores.device and sent_vecs.dtype == torch.float32)
@@ -666,18 +680,10 @@ class QAGNN(nn.Module):
             gnn_input, s = self._head(sent_vecs, concept_ids, node_type_ids, node_scores, adj_lengths, emb_data)
 
         gnn_output = self.gnn(gnn_input, adj, node_type_ids, s)
-        fused = self.pooler.pool_concat(sent_vecs, gnn_output, node_type_ids, adj_lengths) if not self.training else None
-        if fused is not None:  # pool mask + pooling + cat(graph_vecs, sent_vecs, Z) in one kernel (dropout_fc = identity in eval)
-            if cache_output:
-                self.concept_ids, self.adj, self.pool_attn = concept_ids, adj, fused[1]
-            return fused
-        Z_vecs = gnn_output[:, 0]
-        mask = (pos >= adj_lengths.unsqueeze(1)) | (node_type_ids == 3)
-        mask[:, 0] = mask[:, 0] & ~mask.all(1)  # a fully masked row keeps node 0 (:176; written without a host sync)
-        graph_vecs, pool_attn = self.pooler(sent_vecs, gnn_output, mask)
+        concat, pool_attn = decoder_tail(self.pooler, sent_vecs, gnn_output, node_type_ids, adj_lengths,
+                                         fused=not self.training, dropout=self.dropout_fc)
         if cache_output:
             self.concept_ids, self.adj, self.pool_attn = concept_ids, adj, pool_attn
-        concat = self.dropout_fc(torch.cat((graph_vecs, sent_vecs, Z_vecs), 1))
         return concat, pool_attn
 
     def _head(self, sent_vecs, concept_ids, node_type_ids, node_scores, adj_lengths, emb_data):

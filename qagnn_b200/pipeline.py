@@ -27,27 +27,50 @@ import contextlib
 import torch
 
 from . import distributed as _dist
+from .data import PackedAdj
+from .modeling_qagnn import _version_key, decoder_tail
 from .training import answer_loss, check_answer_loss
+
+_EVAL_AUTOCAST = (None, torch.bfloat16)
+_TRAIN_AUTOCAST = (None, torch.float16, torch.bfloat16)
+
+
+def _checked_autocast(dtype, allowed):
+    """`dtype` when it is one of `allowed` (None: no autocast), else ValueError."""
+    if dtype not in allowed:
+        names = [str(d) for d in allowed]
+        raise ValueError(f"autocast_dtype must be {', '.join(names[:-1])} or {names[-1]}")
+    return dtype
+
+
+def _autocast(dtype):
+    """The context a step captures and runs under: torch.autocast(dtype, cache_enabled=False), or none for dtype None."""
+    if dtype is None:
+        return contextlib.nullcontext()
+    return torch.autocast("cuda", dtype=dtype, cache_enabled=False)
 
 
 class StatusWord:
     """Graph prep's index checks across CUDA-graph replays, without blocking the host.  A replay cannot synchronise to
     validate a batch, so inside the capture `record(word)` ORs graph prep's status word into a device word and copies that
     to pinned memory.  `replayed()` marks the end of a replay, and `check()` raises IndexError once the copy of a replay
-    has landed with a bit set: at a later call, never by waiting for the GPU."""
+    has landed with a bit set: at a later call, never by waiting for the GPU.  Built without a device (index checks off),
+    the word does nothing."""
 
-    def __init__(self, device):
-        self.accum = torch.zeros(1, dtype=torch.int32, device=device)
-        self.host = torch.zeros(1, dtype=torch.int32).pin_memory()
+    def __init__(self, device=None):
+        self.accum = None if device is None else torch.zeros(1, dtype=torch.int32, device=device)
+        self.host = None if device is None else torch.zeros(1, dtype=torch.int32).pin_memory()
         self.pending = None  # event after the last replay's copy
 
     def record(self, word):
-        self.accum.bitwise_or_(word)
-        self.host.copy_(self.accum, non_blocking=True)
+        if self.accum is not None:
+            self.accum.bitwise_or_(word)
+            self.host.copy_(self.accum, non_blocking=True)
 
     def replayed(self):
-        self.pending = torch.cuda.Event()
-        self.pending.record()
+        if self.accum is not None:
+            self.pending = torch.cuda.Event()
+            self.pending.record()
 
     def check(self, what):
         if self.pending is None or not self.pending.query():  # the accumulated word is looked at again later
@@ -64,10 +87,10 @@ class StatusWord:
 @contextlib.contextmanager
 def capture_guard(gnn, adj, node_type, what, warmup):
     """Prepares the capture of CUDA graphs that run QAGNN_Message_Passing `gnn` on the batch (adj, node_type) and yields the
-    StatusWord the capture records graph prep's status word into (None with gnn.check_indices off).  Before it yields, it
-    validates the batch once, eagerly, and runs `warmup` twice on a side stream: that folds the weights, sizes the
-    workspaces and loads the kernels.  Inside, gnn.use_cuda_graph and gnn.check_indices are off: the module's kernels
-    become nodes of the caller's graph, and a replay cannot synchronise.  Both are restored on exit.
+    StatusWord the capture records graph prep's status word into (one that does nothing with gnn.check_indices off).
+    Before it yields, it validates the batch once, eagerly, and runs `warmup` twice on a side stream: that folds the
+    weights, sizes the workspaces and loads the kernels.  Inside, gnn.use_cuda_graph and gnn.check_indices are off: the
+    module's kernels become nodes of the caller's graph, and a replay cannot synchronise.  Both are restored on exit.
 
     An adjacency that carries graph_ptr must get the packed prep, else ValueError: the general prep would keep the edge
     count of the batch it was captured on for every later batch written into the same buffers."""
@@ -87,21 +110,22 @@ def capture_guard(gnn, adj, node_type, what, warmup):
         if getattr(adj, "graph_ptr_dev", None) is not None and not gnn._last_prep.packed:
             raise ValueError(f"{what}: the packed graph prep refuses these sub-graphs (too large for one CTA); a captured "
                              "general prep would keep the edge count of this batch for every later one")
-        yield StatusWord(dev) if saved[1] else None
+        yield StatusWord(dev if saved[1] else None)
     finally:
         gnn.use_cuda_graph, gnn.check_indices = saved
 
 
 def capture(gnn, adj, node_type, what, fn):
     """`fn()` captured as one CUDA graph under capture_guard, with graph prep's status word recorded at its end.  Returns
-    (graph, what fn returned, StatusWord or None)."""
+    (graph, what fn returned, StatusWord, kept).  `kept` holds the buffers of `gnn` whose addresses the graph baked in
+    (workspace, folded weights, graph prep): the caller keeps it as long as it keeps the graph, else a later replay reads
+    freed memory once gnn replaces them."""
     with capture_guard(gnn, adj, node_type, what, fn) as status:
         graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(graph):
             out = fn()
-            if status is not None:
-                status.record(gnn._last_prep.status_word())
-    return graph, out, status
+            status.record(gnn._last_prep.status_word())
+    return graph, out, status, (gnn._ws.buf, gnn._folded.blob, gnn._last_prep)
 
 
 class DecoderStep:
@@ -135,10 +159,8 @@ class DecoderStep:
         `max_nodes` n bounds one graph's rows (the loader's max_node_num; `pool_attn` is [n_head*B, n]).  node_ptr is rebuilt
         from adj_lengths on the device in every run, so one capture at N_cap and the edge capacity serves every full batch of a
         split.  `gnn_out` is then [N_cap, D].  Single GPU only."""
-        if autocast_dtype not in (None, torch.bfloat16):
-            raise ValueError("autocast_dtype must be None or torch.bfloat16")
+        self.autocast_dtype = _checked_autocast(autocast_dtype, _EVAL_AUTOCAST)
         self.gnn, self.pooler, self.fc = gnn, pooler, fc
-        self.autocast_dtype = autocast_dtype
         self.inp = {k: inputs[k] for k in self.FIELDS}
         self.adj = (self.inp["edge_index"], self.inp["edge_type"])
         self.ragged = self.inp["H"].dim() == 2
@@ -148,39 +170,30 @@ class DecoderStep:
                 raise ValueError("DecoderStep: ragged batches run on one GPU (world_size == 1)")
             if "graph_ptr" not in inputs or max_edges < 0 or max_nodes is None:
                 raise ValueError("DecoderStep: a ragged step needs inputs['graph_ptr'], max_edges and max_nodes")
-            from .data import PackedAdj
-            self.inp["graph_ptr"] = inputs["graph_ptr"]
             al = self.inp["adj_lengths"]
             self._node_ptr = torch.zeros(al.numel() + 1, dtype=torch.int64, device=al.device)
             self._update_node_ptr()
-            self.adj = PackedAdj(self.inp["edge_index"], self.inp["edge_type"], None, int(max_nodes), None,
-                                 self.inp["graph_ptr"], int(max_edges), -1, self.inp["edge_index"].size(1), None,
-                                 self._node_ptr, self.inp["H"].size(0))
-        elif "graph_ptr" in inputs and max_edges >= 0:
-            from .data import PackedAdj
+        if self.ragged or ("graph_ptr" in inputs and max_edges >= 0):
             self.inp["graph_ptr"] = inputs["graph_ptr"]
-            self.adj = PackedAdj(self.inp["edge_index"], self.inp["edge_type"], None, self.inp["H"].size(1), None,
-                                 self.inp["graph_ptr"], int(max_edges), -1, self.inp["edge_index"].size(1))
+            self.adj = PackedAdj(edge_index=self.inp["edge_index"], edge_type=self.inp["edge_type"], graph_ptr=None,
+                                 n_nodes=int(max_nodes) if self.ragged else self.inp["H"].size(1),
+                                 graph_ptr_dev=self.inp["graph_ptr"], max_edges=int(max_edges),
+                                 edge_capacity=self.inp["edge_index"].size(1), node_ptr_dev=self._node_ptr,
+                                 node_capacity=self.inp["H"].size(0) if self.ragged else -1)
         self.world, self.group = world_size, group
         dev = self.inp["H"].device
         B, D = self.inp["sent_vecs"].size(0), self.inp["H"].size(-1)
         S = self.inp["sent_vecs"].size(1)
         self.full = torch.empty(world_size * B, 2 * D + S, device=dev) if world_size > 1 else None
         self.graph = None
-        self._status = None  # StatusWord of the captured graph prep (None: eager, or check_indices off)
         self.logits = self.pool_attn = self.gnn_out = None
         self.mode = "eager"
         if use_cuda_graph:
             self._capture()
 
-    def _autocast(self):
-        if self.autocast_dtype is None:
-            return contextlib.nullcontext()
-        return torch.autocast("cuda", dtype=self.autocast_dtype, cache_enabled=False)
-
     @torch.no_grad()
     def _eager(self):
-        with self._autocast():
+        with _autocast(self.autocast_dtype):
             return self._eager_body()
 
     def _update_node_ptr(self):
@@ -195,24 +208,14 @@ class DecoderStep:
                                                                d["adj_lengths"], self.adj.n_nodes)
             return self.fc(concat), pool_attn, out
         out = self.gnn(d["H"], self.adj, d["node_type"], d["node_score"])
-        fused = self.pooler.pool_concat(d["sent_vecs"], out, d["node_type"], d["adj_lengths"])  # :172-187 in one kernel
-        if fused is not None:
-            concat, pool_attn = fused
-        else:
-            n = out.size(1)
-            pos = torch.arange(n, device=out.device)
-            mask = (pos >= d["adj_lengths"].unsqueeze(1)) | (d["node_type"] == 3)        # modeling_qagnn.py:174-175
-            mask[:, 0] = mask[:, 0] & ~mask.all(1)                                          # :176
-            graph_vecs, pool_attn = self.pooler(d["sent_vecs"], out, mask)                  # :180
-            concat = torch.cat((graph_vecs, d["sent_vecs"], out[:, 0]), 1)                  # :187 (dropout = identity in eval)
+        concat, pool_attn = decoder_tail(self.pooler, d["sent_vecs"], out, d["node_type"], d["adj_lengths"])  # :172-187
         full = _dist.all_gather_rows(concat, self.world, self.group, True, self.full)       # the path's one collective
         return self.fc(full), pool_attn, out                                                # :188
 
     def _capture(self):
         # the warm-up also opens the NCCL channels of the all-gather
-        self.graph, (self.logits, self.pool_attn, self.gnn_out), self._status = capture(
+        self.graph, (self.logits, self.pool_attn, self.gnn_out), self._status, self._keep = capture(
             self.gnn, self.adj, self.inp["node_type"], "DecoderStep", self._eager)
-        self._keep = (self.gnn._ws.buf, self.gnn._folded.blob, self.gnn._last_prep)  # addresses baked into the graph
         self.mode = "one CUDA graph (prep + k layers + pooling" + (" + all-gather" if self.world > 1 else "") + " + fc)"
 
     def run(self):
@@ -220,11 +223,9 @@ class DecoderStep:
         index out of range (or an edge crossing its sub-graph) raises IndexError at a later call, once the copy of the
         status word has landed; its results were computed from clamped indices."""
         if self.graph is not None:
-            if self._status is not None:
-                self._status.check("DecoderStep")
+            self._status.check("DecoderStep")
             self.graph.replay()
-            if self._status is not None:
-                self._status.replayed()
+            self._status.replayed()
         else:
             self.logits, self.pool_attn, self.gnn_out = self._eager()
         return self.logits, self.pool_attn, self.gnn_out
@@ -237,19 +238,13 @@ class _TrainingGraphs:
     what = None  # the class name in messages
 
     def _init_training(self, decoder, autocast_dtype):
-        if autocast_dtype not in (None, torch.float16, torch.bfloat16):
-            raise ValueError("autocast_dtype must be None, torch.float16 or torch.bfloat16")
+        self.autocast_dtype = _checked_autocast(autocast_dtype, _TRAIN_AUTOCAST)
         if not decoder.training:
             raise ValueError(f"{self.what} captures the training forward: call decoder.train() first")
-        self.decoder, self.autocast_dtype = decoder, autocast_dtype
+        self.decoder = decoder
         self.deterministic = torch.are_deterministic_algorithms_enabled()
-        self._fwd = self._status = None
+        self._fwd = None
         self.mode = "eager"
-
-    def _autocast(self):
-        if self.autocast_dtype is None:
-            return contextlib.nullcontext()
-        return torch.autocast("cuda", dtype=self.autocast_dtype, cache_enabled=False)
 
     def _addresses(self):
         return tuple(t.data_ptr() for t in self._params + self._buffers)
@@ -257,7 +252,7 @@ class _TrainingGraphs:
     def _capture_graphs(self, adj, node_type, forward, backward, owned=()):
         """Captures `forward()` -> (y, ...) and `backward(y, dy)` as two CUDA graphs in one pool, on the batch (adj,
         node_type) already in the static buffers.  capture_guard first validates that batch and runs forward + backward twice
-        (dy = 1) on a side stream; `forward` records graph prep's status word into self._status when that is set.  The
+        (dy = 1) on a side stream; the forward graph ends by recording graph prep's status word into self._status.  The
         warm-up really runs: the decoder's buffers, the .grad of its trainable parameters (self._params), the tensors `owned`
         and the CUDA RNG state are put back afterwards.  Returns (forward's outputs, the static dy buffer, backward's result)."""
         dec = self.decoder
@@ -274,23 +269,20 @@ class _TrainingGraphs:
         rng = torch.cuda.get_rng_state(dev)
         try:
             with capture_guard(dec.gnn, adj, node_type, self.what, warmup) as status:
-                self._status = status
                 pool = torch.cuda.graph_pool_handle()
                 fwd, bwd = torch.cuda.CUDAGraph(), torch.cuda.CUDAGraph()
                 with torch.cuda.graph(fwd, pool=pool):
                     out = forward()
+                    status.record(dec.gnn._last_prep.status_word())
                 dy = torch.empty_like(out[0])
                 with torch.cuda.graph(bwd, pool=pool):
                     res = backward(out[0], dy)
-            self._fwd, self._bwd = fwd, bwd
+            self._fwd, self._bwd, self._status = fwd, bwd, status
             self._bn_buffers = [b for m in dec.modules() if isinstance(m, torch.nn.modules.batchnorm._BatchNorm)
                                 for b in (m.running_mean, m.running_var, m.num_batches_tracked) if b is not None]
             self._ptrs = self._addresses()
             self.mode = "two CUDA graphs (forward + backward)"
             return out, dy, res
-        except BaseException:
-            self._status = None
-            raise
         finally:
             with torch.no_grad():
                 for b, s in zip(self._buffers + list(owned), saved):
@@ -311,12 +303,10 @@ class _TrainingGraphs:
         if torch.are_deterministic_algorithms_enabled() != self.deterministic:
             raise RuntimeError(f"{what} was captured with torch.use_deterministic_algorithms({self.deterministic}) and "
                                f"its backward graph holds that mode's kernels; the flag changed since. Build a new {what}.")
-        if self._status is not None:
-            self._status.check(what)
+        self._status.check(what)
 
     def _replayed(self):
-        if self._status is not None:
-            self._status.replayed()
+        self._status.replayed()
         # the replay changed the running statistics behind autograd's back: the eval path's folded weights key on versions
         torch.autograd.graph.increment_version(self._bn_buffers)
 
@@ -395,8 +385,8 @@ class TrainStep(_TrainingGraphs):
         self._cid, self._nt, self._al = concept_ids.clone(), node_type_ids.clone(), adj_lengths.clone()
         self._edges = torch.zeros(3, K, dtype=torch.int64, device=dev)
         self._gp = torch.zeros(B + 1, dtype=torch.int64, device=dev)
-        from .data import PackedAdj
-        self._adj = PackedAdj(self._edges[:2], self._edges[2], None, n, self._edges, self._gp, self.max_edges, -1, K)
+        self._adj = PackedAdj(edge_index=self._edges[:2], edge_type=self._edges[2], graph_ptr=None, n_nodes=n,
+                              buf=self._edges, graph_ptr_dev=self._gp, max_edges=self.max_edges, edge_capacity=K)
         self._copy_batch(sent_vecs, concept_ids, node_type_ids, node_scores, adj_lengths, packed_adj)
         if use_cuda_graph:
             self._capture()
@@ -427,16 +417,10 @@ class TrainStep(_TrainingGraphs):
             self._edges[2, :ne].copy_(adj.edge_type[:ne], non_blocking=True)
         self._gp.copy_(adj.graph_ptr_dev if adj.graph_ptr_dev is not None else gp, non_blocking=True)
 
-    def _forward(self, sent_vecs, node_scores):
-        logits, pool_attn = self.decoder(sent_vecs, self._cid, self._nt, node_scores, self._al, self._adj)
-        if self._status is not None:
-            self._status.record(self.decoder.gnn._last_prep.status_word())
-        return logits, pool_attn
-
     def _capture(self):
         def forward():
-            with self._autocast():
-                return self._forward(self._sv, self._ns)
+            with _autocast(self.autocast_dtype):
+                return self.decoder(self._sv, self._cid, self._nt, self._ns, self._al, self._adj)
 
         def backward(logits, d_logits):
             return torch.autograd.grad(logits, [self._sv, self._ns] + self._params, d_logits, allow_unused=True)
@@ -449,15 +433,53 @@ class TrainStep(_TrainingGraphs):
         if self._fwd is not None:
             self._check_replay()
         self._copy_batch(sent_vecs, concept_ids, node_type_ids, node_scores, adj_lengths, packed_adj)
-        with self._autocast():
+        with _autocast(self.autocast_dtype):
             if self._fwd is None:
-                return self._forward(sent_vecs, node_scores)
+                return self.decoder(sent_vecs, self._cid, self._nt, node_scores, self._al, self._adj)
             out = _TrainReplay.apply(self, sent_vecs, node_scores, *self._params)
         self._replayed()
         return out
 
 
-class SplitEvalStep:
+class _SplitBatches:
+    """What SplitEvalStep and SplitTrainStep share: static buffers for batches of `batch_size` questions of a DeviceSplit at
+    one edge capacity (and, ragged, one node capacity), the per-call check and upload of the question ids, and the
+    assembly and decoder call their graphs hold.  A subclass provides `what` (its name in messages), `unit` (what a
+    partial batch is called), `decoder`, `_sv` and `_check_sent_vecs`."""
+
+    def _init_split(self, split, batch_size, edge_capacity, max_edges, node_capacity=None):
+        self.split, self.batch_size = split, int(batch_size)
+        self.edge_capacity, self.max_edges = int(edge_capacity), int(max_edges)
+        self.node_capacity = node_capacity
+        self._n_cap = -1 if node_capacity is None else int(node_capacity)
+        self._qids = torch.zeros(self.batch_size, dtype=torch.int64, device=split.device)
+        self._out = split.buffers(self.batch_size, self.edge_capacity, node_capacity)
+        self._adj = split.packed_adj(self._out, self.max_edges, self.edge_capacity, self._n_cap)
+        self.logits = self.pool_attn = None
+        self.captures = 0
+
+    def _load_ids(self, question_ids, sent_vecs):
+        """Checks a call's question ids on the host (DeviceSplit.check), its batch size and its sent_vecs, and only then
+        enqueues the upload of the ids: a refused call leaves the static buffers as they were."""
+        q = self.split.check(question_ids, self.edge_capacity, self.node_capacity)[0]
+        if q.size != self.batch_size:
+            raise ValueError(f"{self.what}: {q.size} questions, the step was built for {self.batch_size}; run a partial "
+                             f"{self.unit} through split.batch + decoder")
+        self._check_sent_vecs(sent_vecs)
+        # a pinned block from the caching host allocator per call: it is not reused before this copy has run
+        self._qids.copy_(torch.from_numpy(q).pin_memory(), non_blocking=True)
+
+    def _assemble(self):
+        """Enqueues the assembly of the loaded ids' batch into the static buffers; returns them."""
+        return self.split.assemble(self._qids, self.edge_capacity, self._n_cap, self._out)
+
+    def _decode(self, out):
+        """decoder(...) on the assembled buffers `out` and the step's sent_vecs: (logits, pool_attn)."""
+        return self.decoder(self._sv, out["concept_ids"], out["node_type_ids"], out["node_scores"], out["adj_lengths"],
+                            self._adj)
+
+
+class SplitEvalStep(_SplitBatches):
     """Evaluation of a split held on the GPU (qagnn_b200.data.DeviceSplit) as one CUDA graph per step: batch assembly from the
     question ids (qagnn_assemble_batch), the node-row gathers and `decoder(...)` itself under no_grad, i.e. QAGNN.forward in
     .eval() (head kernel -> message passing -> pooling tail -> fc).  A call's only inputs are the question ids and sent_vecs:
@@ -486,25 +508,20 @@ class SplitEvalStep:
     `accuracy()` reads them once, `reset_scores()` starts over, and `score(question_ids, logits)` scores a final partial batch
     run through split.batch + decoder with the same ops.  A split without labels is not scored."""
 
+    what, unit = "SplitEvalStep", "batch"
+
     def __init__(self, decoder, split, batch_size, *, edge_capacity, max_edges, node_capacity=None, autocast_dtype=None,
                  use_cuda_graph=True):
-        if autocast_dtype not in (None, torch.bfloat16):
-            raise ValueError("autocast_dtype must be None or torch.bfloat16")
+        self.autocast_dtype = _checked_autocast(autocast_dtype, _EVAL_AUTOCAST)
         if decoder.training:
             raise ValueError("SplitEvalStep runs the eval forward: call decoder.eval() first")
-        self.decoder, self.split, self.autocast_dtype = decoder, split, autocast_dtype
-        self.batch_size, self.edge_capacity, self.max_edges = int(batch_size), int(edge_capacity), int(max_edges)
-        self.node_capacity = node_capacity
-        self._n_cap = -1 if node_capacity is None else int(node_capacity)
+        self.decoder = decoder
+        self._init_split(split, batch_size, edge_capacity, max_edges, node_capacity)
         dev = split.device
-        B = self.batch_size * split.num_choice
-        self._qids = torch.zeros(self.batch_size, dtype=torch.int64, device=dev)
-        self._sv = torch.zeros(B, decoder.svec2nvec.in_features, dtype=torch.float32, device=dev)
-        self._out = split.buffers(self.batch_size, self.edge_capacity, node_capacity)
-        self._adj = split.packed_adj(self._out, self.max_edges, self.edge_capacity, self._n_cap)
+        self._sv = torch.zeros(self.batch_size * split.num_choice, decoder.svec2nvec.in_features, dtype=torch.float32,
+                               device=dev)
         self.use_cuda_graph = use_cuda_graph
-        self.graph, self._status, self._key, self.captures = None, None, None, 0
-        self.logits = self.pool_attn = None
+        self.graph, self._status, self._key = None, StatusWord(), None
         self.mode = "eager"
         self.n_correct = self.n_scored = self.predictions = None
         if split.labels is not None:
@@ -514,36 +531,20 @@ class SplitEvalStep:
             self._pred_slots = torch.full((split.n_questions + 1,), -1, dtype=torch.int64, device=dev)
             self.predictions = self._pred_slots[:-1]
 
-    def _autocast(self):
-        if self.autocast_dtype is None:
-            return contextlib.nullcontext()
-        return torch.autocast("cuda", dtype=self.autocast_dtype, cache_enabled=False)
-
     def _weights_key(self):
         """What the decoder's caches key on: parameter and buffer versions, the folded weights' key and the projected table's."""
-        from .modeling_qagnn import _version_key
         dec = self.decoder
         return (_version_key(list(dec.parameters()) + list(dec.buffers())), dec.gnn._folded.key,
                 getattr(dec.concept_emb, "_ptab_key", None))
 
-    def _load(self, question_ids, sent_vecs):
-        q = self.split.check(question_ids, self.edge_capacity, self.node_capacity)[0]
-        if q.size != self.batch_size:
-            raise ValueError(f"SplitEvalStep: {q.size} questions, the step was built for {self.batch_size}; run a partial "
-                             "batch through split.batch + decoder")
+    def _check_sent_vecs(self, sent_vecs):
         if tuple(sent_vecs.shape) != tuple(self._sv.shape):
             raise ValueError(f"SplitEvalStep: sent_vecs is {tuple(sent_vecs.shape)}, the step was built for {tuple(self._sv.shape)}")
-        # a pinned block from the caching host allocator per call: it is not reused before this copy has run
-        self._qids.copy_(torch.from_numpy(q).pin_memory(), non_blocking=True)
-        if self._sv.data_ptr() != sent_vecs.data_ptr():
-            self._sv.copy_(sent_vecs)
 
     @torch.no_grad()
     def _body(self):
-        with self._autocast():
-            out = self.split.assemble(self._qids, self.edge_capacity, self._n_cap, self._out)
-            logits, pool_attn = self.decoder(self._sv, out["concept_ids"], out["node_type_ids"], out["node_scores"],
-                                             out["adj_lengths"], self._adj)
+        with _autocast(self.autocast_dtype):
+            logits, pool_attn = self._decode(self._assemble())
         if self.n_correct is not None:
             self._score(self._qids, logits)
         return logits, pool_attn
@@ -562,19 +563,18 @@ class SplitEvalStep:
         self._pred_slots.index_copy_(0, slot, pred)
 
     def _capture(self):
-        self.graph = self._status = None  # frees the previous capture's pool before the next one is made
-        gnn = self.decoder.gnn
-        self.split.assemble(self._qids, self.edge_capacity, self._n_cap, self._out)  # capture_guard validates this batch
+        self.graph, self._status = None, StatusWord()  # frees the previous capture's pool before the next one is made
+        self._assemble()  # capture_guard validates this batch
         # capture_guard's warm-up really runs the body twice: keep it out of the scores
         scores = [] if self.n_correct is None else [self.n_correct, self.n_scored, self._pred_slots]
         saved = [t.clone() for t in scores]
         try:
-            self.graph, (self.logits, self.pool_attn), self._status = capture(gnn, self._adj, self._out["node_type_ids"],
-                                                                              "SplitEvalStep", self._body)
+            self.graph, (self.logits, self.pool_attn), self._status, kept = capture(
+                self.decoder.gnn, self._adj, self._out["node_type_ids"], "SplitEvalStep", self._body)
         finally:
             for t, v in zip(scores, saved):
                 t.copy_(v)
-        self._keep = (gnn._ws.buf, gnn._folded.blob, gnn._last_prep, getattr(self.decoder.concept_emb, "_ptab", None))
+        self._keep = kept + (getattr(self.decoder.concept_emb, "_ptab", None),)  # the graph reads the projected table too
         self._key = self._weights_key()
         self.captures += 1
         self.mode = "one CUDA graph (assembly + gathers + head + prep + k layers + pooling + fc)"
@@ -584,17 +584,17 @@ class SplitEvalStep:
         [bs*nc, S] (device); static buffers that the next call overwrites."""
         if self.decoder.training:
             raise RuntimeError("SplitEvalStep runs the eval forward: call decoder.eval() first")
-        if self._status is not None:
-            self._status.check("SplitEvalStep")
-        self._load(question_ids, sent_vecs)
+        self._status.check("SplitEvalStep")
+        self._load_ids(question_ids, sent_vecs)
+        if self._sv.data_ptr() != sent_vecs.data_ptr():
+            self._sv.copy_(sent_vecs)
         if not self.use_cuda_graph:
             self.logits, self.pool_attn = self._body()
             return self.logits, self.pool_attn
         if self.graph is None or self._weights_key() != self._key:
             self._capture()  # on the batch just loaded, which the host checks accepted
         self.graph.replay()
-        if self._status is not None:
-            self._status.replayed()
+        self._status.replayed()
         return self.logits, self.pool_attn
 
     def _require_labels(self):
@@ -654,7 +654,7 @@ class _SplitTrainReplay(torch.autograd.Function):
         return None, None, step._g_sv if ctx.needs_input_grad[2] else None
 
 
-class SplitTrainStep(_TrainingGraphs):
+class SplitTrainStep(_TrainingGraphs, _SplitBatches):
     """A training micro-step on a split held on the GPU (qagnn_b200.data.DeviceSplit built with `labels`) as two CUDA graphs:
     the loop body of qagnn.py:252-278 with `--loss cross_entropy` or `--loss margin_rank`, whose only per-call inputs are the
     question ids and sent_vecs:
@@ -693,7 +693,7 @@ class SplitTrainStep(_TrainingGraphs):
     require grad, and in .eval() (build a new SplitTrainStep).  Every call needs exactly `batch_size` questions: run a final
     partial micro-batch eagerly through split.batch + decoder + training.answer_loss.  Padded batches on one GPU only."""
 
-    what = "SplitTrainStep"
+    what, unit = "SplitTrainStep", "micro-batch"
 
     def __init__(self, decoder, split, batch_size, *, edge_capacity, max_edges, autocast_dtype=None, loss="cross_entropy"):
         """`edge_capacity` K bounds the edges of every micro-batch (FlatAdjCache.max_batch_edges(batch_size)), `max_edges` M
@@ -703,31 +703,30 @@ class SplitTrainStep(_TrainingGraphs):
             raise ValueError("SplitTrainStep: the split has no labels; build the DeviceSplit with labels=")
         check_answer_loss(loss, split.num_choice)
         self.loss = loss
-        self.split, self.batch_size = split, int(batch_size)
-        self.edge_capacity, self.max_edges = int(edge_capacity), int(max_edges)
         largest = int(split.counts.max()) if split.counts.size else 0
-        if self.max_edges < largest:
-            raise ValueError(f"SplitTrainStep: max_edges = {self.max_edges}, the split has a sub-graph of {largest} edges")
-        dev = split.device
-        self._qids = torch.zeros(self.batch_size, dtype=torch.int64, device=dev)
-        self._labels = torch.zeros(self.batch_size, dtype=torch.int64, device=dev)
-        self._out = split.buffers(self.batch_size, self.edge_capacity)
-        self._adj = split.packed_adj(self._out, self.max_edges, self.edge_capacity)
-        self._anchor = torch.empty(0, device=dev, requires_grad=True)
+        if int(max_edges) < largest:
+            raise ValueError(f"SplitTrainStep: max_edges = {int(max_edges)}, the split has a sub-graph of {largest} edges")
+        self._init_split(split, batch_size, edge_capacity, max_edges)
+        self._labels = torch.zeros(self.batch_size, dtype=torch.int64, device=split.device)
+        self._anchor = torch.empty(0, device=split.device, requires_grad=True)
         self._sv = None  # sized by the first call
-        self.logits = self.pool_attn = None
-        self.calls = self.captures = 0
+        self.calls = 0
+
+    def _check_sent_vecs(self, sent_vecs):
+        want = (self.batch_size * self.split.num_choice, self.decoder.svec2nvec.in_features)
+        if self._sv is None and (tuple(sent_vecs.shape) != want or not sent_vecs.is_floating_point()):
+            raise ValueError(f"SplitTrainStep: sent_vecs is {tuple(sent_vecs.shape)} {sent_vecs.dtype}, the step needs "
+                             f"floating-point {want}")
+        if self._sv is not None and (sent_vecs.shape != self._sv.shape or sent_vecs.dtype != self._sv.dtype):
+            raise ValueError(f"SplitTrainStep: sent_vecs is {tuple(sent_vecs.shape)} {sent_vecs.dtype}, the step was built "
+                             f"for {tuple(self._sv.shape)} {self._sv.dtype}")
 
     def _forward(self):
-        nc = self.split.num_choice
-        with self._autocast():
-            out = self.split.assemble(self._qids, self.edge_capacity, -1, self._out)
+        with _autocast(self.autocast_dtype):
+            out = self._assemble()
             torch.index_select(self.split.labels, 0, self._qids, out=self._labels)
-            logits, pool_attn = self.decoder(self._sv, out["concept_ids"], out["node_type_ids"], out["node_scores"],
-                                             out["adj_lengths"], self._adj)
-            loss = answer_loss(logits, self._labels, nc, self.loss)
-        if self._status is not None:
-            self._status.record(self.decoder.gnn._last_prep.status_word())
+            logits, pool_attn = self._decode(out)
+            loss = answer_loss(logits, self._labels, self.split.num_choice, self.loss)
         return loss, logits, pool_attn
 
     def _capture(self):
@@ -740,7 +739,7 @@ class SplitTrainStep(_TrainingGraphs):
             torch._foreach_add_([bufs[i] for i in used], [grads[1 + i] for i in used])
             return grads[0]
 
-        self.split.assemble(self._qids, self.edge_capacity, -1, self._out)  # capture_guard validates this batch
+        self._assemble()  # capture_guard validates this batch
         (self._loss, logits, pool_attn), self._d_loss, self._g_sv = self._capture_graphs(
             self._adj, self._out["node_type_ids"], self._forward, backward, owned=bufs)
         self.logits, self.pool_attn = logits.detach(), pool_attn.detach()
@@ -769,19 +768,7 @@ class SplitTrainStep(_TrainingGraphs):
             if [p.requires_grad for p in self.decoder.parameters()] != self._requires_grad:
                 raise RuntimeError("SplitTrainStep: which decoder parameters require grad changed since capture; the "
                                    "backward graph accumulates the old set. Build a new SplitTrainStep.")
-        q = self.split.check(question_ids, self.edge_capacity)[0]
-        if q.size != self.batch_size:
-            raise ValueError(f"SplitTrainStep: {q.size} questions, the step was built for {self.batch_size}; run a partial "
-                             "micro-batch through split.batch + decoder")
-        want = (self.batch_size * self.split.num_choice, self.decoder.svec2nvec.in_features)
-        if self._sv is None and (tuple(sent_vecs.shape) != want or not sent_vecs.is_floating_point()):
-            raise ValueError(f"SplitTrainStep: sent_vecs is {tuple(sent_vecs.shape)} {sent_vecs.dtype}, the step needs "
-                             f"floating-point {want}")
-        if self._sv is not None and (sent_vecs.shape != self._sv.shape or sent_vecs.dtype != self._sv.dtype):
-            raise ValueError(f"SplitTrainStep: sent_vecs is {tuple(sent_vecs.shape)} {sent_vecs.dtype}, the step was built "
-                             f"for {tuple(self._sv.shape)} {self._sv.dtype}")
-        # a pinned block from the caching host allocator per call: it is not reused before this copy has run
-        self._qids.copy_(torch.from_numpy(q).pin_memory(), non_blocking=True)
+        self._load_ids(question_ids, sent_vecs)
         if self._fwd is None:
             self._sv = sent_vecs.detach().clone().requires_grad_(True)
             try:
