@@ -449,7 +449,9 @@ __device__ __forceinline__ float warp_sum(float v) {
   return v;
 }
 
-// dynamic smem: qk[D] | dxs[D] | dqk[D] | a[n] | g[n] | red[kPoolBwdThreads / 32]
+// dynamic smem: qk[D] | dxs[D] | dqk[D] | red[kPoolBwdThreads / 32].  The per-node vectors stay in global memory: a is the
+// forward's attn row, and g is built in place in its scratch row (da_i first, then the logit gradient), so the shared memory
+// does not grow with n and the kernel takes every node count the forward takes.
 template <typename XT>
 __global__ void __launch_bounds__(kPoolBwdThreads) pool_backward_head_kernel(int n, int D, int nh, int S, int64_t N_rows,
                                                                             const XT* __restrict__ X, const int64_t* __restrict__ node_ptr,
@@ -464,10 +466,10 @@ __global__ void __launch_bounds__(kPoolBwdThreads) pool_backward_head_kernel(int
   float* qk = sm;
   float* dxs = qk + D;
   float* dqk = dxs + D;
-  float* a = dqk + D;
-  float* g = a + n;
-  float* red = g + n;
+  float* red = dqk + D;
   PoolBwdScratch sc(scratch, B, n, D, nh);
+  const float* a = attn + ((size_t)h * B + b) * n;
+  float* g = sc.g + ((size_t)h * B + b) * n;
   int64_t row0;
   int nr;
   ragged_graph_rows(b, n, node_ptr, adj_lengths, N_rows, row0, nr);
@@ -476,7 +478,6 @@ __global__ void __launch_bounds__(kPoolBwdThreads) pool_backward_head_kernel(int
   const float* qsh = qs + (size_t)b * D + h * dk;
   const float* dph = dconcat + (size_t)b * (2 * D + S) + h * dk;  // dpooled_h
   const size_t vo = ((size_t)b * nh + h) * D;
-  for (int i = tid; i < nr; i += kPoolBwdThreads) a[i] = attn[((size_t)h * B + b) * n + i];
   for (int j = tid; j < D; j += kPoolBwdThreads) {
     float q = 0.f, d = 0.f;
     for (int r = 0; r < dk; ++r) {
@@ -512,9 +513,7 @@ __global__ void __launch_bounds__(kPoolBwdThreads) pool_backward_head_kernel(int
   __syncthreads();
   const float sdot = red[0];
   for (int i = tid; i < n; i += kPoolBwdThreads) {
-    const float gi = i < nr ? a[i] * (g[i] - sdot) * inv_temp : 0.f;
-    if (i < nr) g[i] = gi;
-    sc.g[((size_t)h * B + b) * n + i] = gi;
+    g[i] = i < nr ? a[i] * (g[i] - sdot) * inv_temp : 0.f;
   }
   __syncthreads();
   for (int j = tid; j < D; j += kPoolBwdThreads) {
@@ -598,8 +597,20 @@ __global__ void __launch_bounds__(kPoolBwdThreads) pool_backward_weights_kernel(
   }
 }
 
-inline size_t pool_backward_smem_bytes(int n, int D) {
-  return ((size_t)3 * D + 2 * (size_t)n + kPoolBwdThreads / 32) * sizeof(float);
+// (3D + 8) floats: always less than pool_smem_bytes(n, D, nh) (10 nh D + nh n + nh + 16 floats), so the backward takes
+// every shape the forward takes.  Above 48 KB (D > 4093) it opts in, once per device and X type, to the forward's cap.
+inline size_t pool_backward_smem_bytes(int D) { return ((size_t)3 * D + kPoolBwdThreads / 32) * sizeof(float); }
+
+template <typename XT>
+int32_t prepare_pool_backward_launch(size_t smem) {
+  static bool attr_set[kMaxDevices] = {false};
+  const int dev = current_device();
+  if (smem > 48 * 1024 && !attr_set[dev]) {
+    QAGNN_CHECK_CUDA(cudaFuncSetAttribute(pool_backward_head_kernel<XT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                          (int)kPoolSmemCap));
+    attr_set[dev] = true;
+  }
+  return QAGNN_OK;
 }
 
 template <typename XT>
@@ -614,8 +625,9 @@ int32_t pool_backward_ragged(int32_t B, int32_t n, int32_t D, int32_t n_head, in
       !dbv || !scratch)
     return QAGNN_ERR_INVALID_ARGUMENT;
   if (scratch_bytes < PoolBwdScratch::floats(B, n, D, n_head) * sizeof(float)) return QAGNN_ERR_WORKSPACE;
-  const size_t smem = pool_backward_smem_bytes(n, D);
-  if (smem > 48 * 1024) return QAGNN_ERR_UNSUPPORTED;
+  if (pool_smem_bytes(n, D, n_head) > kPoolSmemCap) return QAGNN_ERR_UNSUPPORTED;  // the forward refuses these too
+  const size_t smem = pool_backward_smem_bytes(D);
+  QAGNN_RETURN_IF(prepare_pool_backward_launch<XT>(smem));
   QAGNN_CHECK_CUDA(cudaMemsetAsync(dX, 0, (size_t)N_rows * D * sizeof(float), st));
   pool_backward_head_kernel<XT><<<dim3(B, n_head), kPoolBwdThreads, smem, st>>>(n, D, n_head, S, N_rows, X, node_ptr, adj_lengths,
                                                                                 qs, wk, bk, wv, attn, dconcat, dqs, scratch);
