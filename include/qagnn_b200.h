@@ -431,6 +431,20 @@ int32_t qagnn_adamw_step(int32_t n_tensors, void *const *params, void *const *gr
                          void *const *step_tables, int64_t table_len, const float *found_inf, const float *grad_scale,
                          int32_t *counter, void *stream);
 
+/* fp64 slots qagnn_clip_grad_norm needs for n_tensors tensors of numels[i] elements (one per 8192-element chunk); -1 for a
+ * negative count or size. */
+int64_t qagnn_clip_grad_norm_slots(int32_t n_tensors, const int64_t *numels);
+
+/* torch.nn.utils.clip_grad_norm_(grads, max_norm) over n_tensors contiguous fp32 gradients grads[i] of numels[i] elements on
+ * the current device (qagnn_b200.optim.clip_grad_norm_): a norm launch and a scale launch per 512 tensors.  The L2 norm is
+ * summed in fp64, each square exact, in an order fixed by the tensors' sizes and their order alone (csrc/clip.cu), and rounded
+ * once to fp32 into *total_norm.  *coef = clamp((float)max_norm * (1 / (*total_norm + (float)1e-6)), max=1) in fp32, NaN kept,
+ * and every gradient is multiplied by it in place, unless it is 1.  slots: n_slots >= qagnn_clip_grad_norm_slots(...) device
+ * doubles; counter: a device int32 that is zero between calls (the kernel resets it); total_norm, coef: device fp32.  No host
+ * synchronisation and no floating-point atomics.  QAGNN_ERR_WORKSPACE when n_slots is too small. */
+int32_t qagnn_clip_grad_norm(int32_t n_tensors, void *const *grads, const int64_t *numels, double max_norm, double *slots,
+                             int64_t n_slots, int32_t *counter, float *total_norm, float *coef, void *stream);
+
 /* Launch counters since load (kernels this library enqueued); for bench.py's gpu_launches. */
 int64_t qagnn_launch_count(void);
 

@@ -24,20 +24,18 @@
 //   computes) before its rounding.
 // The host-double scalars (1 - b2, -wd*lr, eps, ...) are rounded to fp32 as torch rounds them.
 //
-// Work split: each tensor is cut into chunks of kChunk elements and a grid-stride loop hands chunks to CTAs; a CTA finds its
-// chunk's tensor by binary search over the per-tensor chunk prefix held in the kernel parameters.  Every CTA reads the step
-// counters, so they are advanced only by the last CTA to finish (a grid-wide arrival counter that the last CTA resets).  A
-// nonzero found_inf leaves p, m, v and every step as they are.
-#include "common.cuh"
+// Work split: multi_tensor.cuh's chunks, launches and arrival counter.  Every CTA reads the step counters, so they are
+// advanced only by the last CTA to finish.  A nonzero found_inf leaves p, m, v and every step as they are.
+#include "multi_tensor.cuh"
 
 namespace qagnn {
 
 namespace {
 
-constexpr int kThreads = 256;
-constexpr int64_t kChunk = 8192;    // elements per chunk: 8 float4 per thread
-constexpr int kMaxTensors = 512;    // per launch: the parameter block below stays under sm_90's 32764 bytes
-constexpr int kMaxGroups = 16;      // distinct param groups per launch
+using mt::kChunk;
+using mt::kMaxTensors;
+using mt::kThreads;
+constexpr int kMaxGroups = 16;  // distinct param groups per launch
 
 enum class Rule { kRAdam, kAdamW };
 enum : int32_t { kKindNone = 0, kKindSgd = 1, kKindRect = 2 };
@@ -117,12 +115,7 @@ __device__ __forceinline__ void step_body(const StepArgs& a) {
   k.inv = k.unscale ? __double2float_rn(__drcp_rn((double)*a.grad_scale)) : 1.f;
   const int32_t total = a.chunk_end[a.n - 1];
   for (int32_t c = blockIdx.x; c < total; c += gridDim.x) {
-    int lo = 0, hi = a.n - 1;  // the first tensor whose chunk_end exceeds c
-    while (lo < hi) {
-      const int mid = (lo + hi) >> 1;
-      if (a.chunk_end[mid] > c) hi = mid; else lo = mid + 1;
-    }
-    const int i = lo;
+    const int i = mt::chunk_owner(a.chunk_end, a.n, c);
     const int64_t c0 = (int64_t)(c - (i ? a.chunk_end[i - 1] : 0)) * kChunk;
     const int64_t n = min(kChunk, a.numel[i] - c0);
     const StepGroup& gr = a.groups[a.group[i]];
@@ -170,15 +163,7 @@ __device__ __forceinline__ void step_body(const StepArgs& a) {
     for (int64_t j = done + threadIdx.x; j < n; j += kThreads) step_scalar<R>(p, g, m, v, j, k);
   }
   // the last CTA to arrive advances the step counters: every CTA has read them by then
-  __shared__ bool last;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    __threadfence();
-    last = atomicAdd(a.counter, 1) == (int32_t)gridDim.x - 1;
-  }
-  __syncthreads();
-  if (!last) return;
-  __threadfence();
+  if (!mt::last_to_arrive(a.counter)) return;
   if (!k.skip)
     for (int i = threadIdx.x; i < a.n; i += kThreads) *a.step[i] += 1;
   if (threadIdx.x == 0) *a.counter = 0;
@@ -203,8 +188,7 @@ void fill_group(StepGroup& gr, double lr, double wd, double b1, double b2, doubl
 
 template <Rule R>
 int32_t launch(const StepArgs& a, cudaStream_t st) {
-  const int64_t chunks = a.chunk_end[a.n - 1];
-  const unsigned blocks = (unsigned)max(min(chunks, (int64_t)kNumSMs * 8), (int64_t)1);
+  const unsigned blocks = mt::launch_blocks(a.chunk_end[a.n - 1]);
   if constexpr (R == Rule::kRAdam)
     radam_kernel<<<blocks, kThreads, 0, st>>>(a);
   else
@@ -228,8 +212,8 @@ int32_t step_all(int32_t n_tensors, void* const* params, void* const* grads, voi
     return QAGNN_ERR_INVALID_ARGUMENT;
   for (int32_t i = 0; i < n_tensors; ++i) {
     const int32_t gi = group_index[i];
-    if (gi < 0 || gi >= n_groups || !steps[i] || numels[i] < 0 ||
-        (numels[i] + kChunk - 1) / kChunk > INT32_MAX) return QAGNN_ERR_INVALID_ARGUMENT;
+    if (gi < 0 || gi >= n_groups || !steps[i] || numels[i] < 0 || mt::chunk_count(numels[i]) > INT32_MAX)
+      return QAGNN_ERR_INVALID_ARGUMENT;
     if (numels[i] > 0 && (!params[i] || !grads[i] || !exp_avgs[i] || !exp_avg_sqs[i])) return QAGNN_ERR_INVALID_ARGUMENT;
     if (!step_tables[gi] || !(beta1[gi] >= 0.0 && beta1[gi] < 1.0) || !(beta2[gi] >= 0.0 && beta2[gi] < 1.0))
       return QAGNN_ERR_INVALID_ARGUMENT;
@@ -246,12 +230,12 @@ int32_t step_all(int32_t n_tensors, void* const* params, void* const* grads, voi
   int64_t chunks = 0;
   for (int32_t i = 0; i < n_tensors; ++i) {
     const int32_t gi = group_index[i];
-    const int64_t nc = (numels[i] + kChunk - 1) / kChunk;
+    const int64_t nc = mt::chunk_count(numels[i]);
     int32_t slot = -1;
     for (int32_t s = 0; s < n_slots; ++s)
       if (slot_of[s] == gi) slot = s;
     // a full launch (tensors, groups or the int32 chunk prefix) goes out first
-    if (a.n == kMaxTensors || (slot < 0 && n_slots == kMaxGroups) || chunks + nc > INT32_MAX) {
+    if (mt::launch_full(a.n, chunks, nc) || (slot < 0 && n_slots == kMaxGroups)) {
       QAGNN_RETURN_IF(launch<R>(a, st));
       a.n = 0;
       n_slots = 0;

@@ -13,7 +13,9 @@ doubles with the original's formula, into a device fp64 table per (device, beta1
 device step.  The host counts its own `step()` calls, which bounds every device step, and grows the table ahead of that count.
 
 `OPTIMIZER_CLASSES` is the reference's `--optim` table, so `from qagnn_b200.optim import OPTIMIZER_CLASSES` replaces the
-reference's import, whose module no longer loads with current `transformers`.
+reference's import, whose module no longer loads with current `transformers`.  `clip_grad_norm_` is the recipe's
+`torch.nn.utils.clip_grad_norm_` in two launches per device (csrc/clip.cu) instead of torch's three foreach passes, so
+the optimiser tail `scaler.unscale_; clip_grad_norm_; scaler.step; scaler.update` never reads the GPU.
 """
 import ctypes as C
 import math
@@ -257,6 +259,65 @@ class AdamW(_DeviceStepOptimizer):
 
     def _rule_flags(self):
         return [int(bool(g["correct_bias"])) for g in self.param_groups]
+
+
+_clip_workspace = {}  # device -> [fp64 slots, int32 arrival counter, fp32 clip coefficient]
+
+
+def _clip_buffers(device, n_slots):
+    ws = _clip_workspace.get(device)
+    if ws is None:
+        ws = _clip_workspace[device] = [torch.empty(0, dtype=torch.float64, device=device),
+                                        torch.zeros(1, dtype=torch.int32, device=device),
+                                        torch.empty(1, dtype=torch.float32, device=device)]
+    if ws[0].numel() < n_slots:
+        ws[0] = torch.empty(max(n_slots, 2 * ws[0].numel()), dtype=torch.float64, device=device)
+    return ws
+
+
+@torch.no_grad()
+def clip_grad_norm_(parameters, max_norm, norm_type=2.0, error_if_nonfinite=False, foreach=None):
+    """torch.nn.utils.clip_grad_norm_ as the reference calls it, in two sm_90a launches on one device (csrc/clip.cu): the
+    L2 norm of every `.grad` (parameters without one are skipped) and `.grad *= min(max_norm / (norm + 1e-6), 1)` in place.
+    Returns the norm as a new 0-dim fp32 tensor on the gradients' device without reading it on the host, or
+    `torch.tensor(0.0)` when no parameter has a gradient.
+
+    The norm is summed in fp64 in an order fixed by the gradients' sizes alone, so it is reproducible bit for bit and within
+    one fp32 ulp of the exact norm; torch's fp32 sum is neither, and its squares overflow (an inf norm) for gradients past
+    about 1.8e19, where this one stays finite.  From the norm on, the coefficient and every gradient are torch's fp32
+    operations bit for bit, and a coefficient of 1 leaves the gradients untouched without rewriting them.  An inf norm gives
+    a coefficient of 0 and a NaN norm a NaN one, as in torch.  Gradients must be dense, contiguous fp32 CUDA tensors on one
+    device.  `norm_type` must be 2 and `error_if_nonfinite` False, which would need a host read; `foreach` is accepted and
+    ignored.  One fp64 slot per 8192 gradient elements is kept per device between calls."""
+    name = "clip_grad_norm_"
+    if float(norm_type) != 2.0:
+        raise ValueError(f"qagnn_b200.optim.{name}: only the L2 norm (norm_type=2) is implemented (got {norm_type})")
+    if error_if_nonfinite:
+        raise ValueError(f"qagnn_b200.optim.{name}: error_if_nonfinite=True needs a host read of the norm; it is not "
+                         f"supported")
+    if isinstance(parameters, torch.Tensor):
+        parameters = [parameters]
+    grads = [p.grad for p in parameters if p.grad is not None]
+    if not grads:
+        return torch.tensor(0.0)
+    for g in grads:
+        if g.layout != torch.strided:
+            raise TypeError(f"qagnn_b200.optim.{name}: the gradient must be dense (got {g.layout})")
+        _check_tensor(g, "gradient", name)
+    device = grads[0].device
+    if any(g.device != device for g in grads):
+        raise ValueError(f"qagnn_b200.optim.{name}: gradients on {sorted({str(g.device) for g in grads})}; all must be on "
+                         f"one device")
+    lib = _lib.load()
+    n = len(grads)
+    numels = (C.c_int64 * n)(*[g.numel() for g in grads])
+    slots, counter, coef = _clip_buffers(device, lib.qagnn_clip_grad_norm_slots(n, numels))
+    total_norm = torch.empty((), dtype=torch.float32, device=device)
+    with torch.cuda.device(device):
+        _lib.check(lib.qagnn_clip_grad_norm(n, (C.c_void_p * n)(*[g.data_ptr() for g in grads]), numels, float(max_norm),
+                                            _lib.ptr(slots), slots.numel(), _lib.ptr(counter), _lib.ptr(total_norm),
+                                            _lib.ptr(coef), _lib.stream_ptr(device)), "qagnn_clip_grad_norm")
+    return total_norm
 
 
 # The reference's --optim table (utils/optimization_utils.py).  'sgd' and 'adam' are torch's own classes, as the reference

@@ -19,10 +19,17 @@ Cases:
               the decoder: kernel ms from CUDA events and, for qagnn, the fraction of 3.35 TB/s at 28 bytes per parameter
   3. batch    one optimiser batch of 64 questions at -mbs 2 under fp16 autocast through SplitTrainStep (32 micro-steps) and
               the tail of case 1 with each optimiser
+  4. clip     the gradient clip alone, torch.nn.utils.clip_grad_norm_(foreach=True) against qagnn_b200.optim.clip_grad_norm_,
+              over the decoder's tensors and over case 2's set, at a max_norm that clips (half the norm) and at one that does
+              not (twice it), each call on the same gradients: wall and host ms, launches and synchronisations, and the
+              kernels' summed device time with its share of 3.35 TB/s at the bytes each route moves per parameter (torch
+              12: a read for the norm, a read and a write for the multiply; qagnn 12 when it clips, 4 when it does not)
+  5. clip_tail  case 1 with qagnn_b200.optim.RAdam under torch's clip (qagnn) and under qagnn_b200's (qagnn_clip)
 Medians with the spread (min, max) over --reps alternated repetitions.  Everything it writes goes to --out.
 
     python tools/bench_optim.py --out profiles/h100_optim.jsonl
     python tools/bench_optim.py --optim adamw --cases tail encoder --out profiles/h100_optim_adamw.jsonl
+    python tools/bench_optim.py --cases clip clip_tail --out profiles/h100_clip.jsonl
 """
 import argparse
 import json
@@ -51,6 +58,7 @@ HBM_TBS = 3.35  # H100 SXM data-sheet HBM3 bandwidth
 
 def make_opt(optim, route, groups):
     from qagnn_b200.optim import AdamW, RAdam
+    route = "qagnn" if route == "qagnn_clip" else route
     if optim == "adamw":
         if route == "oracle":
             return AdamWOracle(groups)
@@ -102,8 +110,13 @@ def profile_counts(fn):
     return launches, syncs
 
 
-def case_tail(dec, dev, reps, optim):
-    routes = ROUTES[optim]
+def clip_of(route):
+    from qagnn_b200.optim import clip_grad_norm_
+    return clip_grad_norm_ if route == "qagnn_clip" else torch.nn.utils.clip_grad_norm_
+
+
+def case_tail(dec, dev, reps, optim, routes=None, case="tail"):
+    routes = routes or ROUTES[optim]
     named = [(n, p) for n, p in dec.named_parameters() if p.requires_grad]
     g = torch.Generator(device=dev).manual_seed(0)
     grads = [torch.randn(p.shape, device=dev, generator=g) * 1e-3 for _, p in named]
@@ -120,7 +133,7 @@ def case_tail(dec, dev, reps, optim):
     def tail(route):
         ps, opt, sc = runs[route]
         sc.unscale_(opt)
-        torch.nn.utils.clip_grad_norm_(ps, 1.0)
+        clip_of(route)(ps, 1.0)
         sc.step(opt)
         sc.update()
 
@@ -144,7 +157,7 @@ def case_tail(dec, dev, reps, optim):
     for route in routes:
         load(route)
         launches, syncs = profile_counts(lambda: tail(route))
-        out.append({"case": "tail", "route": route, "tensors": len(named), "params": sum(p.numel() for _, p in named),
+        out.append({"case": case, "route": route, "tensors": len(named), "params": sum(p.numel() for _, p in named),
                     "wall_ms": stats(wall[route]), "host_ms": stats(host[route]), "launches": launches, "syncs": syncs})
     return out
 
@@ -193,6 +206,77 @@ def case_encoder(dec, dev, reps, optim):
         out.append(line)
     del opts
     torch.cuda.empty_cache()
+    return out
+
+
+def kernel_ms(fn):
+    """Summed duration of the device kernels fn enqueues, from a torch.profiler pass of its own."""
+    from torch.profiler import ProfilerActivity, profile
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        fn()
+        torch.cuda.synchronize()
+    return sum(e.time_range.elapsed_us() for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA) * 1e-3
+
+
+def case_clip(dec, dev, reps):
+    from qagnn_b200.optim import clip_grad_norm_
+    clips = {"torch": lambda ps, m: torch.nn.utils.clip_grad_norm_(ps, m, foreach=True), "qagnn": clip_grad_norm_}
+    named_dec = [p.detach() for p in dec.parameters() if p.requires_grad]
+    torch.manual_seed(0)
+    sets = {"decoder": named_dec,
+            "encoder": [torch.randn(s, device=dev) * 0.02 for _, s in roberta_large_shapes()] + named_dec}
+    out = []
+    for name, base in sets.items():
+        grads = [torch.randn_like(p) * 1e-3 for p in base]
+        n_params = sum(g.numel() for g in grads)
+        norm = float(torch.linalg.vector_norm(torch.stack([torch.linalg.vector_norm(g) for g in grads])))
+        params = {}
+        for route in clips:
+            ps = [torch.nn.Parameter(torch.empty_like(g)) for g in grads]
+            for p, g in zip(ps, grads):
+                p.grad = g.clone()
+            params[route] = ps
+
+        def reload(route):
+            for p, g in zip(params[route], grads):
+                p.grad.copy_(g)
+
+        for clipping, max_norm in (("clips", 0.5 * norm), ("no_clip", 2.0 * norm)):
+            def call(route):
+                clips[route](params[route], max_norm)
+
+            for route in clips:
+                for _ in range(3):
+                    reload(route)
+                    call(route)
+            wall, host, kern = ({r: [] for r in clips} for _ in range(3))
+            for _ in range(reps):
+                for route in clips:
+                    reload(route)
+                    torch.cuda.synchronize()
+                    t0 = time.perf_counter()
+                    call(route)
+                    t1 = time.perf_counter()
+                    torch.cuda.synchronize()
+                    t2 = time.perf_counter()
+                    wall[route].append((t2 - t0) * 1e3)
+                    host[route].append((t1 - t0) * 1e3)
+            for _ in range(5):
+                for route in clips:
+                    reload(route)
+                    kern[route].append(kernel_ms(lambda: call(route)))
+            for route in clips:
+                reload(route)
+                launches, syncs = profile_counts(lambda: call(route))
+                k = stats(kern[route])
+                nbytes = 4 if route == "qagnn" and clipping == "no_clip" else 12
+                out.append({"case": "clip", "set": name, "route": route, "max_norm": clipping, "tensors": len(grads),
+                            "params": n_params, "wall_ms": stats(wall[route]), "host_ms": stats(host[route]),
+                            "launches": launches, "syncs": syncs, "kernel_ms": k, "bytes_per_param": nbytes,
+                            "hbm_fraction": nbytes * n_params / (k["median"] * 1e-3) / (HBM_TBS * 1e12)})
+        del params, grads, base
+        torch.cuda.empty_cache()
     return out
 
 
@@ -262,6 +346,10 @@ def main():
         lines += case_encoder(dec, dev, max(5, args.reps // 3), args.optim)
     if "batch" in args.cases:
         lines += case_batch(dev, max(3, args.reps // 6), args.seed, args.optim)
+    if "clip" in args.cases:
+        lines += case_clip(dec, dev, args.reps)
+    if "clip_tail" in args.cases:
+        lines += case_tail(dec, dev, args.reps, "radam", routes=("qagnn", "qagnn_clip"), case="clip_tail")
     for line in lines:
         line["gpu"] = gpu
         line["optim"] = args.optim
