@@ -445,6 +445,16 @@ int64_t qagnn_clip_grad_norm_slots(int32_t n_tensors, const int64_t *numels);
 int32_t qagnn_clip_grad_norm(int32_t n_tensors, void *const *grads, const int64_t *numels, double max_norm, double *slots,
                              int64_t n_slots, int32_t *counter, float *total_norm, float *coef, void *stream);
 
+/* The ordered sum of one optimiser batch's per-micro-batch gradients into .grad, for data-parallel training
+ * (qagnn_b200.distributed.ordered_grad_sum_): n_tensors contiguous fp32 tensors grads[i] of numels[i] elements on the current
+ * device, and device fp32 slots, row j (j < n_valid, n_valid >= 1) at slots + j * ld holding micro-batch j's gradient of tensor
+ * i at columns [cols[i], cols[i] + numels[i]) <= ld.  Per element: g = init_from_grad[i] ? g + slot 0 : slot 0, then
+ * g = g + slot j for j = 1 ... n_valid - 1, in that order, each one fp32 add rounded to nearest: the adds of one GPU
+ * accumulating the micro-batches into .grad one after another.  One launch per 512 non-empty tensors, none when every tensor
+ * is empty; no host synchronisation and no atomics. */
+int32_t qagnn_ordered_grad_sum(int32_t n_tensors, void *const *grads, const int64_t *numels, const int64_t *cols,
+                               const int32_t *init_from_grad, const float *slots, int64_t ld, int32_t n_valid, void *stream);
+
 /* Launch counters since load (kernels this library enqueued); for bench.py's gpu_launches. */
 int64_t qagnn_launch_count(void);
 
