@@ -21,9 +21,13 @@ question ids and runs QAGNN.forward in .eval() on it, so nothing of the batch is
 
 `SplitTrainStep` trains from such a split: its forward graph assembles the micro-batch, gathers its labels and takes the
 cross-entropy or margin-rank loss; its backward graph adds the parameter gradients into `.grad` itself.
+
+`SplitTrainBatch` runs several such micro-steps of an optimiser batch at once on one GPU, each on a stream of its own, and sums
+their gradients in micro-batch order.
 """
 import contextlib
 
+import numpy as np
 import torch
 
 from . import distributed as _dist
@@ -249,12 +253,13 @@ class _TrainingGraphs:
     def _addresses(self):
         return tuple(t.data_ptr() for t in self._params + self._buffers)
 
-    def _capture_graphs(self, adj, node_type, forward, backward, owned=()):
+    def _capture_graphs(self, adj, node_type, forward, backward, owned=(), stream=None):
         """Captures `forward()` -> (y, ...) and `backward(y, dy)` as two CUDA graphs in one pool, on the batch (adj,
         node_type) already in the static buffers.  capture_guard first validates that batch and runs forward + backward twice
         (dy = 1) on a side stream; the forward graph ends by recording graph prep's status word into self._status.  The
         warm-up really runs: the decoder's buffers, the .grad of its trainable parameters (self._params), the tensors `owned`
-        and the CUDA RNG state are put back afterwards.  Returns (forward's outputs, the static dy buffer, backward's result)."""
+        and the CUDA RNG state are put back afterwards.  Both graphs are captured on `stream` (None: torch.cuda.graph's own
+        side stream).  Returns (forward's outputs, the static dy buffer, backward's result)."""
         dec = self.decoder
         dev = node_type.device
         self._params = [p for p in dec.parameters() if p.requires_grad]
@@ -271,11 +276,11 @@ class _TrainingGraphs:
             with capture_guard(dec.gnn, adj, node_type, self.what, warmup) as status:
                 pool = torch.cuda.graph_pool_handle()
                 fwd, bwd = torch.cuda.CUDAGraph(), torch.cuda.CUDAGraph()
-                with torch.cuda.graph(fwd, pool=pool):
+                with torch.cuda.graph(fwd, pool=pool, stream=stream):
                     out = forward()
                     status.record(dec.gnn._last_prep.status_word())
                 dy = torch.empty_like(out[0])
-                with torch.cuda.graph(bwd, pool=pool):
+                with torch.cuda.graph(bwd, pool=pool, stream=stream):
                     res = backward(out[0], dy)
             self._fwd, self._bwd, self._status = fwd, bwd, status
             self._bn_buffers = [b for m in dec.modules() if isinstance(m, torch.nn.modules.batchnorm._BatchNorm)
@@ -294,6 +299,12 @@ class _TrainingGraphs:
     def _check_replay(self):
         """Before a replay: RuntimeError when the graphs no longer fit the decoder, IndexError when an earlier replay's graph
         prep flagged its batch."""
+        self._check_fit()
+        self._status.check(self.what)
+
+    def _check_fit(self):
+        """RuntimeError when graphs captured on the decoder no longer fit it: eval mode, moved parameters or buffers, or
+        another deterministic flag."""
         what = self.what
         if not self.decoder.training:
             raise RuntimeError(f"{what} replays the training forward: call decoder.train() first")
@@ -303,7 +314,6 @@ class _TrainingGraphs:
         if torch.are_deterministic_algorithms_enabled() != self.deterministic:
             raise RuntimeError(f"{what} was captured with torch.use_deterministic_algorithms({self.deterministic}) and "
                                f"its backward graph holds that mode's kernels; the flag changed since. Build a new {what}.")
-        self._status.check(what)
 
     def _replayed(self):
         self._status.replayed()
@@ -715,10 +725,10 @@ class SplitTrainStep(_TrainingGraphs, _SplitBatches):
     def _check_sent_vecs(self, sent_vecs):
         want = (self.batch_size * self.split.num_choice, self.decoder.svec2nvec.in_features)
         if self._sv is None and (tuple(sent_vecs.shape) != want or not sent_vecs.is_floating_point()):
-            raise ValueError(f"SplitTrainStep: sent_vecs is {tuple(sent_vecs.shape)} {sent_vecs.dtype}, the step needs "
+            raise ValueError(f"{self.what}: sent_vecs is {tuple(sent_vecs.shape)} {sent_vecs.dtype}, the step needs "
                              f"floating-point {want}")
         if self._sv is not None and (sent_vecs.shape != self._sv.shape or sent_vecs.dtype != self._sv.dtype):
-            raise ValueError(f"SplitTrainStep: sent_vecs is {tuple(sent_vecs.shape)} {sent_vecs.dtype}, the step was built "
+            raise ValueError(f"{self.what}: sent_vecs is {tuple(sent_vecs.shape)} {sent_vecs.dtype}, the step was built "
                              f"for {tuple(self._sv.shape)} {self._sv.dtype}")
 
     def _forward(self):
@@ -731,21 +741,27 @@ class SplitTrainStep(_TrainingGraphs, _SplitBatches):
 
     def _capture(self):
         bufs = [torch.zeros_like(p) for p in self.decoder.parameters() if p.requires_grad]
+        used = self._capture_split(lambda used, grads: torch._foreach_add_([bufs[i] for i in used], grads), owned=bufs)
+        self._owned = [(self._params[i], bufs[i]) for i in used]
+
+    def _capture_split(self, sink, owned=(), forward=None, stream=None):
+        """Captures the forward graph (`forward`, default self._forward) and the backward graph, which ends by handing the
+        parameter gradients the loss reaches to `sink(used, grads)`, `used` their indices into self._params.  Returns `used`."""
         used = []
 
         def backward(loss, d_loss):
             grads = torch.autograd.grad(loss, [self._sv] + self._params, d_loss, allow_unused=True)
             used[:] = [i for i, g in enumerate(grads[1:]) if g is not None]
-            torch._foreach_add_([bufs[i] for i in used], [grads[1 + i] for i in used])
+            sink(used, [grads[1 + i] for i in used])
             return grads[0]
 
         self._assemble()  # capture_guard validates this batch
         (self._loss, logits, pool_attn), self._d_loss, self._g_sv = self._capture_graphs(
-            self._adj, self._out["node_type_ids"], self._forward, backward, owned=bufs)
+            self._adj, self._out["node_type_ids"], forward or self._forward, backward, owned=owned, stream=stream)
         self.logits, self.pool_attn = logits.detach(), pool_attn.detach()
-        self._owned = [(self._params[i], bufs[i]) for i in used]
         self._requires_grad = [p.requires_grad for p in self.decoder.parameters()]
         self.captures += 1
+        return used
 
     def _own_grads(self):
         """Makes every accumulated parameter's .grad the step's buffer, holding what .grad held (None counts as zeros)."""
@@ -780,6 +796,324 @@ class SplitTrainStep(_TrainingGraphs, _SplitBatches):
         loss = _SplitTrainReplay.apply(self, self._anchor, sent_vecs)
         self._replayed()
         return loss
+
+
+def _cuda_generator(device):
+    """torch's default CUDA generator of `device`."""
+    index = device.index if device.index is not None else torch.cuda.current_device()
+    return torch.cuda.default_generators[index]
+
+
+def train_chunks(batch, micro_batch_size, branches):
+    """The full micro-batches of `micro_batch_size` questions of the optimiser batch `batch` (host question ids), in order, in
+    lists of at most `branches`.  A final partial micro-batch, batch[len(batch) // micro_batch_size * micro_batch_size:], is
+    not among them."""
+    batch = np.asarray(batch)
+    mbs, S = int(micro_batch_size), int(branches)
+    full = [batch[a:a + mbs] for a in range(0, len(batch) // mbs * mbs, mbs)]
+    return [full[a:a + S] for a in range(0, len(full), S)]
+
+
+class _TrainBranch(SplitTrainStep):
+    """One micro-step of a SplitTrainBatch: a SplitTrainStep's forward and backward graphs in a pool of their own, captured
+    on the branch's stream with the branch's CUDA generator state, with the decoder's BatchNorm buffers pointing at the
+    branch's copies (which the forward graph first loads from the live buffers), and a backward graph that writes the
+    parameter gradients into the branch's row of the batch's slot buffer.  Its ids are the branch's row of the batch's."""
+
+    what = "SplitTrainBatch"
+
+    def __init__(self, tb, index):
+        super().__init__(tb.decoder, tb.split, tb.batch_size, edge_capacity=tb.edge_capacity, max_edges=tb.max_edges,
+                         autocast_dtype=tb.autocast_dtype, loss=tb.loss)
+        # no reference back to `tb`: a cycle would leave its graphs to the garbage collector, which may then destroy
+        # them while another capture is in progress and invalidate it
+        self.index = index
+        self._qids = tb._qids[index]  # filled by the batch's one upload of a chunk's ids
+
+    def capture(self, tb, sent_vecs, stream, rng):
+        b = self.index
+        self._sv = sent_vecs.detach().clone().requires_grad_(True)
+        self.stream = stream
+
+        def forward():
+            with torch.no_grad():  # the chunk's BatchNorm state, read before any branch updates its copies
+                if tb._bns:
+                    torch.cat(tb._bn_live, out=tb._bn_rows[b])
+                    torch.stack(tb._nbt_live, out=tb._nbt_rows[b])
+            return self._forward()
+
+        gen = _cuda_generator(tb.split.device)
+        live_rng = gen.graphsafe_get_state()
+        gen.graphsafe_set_state(rng)
+        try:
+            with tb._branch_buffers(b):
+                self.used = self._capture_split(lambda used, grads: torch._foreach_copy_(tb._row_views(b, used), grads),
+                                                forward=forward, stream=stream)
+        finally:
+            gen.graphsafe_set_state(live_rng)
+        self._keep = (self.decoder.gnn._last_prep,)  # graph prep's buffers, which both graphs baked in
+
+
+class _SplitTrainBatchReplay(torch.autograd.Function):
+    """The captured forward and backward graphs of a chunk's branches as one autograd node.  Its inputs are a zero-element
+    anchor that always requires grad, so the node exists when no sent_vecs requires grad (a frozen encoder), and the chunk's
+    sent_vecs.  The parameters are not inputs: the backward sums the branches' gradient slots into `.grad` itself."""
+
+    @staticmethod
+    def forward(ctx, tb, anchor, *sent_vecs):
+        branches = tb._branches[:len(sent_vecs)]
+        for br, sv in zip(branches, sent_vecs):
+            if br._sv.data_ptr() != sv.data_ptr():
+                br._sv.copy_(sv)
+        tb._replay(branches, "_fwd")
+        ctx.tb, ctx.n, ctx.call = tb, len(branches), tb.calls
+        return torch.stack([br._loss for br in branches])
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, d_losses):
+        tb = ctx.tb
+        if ctx.call != tb.calls:
+            raise RuntimeError("SplitTrainBatch: backward through the losses of an earlier call; the next call's forward "
+                               "replays have overwritten their activations. Run each call's backward before the next call.")
+        branches = tb._branches[:ctx.n]
+        torch._foreach_copy_([br._d_loss for br in branches], list(d_losses.unbind(0)))
+        tb._replay(branches, "_bwd")
+        tb._sum_slots(ctx.n)
+        return (None, None) + tuple(br._g_sv if need else None for br, need in zip(branches, ctx.needs_input_grad[2:]))
+
+
+class SplitTrainBatch(_TrainingGraphs):
+    """The micro-steps of an optimiser batch on a split held on the GPU (qagnn_b200.data.DeviceSplit built with `labels`), up
+    to `branches` of them at a time on one GPU, equal to the plain SplitTrainStep loop:
+
+        tb = SplitTrainBatch(model.decoder.train(), split, mbs, branches=8, edge_capacity=K, max_edges=M,
+                             autocast_dtype=torch.float16, loss=args.loss)
+        optimizer.zero_grad()
+        for chunk in tb.chunks(batch):                     # lists of <= branches full micro-batches (host ids), in order
+            svs = [model.encoder(*lm_inputs_of(q))[0] for q in chunk]
+            losses = tb(chunk, svs)                        # [len(chunk)] fp32: each micro-batch's mean loss
+            scaler.scale((losses * weights).sum()).backward()     # weights[j] = len(chunk[j]) / len(batch)
+        # a final partial micro-batch runs eagerly, as with SplitTrainStep
+
+    A branch is one micro-step: a SplitTrainStep's two graphs (assembly, label gather, `decoder(...)` in .train() and
+    training.answer_loss; torch.autograd.grad), with its own static buffers, graph pool and stream.  Every branch is
+    captured on its own stream and replayed on it, so each bakes in its own cuBLAS workspace; graphs of different branches
+    never share a pool, so they may run at the same time.  A call checks every micro-batch's ids on the host
+    (DeviceSplit.check), uploads the chunk's ids in one copy, copies each sent_vecs into its branch's buffer and replays the
+    chunk's forward graphs, branch j on its stream after the current stream's work; the current stream then waits for all of
+    them.  It reads nothing on the host and returns the losses behind one autograd node.  Its backward seeds branch j's
+    backward graph with d_losses[j], replays the backward graphs the same way (each writes its parameter gradients into its
+    own row of a slot buffer laid out by distributed.slot_columns), then distributed.ordered_grad_sum_ adds the rows in
+    micro-batch order onto `.grad` (onto the first row when `.grad` is None), and dL/dsent_vecs flows back per micro-batch.
+
+    Contracts, as for DataParallelSplitTrain:
+    - the losses, logits, dL/dsent_vecs and every decoder `.grad` equal the plain SplitTrainStep loop's bit for bit under
+      torch.use_deterministic_algorithms(True) with dropout 0, and so do the parameters after the optimiser step: BatchNorm
+      uses batch statistics in training, so its running statistics do not feed back within a batch.  `.grad` becomes a view
+      of a batch-owned buffer when it was None, as SplitTrainStep's becomes a step-owned one;
+    - BatchNorm running statistics: each branch's graphs update branch-owned copies of the decoder's BatchNorm buffers (the
+      node MLPs' and the shared edge encoder's), loaded from the live ones at the start of its forward graph.  After a
+      chunk's forward the copies are folded into the live buffers in micro-batch order by distributed.fold_running_stats, in
+      fp64 rounded once to fp32, and num_batches_tracked advances by the exact count.  The loop rounds after every update, so
+      the statistics agree with it to within the rounding of the updates, not bit for bit;
+    - dropout: each branch draws from a CUDA generator state of its own, seeded at capture from torch's CPU generator, so
+      branches never share a mask and never race on the generator's device-side offset.  With dropout the run is the plain
+      loop in distribution, not bit for bit.  Reseeding torch afterwards does not reseed the branches.
+
+    The first call captures every branch, on its own chunk's micro-batches (cycled over the branches past len(chunk)); the
+    warm-ups restore the BatchNorm buffers, `.grad` and the CUDA generator state.  Refusals: ValueError at construction for
+    `branches` < 1, a split without labels, an unknown loss, autocast dtype or max_edges SplitTrainStep refuses, a BatchNorm
+    with momentum=None (its statistics cannot be folded) and a decoder in .eval(); ValueError at a call, before anything is
+    enqueued, for an empty chunk or one of more than `branches` micro-batches, a micro-batch of another size (a partial one
+    included), another number of sent_vecs than micro-batches and sent_vecs of another shape or dtype; RuntimeError at a call
+    in .eval(), after `.to()` / `.cuda()`, after torch.use_deterministic_algorithms changed or after a change in which decoder
+    parameters require grad (build a new SplitTrainBatch), and at a backward after the next call.  Padded batches, one GPU;
+    branches past the 32 streams of torch's stream pool share streams and do not all overlap."""
+
+    what = "SplitTrainBatch"
+
+    def __init__(self, decoder, split, batch_size, *, branches=8, edge_capacity, max_edges, autocast_dtype=None,
+                 loss="cross_entropy"):
+        if int(branches) < 1:
+            raise ValueError(f"SplitTrainBatch: branches = {int(branches)}; it needs at least 1")
+        self._init_training(decoder, autocast_dtype)
+        self.split, self.batch_size, self.branches = split, int(batch_size), int(branches)
+        self.edge_capacity, self.max_edges, self.loss = int(edge_capacity), int(max_edges), loss
+        self._bns = [m for m in decoder.modules() if isinstance(m, torch.nn.modules.batchnorm._BatchNorm)
+                     and m.track_running_stats]
+        if any(m.momentum is None for m in self._bns):
+            raise ValueError("SplitTrainBatch: a BatchNorm with momentum=None (a cumulative average) cannot be folded across "
+                             "branches")
+        dev = split.device
+        self._qids = torch.zeros(self.branches, self.batch_size, dtype=torch.int64, device=dev)
+        self._branches = [_TrainBranch(self, b) for b in range(self.branches)]  # refuses what SplitTrainStep refuses
+        self._bn_live = [t for m in self._bns for t in (m.running_mean, m.running_var)]
+        self._nbt_live = [m.num_batches_tracked for m in self._bns]
+        L = sum(t.numel() for t in self._bn_live)
+        self._bn_rows = torch.zeros(self.branches, L, dtype=torch.float32, device=dev)
+        self._nbt_rows = torch.zeros(self.branches, len(self._bns), dtype=torch.int64, device=dev)
+        self._bn_owner = torch.tensor([i for i, m in enumerate(self._bns) for _ in range(2 * m.running_mean.numel())],
+                                      dtype=torch.int64, device=dev)
+        self._bn_momentum = torch.tensor([float(m.momentum) for m in self._bns for _ in range(2 * m.running_mean.numel())],
+                                         dtype=torch.float64, device=dev)
+        self._anchor = torch.empty(0, device=dev, requires_grad=True)
+        self._slots = None
+        self._used = None
+        self.calls = 0
+
+    def chunks(self, batch):
+        """train_chunks(batch, batch_size, branches): the chunks of full micro-batches this step takes, in order."""
+        return train_chunks(batch, self.batch_size, self.branches)
+
+    @property
+    def logits(self):
+        """The logits [batch_size * nc, 1] of the last call's micro-batches, one static buffer per branch."""
+        return [br.logits for br in self._branches[:self._n]] if self.calls else []
+
+    # -- a call ---------------------------------------------------------------------------------------------------------
+
+    def __call__(self, chunk, sent_vecs):
+        """The mean losses [len(chunk)] (fp32) of the micro-batches `chunk` (a list of host id arrays of batch_size
+        questions each) with their sent_vecs (a list of device tensors [batch_size*nc, S]); `.backward()` replays the
+        branches' backward graphs and sums their gradients into `.grad`."""
+        if not self.decoder.training:
+            raise RuntimeError("SplitTrainBatch replays the training forward: call decoder.train() first")
+        captured = self._slots is not None
+        if captured:
+            self._check_fit()
+            if [p.requires_grad for p in self.decoder.parameters()] != self._requires_grad:
+                raise RuntimeError("SplitTrainBatch: which decoder parameters require grad changed since capture; the "
+                                   "backward graphs write the old set. Build a new SplitTrainBatch.")
+            for br in self._branches:
+                br._status.check(self.what)
+        chunk, sent_vecs = list(chunk), list(sent_vecs)
+        n = len(chunk)
+        if not 1 <= n <= self.branches:
+            raise ValueError(f"SplitTrainBatch: a chunk of {n} micro-batches; it takes 1 to branches = {self.branches}")
+        if len(sent_vecs) != n:
+            raise ValueError(f"SplitTrainBatch: {len(sent_vecs)} sent_vecs for {n} micro-batches")
+        ids = [self._checked_ids(q, sv, self._branches[j]) for j, (q, sv) in enumerate(zip(chunk, sent_vecs))]
+        rows = n if captured else self.branches  # the capture gives every branch a micro-batch of this chunk
+        ids = np.stack([ids[j % n] for j in range(rows)])
+        # a pinned block from the caching host allocator per call: it is not reused before this copy has run
+        self._qids[:rows].copy_(torch.from_numpy(ids).pin_memory(), non_blocking=True)
+        if not captured:
+            self._capture(sent_vecs)
+        self.calls += 1
+        self._n = n
+        losses = _SplitTrainBatchReplay.apply(self, self._anchor, *sent_vecs)
+        for br in self._branches[:n]:
+            br._status.replayed()
+        self._fold_bn(n)
+        return losses
+
+    def _checked_ids(self, question_ids, sent_vecs, branch):
+        q = self.split.check(question_ids, self.edge_capacity)[0]
+        if q.size != self.batch_size:
+            raise ValueError(f"SplitTrainBatch: a micro-batch of {q.size} questions, the step was built for "
+                             f"{self.batch_size}; run a partial micro-batch through split.batch + decoder")
+        branch._check_sent_vecs(sent_vecs)
+        return q
+
+    def _replay(self, branches, which):
+        """Replays graph `which` of every branch on its stream after the current stream's work; the current stream then
+        waits for all of them."""
+        cur = torch.cuda.current_stream(self.split.device)
+        for br in branches:
+            br.stream.wait_stream(cur)
+            with torch.cuda.stream(br.stream):
+                getattr(br, which).replay()
+        for br in branches:
+            cur.wait_stream(br.stream)
+
+    # -- capture --------------------------------------------------------------------------------------------------------
+
+    def _capture(self, sent_vecs):
+        dev = self.split.device
+        params = [p for p in self.decoder.parameters() if p.requires_grad]
+        # rows as long as every trainable parameter needs: the layout of the reached ones is fixed by the first backward
+        ld = _dist.slot_columns([p.numel() for p in params])[1]
+        self._slots = torch.empty(self.branches, ld, dtype=torch.float32, device=dev)
+        streams = [torch.cuda.Stream(device=dev) for _ in range(self.branches)]  # consecutive: distinct up to 32
+        seeds = torch.randint(0, 2 ** 62, (self.branches,)).tolist()
+        gen = _cuda_generator(dev)
+        try:
+            for br, s, seed in zip(self._branches, streams, seeds):
+                br.capture(self, sent_vecs[br.index % len(sent_vecs)], s, gen.clone_state().manual_seed(seed))
+        except BaseException:
+            self._slots = self._used = None
+            for br in self._branches:
+                br._sv = None
+            raise
+        self._params = params
+        self._buffers = list(self.decoder.buffers())
+        self._ptrs = self._addresses()
+        self._requires_grad = [p.requires_grad for p in self.decoder.parameters()]
+        flat = torch.empty(self._slots.size(1), dtype=torch.float32, device=dev)
+        self._own = [flat[c:c + p.numel()].view_as(p) for p, c in zip(self._used_params(), self._cols)]
+        self.mode = f"{self.branches} branches of two CUDA graphs (forward + backward) on streams of their own"
+
+    @contextlib.contextmanager
+    def _branch_buffers(self, b):
+        """The decoder's BatchNorm buffers pointing at branch b's copies, for the branch's capture."""
+        row, nbt = self._bn_rows[b], self._nbt_rows[b]
+        off = 0
+        for i, m in enumerate(self._bns):
+            c = m.running_mean.numel()
+            m.running_mean, m.running_var = row[off:off + c], row[off + c:off + 2 * c]
+            m.num_batches_tracked = nbt[i]
+            off += 2 * c
+        try:
+            yield
+        finally:
+            for i, m in enumerate(self._bns):
+                m.running_mean, m.running_var = self._bn_live[2 * i], self._bn_live[2 * i + 1]
+                m.num_batches_tracked = self._nbt_live[i]
+
+    def _row_views(self, b, used):
+        """Branch b's slot row as views shaped like the reached parameters `used` (indices into the trainable ones); the
+        first call fixes the layout, distributed.slot_columns of their sizes."""
+        params = self._branches[b]._params
+        if self._used is None:
+            self._used = list(used)
+            self._cols = _dist.slot_columns([params[i].numel() for i in used])[0]
+        elif list(used) != self._used:
+            raise RuntimeError("SplitTrainBatch: the branches' losses reach different decoder parameters")
+        row = self._slots[b]
+        return [row[c:c + params[i].numel()].view_as(params[i]) for i, c in zip(self._used, self._cols)]
+
+    def _used_params(self):
+        return [self._params[i] for i in self._used]
+
+    # -- after the replays ----------------------------------------------------------------------------------------------
+
+    def _sum_slots(self, n):
+        """Adds the first n slot rows onto the reached parameters' `.grad` in micro-batch order (ordered_grad_sum_)."""
+        grads, init = [], []
+        for p, own in zip(self._used_params(), self._own):
+            g = p.grad
+            if g is not None and not g.is_contiguous():
+                own.copy_(g)
+                g = own
+            grads.append(own if g is None else g)
+            init.append(g is not None)
+        _dist.ordered_grad_sum_(grads, self._slots, n, init)
+        for p, g in zip(self._used_params(), grads):
+            if p.grad is not g:
+                p.grad = g
+
+    def _fold_bn(self, n):
+        """The live BatchNorm buffers after the first n branches' updates in micro-batch order (fold_running_stats)."""
+        if not self._bns:
+            return
+        with torch.no_grad():
+            start = torch.cat(self._bn_live)
+            counts = self._nbt_rows[:n] - torch.stack(self._nbt_live)
+            folded = _dist.fold_running_stats(start, self._bn_rows[:n], counts.index_select(1, self._bn_owner),
+                                              self._bn_momentum).to(start.dtype)
+            torch._foreach_copy_(self._bn_live, list(folded.split([t.numel() for t in self._bn_live])))
+            torch._foreach_add_(self._nbt_live, list(counts.sum(0).unbind(0)))
 
 
 def packed_host_batch(adj, H, node_type, node_score, sent_vecs, adj_lengths):
