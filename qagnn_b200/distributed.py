@@ -142,6 +142,42 @@ def ordered_grad_sum_(grads, slots, n_valid, init_from_grad):
             _lib.stream_ptr(slots.device)), "qagnn_ordered_grad_sum")
 
 
+class GradSlots:
+    """Micro-batch j's gradients of the fp32 `tensors` in row j of `slots` [rows, >= ld], laid out by slot_columns (ld its
+    row length), and their ordered sum onto the tensors' `.grad`; `flat` [>= ld] takes the sums that start from no tensor of
+    the caller's.  The caller allocates both.  `rows[j]` and `own` are row j and `flat` as views shaped like the tensors."""
+
+    def __init__(self, tensors, slots, flat):
+        self.tensors, self.slots = list(tensors), slots
+        self.cols = slot_columns([t.numel() for t in self.tensors])[0]
+        self.rows = [self._views(row) for row in slots]
+        self.own = self._views(flat)
+
+    def _views(self, flat):
+        return [flat[c:c + t.numel()].view_as(t) for t, c in zip(self.tensors, self.cols)]
+
+    def copy_row_(self, j, grads):
+        """Copies `grads`, one per tensor, into row j; None counts as zeros."""
+        dst = self.rows[j]
+        if grads and all(g is not None for g in grads):
+            torch._foreach_copy_(dst, list(grads))
+        else:
+            for d, g in zip(dst, grads):
+                d.zero_() if g is None else d.copy_(g)
+
+    def sum_(self, starts, n_valid):
+        """ordered_grad_sum_ of rows 0 ... n_valid - 1 onto `starts`, one per tensor, and each tensor's `.grad` the sum: a start
+        of None sums into `own`, a non-contiguous one is first copied there, a contiguous one is added onto in place."""
+        sums = []
+        for s, own in zip(starts, self.own):
+            if s is not None and not s.is_contiguous():
+                own.copy_(s)
+            sums.append(s if s is not None and s.is_contiguous() else own)
+        ordered_grad_sum_(sums, self.slots, n_valid, [s is not None for s in starts])
+        for t, s in zip(self.tensors, sums):
+            t.grad = s
+
+
 def fold_running_stats(start, ends, counts, momentum):
     """The running statistics one process would hold after W ranks' BatchNorm updates in rank order, from each rank's own:
     `start` [L] the common starting values R_0, `ends` [W, L] rank r's values R_r after `counts` [W, L] updates of its own from
@@ -156,6 +192,53 @@ def fold_running_stats(start, ends, counts, momentum):
     total = counts.sum(0)
     after = total - counts.cumsum(0)
     return torch.pow(a, total) * start + (torch.pow(a, after) * (ends - torch.pow(a, counts) * start)).sum(0)
+
+
+class BatchNormFold:
+    """The running statistics of `decoder`'s BatchNorms that track them, read as one flat [mean_0, var_0, mean_1, var_1, ...]
+    vector of L elements and T num_batches_tracked counts, and folded into the live buffers from copies that several branches
+    or ranks (`across`) updated on their own.  Raises ValueError, naming the caller `what`, for a BatchNorm with momentum=None."""
+
+    def __init__(self, decoder, what, across):
+        self.bns = [m for m in decoder.modules() if isinstance(m, torch.nn.modules.batchnorm._BatchNorm)
+                    and m.track_running_stats]
+        if any(m.momentum is None for m in self.bns):
+            raise ValueError(f"{what}: a BatchNorm with momentum=None (a cumulative average) cannot be folded across {across}")
+        self.live = [t for m in self.bns for t in (m.running_mean, m.running_var)]
+        self.live_counts = [m.num_batches_tracked for m in self.bns]
+        self.sizes = [t.numel() for t in self.live]
+        dev = self.live[0].device if self.live else None
+        owner = [i for i, m in enumerate(self.bns) for _ in range(2 * m.running_mean.numel())]
+        self._owner = torch.tensor(owner, dtype=torch.int64, device=dev)
+        self._momentum = torch.tensor([float(self.bns[i].momentum) for i in owner], dtype=torch.float64, device=dev)
+
+    def read(self, stats=None, counts=None):
+        """(the flat statistics [L], num_batches_tracked [T]) of the live buffers, written into `stats` / `counts` if given."""
+        return torch.cat(self.live, out=stats), torch.stack(self.live_counts, out=counts)
+
+    def fold_(self, start, ends):
+        """The live buffers after the updates of every row of `ends` (stats [W, L], counts [W, T]), in row order, each row's
+        from `start` (stats [L], counts [T], as read() returns them): fold_running_stats in fp64, rounded once, and
+        num_batches_tracked the start count plus the exact sum of the rows' counts."""
+        (stats, counts), (end_stats, end_counts) = start, ends
+        n = end_counts - counts
+        with torch.no_grad():
+            folded = fold_running_stats(stats, end_stats, n.index_select(1, self._owner), self._momentum)
+            torch._foreach_copy_(self.live, list(folded.to(stats.dtype).split(self.sizes)))
+            torch._foreach_copy_(self.live_counts, list((counts + n.sum(0).to(counts.dtype)).unbind(0)))
+
+    @contextlib.contextmanager
+    def pointing_at(self, stats, counts):
+        """The modules' buffers pointing at `stats` [L] and `counts` [T] (rows of a [rows, L] / [rows, T] pair) in the block."""
+        self._point(stats.split(self.sizes), counts)
+        try:
+            yield
+        finally:
+            self._point(self.live, self.live_counts)
+
+    def _point(self, stats, counts):
+        for i, m in enumerate(self.bns):
+            m.running_mean, m.running_var, m.num_batches_tracked = stats[2 * i], stats[2 * i + 1], counts[i]
 
 
 class DataParallelSplitTrain:
@@ -210,21 +293,11 @@ class DataParallelSplitTrain:
                 raise ValueError(f"DataParallelSplitTrain: a full batch of {M} micro-batches leaves rank {r} of {W} "
                                  f"{'none' if hi == lo else 'only the partial one'}; every rank must capture its step on a "
                                  f"full micro-batch of the first batch")
-        dec = step.decoder
-        self._bns = [m for m in dec.modules() if isinstance(m, torch.nn.modules.batchnorm._BatchNorm)
-                     and m.track_running_stats]
-        for m in self._bns:
-            if m.momentum is None:
-                raise ValueError("DataParallelSplitTrain: a BatchNorm with momentum=None (a cumulative average) cannot be "
-                                 "folded across ranks")
-        if self._bns:
-            self._bn_momentum = torch.cat([torch.full((2 * m.running_mean.numel(),), float(m.momentum), dtype=torch.float64)
-                                           for m in self._bns]).to(split.device)
-            self._bn_owner = torch.cat([torch.full((2 * m.running_mean.numel(),), i) for i, m in enumerate(self._bns)]
-                                       ).to(split.device)
-        self._params = [p for p in dec.parameters() if p.requires_grad]
+        self._bn = BatchNormFold(step.decoder, "DataParallelSplitTrain", "ranks")
+        self._params = [p for p in step.decoder.parameters() if p.requires_grad]
         self._other = list(other_params)
         self._reached = None       # indices into self._params the step's capture reaches, in order
+        self._grad_slots = None         # the reached parameters' GradSlots
         self._other_pattern = None  # the requires-grad flags of self._other that self._other_reached was exchanged for
         self._other_reached = None  # indices into self._other the loss reaches under that pattern
         self._batch = None         # (n, M, m, first row, count) between micro_batches() and reduce_()
@@ -244,8 +317,8 @@ class DataParallelSplitTrain:
         self._batch = (n, M, -(-M // W), lo, hi - lo)
         self._done = 0
         # .grad from before the batch: the decoder's adds on top of it in order; the other parameters' after the sum
-        self._before = [g if g is None or self._is_own(i, g) else g.detach().clone()
-                        for i, g in enumerate(p.grad for p in self._params)]
+        own = {id(g) for g in self._grad_slots.own} if self._grad_slots is not None else set()
+        self._before = [g if g is None or id(g) in own else g.detach().clone() for g in (p.grad for p in self._params)]
         self._pattern = tuple(p.requires_grad for p in self._other)
         self._trainable = [i for i, t in enumerate(self._pattern) if t]
         self._other_before = {i: self._other[i].grad for i in self._trainable}
@@ -253,7 +326,7 @@ class DataParallelSplitTrain:
             p.grad = None
         for i in self._trainable:
             self._other[i].grad = None
-        self._bn_start = self._bn_state() if W > 1 else None
+        self._bn_start = self._bn.read() if W > 1 and self._bn.bns else None
         return [batch[j * mbs:(j + 1) * mbs] for j in range(lo, hi)]
 
     @contextlib.contextmanager
@@ -268,13 +341,7 @@ class DataParallelSplitTrain:
             self._set_layout()
         if any(self._params[i].grad is not None for i in self._unreached):
             raise RuntimeError("DataParallelSplitTrain: a micro-step reached decoder parameters its step's capture does not")
-        dst = self._row_views[self._batch[2] * self.rank + self._done]
-        src = [self._params[i].grad for i in self._reached]
-        if src and all(g is not None for g in src):
-            torch._foreach_copy_(dst, src)
-        else:
-            for d, g in zip(dst, src):
-                d.zero_() if g is None else d.copy_(g)
+        self._grad_slots.copy_row_(self._batch[2] * self.rank + self._done, [p.grad for p in self._grad_slots.tensors])
         self._done += 1
 
     def loss(self, question_ids, sent_vecs):
@@ -318,19 +385,12 @@ class DataParallelSplitTrain:
     def _gather_slots(self):
         if self.world_size > 1:
             m = self._batch[2]
-            rows = self._slots[:self.world_size * m]
+            rows = self._grad_slots.slots[:self.world_size * m]
             dist.all_gather_into_tensor(rows, rows[self.rank * m:(self.rank + 1) * m], group=self.group)
 
     def _sum_slots(self):
-        grads, init = [], []
-        for i, c in zip(self._reached, self._cols):
-            before = self._before[i]
-            grads.append(self._own[i] if before is None else before)
-            init.append(before is not None)
-        ordered_grad_sum_(grads, self._slots, self._batch[1], init)
-        for i, g in zip(self._reached, grads):
-            self._params[i].grad = g
-        for i in set(range(len(self._params))) - set(self._reached):
+        self._grad_slots.sum_([self._before[i] for i in self._reached], self._batch[1])
+        for i in self._unreached:
             self._params[i].grad = self._before[i]
 
     def _reduce_other(self):
@@ -366,56 +426,32 @@ class DataParallelSplitTrain:
         return local
 
     def _fold_bn(self):
-        if self.world_size == 1 or not self._bns:
+        if self.world_size == 1 or not self._bn.bns:
             return
-        start, n0 = self._bn_start
-        end, n1 = self._bn_state()
-        mine = torch.cat([end, (n1 - n0).double()])
+        stats, counts = self._bn.read()
+        mine = torch.cat([stats.double(), counts.double()])
         every = torch.empty(self.world_size * mine.numel(), dtype=torch.float64, device=mine.device)
         dist.all_gather_into_tensor(every, mine, group=self.group)
         every = every.view(self.world_size, -1)
-        L = start.numel()
-        counts = every[:, L:]
-        folded = fold_running_stats(start, every[:, :L], counts.index_select(1, self._bn_owner), self._bn_momentum)
-        total = n0 + counts.sum(0).round().long()
-        off = 0
-        with torch.no_grad():
-            for i, m in enumerate(self._bns):
-                c = m.running_mean.numel()
-                m.running_mean.copy_(folded[off:off + c])
-                m.running_var.copy_(folded[off + c:off + 2 * c])
-                m.num_batches_tracked.copy_(total[i])
-                off += 2 * c
+        self._bn.fold_(self._bn_start, (every[:, :stats.numel()], every[:, stats.numel():]))
 
     # -- helpers --------------------------------------------------------------------------------------------------------
 
-    def _bn_state(self):
-        if not self._bns:
-            return None
-        stats = torch.cat([t.detach().double().reshape(-1) for m in self._bns for t in (m.running_mean, m.running_var)])
-        return stats, torch.stack([m.num_batches_tracked.detach().clone() for m in self._bns])
-
-    def _is_own(self, i, g):
-        return self._reached is not None and i in self._own and g is self._own[i]
-
     def _set_layout(self):
-        """The decoder parameters the step's capture reaches, their slot columns, the slot rows and the flat `.grad`."""
+        """The decoder parameters the step's capture reaches and their gradient slots, the rows of a full batch."""
         step = self.step
         if step._fwd is None:
             raise RuntimeError("DataParallelSplitTrain: the first micro-step ran eagerly; the first batch must be full")
         where = {id(p): i for i, p in enumerate(self._params)}
         self._reached = sorted(where[id(p)] for p, _ in step._owned)
-        numels = [self._params[i].numel() for i in self._reached]
-        self._cols, ld = slot_columns(numels)
+        self._unreached = sorted(set(range(len(self._params))) - set(self._reached))
+        reached = [self._params[i] for i in self._reached]
+        ld = slot_columns([p.numel() for p in reached])[1]
         full = -(-self.batch_size // self.micro_batch_size)
         m = -(-full // self.world_size)
         dev = self.split.device
-        self._slots = torch.empty(self.world_size * m, ld, dtype=torch.float32, device=dev)
-        flat = torch.empty(ld, dtype=torch.float32, device=dev)
-        self._own = {i: flat[c:c + n].view_as(self._params[i]) for i, c, n in zip(self._reached, self._cols, numels)}
-        self._row_views = [[row[c:c + n].view_as(self._params[i]) for i, c, n in zip(self._reached, self._cols, numels)]
-                           for row in self._slots]
-        self._unreached = sorted(set(range(len(self._params))) - set(self._reached))
+        self._grad_slots = GradSlots(reached, torch.empty(self.world_size * m, ld, dtype=torch.float32, device=dev),
+                                torch.empty(ld, dtype=torch.float32, device=dev))
 
     def _exchange_reached(self):
         """Once per requires-grad pattern of other_params: every rank's reached decoder parameters must agree; the other

@@ -315,6 +315,12 @@ class _TrainingGraphs:
             raise RuntimeError(f"{what} was captured with torch.use_deterministic_algorithms({self.deterministic}) and "
                                f"its backward graph holds that mode's kernels; the flag changed since. Build a new {what}.")
 
+    def _check_requires_grad(self):
+        """RuntimeError when which decoder parameters require grad changed since capture."""
+        if [p.requires_grad for p in self.decoder.parameters()] != self._requires_grad:
+            raise RuntimeError(f"{self.what}: which decoder parameters require grad changed since capture; the backward "
+                               f"graphs hold the old set. Build a new {self.what}.")
+
     def _replayed(self):
         self._status.replayed()
         # the replay changed the running statistics behind autograd's back: the eval path's folded weights key on versions
@@ -781,9 +787,7 @@ class SplitTrainStep(_TrainingGraphs, _SplitBatches):
             raise RuntimeError("SplitTrainStep replays the training forward: call decoder.train() first")
         if self._fwd is not None:
             self._check_replay()
-            if [p.requires_grad for p in self.decoder.parameters()] != self._requires_grad:
-                raise RuntimeError("SplitTrainStep: which decoder parameters require grad changed since capture; the "
-                                   "backward graph accumulates the old set. Build a new SplitTrainStep.")
+            self._check_requires_grad()
         self._load_ids(question_ids, sent_vecs)
         if self._fwd is None:
             self._sv = sent_vecs.detach().clone().requires_grad_(True)
@@ -837,18 +841,17 @@ class _TrainBranch(SplitTrainStep):
 
         def forward():
             with torch.no_grad():  # the chunk's BatchNorm state, read before any branch updates its copies
-                if tb._bns:
-                    torch.cat(tb._bn_live, out=tb._bn_rows[b])
-                    torch.stack(tb._nbt_live, out=tb._nbt_rows[b])
+                if tb._bn.bns:
+                    tb._bn.read(tb._bn_rows[b], tb._nbt_rows[b])
             return self._forward()
 
         gen = _cuda_generator(tb.split.device)
         live_rng = gen.graphsafe_get_state()
         gen.graphsafe_set_state(rng)
         try:
-            with tb._branch_buffers(b):
-                self.used = self._capture_split(lambda used, grads: torch._foreach_copy_(tb._row_views(b, used), grads),
-                                                forward=forward, stream=stream)
+            with tb._bn.pointing_at(tb._bn_rows[b], tb._nbt_rows[b]):
+                self._capture_split(lambda used, grads: torch._foreach_copy_(tb._row_views(b, used), grads),
+                                    forward=forward, stream=stream)
         finally:
             gen.graphsafe_set_state(live_rng)
         self._keep = (self.decoder.gnn._last_prep,)  # graph prep's buffers, which both graphs baked in
@@ -879,7 +882,7 @@ class _SplitTrainBatchReplay(torch.autograd.Function):
         branches = tb._branches[:ctx.n]
         torch._foreach_copy_([br._d_loss for br in branches], list(d_losses.unbind(0)))
         tb._replay(branches, "_bwd")
-        tb._sum_slots(ctx.n)
+        tb._grad_slots.sum_([p.grad for p in tb._grad_slots.tensors], ctx.n)
         return (None, None) + tuple(br._g_sv if need else None for br, need in zip(branches, ctx.needs_input_grad[2:]))
 
 
@@ -940,26 +943,14 @@ class SplitTrainBatch(_TrainingGraphs):
         self._init_training(decoder, autocast_dtype)
         self.split, self.batch_size, self.branches = split, int(batch_size), int(branches)
         self.edge_capacity, self.max_edges, self.loss = int(edge_capacity), int(max_edges), loss
-        self._bns = [m for m in decoder.modules() if isinstance(m, torch.nn.modules.batchnorm._BatchNorm)
-                     and m.track_running_stats]
-        if any(m.momentum is None for m in self._bns):
-            raise ValueError("SplitTrainBatch: a BatchNorm with momentum=None (a cumulative average) cannot be folded across "
-                             "branches")
+        self._bn = _dist.BatchNormFold(decoder, self.what, "branches")
         dev = split.device
         self._qids = torch.zeros(self.branches, self.batch_size, dtype=torch.int64, device=dev)
         self._branches = [_TrainBranch(self, b) for b in range(self.branches)]  # refuses what SplitTrainStep refuses
-        self._bn_live = [t for m in self._bns for t in (m.running_mean, m.running_var)]
-        self._nbt_live = [m.num_batches_tracked for m in self._bns]
-        L = sum(t.numel() for t in self._bn_live)
-        self._bn_rows = torch.zeros(self.branches, L, dtype=torch.float32, device=dev)
-        self._nbt_rows = torch.zeros(self.branches, len(self._bns), dtype=torch.int64, device=dev)
-        self._bn_owner = torch.tensor([i for i, m in enumerate(self._bns) for _ in range(2 * m.running_mean.numel())],
-                                      dtype=torch.int64, device=dev)
-        self._bn_momentum = torch.tensor([float(m.momentum) for m in self._bns for _ in range(2 * m.running_mean.numel())],
-                                         dtype=torch.float64, device=dev)
+        self._bn_rows = torch.zeros(self.branches, sum(self._bn.sizes), dtype=torch.float32, device=dev)
+        self._nbt_rows = torch.zeros(self.branches, len(self._bn.bns), dtype=torch.int64, device=dev)
         self._anchor = torch.empty(0, device=dev, requires_grad=True)
-        self._slots = None
-        self._used = None
+        self._slots = self._flat = self._used = self._grad_slots = None  # set by the capture
         self.calls = 0
 
     def chunks(self, batch):
@@ -982,9 +973,7 @@ class SplitTrainBatch(_TrainingGraphs):
         captured = self._slots is not None
         if captured:
             self._check_fit()
-            if [p.requires_grad for p in self.decoder.parameters()] != self._requires_grad:
-                raise RuntimeError("SplitTrainBatch: which decoder parameters require grad changed since capture; the "
-                                   "backward graphs write the old set. Build a new SplitTrainBatch.")
+            self._check_requires_grad()
             for br in self._branches:
                 br._status.check(self.what)
         chunk, sent_vecs = list(chunk), list(sent_vecs)
@@ -1005,7 +994,8 @@ class SplitTrainBatch(_TrainingGraphs):
         losses = _SplitTrainBatchReplay.apply(self, self._anchor, *sent_vecs)
         for br in self._branches[:n]:
             br._status.replayed()
-        self._fold_bn(n)
+        if self._bn.bns:  # the branches' BatchNorm rows into the live buffers, in micro-batch order
+            self._bn.fold_(self._bn.read(), (self._bn_rows[:n], self._nbt_rows[:n]))
         return losses
 
     def _checked_ids(self, question_ids, sent_vecs, branch):
@@ -1032,9 +1022,11 @@ class SplitTrainBatch(_TrainingGraphs):
     def _capture(self, sent_vecs):
         dev = self.split.device
         params = [p for p in self.decoder.parameters() if p.requires_grad]
-        # rows as long as every trainable parameter needs: the layout of the reached ones is fixed by the first backward
+        # allocated before any capture, as long as every trainable parameter needs: the first branch's backward fixes which
+        # of them the losses reach, and so the layout
         ld = _dist.slot_columns([p.numel() for p in params])[1]
         self._slots = torch.empty(self.branches, ld, dtype=torch.float32, device=dev)
+        self._flat = torch.empty(ld, dtype=torch.float32, device=dev)
         streams = [torch.cuda.Stream(device=dev) for _ in range(self.branches)]  # consecutive: distinct up to 32
         seeds = torch.randint(0, 2 ** 62, (self.branches,)).tolist()
         gen = _cuda_generator(dev)
@@ -1042,7 +1034,7 @@ class SplitTrainBatch(_TrainingGraphs):
             for br, s, seed in zip(self._branches, streams, seeds):
                 br.capture(self, sent_vecs[br.index % len(sent_vecs)], s, gen.clone_state().manual_seed(seed))
         except BaseException:
-            self._slots = self._used = None
+            self._slots = self._flat = self._used = self._grad_slots = None
             for br in self._branches:
                 br._sv = None
             raise
@@ -1050,70 +1042,18 @@ class SplitTrainBatch(_TrainingGraphs):
         self._buffers = list(self.decoder.buffers())
         self._ptrs = self._addresses()
         self._requires_grad = [p.requires_grad for p in self.decoder.parameters()]
-        flat = torch.empty(self._slots.size(1), dtype=torch.float32, device=dev)
-        self._own = [flat[c:c + p.numel()].view_as(p) for p, c in zip(self._used_params(), self._cols)]
         self.mode = f"{self.branches} branches of two CUDA graphs (forward + backward) on streams of their own"
-
-    @contextlib.contextmanager
-    def _branch_buffers(self, b):
-        """The decoder's BatchNorm buffers pointing at branch b's copies, for the branch's capture."""
-        row, nbt = self._bn_rows[b], self._nbt_rows[b]
-        off = 0
-        for i, m in enumerate(self._bns):
-            c = m.running_mean.numel()
-            m.running_mean, m.running_var = row[off:off + c], row[off + c:off + 2 * c]
-            m.num_batches_tracked = nbt[i]
-            off += 2 * c
-        try:
-            yield
-        finally:
-            for i, m in enumerate(self._bns):
-                m.running_mean, m.running_var = self._bn_live[2 * i], self._bn_live[2 * i + 1]
-                m.num_batches_tracked = self._nbt_live[i]
 
     def _row_views(self, b, used):
         """Branch b's slot row as views shaped like the reached parameters `used` (indices into the trainable ones); the
-        first call fixes the layout, distributed.slot_columns of their sizes."""
-        params = self._branches[b]._params
-        if self._used is None:
+        first call fixes them and so the layout."""
+        if self._grad_slots is None:
+            params = self._branches[b]._params
             self._used = list(used)
-            self._cols = _dist.slot_columns([params[i].numel() for i in used])[0]
+            self._grad_slots = _dist.GradSlots([params[i] for i in used], self._slots, self._flat)
         elif list(used) != self._used:
             raise RuntimeError("SplitTrainBatch: the branches' losses reach different decoder parameters")
-        row = self._slots[b]
-        return [row[c:c + params[i].numel()].view_as(params[i]) for i, c in zip(self._used, self._cols)]
-
-    def _used_params(self):
-        return [self._params[i] for i in self._used]
-
-    # -- after the replays ----------------------------------------------------------------------------------------------
-
-    def _sum_slots(self, n):
-        """Adds the first n slot rows onto the reached parameters' `.grad` in micro-batch order (ordered_grad_sum_)."""
-        grads, init = [], []
-        for p, own in zip(self._used_params(), self._own):
-            g = p.grad
-            if g is not None and not g.is_contiguous():
-                own.copy_(g)
-                g = own
-            grads.append(own if g is None else g)
-            init.append(g is not None)
-        _dist.ordered_grad_sum_(grads, self._slots, n, init)
-        for p, g in zip(self._used_params(), grads):
-            if p.grad is not g:
-                p.grad = g
-
-    def _fold_bn(self, n):
-        """The live BatchNorm buffers after the first n branches' updates in micro-batch order (fold_running_stats)."""
-        if not self._bns:
-            return
-        with torch.no_grad():
-            start = torch.cat(self._bn_live)
-            counts = self._nbt_rows[:n] - torch.stack(self._nbt_live)
-            folded = _dist.fold_running_stats(start, self._bn_rows[:n], counts.index_select(1, self._bn_owner),
-                                              self._bn_momentum).to(start.dtype)
-            torch._foreach_copy_(self._bn_live, list(folded.split([t.numel() for t in self._bn_live])))
-            torch._foreach_add_(self._nbt_live, list(counts.sum(0).unbind(0)))
+        return self._grad_slots.rows[b]
 
 
 def packed_host_batch(adj, H, node_type, node_score, sent_vecs, adj_lengths):

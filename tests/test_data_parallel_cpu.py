@@ -1,7 +1,7 @@
 """Data-parallel training of a split on the CPU: the block partition of an optimiser batch's micro-batches over the ranks
 (DataParallelSplitTrain.micro_batches), the BatchNorm fold (distributed.fold_running_stats) against a sequential fp64 EMA and
-against nn.BatchNorm1d(momentum=0.1) stepped micro-batch by micro-batch, the constructor's refusals, the slot layout, and
-the ordered-sum kernel's SASS (no floating-point atomics, no spills)."""
+against nn.BatchNorm1d stepped micro-batch by micro-batch (BatchNormFold over mixed widths and momenta included), the
+constructor's refusals, the slot layout, and the ordered-sum kernel's SASS (no floating-point atomics, no spills)."""
 import os
 import re
 import shutil
@@ -148,6 +148,52 @@ def test_the_fold_of_batchnorm1d_is_within_the_bar(W, micro):
         assert float((folded - ref).abs().max()) <= BN_BAR * float(ref.abs().max()), name
     assert int(one.num_batches_tracked) == int(start["num_batches_tracked"]) + sum(
         int(bn.num_batches_tracked - start["num_batches_tracked"]) for bn in ranks)
+
+
+@pytest.mark.parametrize("fp64", [False, True], ids=["rows", "gathered"])
+@pytest.mark.parametrize("W,micro", [(2, 4), (3, 7), (8, 32)])
+def test_the_fold_of_batchnorms_of_other_widths_and_momenta_is_within_the_bar(W, micro, fp64):
+    """BatchNormFold over two BatchNorm1d of widths 200 and 48 and momenta 0.1 and 0.3, which a micro-batch updates 3 times and
+    once: one process steps them micro-batch by micro-batch, W copies each step their block, and the fold of the copies'
+    statistics (fp32 rows with int64 counts as SplitTrainBatch holds them, or the fp64 block DataParallelSplitTrain
+    gathers) is within the bar of the one process, its num_batches_tracked equal."""
+    torch.manual_seed(W)
+
+    def make():
+        return torch.nn.ModuleList([torch.nn.BatchNorm1d(200, momentum=0.1), torch.nn.BatchNorm1d(48, momentum=0.3)]).train()
+
+    data = [([torch.randn(40, 200) * 5 + 3 for _ in range(3)], [torch.randn(40, 48) * 2 - 1]) for _ in range(micro)]
+    one = make()
+    for bn in one:
+        bn.running_mean.normal_(0, 2)
+        bn.running_var.uniform_(0.5, 4)
+    start = {k: v.clone() for k, v in one.state_dict().items()}
+    ranks = [make() for _ in range(W)]
+    for m in ranks:
+        m.load_state_dict(start)
+
+    def step(m, micro_batches):
+        for mb in micro_batches:
+            for bn, xs in zip(m, mb):
+                for x in xs:
+                    bn(x)
+    step(one, data)
+    for r, m in enumerate(ranks):
+        lo, hi = D.shard_bounds(micro, r, W)
+        step(m, data[lo:hi])
+    folded = make()
+    folded.load_state_dict(start)
+    fold = D.BatchNormFold(folded, "test", "ranks")
+    ends = [D.BatchNormFold(m, "test", "ranks").read() for m in ranks]
+    stats, counts = torch.stack([s for s, _ in ends]), torch.stack([c for _, c in ends])
+    fold.fold_(fold.read(), (stats.double(), counts.double()) if fp64 else (stats, counts))
+    for got, ref in zip(folded, one):
+        for name in ("running_mean", "running_var"):
+            a, b = getattr(got, name), getattr(ref, name)
+            assert a.dtype == torch.float32
+            assert float((a - b).abs().max()) <= BN_BAR * float(b.abs().max()), name
+        assert torch.equal(got.num_batches_tracked, ref.num_batches_tracked)
+    assert [int(bn.num_batches_tracked) for bn in folded] == [3 * micro, micro]
 
 
 # ---- the kernel ----------------------------------------------------------------------------------------------------------

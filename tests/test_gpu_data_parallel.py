@@ -1,8 +1,9 @@
 """Data-parallel training of a split (qagnn_b200.distributed.DataParallelSplitTrain) on the GPU.  ordered_grad_sum_ equals a
 Python loop of torch._foreach_add_ bit for bit over the recipe decoder's 86 gradients, sizes 0, 1, 3 and 8193, odd-offset
-views, 700 tensors (two launches), 1, 2, 33 and 64 slots, `.grad` None or zeroed, and slots holding -0.0, inf and NaN.  With
-one rank, under torch.use_deterministic_algorithms(True) with dropout 0, two optimiser batches (the second ending in a
-partial micro-batch) equal the plain SplitTrainStep loop bit for bit: every `.grad`, the BatchNorm buffers and the parameters
+views, 700 tensors (two launches), 1, 2, 33 and 64 slots, `.grad` None or zeroed, and slots holding -0.0, inf and NaN; so
+does GradSlots onto a `.grad` that is None, transposed or held by the caller.  With one rank, under
+torch.use_deterministic_algorithms(True) with dropout 0, two optimiser batches (the second ending in a partial
+micro-batch) equal the plain SplitTrainStep loop bit for bit: every `.grad`, the BatchNorm buffers and the parameters
 after optim.RAdam, in fp32, fp16 with a GradScaler and bf16, and reduce_ reads nothing on the host.  With 2, 4 and 8 ranks
 (NCCL, one process per GPU; skipped when fewer than 2 GPUs are visible) the decoder's `.grad` and the parameters after RAdam
 equal the one-GPU run bit for bit, a batch with fewer micro-batches than ranks included; the BatchNorm statistics are within
@@ -126,6 +127,28 @@ def test_refusals():
         D.ordered_grad_sum_([x.half()], torch.zeros(2, 4, device=DEV), 1, False)
     with pytest.raises(ValueError, match="init_from_grad"):
         D.ordered_grad_sum_([x], torch.zeros(2, 4, device=DEV), 1, [True, False])
+
+
+def test_grad_slots_sum_onto_none_a_transposed_grad_and_a_held_one():
+    """GradSlots: rows written by copy_row_ (None as zeros) and summed by sum_ equal the foreach loop bit for bit, and `.grad`
+    becomes a view of the helper's own buffer for a start of None or a non-contiguous one, the start itself otherwise."""
+    g = torch.Generator(device=DEV).manual_seed(6)
+    params = [torch.nn.Parameter(torch.empty(s, device=DEV)) for s in ((3, 5), (4, 6), (7,))]
+    rows = [[torch.randn(p.shape, device=DEV, generator=g) for p in params] for _ in range(3)]
+    rows[1][0] = None
+    ld = D.slot_columns([p.numel() for p in params])[1]
+    gs = D.GradSlots(params, torch.full((4, ld), float("nan"), device=DEV), torch.empty(ld, device=DEV))
+    for j, row in enumerate(rows):
+        gs.copy_row_(j, row)
+    held = torch.randn(7, device=DEV, generator=g)
+    starts = [None, torch.randn(6, 4, device=DEV, generator=g).t(), held]
+    ref = _loop([None if s is None else s.clone() for s in starts],
+                [[torch.zeros(p.shape, device=DEV) if t is None else t for p, t in zip(params, row)] for row in rows], 3)
+    gs.sum_(starts, 3)
+    for p, r in zip(params, ref):
+        assert torch.equal(p.grad.view(torch.int32), r.view(torch.int32))
+    assert params[0].grad.data_ptr() == gs.own[0].data_ptr() and params[1].grad.data_ptr() == gs.own[1].data_ptr()
+    assert params[1].grad.is_contiguous() and params[2].grad is held
 
 
 # ---- the training loop ---------------------------------------------------------------------------------------------------

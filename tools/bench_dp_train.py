@@ -192,7 +192,7 @@ def main():
         n = len(outs)
         cargs = (n, (C.c_void_p * n)(*[o.data_ptr() for o in outs]), (C.c_int64 * n)(*[o.numel() for o in outs]),
                  (C.c_int64 * n)(*D.slot_columns([o.numel() for o in outs])[0]), (C.c_int32 * n)(*([0] * n)),
-                 _lib.ptr(dp._slots), dp._slots.stride(0), M, _lib.stream_ptr(dev))
+                 _lib.ptr(dp._grad_slots.slots), dp._grad_slots.slots.stride(0), M, _lib.stream_ptr(dev))
         lib = _lib.load()
         _lib.check(lib.qagnn_ordered_grad_sum(*cargs), "qagnn_ordered_grad_sum")
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
