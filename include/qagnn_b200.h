@@ -445,6 +445,38 @@ int64_t qagnn_clip_grad_norm_slots(int32_t n_tensors, const int64_t *numels);
 int32_t qagnn_clip_grad_norm(int32_t n_tensors, void *const *grads, const int64_t *numels, double max_norm, double *slots,
                              int64_t n_slots, int32_t *counter, float *total_norm, float *coef, void *stream);
 
+/* The update rule of a captured optimiser tail: qagnn_radam_step's or qagnn_adamw_step's. */
+enum { QAGNN_RULE_RADAM = 0, QAGNN_RULE_ADAMW = 1 };
+
+/* Bytes of the captured tail's per-call block for n_groups param groups; -1 when n_groups < 1. */
+int64_t qagnn_step_tail_block_bytes(int32_t n_groups);
+
+/* Writes the captured tail's per-call block into host memory `block` of n_bytes, for a copy to the device before each replay
+ * of qagnn_step_tail: per group (lr, weight_decay, beta1, beta2, eps, rule_flag and step_tables as for qagnn_radam_step /
+ * qagnn_adamw_step, every group's table non-null), rounded as those entries round them, then table_len, (float)max_norm and
+ * GradScaler's growth_factor, backoff_factor and growth_interval.  Host only.  QAGNN_ERR_WORKSPACE when n_bytes is short. */
+int32_t qagnn_step_tail_fill(int32_t rule, int32_t n_groups, const double *lr, const double *weight_decay, const double *beta1,
+                             const double *beta2, const double *eps, const int32_t *rule_flag, void *const *step_tables,
+                             int64_t table_len, double max_norm, double growth_factor, double backoff_factor,
+                             int32_t growth_interval, void *block, int64_t n_bytes);
+
+/* The recipe's optimiser tail, scaler.unscale_; clip_grad_norm_; scaler.step; scaler.update, on the current device with no
+ * host read and every per-call value taken from the device block (qagnn_b200.optim.CapturedTail), so a CUDA graph can replay
+ * it.  Pass 1, when clip is nonzero or scale is given: over the n_norm gradients norm_grads / norm_numels, sets *found_inf to
+ * 1 for a non-finite gradient (when scale is given) and, when clip is nonzero, writes qagnn_clip_grad_norm's *total_norm and
+ * *coef for the gradients times (float)(1 / (double)*scale) (times 1 without a scale), with the block's max_norm.  Pass 2: the
+ * rule's step over the tensors (laid out as for qagnn_radam_step; group_index into the block's groups), each gradient first
+ * unscaled and clipped as the eager tail would leave it in .grad; nothing else changes when *found_inf is nonzero.  Without
+ * a clip the step unscales as qagnn_radam_step does with grad_scale = scale.  With a scale, the call ends with
+ * torch._amp_update_scale_ on *scale and *growth_tracker (device int32) and clears *found_inf.  found_inf (device fp32) and
+ * counter (device int32) are zero between calls; slots as for qagnn_clip_grad_norm over the norm list.  Launches: one per pass
+ * per 512 tensors (pass 2 also per 16 groups). */
+int32_t qagnn_step_tail(int32_t rule, int32_t n_tensors, void *const *params, void *const *grads, void *const *exp_avgs,
+                        void *const *exp_avg_sqs, void *const *steps, const int64_t *numels, const int32_t *group_index,
+                        int32_t n_groups, int32_t n_norm, void *const *norm_grads, const int64_t *norm_numels, int32_t clip,
+                        const void *block, double *slots, int64_t n_slots, int32_t *counter, float *total_norm, float *coef,
+                        float *found_inf, float *scale, int32_t *growth_tracker, void *stream);
+
 /* The ordered sum of one optimiser batch's per-micro-batch gradients into .grad, for data-parallel training
  * (qagnn_b200.distributed.ordered_grad_sum_): n_tensors contiguous fp32 tensors grads[i] of numels[i] elements on the current
  * device, and device fp32 slots, row j (j < n_valid, n_valid >= 1) at slots + j * ld holding micro-batch j's gradient of tensor

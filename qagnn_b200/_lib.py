@@ -109,7 +109,12 @@ EXPORTS = {
                                      _P, _P, _P, _P]),
     "qagnn_clip_grad_norm_slots": (C.c_int64, [C.c_int32, _P]),
     "qagnn_clip_grad_norm": (C.c_int32, [C.c_int32, _P, _P, C.c_double, _P, C.c_int64, _P, _P, _P, _P]),
-    "qagnn_ordered_grad_sum": (C.c_int32, [C.c_int32, _P, _P, _P, _P, _P, C.c_int64, C.c_int32, _P]),
+    "qagnn_step_tail_block_bytes": (C.c_int64, [C.c_int32]),
+    "qagnn_step_tail_fill": (C.c_int32, [C.c_int32, C.c_int32, _P, _P, _P, _P, _P, _P, _P, C.c_int64, C.c_double, C.c_double,
+                                         C.c_double, C.c_int32, _P, C.c_int64]),
+    "qagnn_step_tail": (C.c_int32, [C.c_int32, C.c_int32, _P, _P, _P, _P, _P, _P, _P, C.c_int32, C.c_int32, _P, _P, C.c_int32, _P,
+                                    _P, C.c_int64, _P, _P, _P, _P, _P, _P, _P]),
+    "qagnn_ordered_grad_sum":(C.c_int32, [C.c_int32, _P, _P, _P, _P, _P, C.c_int64, C.c_int32, _P]),
     "qagnn_launch_count": (C.c_int64, []),
     "qagnn_profile_enable": (C.c_int32, [C.c_int32]),
     "qagnn_profile_read": (C.c_int32, [C.POINTER(C.c_double), C.POINTER(C.c_int64)]),

@@ -15,12 +15,14 @@ device step.  The host counts its own `step()` calls, which bounds every device 
 `OPTIMIZER_CLASSES` is the reference's `--optim` table, so `from qagnn_b200.optim import OPTIMIZER_CLASSES` replaces the
 reference's import, whose module no longer loads with current `transformers`.  `clip_grad_norm_` is the recipe's
 `torch.nn.utils.clip_grad_norm_` in two launches per device (csrc/clip.cu) instead of torch's three foreach passes, so
-the optimiser tail `scaler.unscale_; clip_grad_norm_; scaler.step; scaler.update` never reads the GPU.
+the optimiser tail `scaler.unscale_; clip_grad_norm_; scaler.step; scaler.update` never reads the GPU.  `CapturedTail` runs
+that whole tail, scheduler step included, as one CUDA graph replay of two launches (csrc/tail.cu).
 """
 import ctypes as C
 import math
 
 import torch
+from torch.amp.grad_scaler import OptState
 
 from . import _lib
 
@@ -126,6 +128,14 @@ class _DeviceStepOptimizer(torch.optim.Optimizer):
             c = self._counters[device] = torch.zeros(1, dtype=torch.int32, device=device)
         return c
 
+    def _state_for(self, p):
+        st = self.state[p]
+        if len(st) == 0:
+            st["step"] = torch.zeros((), dtype=torch.int64, device=p.device)
+            st["exp_avg"] = torch.zeros_like(p, memory_format=torch.contiguous_format)
+            st["exp_avg_sq"] = torch.zeros_like(p, memory_format=torch.contiguous_format)
+        return st
+
     @torch.no_grad()
     def step(self, closure=None):
         loss = None
@@ -161,14 +171,7 @@ class _DeviceStepOptimizer(torch.optim.Optimizer):
         lr, wd, b1, b2, eps = (arr(C.c_double, col) for col in zip(*hyper))
         flags = arr(C.c_int32, self._rule_flags())
         for device, items in work.items():
-            states = []
-            for _, p in items:
-                st = self.state[p]
-                if len(st) == 0:
-                    st["step"] = torch.zeros((), dtype=torch.int64, device=device)
-                    st["exp_avg"] = torch.zeros_like(p, memory_format=torch.contiguous_format)
-                    st["exp_avg_sq"] = torch.zeros_like(p, memory_format=torch.contiguous_format)
-                states.append(st)
+            states = [self._state_for(p) for _, p in items]
             tables = [None] * n_groups
             for gi in {gi for gi, _ in items}:
                 tables[gi] = self._table(device, hyper[gi][2], hyper[gi][3])
@@ -318,6 +321,170 @@ def clip_grad_norm_(parameters, max_norm, norm_type=2.0, error_if_nonfinite=Fals
                                             _lib.ptr(slots), slots.numel(), _lib.ptr(counter), _lib.ptr(total_norm),
                                             _lib.ptr(coef), _lib.stream_ptr(device)), "qagnn_clip_grad_norm")
     return total_norm
+
+
+class CapturedTail:
+    """The recipe's optimiser tail as one CUDA graph replay per optimiser batch (csrc/tail.cu).  `tail()` does what
+
+        scaler.unscale_(optimizer); clip_grad_norm_(clip_parameters, max_grad_norm)   # both only when max_grad_norm > 0
+        scheduler.step(); scaler.step(optimizer); scaler.update()
+
+    does with this module's `optimizer` and `clip_grad_norm_` and torch's GradScaler, bit for bit in the parameters, their
+    state, `.grad`, the norm and the scaler's scale and growth tracker, in two sm_90a launches (two more per 512 tensors or
+    16 groups) and with no host read.  It returns the norm as a new 0-dim device tensor, or None when max_grad_norm <= 0.
+
+    `optimizer` is a `RAdam` or an `AdamW`; `scaler` a `torch.amp.GradScaler` or None (a disabled one counts as None);
+    `scheduler` any LR scheduler or None.  `clip_parameters` defaults to the optimizer's parameters; those with a `.grad` must
+    be the optimizer's parameters with a `.grad`, in any order.  Every call first steps the scheduler on the host, then
+    writes what a replay must not freeze (each group's hyperparameters, the step tables, max_grad_norm and the scaler's
+    factors) into a device block through a fresh pinned buffer, replays the graph and counts the step on the host, so eager
+    `optimizer.step()` calls can be mixed in.  The graph holds the tensors' addresses: a call whose parameters, gradients,
+    optimiser state or scaler tensors moved (a frozen or unfrozen encoder, `zero_grad(set_to_none=True)`,
+    `load_state_dict`) first runs its kernels directly and captures them again; `captures` counts the captures.  The
+    scaler's Python bookkeeping is not touched, so `scaler.scale`, `get_scale` and `state_dict` keep working.  Gradients
+    must be dense, contiguous fp32 tensors on one CUDA device, as for the optimiser."""
+
+    def __init__(self, optimizer, scaler=None, scheduler=None, max_grad_norm=0.0, clip_parameters=None):
+        if not isinstance(optimizer, (RAdam, AdamW)):
+            raise ValueError(f"qagnn_b200.optim.CapturedTail: {type(optimizer).__module__}.{type(optimizer).__name__} is not "
+                             f"qagnn_b200.optim.RAdam or AdamW; run the eager tail (scaler.unscale_, clip_grad_norm_, "
+                             f"scheduler.step, scaler.step, scaler.update) for it")
+        if scaler is not None and not scaler.is_enabled():
+            scaler = None
+        self.optimizer, self.scaler, self.scheduler = optimizer, scaler, scheduler
+        self.max_grad_norm = float(max_grad_norm)
+        if isinstance(clip_parameters, torch.Tensor):
+            clip_parameters = [clip_parameters]
+        self._clip_parameters = None if clip_parameters is None else list(clip_parameters)
+        self._rule = 0 if isinstance(optimizer, RAdam) else 1  # QAGNN_RULE_*
+        self.captures = 0
+        self._key = None
+        self._graph = None
+        self._bufs = None
+
+    def _work(self):
+        """[(group index, p)] of the parameters with a gradient, checked as the optimiser and the clip check them."""
+        opt, name = self.optimizer, "CapturedTail"
+        items = []
+        for gi, group in enumerate(opt.param_groups):
+            opt._check_group(group)
+            for p in group["params"]:
+                if p.grad is None:
+                    continue
+                if p.grad.layout != torch.strided:
+                    raise TypeError(f"qagnn_b200.optim.{name}: the gradient must be dense (got {p.grad.layout})")
+                _check_tensor(p, "parameter", name)
+                _check_tensor(p.grad, "gradient", name)
+                if p.grad.shape != p.shape or p.grad.device != p.device:
+                    raise ValueError(f"qagnn_b200.optim.{name}: a gradient of shape {tuple(p.grad.shape)} on {p.grad.device} "
+                                     f"for a parameter of shape {tuple(p.shape)} on {p.device}")
+                items.append((gi, p))
+        if not items:
+            raise RuntimeError(f"qagnn_b200.optim.{name}: no parameter has a gradient")
+        devices = {p.device for _, p in items}
+        if len(devices) != 1:
+            raise ValueError(f"qagnn_b200.optim.{name}: parameters on {sorted(str(d) for d in devices)}; all must be on one "
+                             f"device (the eager tail handles several)")
+        return items, items[0][1].device
+
+    def _norm_grads(self, items):
+        if self._clip_parameters is None:
+            return [p.grad for _, p in items]
+        grads = [p.grad for p in self._clip_parameters if p.grad is not None]
+        if {id(g) for g in grads} != {id(p.grad) for _, p in items} or len(grads) != len(items):
+            raise ValueError("qagnn_b200.optim.CapturedTail: the clip_parameters with a .grad must be the optimizer's "
+                             "parameters with a .grad; run the eager tail for other sets")
+        return grads
+
+    def _scaler_tensors(self, device):
+        scaler = self.scaler
+        if scaler is None:
+            return None, None
+        if scaler._scale is None or scaler._growth_tracker is None:
+            raise RuntimeError("qagnn_b200.optim.CapturedTail: the scaler has no scale yet; call scaler.scale(loss) first")
+        if scaler._scale.device != device:
+            raise ValueError(f"qagnn_b200.optim.CapturedTail: the scaler's scale is on {scaler._scale.device}, the "
+                             f"parameters on {device}")
+        return scaler._scale, scaler._growth_tracker
+
+    @torch.no_grad()
+    def __call__(self):
+        opt = self.optimizer
+        st = None if self.scaler is None else self.scaler._per_optimizer_states.get(id(opt))
+        if st is not None and st["stage"] is OptState.UNSCALED:
+            raise RuntimeError("qagnn_b200.optim.CapturedTail: scaler.unscale_(optimizer) was already called since the last "
+                               "update(); the tail unscales the gradients itself")
+        items, device = self._work()
+        clip = self.max_grad_norm > 0
+        scale, tracker = self._scaler_tensors(device)
+        norm_grads = self._norm_grads(items) if clip else [p.grad for _, p in items]
+        states = [opt._state_for(p) for _, p in items]
+        key = (device, clip, None if scale is None else (scale.data_ptr(), tracker.data_ptr()), len(opt.param_groups),
+               tuple((gi, p.data_ptr(), p.grad.data_ptr(), s["exp_avg"].data_ptr(), s["exp_avg_sq"].data_ptr(),
+                      s["step"].data_ptr(), p.numel()) for (gi, p), s in zip(items, states)),
+               tuple((g.data_ptr(), g.numel()) for g in norm_grads))
+
+        if self.scheduler is not None:
+            self.scheduler.step()
+        opt._host_steps += 1
+        lib = _lib.load()
+        hyper = [(float(g["lr"]), float(g["weight_decay"]), float(g["betas"][0]), float(g["betas"][1]), float(g["eps"]))
+                 for g in opt.param_groups]
+        tables = [opt._table(device, h[2], h[3]) for h in hyper]
+        arr = lambda ct, vals: (ct * len(vals))(*vals)  # noqa: E731
+        lr, wd, b1, b2, eps = (arr(C.c_double, col) for col in zip(*hyper))
+        n_groups = len(hyper)
+        n_bytes = lib.qagnn_step_tail_block_bytes(n_groups)
+        if self._key != key:
+            self._bufs = self._buffers(device, n_bytes, norm_grads, lib)
+        bufs = self._bufs
+        # a fresh pinned buffer per call from the caching host allocator, which keeps it until its copy has run
+        staging = torch.empty(n_bytes, dtype=torch.uint8, pin_memory=True)
+        sc = self.scaler
+        _lib.check(lib.qagnn_step_tail_fill(
+            self._rule, n_groups, lr, wd, b1, b2, eps, arr(C.c_int32, opt._rule_flags()),
+            arr(C.c_void_p, [t.data_ptr() for t in tables]), min(t.shape[0] for t in tables), self.max_grad_norm,
+            float(sc._growth_factor) if sc else 2.0, float(sc._backoff_factor) if sc else 0.5,
+            int(sc._growth_interval) if sc else 1, C.c_void_p(staging.data_ptr()), n_bytes), "qagnn_step_tail_fill")
+        bufs["block"].copy_(staging, non_blocking=True)
+        if self._key == key:
+            self._graph.replay()
+        else:
+            # this call's step runs directly, which also loads the kernels; the capture then records the same launches
+            self._graph = None
+            launch = self._launcher(lib, device, items, states, norm_grads, clip, scale, tracker, n_groups)
+            launch()
+            graph = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(graph):
+                launch()
+            self._graph, self._key = graph, key
+            self.captures += 1
+        return bufs["total_norm"].clone() if clip else None
+
+    def _buffers(self, device, n_bytes, norm_grads, lib):
+        n = len(norm_grads)
+        n_slots = lib.qagnn_clip_grad_norm_slots(n, (C.c_int64 * n)(*[g.numel() for g in norm_grads]))
+        z = lambda dt: torch.zeros(1, dtype=dt, device=device)  # noqa: E731
+        return dict(block=torch.empty(n_bytes, dtype=torch.uint8, device=device),
+                    slots=torch.empty(max(n_slots, 1), dtype=torch.float64, device=device),
+                    counter=z(torch.int32), found_inf=z(torch.float32), coef=z(torch.float32),
+                    total_norm=torch.zeros((), dtype=torch.float32, device=device))
+
+    def _launcher(self, lib, device, items, states, norm_grads, clip, scale, tracker, n_groups):
+        arr = lambda ct, vals: (ct * len(vals))(*vals)  # noqa: E731
+        ptrs = lambda ts: arr(C.c_void_p, [t.data_ptr() for t in ts])  # noqa: E731
+        n, nn, b = len(items), len(norm_grads), self._bufs
+        args = (self._rule, n, ptrs([p for _, p in items]), ptrs([p.grad for _, p in items]),
+                ptrs([s["exp_avg"] for s in states]), ptrs([s["exp_avg_sq"] for s in states]), ptrs([s["step"] for s in states]),
+                arr(C.c_int64, [p.numel() for _, p in items]), arr(C.c_int32, [gi for gi, _ in items]), n_groups,
+                nn, ptrs(norm_grads), arr(C.c_int64, [g.numel() for g in norm_grads]), int(clip), _lib.ptr(b["block"]),
+                _lib.ptr(b["slots"]), b["slots"].numel(), _lib.ptr(b["counter"]), _lib.ptr(b["total_norm"]),
+                _lib.ptr(b["coef"]), _lib.ptr(b["found_inf"]), _lib.ptr(scale), _lib.ptr(tracker))
+
+        def launch():
+            with torch.cuda.device(device):
+                _lib.check(lib.qagnn_step_tail(*args, _lib.stream_ptr(device)), "qagnn_step_tail")
+        return launch
 
 
 # The reference's --optim table (utils/optimization_utils.py).  'sgd' and 'adam' are torch's own classes, as the reference
