@@ -431,6 +431,33 @@ int32_t qagnn_adamw_step(int32_t n_tensors, void *const *params, void *const *gr
                          void *const *step_tables, int64_t table_len, const float *found_inf, const float *grad_scale,
                          int32_t *counter, void *stream);
 
+/* One step of torch.optim.Adam as torch 2.11 steps it by default on CUDA (the foreach implementation; amsgrad, maximize and
+ * decoupled_weight_decay off; qagnn_b200.optim.Adam), with the argument layout of qagnn_radam_step; rule_flag is unused.
+ * Per element: d = g + weight_decay * p when weight_decay != 0 (.grad keeps g), m = lerp(m, d, 1 - b1),
+ * v = b2 v + (1 - b2) d^2, p += step_size * m / (sqrt(v) / bc2_sqrt + eps), each rounded as torch's kernels round it.
+ * step_tables[g] is a device fp64 [table_len, 2] table of ((1 - b2^t) ** 0.5, 1 - b1^t) for t = row, in Python doubles;
+ * the kernel forms step_size = -(lr / (1 - b1^t)) in IEEE fp64 before rounding it to fp32.  found_inf, grad_scale and
+ * counter as for qagnn_radam_step.  Every element is torch's result bit for bit; no host synchronisation. */
+int32_t qagnn_adam_step(int32_t n_tensors, void *const *params, void *const *grads, void *const *exp_avgs,
+                        void *const *exp_avg_sqs, void *const *steps, const int64_t *numels, const int32_t *group_index,
+                        int32_t n_groups, const double *lr, const double *weight_decay, const double *beta1,
+                        const double *beta2, const double *eps, const int32_t *rule_flag, void *const *step_tables,
+                        int64_t table_len, const float *found_inf, const float *grad_scale, int32_t *counter, void *stream);
+
+/* One step of torch.optim.SGD as torch 2.11 steps it by default on CUDA (the foreach implementation; maximize off;
+ * qagnn_b200.optim.SGD), with the argument layout of qagnn_radam_step: exp_avgs holds the momentum buffers, beta1 is each
+ * group's momentum (finite, >= 0), beta2 its dampening, rule_flag its nesterov; exp_avg_sqs, eps, step_tables and table_len
+ * are unused and may be null / 0.  A group with momentum 0 keeps no buffer (its exp_avgs[i] may be null).  Per element:
+ * d = g + weight_decay * p when weight_decay != 0, then with momentum buf = d at device step 0, else
+ * buf = momentum buf + (1 - dampening) d, and d = d + momentum buf (nesterov; written to .grad when weight_decay == 0, as
+ * torch does) or buf; then p += -lr d.  Buffers are zero before their first step.  found_inf, grad_scale and counter as for
+ * qagnn_radam_step.  Every element is torch's result bit for bit; no host synchronisation. */
+int32_t qagnn_sgd_step(int32_t n_tensors, void *const *params, void *const *grads, void *const *momentum_buffers,
+                       void *const *exp_avg_sqs, void *const *steps, const int64_t *numels, const int32_t *group_index,
+                       int32_t n_groups, const double *lr, const double *weight_decay, const double *momentum,
+                       const double *dampening, const double *eps, const int32_t *nesterov, void *const *step_tables,
+                       int64_t table_len, const float *found_inf, const float *grad_scale, int32_t *counter, void *stream);
+
 /* fp64 slots qagnn_clip_grad_norm needs for n_tensors tensors of numels[i] elements (one per 8192-element chunk); -1 for a
  * negative count or size. */
 int64_t qagnn_clip_grad_norm_slots(int32_t n_tensors, const int64_t *numels);
@@ -445,15 +472,16 @@ int64_t qagnn_clip_grad_norm_slots(int32_t n_tensors, const int64_t *numels);
 int32_t qagnn_clip_grad_norm(int32_t n_tensors, void *const *grads, const int64_t *numels, double max_norm, double *slots,
                              int64_t n_slots, int32_t *counter, float *total_norm, float *coef, void *stream);
 
-/* The update rule of a captured optimiser tail: qagnn_radam_step's or qagnn_adamw_step's. */
-enum { QAGNN_RULE_RADAM = 0, QAGNN_RULE_ADAMW = 1 };
+/* The update rule of a captured optimiser tail: qagnn_radam_step's, qagnn_adamw_step's, qagnn_adam_step's or
+ * qagnn_sgd_step's. */
+enum { QAGNN_RULE_RADAM = 0, QAGNN_RULE_ADAMW = 1, QAGNN_RULE_ADAM = 2, QAGNN_RULE_SGD = 3 };
 
 /* Bytes of the captured tail's per-call block for n_groups param groups; -1 when n_groups < 1. */
 int64_t qagnn_step_tail_block_bytes(int32_t n_groups);
 
 /* Writes the captured tail's per-call block into host memory `block` of n_bytes, for a copy to the device before each replay
  * of qagnn_step_tail: per group (lr, weight_decay, beta1, beta2, eps, rule_flag and step_tables as for qagnn_radam_step /
- * qagnn_adamw_step, every group's table non-null), rounded as those entries round them, then table_len, (float)max_norm and
+ * qagnn_adamw_step / qagnn_adam_step / qagnn_sgd_step, every group's table non-null except SGD's), rounded as those entries round them, then table_len, (float)max_norm and
  * GradScaler's growth_factor, backoff_factor and growth_interval.  Host only.  QAGNN_ERR_WORKSPACE when n_bytes is short. */
 int32_t qagnn_step_tail_fill(int32_t rule, int32_t n_groups, const double *lr, const double *weight_decay, const double *beta1,
                              const double *beta2, const double *eps, const int32_t *rule_flag, void *const *step_tables,

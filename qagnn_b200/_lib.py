@@ -107,6 +107,10 @@ EXPORTS = {
                                      _P, _P, _P, _P]),
     "qagnn_adamw_step": (C.c_int32, [C.c_int32, _P, _P, _P, _P, _P, _P, _P, C.c_int32, _P, _P, _P, _P, _P, _P, _P, C.c_int64,
                                      _P, _P, _P, _P]),
+    "qagnn_adam_step": (C.c_int32, [C.c_int32, _P, _P, _P, _P, _P, _P, _P, C.c_int32, _P, _P, _P, _P, _P, _P, _P, C.c_int64,
+                                    _P, _P, _P, _P]),
+    "qagnn_sgd_step": (C.c_int32, [C.c_int32, _P, _P, _P, _P, _P, _P, _P, C.c_int32, _P, _P, _P, _P, _P, _P, _P, C.c_int64,
+                                   _P, _P, _P, _P]),
     "qagnn_clip_grad_norm_slots": (C.c_int64, [C.c_int32, _P]),
     "qagnn_clip_grad_norm": (C.c_int32, [C.c_int32, _P, _P, C.c_double, _P, C.c_int64, _P, _P, _P, _P]),
     "qagnn_step_tail_block_bytes": (C.c_int64, [C.c_int32]),

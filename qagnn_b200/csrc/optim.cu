@@ -23,8 +23,10 @@
 //   (sqrt(1 - b2^t), 1 - b1^t) from Python's libm pow, and the kernel forms -((lr * sq) / bc1) in IEEE fp64 (the bits Python
 //   computes) before its rounding.
 // The host-double scalars (1 - b2, -wd*lr, eps, ...) are rounded to fp32 as torch rounds them.
+// torch.optim.Adam and SGD (Rule::kAdam, kSgd) run on the same body; optim_torch.cu states their rules and rounding.
 //
-// The body and the packing live in optim.cuh, which the captured optimiser tail (tail.cu) shares.
+// The body, the packing and the entries' host side live in optim.cuh, which torch's Adam and SGD (optim_torch.cu) and the
+// captured optimiser tail (tail.cu) share.
 // Work split: multi_tensor.cuh's chunks, launches and arrival counter.  Every CTA reads the step counters, so they are
 // advanced only by the last CTA to finish.  A nonzero found_inf leaves p, m, v and every step as they are.
 #include "optim.cuh"
@@ -48,39 +50,6 @@ int32_t launch(const StepArgs& a, cudaStream_t st) {
   return QAGNN_OK;
 }
 
-// The shared host side of both entries: validation, per-launch packing (512 tensors, 16 groups, an int32 chunk prefix) and
-// the launches.  rule_flag is RAdam's degenerated_to_sgd or AdamW's correct_bias, per group.
-template <Rule R>
-int32_t step_all(int32_t n_tensors, void* const* params, void* const* grads, void* const* exp_avgs, void* const* exp_avg_sqs,
-                 void* const* steps, const int64_t* numels, const int32_t* group_index, int32_t n_groups, const double* lr,
-                 const double* weight_decay, const double* beta1, const double* beta2, const double* eps,
-                 const int32_t* rule_flag, void* const* step_tables, int64_t table_len, const float* found_inf,
-                 const float* grad_scale, int32_t* counter, void* stream) {
-  if (n_tensors < 0 || n_groups < 0) return QAGNN_ERR_INVALID_ARGUMENT;
-  if (n_tensors == 0) return QAGNN_OK;
-  if (!tensors_valid(n_tensors, params, grads, exp_avgs, exp_avg_sqs, steps, numels, group_index, n_groups) || !lr ||
-      !weight_decay || !beta1 || !beta2 || !eps || !rule_flag || !step_tables || table_len < 2 || !counter)
-    return QAGNN_ERR_INVALID_ARGUMENT;
-  for (int32_t i = 0; i < n_tensors; ++i) {
-    const int32_t gi = group_index[i];
-    if (!step_tables[gi] || !(beta1[gi] >= 0.0 && beta1[gi] < 1.0) || !(beta2[gi] >= 0.0 && beta2[gi] < 1.0))
-      return QAGNN_ERR_INVALID_ARGUMENT;
-  }
-  cudaStream_t st = (cudaStream_t)stream;
-  static thread_local StepArgs a;  // 28 KB: kept off the stack
-  a.table_len = table_len;
-  a.found_inf = found_inf;
-  a.grad_scale = grad_scale;
-  a.counter = counter;
-  return pack_launches(
-      a, n_tensors, params, grads, exp_avgs, exp_avg_sqs, steps, numels, group_index,
-      [&](int32_t slot, int32_t gi) {
-        fill_group(a.groups[slot], lr[gi], weight_decay[gi], beta1[gi], beta2[gi], eps[gi],
-                   group_flags<R>(weight_decay[gi], rule_flag[gi]), (const double*)step_tables[gi]);
-      },
-      [&](bool) { return launch<R>(a, st); });
-}
-
 }  // namespace
 
 }  // namespace qagnn
@@ -95,7 +64,8 @@ extern "C" int32_t qagnn_radam_step(int32_t n_tensors, void* const* params, void
                                     const float* found_inf, const float* grad_scale, int32_t* counter, void* stream) {
   return step_all<Rule::kRAdam>(n_tensors, params, grads, exp_avgs, exp_avg_sqs, steps, numels, group_index, n_groups, lr,
                                 weight_decay, beta1, beta2, eps, degenerated_to_sgd, step_tables, table_len, found_inf,
-                                grad_scale, counter, stream);
+                                grad_scale, counter,
+                                [&](const StepArgs& a) { return launch<Rule::kRAdam>(a, (cudaStream_t)stream); });
 }
 
 extern "C" int32_t qagnn_adamw_step(int32_t n_tensors, void* const* params, void* const* grads, void* const* exp_avgs,
@@ -106,5 +76,6 @@ extern "C" int32_t qagnn_adamw_step(int32_t n_tensors, void* const* params, void
                                     const float* grad_scale, int32_t* counter, void* stream) {
   return step_all<Rule::kAdamW>(n_tensors, params, grads, exp_avgs, exp_avg_sqs, steps, numels, group_index, n_groups, lr,
                                 weight_decay, beta1, beta2, eps, correct_bias, step_tables, table_len, found_inf,
-                                grad_scale, counter, stream);
+                                grad_scale, counter,
+                                [&](const StepArgs& a) { return launch<Rule::kAdamW>(a, (cudaStream_t)stream); });
 }

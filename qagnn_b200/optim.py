@@ -1,19 +1,21 @@
 """The reference's optimisers as one multi-tensor sm_90a launch per device (csrc/optim.cu).
 
 `RAdam` is the reference's `utils.optimization_utils.RAdam` (qagnn_radam_step) and `AdamW` is transformers' `AdamW` (3.4.0,
-the version the reference pins; qagnn_adamw_step).  Each takes its original's arguments and param groups and reproduces its
+the version the reference pins; qagnn_adamw_step).  `Adam` and `SGD` are torch.optim's, as torch 2.11 steps them by default
+on CUDA (qagnn_adam_step, qagnn_sgd_step; csrc/optim_torch.cu).  Each takes its original's arguments and param groups and reproduces its
 update bit for bit: the same fp32 operations in the same order, with the same rounding of every Python scalar.  They differ
 from the originals in how they run:
 - one kernel launch per device per `step()` (one per 512 tensors), instead of about ten element-wise ops per tensor;
 - `state[p]['step']` is an int64 0-dim tensor on p's device, advanced by the kernel, so `step()` never reads the GPU;
 - they declare `_step_supports_amp_scaling`: `GradScaler.step` hands them `found_inf` and, when `unscale_` was not called,
   `grad_scale`, and the kernel skips the step or unscales the gradients on the device instead of the scaler's `.item()`.
-What depends on the step t alone (RAdam's step size and branch, AdamW's bias corrections) is computed on the host in Python
+What depends on the step t alone (RAdam's step size and branch, AdamW's and Adam's bias corrections) is computed on the host in Python
 doubles with the original's formula, into a device fp64 table per (device, beta1, beta2) that the kernel indexes with the
 device step.  The host counts its own `step()` calls, which bounds every device step, and grows the table ahead of that count.
 
 `OPTIMIZER_CLASSES` is the reference's `--optim` table, so `from qagnn_b200.optim import OPTIMIZER_CLASSES` replaces the
-reference's import, whose module no longer loads with current `transformers`.  `clip_grad_norm_` is the recipe's
+reference's import, whose module no longer loads with current `transformers`; `DEVICE_OPTIMIZER_CLASSES` maps the same names
+to the four device optimisers.  `clip_grad_norm_` is the recipe's
 `torch.nn.utils.clip_grad_norm_` in two launches per device (csrc/clip.cu) instead of torch's three foreach passes, so
 the optimiser tail `scaler.unscale_; clip_grad_norm_; scaler.step; scaler.update` never reads the GPU.  `CapturedTail` runs
 that whole tail, scheduler step included, as one CUDA graph replay of two launches (csrc/tail.cu).
@@ -59,6 +61,27 @@ def bias_correction_table(beta1, beta2, length):
     return torch.tensor(rows, dtype=torch.float64)
 
 
+def adam_bias_correction_row(beta1, beta2, t):
+    """(bias_correction2_sqrt, bias_correction1) of torch.optim.Adam's default CUDA step at step t >= 1, in Python doubles as
+    torch forms them from its fp32 step count; its step size is (lr / row[1]) * -1."""
+    t = float(t)
+    return (1 - beta2 ** t) ** 0.5, 1 - beta1 ** t
+
+
+def adam_bias_correction_table(beta1, beta2, length):
+    """fp64 [length, 2]: row t is adam_bias_correction_row(beta1, beta2, t); row 0 (never indexed) is (0, 0)."""
+    rows = [(0.0, 0.0)] + [adam_bias_correction_row(beta1, beta2, t) for t in range(1, length)]
+    return torch.tensor(rows, dtype=torch.float64)
+
+
+def _refuse(name, options):
+    """ValueError for options set to what the device step does not implement: [(option, value)] that must be falsy."""
+    on = [k for k, v in options if v]
+    if on:
+        raise ValueError(f"qagnn_b200.optim.{name}: {', '.join(f'{k}=True' for k in on)} is not implemented on the device; "
+                         f"use torch.optim.{name} for it")
+
+
 def _check_hyper(lr, betas, eps):
     # the reference's checks and messages
     if not 0.0 <= lr:
@@ -93,16 +116,25 @@ def _check_tensor(t, what, name):
 
 
 class _DeviceStepOptimizer(torch.optim.Optimizer):
-    """What RAdam and AdamW share: the per-device work lists, the state, the step tables, the kernel's arrival counter, the
-    GradScaler hand-off and state_dict loading.  A subclass names its C entry (`_entry`), its table builder (`_table_rows`,
-    fp64 [length, 2] for (beta1, beta2)), its original's sparse-gradient message and host caches in the groups, and supplies
-    `_check_group` and `_rule_flags` (one int32 per group: the entry's per-group flag)."""
+    """What RAdam, AdamW, Adam and SGD share: the per-device work lists, the state, the step tables, the kernel's arrival
+    counter, the GradScaler hand-off and state_dict loading.  A subclass names its C entry (`_entry`) and tail rule
+    (`_rule`, QAGNN_RULE_*), its table builder (`_table_rows`, fp64 [length, 2] for (beta1, beta2); None for no table), its
+    state tensors (`_state_keys`: the entry's exp_avgs and exp_avg_sqs), its original's sparse-gradient message and host
+    caches in the groups, and supplies `_check_group` and `_rule_flags` (one int32 per group: the entry's per-group flag)."""
 
     _step_supports_amp_scaling = True
     _entry = None
+    _rule = None
     _table_rows = None
+    _state_keys = ("exp_avg", "exp_avg_sq")
     _sparse_message = None
     _host_caches = ()
+
+    @staticmethod
+    def _hyper(group):
+        """The entry's per-group doubles (lr, weight_decay, beta1, beta2, eps)."""
+        return float(group["lr"]), float(group["weight_decay"]), float(group["betas"][0]), float(group["betas"][1]), float(
+            group["eps"])
 
     def __init__(self, params, defaults):
         super().__init__(params, defaults)
@@ -128,13 +160,27 @@ class _DeviceStepOptimizer(torch.optim.Optimizer):
             c = self._counters[device] = torch.zeros(1, dtype=torch.int32, device=device)
         return c
 
-    def _state_for(self, p):
+    def _state_for(self, p, group):
         st = self.state[p]
         if len(st) == 0:
             st["step"] = torch.zeros((), dtype=torch.int64, device=p.device)
-            st["exp_avg"] = torch.zeros_like(p, memory_format=torch.contiguous_format)
-            st["exp_avg_sq"] = torch.zeros_like(p, memory_format=torch.contiguous_format)
+            for k in self._state_keys:
+                st[k] = torch.zeros_like(p, memory_format=torch.contiguous_format)
         return st
+
+    def _state_tensors(self, st):
+        """The entry's exp_avgs[i] and exp_avg_sqs[i] of one parameter's state (None: a null pointer)."""
+        return st["exp_avg"], st["exp_avg_sq"]
+
+    def _group_tables(self, device, hyper, groups):
+        """Each listed group's step table on device (None for the others, and for a rule without tables) and the shortest
+        table's length."""
+        tables = [None] * len(hyper)
+        if self._table_rows is None:
+            return tables, 0
+        for gi in groups:
+            tables[gi] = self._table(device, hyper[gi][2], hyper[gi][3])
+        return tables, min(t.shape[0] for t in tables if t is not None)
 
     @torch.no_grad()
     def step(self, closure=None):
@@ -165,35 +211,37 @@ class _DeviceStepOptimizer(torch.optim.Optimizer):
         lib = _lib.load()
         entry = getattr(lib, self._entry)
         n_groups = len(self.param_groups)
-        hyper = [(float(g["lr"]), float(g["weight_decay"]), float(g["betas"][0]), float(g["betas"][1]), float(g["eps"]))
-                 for g in self.param_groups]
+        hyper = [self._hyper(g) for g in self.param_groups]
         arr = lambda ct, vals: (ct * len(vals))(*vals)  # noqa: E731
         lr, wd, b1, b2, eps = (arr(C.c_double, col) for col in zip(*hyper))
         flags = arr(C.c_int32, self._rule_flags())
         for device, items in work.items():
-            states = [self._state_for(p) for _, p in items]
-            tables = [None] * n_groups
-            for gi in {gi for gi, _ in items}:
-                tables[gi] = self._table(device, hyper[gi][2], hyper[gi][3])
-            length = min(t.shape[0] for t in tables if t is not None)
+            states = [self._state_for(p, self.param_groups[gi]) for gi, p in items]
+            moments = [self._state_tensors(st) for st in states]
+            tables, length = self._group_tables(device, hyper, {gi for gi, _ in items})
             # GradScaler keeps found_inf and the scale on its own device: the copies to this one are enqueued, never read
             fi = None if found_inf is None else found_inf.to(device, torch.float32, non_blocking=True)
             gs = None if grad_scale is None else grad_scale.to(device, torch.float32, non_blocking=True)
             n = len(items)
-            ptrs = lambda ts: arr(C.c_void_p, [t.data_ptr() for t in ts])  # noqa: E731
+            ptrs = lambda ts: arr(C.c_void_p, [None if t is None else t.data_ptr() for t in ts])  # noqa: E731
             with torch.cuda.device(device):
                 _lib.check(entry(
-                    n, ptrs([p for _, p in items]), ptrs([p.grad for _, p in items]), ptrs([s["exp_avg"] for s in states]),
-                    ptrs([s["exp_avg_sq"] for s in states]), ptrs([s["step"] for s in states]),
+                    n, ptrs([p for _, p in items]), ptrs([p.grad for _, p in items]), ptrs([m for m, _ in moments]),
+                    ptrs([v for _, v in moments]), ptrs([s["step"] for s in states]),
                     arr(C.c_int64, [p.numel() for _, p in items]), arr(C.c_int32, [gi for gi, _ in items]), n_groups,
                     lr, wd, b1, b2, eps, flags,
                     arr(C.c_void_p, [0 if t is None else t.data_ptr() for t in tables]), length,
                     _lib.ptr(fi), _lib.ptr(gs), _lib.ptr(self._counter(device)), _lib.stream_ptr(device)), self._entry)
         return loss
 
+    def _missing_step(self, st):
+        """The step of an original's state that keeps none (torch's SGD)."""
+        raise KeyError("step")
+
     def load_state_dict(self, state_dict):
-        """Loads this optimiser's state_dict or its original's, whose 'step' is a Python int.  Every step becomes an int64
-        0-dim tensor on its parameter's device, and the step counts are read once to bound the step tables."""
+        """Loads this optimiser's state_dict or its original's, whose 'step' is a Python int or a CPU tensor.  Every step
+        becomes an int64 0-dim tensor on its parameter's device, and the step counts are read once to bound the step
+        tables."""
         super().load_state_dict(state_dict)
         top = self._host_steps
         steps = {}
@@ -204,14 +252,15 @@ class _DeviceStepOptimizer(torch.optim.Optimizer):
                 st = self.state.get(p)
                 if not st:
                     continue
-                step = st["step"]
+                step = st["step"] if "step" in st else self._missing_step(st)
                 if isinstance(step, torch.Tensor):
                     step = step.to(device=p.device, dtype=torch.int64).reshape(())
                 else:
                     step = torch.tensor(int(step), dtype=torch.int64, device=p.device)
                 st["step"] = step
-                for k in ("exp_avg", "exp_avg_sq"):
-                    st[k] = st[k].to(device=p.device, dtype=torch.float32).contiguous()
+                for k in self._state_keys:
+                    st[k] = (torch.zeros_like(p, memory_format=torch.contiguous_format) if st.get(k) is None else
+                             st[k].to(device=p.device, dtype=torch.float32).contiguous())
                 steps.setdefault(p.device, []).append(step)
         for ss in steps.values():
             top = max(top, int(torch.stack(ss).max()))
@@ -225,6 +274,7 @@ class RAdam(_DeviceStepOptimizer):
     hyperparameter) is read from each group at every `step()`, so LambdaLR schedules work as with the reference."""
 
     _entry = "qagnn_radam_step"
+    _rule = 0
     _table_rows = staticmethod(step_size_table)
     _sparse_message = "RAdam does not support sparse gradients"
     _host_caches = ("buffer",)  # the reference's host cache of step sizes
@@ -250,6 +300,7 @@ class AdamW(_DeviceStepOptimizer):
     included, is read from each group at every `step()`."""
 
     _entry = "qagnn_adamw_step"
+    _rule = 1
     _table_rows = staticmethod(bias_correction_table)
     _sparse_message = "Adam does not support sparse gradients, please consider SparseAdam instead"
 
@@ -262,6 +313,120 @@ class AdamW(_DeviceStepOptimizer):
 
     def _rule_flags(self):
         return [int(bool(g["correct_bias"])) for g in self.param_groups]
+
+
+class Adam(_DeviceStepOptimizer):
+    """Adam(params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0, amsgrad=False, *, foreach=None, maximize=False,
+    capturable=False, differentiable=False, fused=None, decoupled_weight_decay=False): torch.optim.Adam, the reference's
+    `--optim adam`, stepped on the GPU (qagnn_adam_step) bit for bit as torch 2.11 steps it by default on CUDA (its foreach
+    implementation).  The constructor, defaults, checks and param-group keys are torch's; amsgrad, maximize,
+    decoupled_weight_decay and foreach / fused / capturable / differentiable set to True are refused (torch.optim.Adam has
+    them).  The state keeps torch's keys, with `step` an int64 0-dim tensor on the parameter's device; `load_state_dict`
+    takes torch's own state dict, whose fp32 CPU steps it converts.  Parameters and their gradients must be contiguous fp32
+    CUDA tensors; a parameter whose `.grad` is None is skipped and its step does not advance."""
+
+    _entry = "qagnn_adam_step"
+    _rule = 2
+    _table_rows = staticmethod(adam_bias_correction_table)
+    _sparse_message = "Adam does not support sparse gradients, please consider SparseAdam instead"
+
+    def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0, amsgrad=False, *, foreach=None,
+                 maximize=False, capturable=False, differentiable=False, fused=None, decoupled_weight_decay=False):
+        if isinstance(lr, torch.Tensor) or any(isinstance(b, torch.Tensor) for b in betas):
+            raise ValueError("qagnn_b200.optim.Adam: a Tensor lr or betas is not implemented on the device; use "
+                             "torch.optim.Adam for it")
+        # torch's checks and messages
+        if not 0.0 <= lr:
+            raise ValueError(f"Invalid learning rate: {lr}")
+        if not 0.0 <= eps:
+            raise ValueError(f"Invalid epsilon value: {eps}")
+        if not 0.0 <= betas[0] < 1.0:
+            raise ValueError(f"Invalid beta parameter at index 0: {betas[0]}")
+        if not 0.0 <= betas[1] < 1.0:
+            raise ValueError(f"Invalid beta parameter at index 1: {betas[1]}")
+        if not 0.0 <= weight_decay:
+            raise ValueError(f"Invalid weight_decay value: {weight_decay}")
+        if not (isinstance(betas[0], float) and isinstance(betas[1], float)):
+            raise ValueError("betas must be either both floats or both Tensors")
+        defaults = dict(lr=lr, betas=tuple(betas), eps=eps, weight_decay=weight_decay, amsgrad=amsgrad, maximize=maximize,
+                        foreach=foreach, capturable=capturable, differentiable=differentiable, fused=fused,
+                        decoupled_weight_decay=decoupled_weight_decay)
+        self._check_group(defaults)
+        super().__init__(params, defaults)
+
+    def _check_group(self, group):
+        _refuse("Adam", [(k, group.get(k)) for k in ("amsgrad", "maximize", "decoupled_weight_decay", "foreach", "fused",
+                                                      "capturable", "differentiable")])
+        _check_hyper(group["lr"], group["betas"], group["eps"])
+
+    def _rule_flags(self):
+        return [0] * len(self.param_groups)
+
+
+class SGD(_DeviceStepOptimizer):
+    """SGD(params, lr=1e-3, momentum=0, dampening=0, weight_decay=0, nesterov=False, *, maximize=False, foreach=None,
+    differentiable=False, fused=None): torch.optim.SGD, the reference's `--optim sgd`, stepped on the GPU (qagnn_sgd_step)
+    bit for bit as torch 2.11 steps it by default on CUDA (its foreach implementation).  The constructor, defaults, checks and
+    param-group keys are torch's; maximize, fused and differentiable set to True are refused (torch.optim.SGD has them).  With
+    momentum the state keeps torch's `momentum_buffer`, allocated as zeros, plus `step`, an int64 0-dim tensor on the
+    parameter's device: the buffer is set from the gradient where the device step is 0, so a first step that GradScaler
+    skips on the device is handled as torch handles it.  `load_state_dict` takes torch's own state dict (a buffer counts as
+    set).  Parameters and their gradients must be contiguous fp32 CUDA tensors; a parameter whose `.grad` is None is
+    skipped."""
+
+    _entry = "qagnn_sgd_step"
+    _rule = 3
+    _state_keys = ("momentum_buffer",)
+    _sparse_message = "qagnn_b200.optim.SGD does not support sparse gradients; use torch.optim.SGD for them"
+
+    def __init__(self, params, lr=1e-3, momentum=0, dampening=0, weight_decay=0, nesterov=False, *, maximize=False,
+                 foreach=None, differentiable=False, fused=None):
+        if isinstance(lr, torch.Tensor):
+            raise ValueError("qagnn_b200.optim.SGD: a Tensor lr is not implemented on the device; use torch.optim.SGD for it")
+        # torch's checks and messages
+        if lr < 0.0:
+            raise ValueError(f"Invalid learning rate: {lr}")
+        if momentum < 0.0:
+            raise ValueError(f"Invalid momentum value: {momentum}")
+        if weight_decay < 0.0:
+            raise ValueError(f"Invalid weight_decay value: {weight_decay}")
+        defaults = dict(lr=lr, momentum=momentum, dampening=dampening, weight_decay=weight_decay, nesterov=nesterov,
+                        maximize=maximize, foreach=foreach, differentiable=differentiable, fused=fused)
+        if nesterov and (momentum <= 0 or dampening != 0):
+            raise ValueError("Nesterov momentum requires a momentum and zero dampening")
+        self._check_group(defaults)
+        super().__init__(params, defaults)
+
+    @staticmethod
+    def _hyper(group):
+        # qagnn_sgd_step's beta1 and beta2 are the momentum and the dampening
+        return float(group["lr"]), float(group["weight_decay"]), float(group["momentum"]), float(group["dampening"]), 0.0
+
+    def _check_group(self, group):
+        _refuse("SGD", [(k, group.get(k)) for k in ("maximize", "fused", "differentiable")])
+        if not 0.0 <= group["lr"]:
+            raise ValueError(f"Invalid learning rate: {group['lr']}")
+        if not 0.0 <= group["momentum"] < math.inf:
+            raise ValueError(f"Invalid momentum value: {group['momentum']}")
+
+    def _rule_flags(self):
+        return [int(bool(g["nesterov"])) for g in self.param_groups]
+
+    def _state_for(self, p, group):
+        st = self.state[p]
+        if "step" not in st:
+            st["step"] = torch.zeros((), dtype=torch.int64, device=p.device)
+        if group["momentum"] != 0 and st.get("momentum_buffer") is None:
+            st["momentum_buffer"] = torch.zeros_like(p, memory_format=torch.contiguous_format)
+            st["step"].zero_()  # a fresh buffer is set from the next gradient, as torch sets a missing one
+        return st
+
+    def _state_tensors(self, st):
+        return st.get("momentum_buffer"), None
+
+    def _missing_step(self, st):
+        # torch's SGD keeps no step: a buffer it saved has been set
+        return 0 if st.get("momentum_buffer") is None else 1
 
 
 _clip_workspace = {}  # device -> [fp64 slots, int32 arrival counter, fp32 clip coefficient]
@@ -333,7 +498,7 @@ class CapturedTail:
     state, `.grad`, the norm and the scaler's scale and growth tracker, in two sm_90a launches (two more per 512 tensors or
     16 groups) and with no host read.  It returns the norm as a new 0-dim device tensor, or None when max_grad_norm <= 0.
 
-    `optimizer` is a `RAdam` or an `AdamW`; `scaler` a `torch.amp.GradScaler` or None (a disabled one counts as None);
+    `optimizer` is a `RAdam`, `AdamW`, `Adam` or `SGD`; `scaler` a `torch.amp.GradScaler` or None (a disabled one counts as None);
     `scheduler` any LR scheduler or None.  `clip_parameters` defaults to the optimizer's parameters; those with a `.grad` must
     be the optimizer's parameters with a `.grad`, in any order.  Every call first steps the scheduler on the host, then
     writes what a replay must not freeze (each group's hyperparameters, the step tables, max_grad_norm and the scaler's
@@ -345,9 +510,9 @@ class CapturedTail:
     must be dense, contiguous fp32 tensors on one CUDA device, as for the optimiser."""
 
     def __init__(self, optimizer, scaler=None, scheduler=None, max_grad_norm=0.0, clip_parameters=None):
-        if not isinstance(optimizer, (RAdam, AdamW)):
+        if not isinstance(optimizer, (RAdam, AdamW, Adam, SGD)):
             raise ValueError(f"qagnn_b200.optim.CapturedTail: {type(optimizer).__module__}.{type(optimizer).__name__} is not "
-                             f"qagnn_b200.optim.RAdam or AdamW; run the eager tail (scaler.unscale_, clip_grad_norm_, "
+                             f"qagnn_b200.optim.RAdam, AdamW, Adam or SGD; run the eager tail (scaler.unscale_, clip_grad_norm_, "
                              f"scheduler.step, scaler.step, scaler.update) for it")
         if scaler is not None and not scaler.is_enabled():
             scaler = None
@@ -356,7 +521,7 @@ class CapturedTail:
         if isinstance(clip_parameters, torch.Tensor):
             clip_parameters = [clip_parameters]
         self._clip_parameters = None if clip_parameters is None else list(clip_parameters)
-        self._rule = 0 if isinstance(optimizer, RAdam) else 1  # QAGNN_RULE_*
+        self._rule = optimizer._rule
         self.captures = 0
         self._key = None
         self._graph = None
@@ -418,19 +583,20 @@ class CapturedTail:
         clip = self.max_grad_norm > 0
         scale, tracker = self._scaler_tensors(device)
         norm_grads = self._norm_grads(items) if clip else [p.grad for _, p in items]
-        states = [opt._state_for(p) for _, p in items]
+        states = [opt._state_for(p, opt.param_groups[gi]) for gi, p in items]
+        moments = [opt._state_tensors(st) for st in states]
+        addr = lambda t: None if t is None else t.data_ptr()  # noqa: E731
         key = (device, clip, None if scale is None else (scale.data_ptr(), tracker.data_ptr()), len(opt.param_groups),
-               tuple((gi, p.data_ptr(), p.grad.data_ptr(), s["exp_avg"].data_ptr(), s["exp_avg_sq"].data_ptr(),
-                      s["step"].data_ptr(), p.numel()) for (gi, p), s in zip(items, states)),
+               tuple((gi, p.data_ptr(), p.grad.data_ptr(), addr(m), addr(v), s["step"].data_ptr(), p.numel())
+                     for (gi, p), s, (m, v) in zip(items, states, moments)),
                tuple((g.data_ptr(), g.numel()) for g in norm_grads))
 
         if self.scheduler is not None:
             self.scheduler.step()
         opt._host_steps += 1
         lib = _lib.load()
-        hyper = [(float(g["lr"]), float(g["weight_decay"]), float(g["betas"][0]), float(g["betas"][1]), float(g["eps"]))
-                 for g in opt.param_groups]
-        tables = [opt._table(device, h[2], h[3]) for h in hyper]
+        hyper = [opt._hyper(g) for g in opt.param_groups]
+        tables, table_len = opt._group_tables(device, hyper, range(len(hyper)))
         arr = lambda ct, vals: (ct * len(vals))(*vals)  # noqa: E731
         lr, wd, b1, b2, eps = (arr(C.c_double, col) for col in zip(*hyper))
         n_groups = len(hyper)
@@ -443,7 +609,7 @@ class CapturedTail:
         sc = self.scaler
         _lib.check(lib.qagnn_step_tail_fill(
             self._rule, n_groups, lr, wd, b1, b2, eps, arr(C.c_int32, opt._rule_flags()),
-            arr(C.c_void_p, [t.data_ptr() for t in tables]), min(t.shape[0] for t in tables), self.max_grad_norm,
+            arr(C.c_void_p, [None if t is None else t.data_ptr() for t in tables]), table_len, self.max_grad_norm,
             float(sc._growth_factor) if sc else 2.0, float(sc._backoff_factor) if sc else 0.5,
             int(sc._growth_interval) if sc else 1, C.c_void_p(staging.data_ptr()), n_bytes), "qagnn_step_tail_fill")
         bufs["block"].copy_(staging, non_blocking=True)
@@ -452,7 +618,7 @@ class CapturedTail:
         else:
             # this call's step runs directly, which also loads the kernels; the capture then records the same launches
             self._graph = None
-            launch = self._launcher(lib, device, items, states, norm_grads, clip, scale, tracker, n_groups)
+            launch = self._launcher(lib, device, items, states, moments, norm_grads, clip, scale, tracker, n_groups)
             launch()
             graph = torch.cuda.CUDAGraph()
             with torch.cuda.graph(graph):
@@ -470,12 +636,12 @@ class CapturedTail:
                     counter=z(torch.int32), found_inf=z(torch.float32), coef=z(torch.float32),
                     total_norm=torch.zeros((), dtype=torch.float32, device=device))
 
-    def _launcher(self, lib, device, items, states, norm_grads, clip, scale, tracker, n_groups):
+    def _launcher(self, lib, device, items, states, moments, norm_grads, clip, scale, tracker, n_groups):
         arr = lambda ct, vals: (ct * len(vals))(*vals)  # noqa: E731
-        ptrs = lambda ts: arr(C.c_void_p, [t.data_ptr() for t in ts])  # noqa: E731
+        ptrs = lambda ts: arr(C.c_void_p, [None if t is None else t.data_ptr() for t in ts])  # noqa: E731
         n, nn, b = len(items), len(norm_grads), self._bufs
         args = (self._rule, n, ptrs([p for _, p in items]), ptrs([p.grad for _, p in items]),
-                ptrs([s["exp_avg"] for s in states]), ptrs([s["exp_avg_sq"] for s in states]), ptrs([s["step"] for s in states]),
+                ptrs([m for m, _ in moments]), ptrs([v for _, v in moments]), ptrs([s["step"] for s in states]),
                 arr(C.c_int64, [p.numel() for _, p in items]), arr(C.c_int32, [gi for gi, _ in items]), n_groups,
                 nn, ptrs(norm_grads), arr(C.c_int64, [g.numel() for g in norm_grads]), int(clip), _lib.ptr(b["block"]),
                 _lib.ptr(b["slots"]), b["slots"].numel(), _lib.ptr(b["counter"]), _lib.ptr(b["total_norm"]),
@@ -489,10 +655,19 @@ class CapturedTail:
 
 # The reference's --optim table (utils/optimization_utils.py).  'sgd' and 'adam' are torch's own classes, as the reference
 # imports them: they do not declare `_step_supports_amp_scaling`, so under GradScaler `scaler.step` still reads found_inf on
-# the host for them.
+# the host for them, and CapturedTail refuses them.
 OPTIMIZER_CLASSES = {
     "sgd": torch.optim.SGD,
     "adam": torch.optim.Adam,
+    "adamw": AdamW,
+    "radam": RAdam,
+}
+
+# The same table stepped on the device throughout: this module's Adam and SGD step as torch's do, bit for bit, take
+# GradScaler's inf skip on the device and run in CapturedTail.
+DEVICE_OPTIMIZER_CLASSES = {
+    "sgd": SGD,
+    "adam": Adam,
     "adamw": AdamW,
     "radam": RAdam,
 }

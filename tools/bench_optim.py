@@ -11,6 +11,12 @@
   torch_adamw  torch.optim.AdamW(foreach=True): a speed yardstick only, since it is not the same update
   qagnn        qagnn_b200.optim.AdamW
 
+--optim adam / --optim sgd (as the reference constructs them: torch's defaults, SGD without momentum):
+
+  torch_adam / torch_sgd  torch.optim.Adam / SGD(foreach=True), torch's default CUDA step; GradScaler.step reads found_inf
+                          on the host before it calls step()
+  qagnn                   qagnn_b200.optim.Adam / SGD: the same update bit for bit in one launch per device
+
 Cases:
   1. tail     the recipes' fp16 optimiser tail (unscale_, clip_grad_norm_(1.0), scaler.step, scaler.update) over the
               decoder's trainable tensors (k = 5, D = 200, sent_dim 1024): wall ms (ending in a synchronise), host ms (the
@@ -30,6 +36,7 @@ Medians with the spread (min, max) over --reps alternated repetitions.  Everythi
     python tools/bench_optim.py --out profiles/h100_optim.jsonl
     python tools/bench_optim.py --optim adamw --cases tail encoder --out profiles/h100_optim_adamw.jsonl
     python tools/bench_optim.py --cases clip clip_tail --out profiles/h100_clip.jsonl
+    python tools/bench_optim.py --optim adam --cases tail encoder --out profiles/h100_optim_adam.jsonl
 """
 import argparse
 import json
@@ -52,13 +59,19 @@ from tests.adamw_oracle import AdamWOracle  # noqa: E402
 from tests.radam_oracle import RAdamOracle  # noqa: E402
 
 NO_DECAY = ("bias", "LayerNorm.bias", "LayerNorm.weight")
-ROUTES = {"radam": ("oracle", "torch_radam", "qagnn"), "adamw": ("oracle", "torch_adamw", "qagnn")}
+ROUTES = {"radam": ("oracle", "torch_radam", "qagnn"), "adamw": ("oracle", "torch_adamw", "qagnn"),
+          "adam": ("torch_adam", "qagnn"), "sgd": ("torch_sgd", "qagnn")}
+STEP_BYTES = {"radam": 28, "adamw": 28, "adam": 28, "sgd": 12}  # per parameter: p, g, m, v read, p, m, v written; SGD p, g, p
 HBM_TBS = 3.35  # H100 SXM data-sheet HBM3 bandwidth
 
 
 def make_opt(optim, route, groups):
-    from qagnn_b200.optim import AdamW, RAdam
+    from qagnn_b200.optim import DEVICE_OPTIMIZER_CLASSES, AdamW, RAdam
     route = "qagnn" if route == "qagnn_clip" else route
+    if optim in ("adam", "sgd"):
+        if route == "qagnn":
+            return DEVICE_OPTIMIZER_CLASSES[optim](groups)
+        return (torch.optim.Adam if optim == "adam" else torch.optim.SGD)(groups, foreach=True)
     if optim == "adamw":
         if route == "oracle":
             return AdamWOracle(groups)
@@ -201,8 +214,9 @@ def case_encoder(dec, dev, reps, optim):
                 "step_ms": stats(ms[route])}
         if route == "qagnn":
             line["kernel_ms"] = stats([u * 1e-3 for u in kernel_us])
-            line["hbm_fraction"] = 28 * n_params / (line["kernel_ms"]["median"] * 1e-3) / (HBM_TBS * 1e12)
-            line["datasheet_ms"] = 28 * n_params / (HBM_TBS * 1e12) * 1e3
+            nb = STEP_BYTES[optim]
+            line["hbm_fraction"] = nb * n_params / (line["kernel_ms"]["median"] * 1e-3) / (HBM_TBS * 1e12)
+            line["datasheet_ms"] = nb * n_params / (HBM_TBS * 1e12) * 1e3
         out.append(line)
     del opts
     torch.cuda.empty_cache()

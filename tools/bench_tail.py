@@ -1,4 +1,5 @@
-"""Times the recipe's optimiser tail two ways, alternated in one process, with --optim radam (the default) or adamw:
+"""Times the recipe's optimiser tail two ways, alternated in one process, with --optim radam (the default), adamw, adam or
+sgd (qagnn_b200.optim.DEVICE_OPTIMIZER_CLASSES, constructed as the reference constructs them):
 
   eager     scaler.unscale_(opt); qagnn_b200.optim.clip_grad_norm_(params, max_norm); scheduler.step(); scaler.step(opt);
             scaler.update(), with qagnn_b200.optim's optimiser
@@ -16,6 +17,7 @@ the bytes each route moves per parameter (traffic()).  Medians with the spread (
 
     python tools/bench_tail.py --out profiles/h100_tail.jsonl
     python tools/bench_tail.py --optim adamw --out profiles/h100_tail.jsonl --append
+    python tools/bench_tail.py --optim sgd --cases decoder encoder --out profiles/h100_optim_sgd.jsonl --append
 """
 import argparse
 import json
@@ -38,16 +40,17 @@ from bench_stream_split import gpu_info  # noqa: E402
 ROUTES = ("eager", "captured")
 
 
-def traffic(route, clip, scaler):
-    """Compulsory bytes per fp32 parameter of one tail, from shapes alone.  eager: unscale_ reads and writes g (8), the
-    clip reads g for the norm (4) and reads and writes it to scale it (8), the step reads g, p, m, v and writes p, m, v (28)
-    or, when it unscales, g too (32).  captured: pass 1 reads g (4, when it runs), pass 2 reads p, g, m, v and writes them
-    back (32) whenever it unscales or clips, else p, m, v (28)."""
+def traffic(route, clip, scaler, optim="radam"):
+    """Compulsory bytes per fp32 parameter of one tail, from shapes alone.  The step alone reads g, p, m, v and writes p, m,
+    v (28; SGD without momentum reads g, p and writes p: 12).  eager: unscale_ reads and writes g (8), the clip reads g for
+    the norm (4) and reads and writes it to scale it (8), then the step, which also writes g (4) when it unscales.
+    captured: pass 1 reads g (4, when it runs), pass 2 is the step and writes g back (4) whenever it unscales or clips."""
+    step = 12 if optim == "sgd" else 28
     if route == "eager":
         if clip:
-            return (8 if scaler else 0) + 4 + 8 + 28
-        return 32 if scaler else 28
-    return (4 if clip or scaler else 0) + (32 if clip or scaler else 28)
+            return (8 if scaler else 0) + 4 + 8 + step
+        return step + 4 if scaler else step
+    return (4 if clip or scaler else 0) + (step + 4 if clip or scaler else step)
 
 
 class Run:
@@ -55,7 +58,7 @@ class Run:
         from qagnn_b200 import optim as O
         self.ps = [torch.nn.Parameter(p.detach().clone()) for _, p in named]
         groups = recipe_groups(list(zip([n for n, _ in named], self.ps)), 1e-3)
-        self.opt = (O.RAdam if optim == "radam" else O.AdamW)(groups)
+        self.opt = O.DEVICE_OPTIMIZER_CLASSES[optim](groups)
         self.scaler = torch.amp.GradScaler("cuda")
         self.scaler.scale(torch.ones((), device=dev))
         self.sched = torch.optim.lr_scheduler.LambdaLR(self.opt, lambda s: min(1.0, (s + 1) / 100))
@@ -115,7 +118,7 @@ def case_set(name, named, dev, reps, optim, clipping):
         load(r)
         launches, syncs = profile_counts(runs[r])
         k = stats(kern[r])
-        nbytes = traffic(r, max_norm > 0, True)
+        nbytes = traffic(r, max_norm > 0, True, optim)
         out.append({"case": name, "route": r, "max_norm": clipping, "tensors": len(named), "params": n_params,
                     "wall_ms": stats(wall[r]), "host_ms": stats(host[r]), "launches": launches, "syncs": syncs,
                     "kernel_ms": k, "bytes_per_param": nbytes,
@@ -147,7 +150,7 @@ def case_batch(dev, reps, seed, optim):
         run = Run(optim, r, named, 1.0, dev)
         run.ps = [p for _, p in named]  # train the decoder's own parameters
         from qagnn_b200 import optim as O
-        run.opt = (O.RAdam if optim == "radam" else O.AdamW)(recipe_groups(named, 1e-3))
+        run.opt = O.DEVICE_OPTIMIZER_CLASSES[optim](recipe_groups(named, 1e-3))
         run.sched = torch.optim.lr_scheduler.LambdaLR(run.opt, lambda s: min(1.0, (s + 1) / 100))
         if r == "captured":
             run.tail = O.CapturedTail(run.opt, run.scaler, run.sched, 1.0, run.ps)
@@ -183,7 +186,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=30)
     ap.add_argument("--seed", type=int, default=0)
-    ap.add_argument("--optim", choices=("radam", "adamw"), default="radam")
+    ap.add_argument("--optim", choices=("radam", "adamw", "adam", "sgd"), default="radam")
     ap.add_argument("--cases", nargs="+", default=["decoder", "encoder", "batch"])
     ap.add_argument("--out", default=None)
     ap.add_argument("--append", action="store_true")
