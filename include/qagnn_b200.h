@@ -515,6 +515,24 @@ int32_t qagnn_step_tail(int32_t rule, int32_t n_tensors, void *const *params, vo
 int32_t qagnn_ordered_grad_sum(int32_t n_tensors, void *const *grads, const int64_t *numels, const int64_t *cols,
                                const int32_t *init_from_grad, const float *slots, int64_t ld, int32_t n_valid, void *stream);
 
+/* Keyed dropout (qagnn_b200.training.keyed_dropout): a mask that depends on what is dropped, not on launch order.  x and y are
+ * contiguous `dtype` (QAGNN_DTYPE_*) tensors viewed as [A, G, L]; element (a, g, l) belongs to question qids[g / nc] (device
+ * int64 [G / nc]) and choice g % nc, and has the in-graph index e = a L + l.  Its uniform u is word e & 3 of Philox4x32-10 with
+ * key (seed lo 32, seed hi 32) and counter (e >> 2, site + 256 choice, question id lo 32, *draw lo 32), `draw` a device int64
+ * read by the kernel.  The element is kept when u >= min(floor(p 2^32), 2^32 - 1), computed in fp64 on the host, and never
+ * at p = 1; a kept element is x * (float)(1 / (1 - p)) rounded once to `dtype`, a dropped one 0.  `mask` receives
+ * ceil(A G L / 32) words, bit i of word i / 32 set when flat element i is kept.  p in [0, 1], nc >= 1 dividing G, site in
+ * [0, 255], else QAGNN_ERR_INVALID_ARGUMENT; more than 2^31 elements: QAGNN_ERR_UNSUPPORTED.  One launch, none when empty; no
+ * host synchronisation. */
+int32_t qagnn_keyed_dropout_forward_typed(int32_t dtype, int64_t A, int64_t G, int64_t L, double p, int64_t seed,
+                                          const int64_t *draw, const int64_t *qids, int32_t nc, int32_t site, const void *x,
+                                          void *y, uint32_t *mask, void *stream);
+
+/* The backward of qagnn_keyed_dropout_forward_typed over its n elements: dx = kept ? dy * (float)(1 / (1 - p)) rounded once
+ * to `dtype` : 0, from the forward's `mask` alone. */
+int32_t qagnn_keyed_dropout_backward_typed(int32_t dtype, int64_t n, double p, const uint32_t *mask, const void *dy, void *dx,
+                                           void *stream);
+
 /* Launch counters since load (kernels this library enqueued); for bench.py's gpu_launches. */
 int64_t qagnn_launch_count(void);
 

@@ -119,6 +119,9 @@ EXPORTS = {
     "qagnn_step_tail": (C.c_int32, [C.c_int32, C.c_int32, _P, _P, _P, _P, _P, _P, _P, C.c_int32, C.c_int32, _P, _P, C.c_int32, _P,
                                     _P, C.c_int64, _P, _P, _P, _P, _P, _P, _P]),
     "qagnn_ordered_grad_sum":(C.c_int32, [C.c_int32, _P, _P, _P, _P, _P, C.c_int64, C.c_int32, _P]),
+    "qagnn_keyed_dropout_forward_typed": (C.c_int32, [C.c_int32, C.c_int64, C.c_int64, C.c_int64, C.c_double, C.c_int64, _P, _P,
+                                                      C.c_int32, C.c_int32, _P, _P, _P, _P]),
+    "qagnn_keyed_dropout_backward_typed": (C.c_int32, [C.c_int32, C.c_int64, C.c_double, _P, _P, _P, _P]),
     "qagnn_launch_count": (C.c_int64, []),
     "qagnn_profile_enable": (C.c_int32, [C.c_int32]),
     "qagnn_profile_read": (C.c_int32, [C.POINTER(C.c_double), C.POINTER(C.c_int64)]),

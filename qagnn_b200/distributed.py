@@ -13,7 +13,7 @@ import torch
 import torch.distributed as dist
 
 from . import _lib
-from .training import answer_loss
+from .training import answer_loss, keyed_dropout
 
 
 def shard_bounds(n_questions, rank, world_size):
@@ -265,9 +265,12 @@ class DataParallelSplitTrain:
 
     The recipe's tail (GradScaler.unscale_, clip_grad_norm_, the scheduler and optimiser steps) then runs unchanged on every
     rank and takes the same step.  That step is the one-GPU step bit for bit when the encoder is frozen or the clip's norm
-    leaves its gradients out; otherwise the encoder's sums can move the clip coefficient in its last bits.  Each rank seeds its own dropout stream, so with dropout the ranks draw other masks than one
-    GPU would: the run is then the one-GPU run in distribution, not bit for bit.  With one rank (W = 1, no process group) the
-    reduction is the ordered sum of the local rows and nothing else changes.
+    leaves its gradients out; otherwise the encoder's sums can move the clip coefficient in its last bits.  Dropout: with the
+    step's `dropout_key` (training.DropoutKey, the same seed on every rank) every micro-batch, the eager partial one in
+    `loss()` included, draws the masks one GPU draws for its questions, and the above holds at any dropout; advance the key
+    on every rank once per optimiser batch, after the optimiser step.  Without a key each rank seeds its own dropout stream,
+    so the ranks draw other masks than one GPU would: the run is then the one-GPU run in distribution, not bit for bit.  With
+    one rank (W = 1, no process group) the reduction is the ordered sum of the local rows and nothing else changes.
 
     Construction raises ValueError when step.batch_size is not `micro_batch_size`, when `batch_size` is less than it, when a
     full batch would leave a rank without a micro-batch or start a rank's block with the partial micro-batch (every rank
@@ -346,13 +349,15 @@ class DataParallelSplitTrain:
 
     def loss(self, question_ids, sent_vecs):
         """The micro-batch's mean loss: the step's for a full micro-batch, else the eager decoder and answer loss of the
-        same autocast, as the one-GPU loop runs its partial micro-batch."""
+        same autocast and dropout key, as the one-GPU loop runs its partial micro-batch."""
         step = self.step
         if len(question_ids) == step.batch_size:
             return step(question_ids, sent_vecs)
         from .pipeline import _autocast
         q = torch.from_numpy(np.asarray(question_ids, dtype=np.int64)).to(self.split.device)
-        with _autocast(step.autocast_dtype):
+        keyed = (contextlib.nullcontext() if step.dropout_key is None
+                 else keyed_dropout(step.dropout_key, q, self.split.num_choice))
+        with _autocast(step.autocast_dtype), keyed:
             logits, _ = step.decoder(sent_vecs, *self.split.batch(question_ids, step.edge_capacity))
             return answer_loss(logits, self.split.labels[q], self.split.num_choice, step.loss)
 

@@ -12,6 +12,8 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
+from . import training as _training
+
 
 # node-feature dtypes the fused pooling kernels read: fp32, and bf16 (the eval forward's output under bf16 autocast)
 _POOL_X_DTYPES = (torch.float32, torch.bfloat16)
@@ -55,7 +57,10 @@ class MLP(nn.Module):
             self.layers[-1].bias.data.zero_()
 
     def forward(self, x):
-        return self.layers(x)
+        for name, m in self.layers.named_children():  # block i's Dropout is keyed dropout site SITE_MLP + i
+            x = (_training.dropout(x, m.p, m.training, _training.SITE_MLP + int(name.split("-")[0]))
+                 if isinstance(m, nn.Dropout) else m(x))
+        return x
 
 
 class MultiheadAttPoolLayer(nn.Module):
@@ -163,9 +168,11 @@ class MultiheadAttPoolLayer(nn.Module):
         logits = torch.einsum("bhd,blhd->hbl", qs, ks) / self.temperature
         if mask is not None:
             logits = logits.masked_fill(mask.unsqueeze(0), float("-inf"))
-        attn = self.attn_dropout(torch.softmax(logits, dim=2))
+        attn = _training.dropout(torch.softmax(logits, dim=2), self.attn_dropout.p, self.attn_dropout.training,
+                                 _training.SITE_POOL_ATTN, graph_dim=1)
         pooled = torch.einsum("hbl,blhd->bhd", attn, vs).reshape(b, nh * dv)
-        return self.dropout(pooled), attn.reshape(nh * b, l)
+        return (_training.dropout(pooled, self.dropout.p, self.dropout.training, _training.SITE_POOL_OUT),
+                attn.reshape(nh * b, l))
 
 
 class _RaggedPoolConcat(torch.autograd.Function):

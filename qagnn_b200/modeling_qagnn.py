@@ -23,6 +23,7 @@ import torch
 import torch.nn as nn
 
 from . import _lib
+from . import training as TR
 from .layers import GELU, MLP, CustomizedEmbedding, MultiheadAttPoolLayer
 
 # head counts GATConvE accepts: every message-passing path (tiled, column-sliced, basic CSR, training backward) runs them
@@ -365,7 +366,6 @@ class GATConvE(nn.Module):
         if getattr(edge_index, "ragged", False):
             _refuse_ragged_training(self, "GATConvE")
         if _wants_autograd(self, x, node_feature_extra):  # autograd through the CUDA message passing, this module's mode
-            from . import training as TR
             if prep is None:
                 prep = self._prep(edge_index, edge_type, node_type)
             tab = TR.edge_table(self.edge_encoder, TR.combo_onehot_table(self.n_ntype, self.n_etype, x.device), prep, 1)
@@ -518,7 +518,6 @@ class QAGNN_Message_Passing(nn.Module):
             status.check("QAGNN_Message_Passing")
         self._replayed = [s for s in self._replayed if s.pending is not None]
         if _wants_autograd(self, H, node_score):  # autograd through the CUDA message passing, this module's mode (training.py)
-            from . import training as TR
             if prep is None:  # a PackedAdj (possibly at an edge capacity) gets the packed prep, a plain pair the general one
                 n = H.size(1) if getattr(A, "graph_ptr_dev", None) is not None else 0
                 prep = graph_prep(A, node_type, n, self.n_ntype, self.n_etype, self.check_indices)
@@ -680,8 +679,10 @@ class QAGNN(nn.Module):
             gnn_input, s = self._head(sent_vecs, concept_ids, node_type_ids, node_scores, adj_lengths, emb_data)
 
         gnn_output = self.gnn(gnn_input, adj, node_type_ids, s)
+        fc_in = self.dropout_fc
         concat, pool_attn = decoder_tail(self.pooler, sent_vecs, gnn_output, node_type_ids, adj_lengths,
-                                         fused=not self.training, dropout=self.dropout_fc)
+                                         fused=not self.training,
+                                         dropout=lambda c: TR.dropout(c, fc_in.p, fc_in.training, TR.SITE_FC_IN))
         if cache_output:
             self.concept_ids, self.adj, self.pool_attn = concept_ids, adj, pool_attn
         return concat, pool_attn
@@ -691,7 +692,8 @@ class QAGNN(nn.Module):
         n = node_scores.size(1)
         gnn_input0 = self.activation(self.svec2nvec(sent_vecs)).unsqueeze(1)
         gnn_input1 = self.concept_emb(concept_ids[:, 1:] - 1, emb_data).to(node_type_ids.device)
-        gnn_input = self.dropout_e(torch.cat([gnn_input0, gnn_input1], dim=1))
+        gnn_input = TR.dropout(torch.cat([gnn_input0, gnn_input1], dim=1), self.dropout_e.p, self.dropout_e.training,
+                               TR.SITE_EMB)
         valid = (torch.arange(n, device=node_scores.device) < adj_lengths.unsqueeze(1)).float()
         s = -node_scores
         s = (s - s[:, 0:1, :]).squeeze(2) * valid

@@ -33,7 +33,7 @@ import torch
 from . import distributed as _dist
 from .data import PackedAdj
 from .modeling_qagnn import _version_key, decoder_tail
-from .training import answer_loss, check_answer_loss
+from .training import answer_loss, check_answer_loss, keyed_dropout
 
 _EVAL_AUTOCAST = (None, torch.bfloat16)
 _TRAIN_AUTOCAST = (None, torch.float16, torch.bfloat16)
@@ -704,6 +704,10 @@ class SplitTrainStep(_TrainingGraphs, _SplitBatches):
 
     The first call captures, on its own batch: the warm-up that precedes the capture restores BatchNorm buffers, `.grad` and
     the CUDA RNG state.  Dropout draws a new mask on every replay and BatchNorm running statistics advance on every replay.
+    With `dropout_key` (training.DropoutKey) the masks are keyed instead: a pure function of the key's seed and draw, the
+    question, its choice, the dropout site and the element, read on the device at every replay.  Advance the key once per
+    optimiser batch, after the optimiser step, and run the final partial micro-batch under training.keyed_dropout with the
+    same key; the loop is then reproducible bit for bit, and SplitTrainBatch and DataParallelSplitTrain with that key equal it.
     Optimiser steps and load_state_dict keep the parameters' addresses, so the graphs stay valid; a call raises RuntimeError
     after `.to()` / `.cuda()`, after torch.use_deterministic_algorithms changed, after a change in which decoder parameters
     require grad, and in .eval() (build a new SplitTrainStep).  Every call needs exactly `batch_size` questions: run a final
@@ -711,12 +715,18 @@ class SplitTrainStep(_TrainingGraphs, _SplitBatches):
 
     what, unit = "SplitTrainStep", "micro-batch"
 
-    def __init__(self, decoder, split, batch_size, *, edge_capacity, max_edges, autocast_dtype=None, loss="cross_entropy"):
+    def __init__(self, decoder, split, batch_size, *, edge_capacity, max_edges, autocast_dtype=None, loss="cross_entropy",
+                 dropout_key=None):
         """`edge_capacity` K bounds the edges of every micro-batch (FlatAdjCache.max_batch_edges(batch_size)), `max_edges` M
-        those of one sub-graph over the split (FlatAdjCache.max_graph_edges()): one capture then serves every micro-batch."""
+        those of one sub-graph over the split (FlatAdjCache.max_graph_edges()): one capture then serves every micro-batch.
+        `dropout_key` (training.DropoutKey on the split's device): the forward graph runs under training.keyed_dropout with
+        the micro-batch's question ids."""
         self._init_training(decoder, autocast_dtype)
         if split.labels is None:
             raise ValueError("SplitTrainStep: the split has no labels; build the DeviceSplit with labels=")
+        if dropout_key is not None and dropout_key.device != torch.device(split.device):
+            raise ValueError(f"{self.what}: the dropout key is on {dropout_key.device}, the split on {split.device}")
+        self.dropout_key = dropout_key
         check_answer_loss(loss, split.num_choice)
         self.loss = loss
         largest = int(split.counts.max()) if split.counts.size else 0
@@ -737,8 +747,14 @@ class SplitTrainStep(_TrainingGraphs, _SplitBatches):
             raise ValueError(f"{self.what}: sent_vecs is {tuple(sent_vecs.shape)} {sent_vecs.dtype}, the step was built "
                              f"for {tuple(self._sv.shape)} {self._sv.dtype}")
 
+    def _keyed(self):
+        """training.keyed_dropout over the step's question ids, or nothing without a key."""
+        if self.dropout_key is None:
+            return contextlib.nullcontext()
+        return keyed_dropout(self.dropout_key, self._qids, self.split.num_choice)
+
     def _forward(self):
-        with _autocast(self.autocast_dtype):
+        with _autocast(self.autocast_dtype), self._keyed():
             out = self._assemble()
             torch.index_select(self.split.labels, 0, self._qids, out=self._labels)
             logits, pool_attn = self._decode(out)
@@ -828,7 +844,7 @@ class _TrainBranch(SplitTrainStep):
 
     def __init__(self, tb, index):
         super().__init__(tb.decoder, tb.split, tb.batch_size, edge_capacity=tb.edge_capacity, max_edges=tb.max_edges,
-                         autocast_dtype=tb.autocast_dtype, loss=tb.loss)
+                         autocast_dtype=tb.autocast_dtype, loss=tb.loss, dropout_key=tb.dropout_key)
         # no reference back to `tb`: a cycle would leave its graphs to the garbage collector, which may then destroy
         # them while another capture is in progress and invalidate it
         self.index = index
@@ -890,14 +906,16 @@ class SplitTrainBatch(_TrainingGraphs):
     """The micro-steps of an optimiser batch on a split held on the GPU (qagnn_b200.data.DeviceSplit built with `labels`), up
     to `branches` of them at a time on one GPU, equal to the plain SplitTrainStep loop:
 
+        key = training.DropoutKey(seed, device)            # optional: dropout masks keyed to the questions
         tb = SplitTrainBatch(model.decoder.train(), split, mbs, branches=8, edge_capacity=K, max_edges=M,
-                             autocast_dtype=torch.float16, loss=args.loss)
+                             autocast_dtype=torch.float16, loss=args.loss, dropout_key=key)
         optimizer.zero_grad()
         for chunk in tb.chunks(batch):                     # lists of <= branches full micro-batches (host ids), in order
             svs = [model.encoder(*lm_inputs_of(q))[0] for q in chunk]
             losses = tb(chunk, svs)                        # [len(chunk)] fp32: each micro-batch's mean loss
             scaler.scale((losses * weights).sum()).backward()     # weights[j] = len(chunk[j]) / len(batch)
-        # a final partial micro-batch runs eagerly, as with SplitTrainStep
+        # a final partial micro-batch runs eagerly, as with SplitTrainStep (under training.keyed_dropout with the key)
+        # ... the optimiser tail, then key.advance_()
 
     A branch is one micro-step: a SplitTrainStep's two graphs (assembly, label gather, `decoder(...)` in .train() and
     training.answer_loss; torch.autograd.grad), with its own static buffers, graph pool and stream.  Every branch is
@@ -912,7 +930,7 @@ class SplitTrainBatch(_TrainingGraphs):
 
     Contracts, as for DataParallelSplitTrain:
     - the losses, logits, dL/dsent_vecs and every decoder `.grad` equal the plain SplitTrainStep loop's bit for bit under
-      torch.use_deterministic_algorithms(True) with dropout 0, and so do the parameters after the optimiser step: BatchNorm
+      torch.use_deterministic_algorithms(True) with dropout 0 or a dropout key, and so do the parameters after the optimiser step: BatchNorm
       uses batch statistics in training, so its running statistics do not feed back within a batch.  `.grad` becomes a view
       of a batch-owned buffer when it was None, as SplitTrainStep's becomes a step-owned one;
     - BatchNorm running statistics: each branch's graphs update branch-owned copies of the decoder's BatchNorm buffers (the
@@ -920,13 +938,17 @@ class SplitTrainBatch(_TrainingGraphs):
       chunk's forward the copies are folded into the live buffers in micro-batch order by distributed.fold_running_stats, in
       fp64 rounded once to fp32, and num_batches_tracked advances by the exact count.  The loop rounds after every update, so
       the statistics agree with it to within the rounding of the updates, not bit for bit;
-    - dropout: each branch draws from a CUDA generator state of its own, seeded at capture from torch's CPU generator, so
-      branches never share a mask and never race on the generator's device-side offset.  With dropout the run is the plain
-      loop in distribution, not bit for bit.  Reseeding torch afterwards does not reseed the branches.
+    - dropout with `dropout_key` (training.DropoutKey): every branch's forward graph runs under training.keyed_dropout with
+      its micro-batch's question ids, so a question draws the masks it draws in the keyed SplitTrainStep loop whatever its
+      branch, stream or chunk, and the contracts above hold bit for bit at any dropout.  Advance the key once per optimiser
+      batch, after the optimiser step, and run the final partial micro-batch under keyed_dropout with the same key;
+    - dropout without a key: each branch draws from a CUDA generator state of its own, seeded at capture from torch's CPU
+      generator, so branches never share a mask and never race on the generator's device-side offset.  The run is then the
+      plain loop in distribution, not bit for bit.  Reseeding torch afterwards does not reseed the branches.
 
     The first call captures every branch, on its own chunk's micro-batches (cycled over the branches past len(chunk)); the
     warm-ups restore the BatchNorm buffers, `.grad` and the CUDA generator state.  Refusals: ValueError at construction for
-    `branches` < 1, a split without labels, an unknown loss, autocast dtype or max_edges SplitTrainStep refuses, a BatchNorm
+    `branches` < 1, a split without labels, a dropout key on another device, an unknown loss, autocast dtype or max_edges SplitTrainStep refuses, a BatchNorm
     with momentum=None (its statistics cannot be folded) and a decoder in .eval(); ValueError at a call, before anything is
     enqueued, for an empty chunk or one of more than `branches` micro-batches, a micro-batch of another size (a partial one
     included), another number of sent_vecs than micro-batches and sent_vecs of another shape or dtype; RuntimeError at a call
@@ -937,11 +959,12 @@ class SplitTrainBatch(_TrainingGraphs):
     what = "SplitTrainBatch"
 
     def __init__(self, decoder, split, batch_size, *, branches=8, edge_capacity, max_edges, autocast_dtype=None,
-                 loss="cross_entropy"):
+                 loss="cross_entropy", dropout_key=None):
         if int(branches) < 1:
             raise ValueError(f"SplitTrainBatch: branches = {int(branches)}; it needs at least 1")
         self._init_training(decoder, autocast_dtype)
         self.split, self.batch_size, self.branches = split, int(batch_size), int(branches)
+        self.dropout_key = dropout_key
         self.edge_capacity, self.max_edges, self.loss = int(edge_capacity), int(max_edges), loss
         self._bn = _dist.BatchNormFold(decoder, self.what, "branches")
         dev = split.device

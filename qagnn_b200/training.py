@@ -19,8 +19,11 @@ BatchNorm of the edge encoder: the reference feeds it one row per edge (E+N rows
 edge's combo, so the batch mean / variance are the combo-histogram-weighted moments of the C distinct rows; the running
 statistics receive the k momentum updates the reference's k calls of the shared module apply.
 """
+import contextlib
 import ctypes as C
 import functools
+import math
+import threading
 
 import torch
 import torch.nn.functional as F
@@ -244,8 +247,132 @@ def mp_forward_autograd(mod, H, A, node_type, node_score, prep):
     extra = torch.cat([type_emb, score_emb], dim=1)                          # :86
     tab = edge_table(mod.edge_encoder, combo_onehot_table(mod.n_ntype, mod.n_etype, H.device), prep, max(mod.k, 1))
     X = H.reshape(-1, D)
-    for layer in mod.gnn_layers:                                             # mp_helper :45-50
+    if mod.training and keyed_active() and len(mod.gnn_layers) > MAX_GNN_LAYERS:
+        raise ValueError(f"keyed dropout: {len(mod.gnn_layers)} message-passing layers; the site table has room for "
+                         f"{MAX_GNN_LAYERS}")
+    for l, layer in enumerate(mod.gnn_layers):                               # mp_helper :45-50
         X = mod.activation(gatconve_autograd(layer, X, extra, nt, prep, tab))
-        X = F.dropout(X, mod.dropout_rate, training=mod.training)
+        X = dropout(X.view(H.shape), mod.dropout_rate, mod.training, SITE_GNN_LAYER + l).view(-1, D)
     out = mod.activation(mod.Vh(H) + mod.Vx(X.view(H.shape)))                # :92
-    return mod.dropout(out)                                                  # :93
+    return dropout(out, mod.dropout.p, mod.dropout.training, SITE_GNN_OUT)   # :93
+
+
+# ---- keyed dropout ------------------------------------------------------------------------------------------------------
+# Under keyed_dropout, a training-mode dropout site of the decoder draws its mask from (seed, draw, question id, choice,
+# site, element) instead of torch's generator, so a question's masks do not depend on which launches ran before it, on which
+# stream or on which rank.  The site ids are part of the mask definition (DESIGN.md §2b).
+SITE_EMB = 0          # QAGNN.dropout_e on the GNN input [B, n, D]
+SITE_GNN_LAYER = 1    # + l: the dropout after message-passing layer l (l < 31)
+SITE_GNN_OUT = 32     # QAGNN_Message_Passing.dropout on its output [B, n, D]
+SITE_POOL_ATTN = 33   # MultiheadAttPoolLayer.attn_dropout on the attention [n_head, B, n]
+SITE_POOL_OUT = 34    # MultiheadAttPoolLayer.dropout on the pooled [B, n_head d_v]
+SITE_FC_IN = 35       # QAGNN.dropout_fc on the concat [B, 2D + S]
+SITE_MLP = 36         # + i: the Dropout of MLP block i
+MAX_GNN_LAYERS = SITE_GNN_OUT - SITE_GNN_LAYER
+
+_keyed = threading.local()
+
+
+class DropoutKey:
+    """The key of keyed_dropout: a seed (0 <= seed < 2^64) and a device int64 `draw` counter [1] on `device`.  The masks of an
+    optimiser batch are those of (seed, draw): advance the key once per optimiser batch, after the optimiser step.
+    `advance_()` is one in-place add on the device, so it reads nothing on the host and may be captured; read `draw` on the
+    host (int(key.draw)) for logs only.  Every rank of a data-parallel run builds the same key."""
+
+    def __init__(self, seed, device):
+        seed = int(seed)
+        if not 0 <= seed < 2 ** 64:
+            raise ValueError(f"DropoutKey: seed must be in [0, 2^64), got {seed}")
+        device = torch.device(device)
+        if device.type != "cuda":
+            raise ValueError(f"DropoutKey: the key lives on a CUDA device, got {device}")
+        if device.index is None:
+            device = torch.device("cuda", torch.cuda.current_device())
+        self.seed, self.device = seed, device
+        self.draw = torch.zeros(1, dtype=torch.int64, device=device)
+
+    def advance_(self):
+        self.draw.add_(1)
+        return self
+
+
+@contextlib.contextmanager
+def keyed_dropout(key, question_ids, num_choice):
+    """While active, the decoder's training-mode dropout sites draw keyed masks: element e of graph g (choice g % num_choice
+    of question question_ids[g // num_choice], device int64 [B / num_choice]) at site s is kept or dropped by
+    Philox4x32-10 under `key` (qagnn_keyed_dropout_forward_typed).  Outside it, and in .eval(), dropout is torch's."""
+    nc = int(num_choice)
+    if nc < 1:
+        raise ValueError(f"keyed_dropout: num_choice = {nc}")
+    if (not isinstance(question_ids, torch.Tensor) or question_ids.dtype != torch.int64 or question_ids.dim() != 1
+            or question_ids.device != key.device):
+        raise ValueError(f"keyed_dropout: question_ids must be a 1-d int64 tensor on the key's device {key.device}")
+    prev = getattr(_keyed, "ctx", None)
+    _keyed.ctx = (key, question_ids, nc)
+    try:
+        yield
+    finally:
+        _keyed.ctx = prev
+
+
+def keyed_active():
+    """True inside keyed_dropout."""
+    return getattr(_keyed, "ctx", None) is not None
+
+
+def dropout(x, p, training, site, graph_dim=0):
+    """F.dropout(x, p, training); in training under keyed_dropout, the keyed mask of `site` instead.  x's dim `graph_dim` is
+    the graph (0 for [B, ...], 1 for the pooler's [n_head, B, n]); the dims before it are A, those after it L."""
+    ctx = getattr(_keyed, "ctx", None)
+    if ctx is None or not training:
+        return F.dropout(x, p, training)
+    key, qids, nc = ctx
+    p = float(p)
+    if not 0.0 <= p <= 1.0:
+        raise ValueError(f"keyed dropout: p = {p}; it must be in [0, 1]")
+    if not 0 <= site <= 255:
+        raise ValueError(f"keyed dropout: site {site} is outside [0, 255]")
+    if x.device != key.device:
+        raise ValueError(f"keyed dropout: the key is on {key.device}, the batch on {x.device}")
+    G = x.size(graph_dim)
+    if G != qids.numel() * nc:
+        raise ValueError(f"keyed dropout: {qids.numel()} question ids with {nc} choices, the batch has {G} graphs")
+    A = math.prod(x.shape[:graph_dim])
+    return _KeyedDropout.apply(x, key, qids, nc, p, site, A, G)
+
+
+class _KeyedDropout(torch.autograd.Function):
+    """y = keyed dropout of x (qagnn_keyed_dropout_forward_typed); the backward reads only the forward's 1-bit keep mask."""
+
+    @staticmethod
+    def forward(ctx, x, key, qids, nc, p, site, A, G):
+        if x.dtype not in _lib.DTYPE_CODES:
+            raise TypeError(f"keyed dropout: float32, float16 or bfloat16 input, got {x.dtype}")
+        lib = _lib.load()
+        xc = x.detach().contiguous()
+        n = xc.numel()
+        L = n // (A * G) if A * G else 0
+        y = torch.empty_like(xc)
+        mask = torch.empty((n + 31) // 32, dtype=torch.int32, device=x.device)
+        seed = key.seed - 2 ** 64 if key.seed >= 2 ** 63 else key.seed
+        with torch.cuda.device(x.device):
+            st = lib.qagnn_keyed_dropout_forward_typed(_lib.DTYPE_CODES[xc.dtype], A, G, L, p, seed, _lib.ptr(key.draw),
+                                                       _lib.ptr(_lib.i64c(qids, "question_ids")), nc, site, _lib.ptr(xc),
+                                                       _lib.ptr(y), _lib.ptr(mask), _lib.stream_ptr(x.device))
+        _lib.check(st, "qagnn_keyed_dropout_forward_typed")
+        ctx.save_for_backward(mask)
+        ctx.p = p
+        return y
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, dy):
+        lib = _lib.load()
+        (mask,) = ctx.saved_tensors
+        dyc = dy.contiguous()
+        dx = torch.empty_like(dyc)
+        with torch.cuda.device(dy.device):
+            st = lib.qagnn_keyed_dropout_backward_typed(_lib.DTYPE_CODES[dyc.dtype], dyc.numel(), ctx.p, _lib.ptr(mask),
+                                                        _lib.ptr(dyc), _lib.ptr(dx), _lib.stream_ptr(dy.device))
+        _lib.check(st, "qagnn_keyed_dropout_backward_typed")
+        return dx.view(dy.shape), None, None, None, None, None, None, None
