@@ -399,64 +399,46 @@ int32_t qagnn_assemble_batch(const int32_t *src, const int32_t *tgt, const int16
                              const int64_t *question_ids, int32_t bs, int64_t K, int64_t N_cap, int64_t *edges,
                              int64_t *graph_ptr_out, int64_t *node_ptr_out, void *stream);
 
-/* One step of the reference's RAdam (utils/optimization_utils.py) over n_tensors fp32 tensors of the current device, in one
- * launch per 512 tensors or 16 distinct groups (qagnn_b200.optim.RAdam).  Tensor i: contiguous params[i], grads[i], exp_avgs[i],
- * exp_avg_sqs[i] of numels[i] elements, its int64 device step counter steps[i], and its group group_index[i] < n_groups.  The
- * per-group host arrays lr, weight_decay, beta1, beta2, eps and degenerated_to_sgd hold the Python values; each scalar the
- * update uses is rounded to fp32 as torch rounds it.  step_tables[g] is a device fp64 [table_len, 2] table of (1.0 when
- * rho_t >= 5 else 0.0, step size) for t = row, built with the reference's formula for the group's betas; the device step after
- * the increment indexes it, so table_len must exceed every step counter.  found_inf (optional, device fp32): nonzero leaves
- * every tensor and step as it is.  grad_scale (optional, device fp32): the gradients are first multiplied by
- * (float)(1.0 / (double)*grad_scale), as GradScaler.unscale_ does, and written back.  counter: a device int32 that is zero
- * between calls (the kernel resets it).  Every element is the eager torch op sequence's result bit for bit; no host
- * synchronisation. */
-int32_t qagnn_radam_step(int32_t n_tensors, void *const *params, void *const *grads, void *const *exp_avgs,
+/* The optimiser update rules of qagnn_optim_step and the captured tail (qagnn_step_tail_fill, qagnn_step_tail).  Per element,
+ * t = the tensor's step + 1 and each scalar the update uses rounded to fp32 as torch rounds it:
+ *   RADAM: the reference's RAdam (utils/optimization_utils.py; qagnn_b200.optim.RAdam).  step_tables[g] holds (1.0 when
+ *     rho_t >= 5 else 0.0, step size) for t = row, built with the reference's formula for the group's betas; rule_flag is
+ *     degenerated_to_sgd.
+ *   ADAMW: transformers' AdamW (3.4.0, the version the reference pins; qagnn_b200.optim.AdamW), in its order:
+ *     m = b1 m + (1 - b1) g, v = b2 v + (1 - b2) g^2, p -= step_size * m / (sqrt(v) + eps), then, when weight_decay > 0,
+ *     p += (-lr * weight_decay) * p on the new p.  step_size is lr * sqrt(1 - b2^t) / (1 - b1^t) when rule_flag (correct_bias)
+ *     is nonzero, else lr.  step_tables[g] holds (sqrt(1 - b2^t), 1 - b1^t) for t = row in Python doubles; the kernel forms
+ *     the step size from it and lr in IEEE fp64 before rounding it to fp32.
+ *   ADAM: torch.optim.Adam as torch 2.11 steps it by default on CUDA (the foreach implementation; amsgrad, maximize and
+ *     decoupled_weight_decay off; qagnn_b200.optim.Adam); rule_flag is unused.  d = g + weight_decay * p when
+ *     weight_decay != 0 (.grad keeps g), m = lerp(m, d, 1 - b1), v = b2 v + (1 - b2) d^2,
+ *     p += step_size * m / (sqrt(v) / bc2_sqrt + eps), each rounded as torch's kernels round it.  step_tables[g] holds
+ *     ((1 - b2^t) ** 0.5, 1 - b1^t) for t = row in Python doubles; the kernel forms step_size = -(lr / (1 - b1^t)) in IEEE
+ *     fp64 before rounding it to fp32.
+ *   SGD: torch.optim.SGD as torch 2.11 steps it by default on CUDA (the foreach implementation; maximize off;
+ *     qagnn_b200.optim.SGD).  exp_avgs holds the momentum buffers, beta1 is each group's momentum (finite, >= 0), beta2 its
+ *     dampening (finite), rule_flag its nesterov; exp_avg_sqs, eps, step_tables and table_len are unused and may be null / 0.
+ *     A group with momentum 0 keeps no buffer (its exp_avgs[i] may be null).  d = g + weight_decay * p when
+ *     weight_decay != 0, then with momentum buf = d at device step 0, else buf = momentum buf + (1 - dampening) d, and
+ *     d = d + momentum buf (nesterov; written to .grad when weight_decay == 0, as torch does) or buf; then p += -lr d.
+ *     Buffers are zero before their first step.
+ * Every element is the original's result bit for bit. */
+enum { QAGNN_RULE_RADAM = 0, QAGNN_RULE_ADAMW = 1, QAGNN_RULE_ADAM = 2, QAGNN_RULE_SGD = 3 };
+
+/* One step of `rule` (QAGNN_RULE_*) over n_tensors fp32 tensors of the current device, in one launch per 512 tensors or 16
+ * distinct groups (qagnn_b200.optim).  Tensor i: contiguous params[i], grads[i], exp_avgs[i], exp_avg_sqs[i] of numels[i]
+ * elements, its int64 device step counter steps[i], and its group group_index[i] < n_groups.  The per-group host arrays lr,
+ * weight_decay, beta1, beta2, eps and rule_flag hold the Python values.  But for SGD, beta1 and beta2 are in [0, 1) and
+ * step_tables[g] is a device fp64 [table_len, 2] table for the group's betas, indexed by the device step after the increment,
+ * so table_len (>= 2) must exceed every step counter.  found_inf (optional, device fp32): nonzero leaves every tensor and
+ * step as it is.  grad_scale (optional, device fp32): the gradients are first multiplied by (float)(1.0 / (double)*grad_scale),
+ * as GradScaler.unscale_ does, and written back.  counter: a device int32 that is zero between calls (the kernel resets it).
+ * No host synchronisation. */
+int32_t qagnn_optim_step(int32_t rule, int32_t n_tensors, void *const *params, void *const *grads, void *const *exp_avgs,
                          void *const *exp_avg_sqs, void *const *steps, const int64_t *numels, const int32_t *group_index,
                          int32_t n_groups, const double *lr, const double *weight_decay, const double *beta1,
-                         const double *beta2, const double *eps, const int32_t *degenerated_to_sgd,
-                         void *const *step_tables, int64_t table_len, const float *found_inf, const float *grad_scale,
-                         int32_t *counter, void *stream);
-
-/* One step of transformers' AdamW (3.4.0, the version the reference pins; qagnn_b200.optim.AdamW), with the argument layout of
- * qagnn_radam_step.  Per element, in transformers' order: m = b1 m + (1 - b1) g, v = b2 v + (1 - b2) g^2,
- * p -= step_size * m / (sqrt(v) + eps), then, when weight_decay > 0, p += (-lr * weight_decay) * p on the new p.  step_size
- * is lr * sqrt(1 - b2^t) / (1 - b1^t) when correct_bias[g] is nonzero, else lr.  step_tables[g] is a device fp64
- * [table_len, 2] table of (sqrt(1 - b2^t), 1 - b1^t) for t = row, built in Python doubles for the group's betas; the kernel
- * forms the step size from it and lr in IEEE fp64 before rounding it to fp32.  found_inf, grad_scale and counter as for
- * qagnn_radam_step.  Every element is the eager torch op sequence's result bit for bit; no host synchronisation. */
-int32_t qagnn_adamw_step(int32_t n_tensors, void *const *params, void *const *grads, void *const *exp_avgs,
-                         void *const *exp_avg_sqs, void *const *steps, const int64_t *numels, const int32_t *group_index,
-                         int32_t n_groups, const double *lr, const double *weight_decay, const double *beta1,
-                         const double *beta2, const double *eps, const int32_t *correct_bias,
-                         void *const *step_tables, int64_t table_len, const float *found_inf, const float *grad_scale,
-                         int32_t *counter, void *stream);
-
-/* One step of torch.optim.Adam as torch 2.11 steps it by default on CUDA (the foreach implementation; amsgrad, maximize and
- * decoupled_weight_decay off; qagnn_b200.optim.Adam), with the argument layout of qagnn_radam_step; rule_flag is unused.
- * Per element: d = g + weight_decay * p when weight_decay != 0 (.grad keeps g), m = lerp(m, d, 1 - b1),
- * v = b2 v + (1 - b2) d^2, p += step_size * m / (sqrt(v) / bc2_sqrt + eps), each rounded as torch's kernels round it.
- * step_tables[g] is a device fp64 [table_len, 2] table of ((1 - b2^t) ** 0.5, 1 - b1^t) for t = row, in Python doubles;
- * the kernel forms step_size = -(lr / (1 - b1^t)) in IEEE fp64 before rounding it to fp32.  found_inf, grad_scale and
- * counter as for qagnn_radam_step.  Every element is torch's result bit for bit; no host synchronisation. */
-int32_t qagnn_adam_step(int32_t n_tensors, void *const *params, void *const *grads, void *const *exp_avgs,
-                        void *const *exp_avg_sqs, void *const *steps, const int64_t *numels, const int32_t *group_index,
-                        int32_t n_groups, const double *lr, const double *weight_decay, const double *beta1,
-                        const double *beta2, const double *eps, const int32_t *rule_flag, void *const *step_tables,
-                        int64_t table_len, const float *found_inf, const float *grad_scale, int32_t *counter, void *stream);
-
-/* One step of torch.optim.SGD as torch 2.11 steps it by default on CUDA (the foreach implementation; maximize off;
- * qagnn_b200.optim.SGD), with the argument layout of qagnn_radam_step: exp_avgs holds the momentum buffers, beta1 is each
- * group's momentum (finite, >= 0), beta2 its dampening, rule_flag its nesterov; exp_avg_sqs, eps, step_tables and table_len
- * are unused and may be null / 0.  A group with momentum 0 keeps no buffer (its exp_avgs[i] may be null).  Per element:
- * d = g + weight_decay * p when weight_decay != 0, then with momentum buf = d at device step 0, else
- * buf = momentum buf + (1 - dampening) d, and d = d + momentum buf (nesterov; written to .grad when weight_decay == 0, as
- * torch does) or buf; then p += -lr d.  Buffers are zero before their first step.  found_inf, grad_scale and counter as for
- * qagnn_radam_step.  Every element is torch's result bit for bit; no host synchronisation. */
-int32_t qagnn_sgd_step(int32_t n_tensors, void *const *params, void *const *grads, void *const *momentum_buffers,
-                       void *const *exp_avg_sqs, void *const *steps, const int64_t *numels, const int32_t *group_index,
-                       int32_t n_groups, const double *lr, const double *weight_decay, const double *momentum,
-                       const double *dampening, const double *eps, const int32_t *nesterov, void *const *step_tables,
-                       int64_t table_len, const float *found_inf, const float *grad_scale, int32_t *counter, void *stream);
+                         const double *beta2, const double *eps, const int32_t *rule_flag, void *const *step_tables,
+                         int64_t table_len, const float *found_inf, const float *grad_scale, int32_t *counter, void *stream);
 
 /* fp64 slots qagnn_clip_grad_norm needs for n_tensors tensors of numels[i] elements (one per 8192-element chunk); -1 for a
  * negative count or size. */
@@ -472,16 +454,12 @@ int64_t qagnn_clip_grad_norm_slots(int32_t n_tensors, const int64_t *numels);
 int32_t qagnn_clip_grad_norm(int32_t n_tensors, void *const *grads, const int64_t *numels, double max_norm, double *slots,
                              int64_t n_slots, int32_t *counter, float *total_norm, float *coef, void *stream);
 
-/* The update rule of a captured optimiser tail: qagnn_radam_step's, qagnn_adamw_step's, qagnn_adam_step's or
- * qagnn_sgd_step's. */
-enum { QAGNN_RULE_RADAM = 0, QAGNN_RULE_ADAMW = 1, QAGNN_RULE_ADAM = 2, QAGNN_RULE_SGD = 3 };
-
 /* Bytes of the captured tail's per-call block for n_groups param groups; -1 when n_groups < 1. */
 int64_t qagnn_step_tail_block_bytes(int32_t n_groups);
 
 /* Writes the captured tail's per-call block into host memory `block` of n_bytes, for a copy to the device before each replay
- * of qagnn_step_tail: per group (lr, weight_decay, beta1, beta2, eps, rule_flag and step_tables as for qagnn_radam_step /
- * qagnn_adamw_step / qagnn_adam_step / qagnn_sgd_step, every group's table non-null except SGD's), rounded as those entries round them, then table_len, (float)max_norm and
+ * of qagnn_step_tail: per group (lr, weight_decay, beta1, beta2, eps, rule_flag and step_tables as qagnn_optim_step takes them
+ * for `rule`, every group's table non-null except SGD's), rounded as it rounds them, then table_len, (float)max_norm and
  * GradScaler's growth_factor, backoff_factor and growth_interval.  Host only.  QAGNN_ERR_WORKSPACE when n_bytes is short. */
 int32_t qagnn_step_tail_fill(int32_t rule, int32_t n_groups, const double *lr, const double *weight_decay, const double *beta1,
                              const double *beta2, const double *eps, const int32_t *rule_flag, void *const *step_tables,
@@ -493,9 +471,9 @@ int32_t qagnn_step_tail_fill(int32_t rule, int32_t n_groups, const double *lr, c
  * it.  Pass 1, when clip is nonzero or scale is given: over the n_norm gradients norm_grads / norm_numels, sets *found_inf to
  * 1 for a non-finite gradient (when scale is given) and, when clip is nonzero, writes qagnn_clip_grad_norm's *total_norm and
  * *coef for the gradients times (float)(1 / (double)*scale) (times 1 without a scale), with the block's max_norm.  Pass 2: the
- * rule's step over the tensors (laid out as for qagnn_radam_step; group_index into the block's groups), each gradient first
+ * rule's step over the tensors (laid out as for qagnn_optim_step; group_index into the block's groups), each gradient first
  * unscaled and clipped as the eager tail would leave it in .grad; nothing else changes when *found_inf is nonzero.  Without
- * a clip the step unscales as qagnn_radam_step does with grad_scale = scale.  With a scale, the call ends with
+ * a clip the step unscales as qagnn_optim_step does with grad_scale = scale.  With a scale, the call ends with
  * torch._amp_update_scale_ on *scale and *growth_tracker (device int32) and clears *found_inf.  found_inf (device fp32) and
  * counter (device int32) are zero between calls; slots as for qagnn_clip_grad_norm over the norm list.  Launches: one per pass
  * per 512 tensors (pass 2 also per 16 groups). */

@@ -103,14 +103,8 @@ EXPORTS = {
                                                          C.c_int64] + [_P] * 16 + [C.c_size_t, _P]),
     "qagnn_assemble_batch": (C.c_int32, [_P, _P, _P, _P, _P, C.c_int64, C.c_int32, C.c_int32, _P, C.c_int32, C.c_int64,
                                          C.c_int64, _P, _P, _P, _P]),
-    "qagnn_radam_step": (C.c_int32, [C.c_int32, _P, _P, _P, _P, _P, _P, _P, C.c_int32, _P, _P, _P, _P, _P, _P, _P, C.c_int64,
-                                     _P, _P, _P, _P]),
-    "qagnn_adamw_step": (C.c_int32, [C.c_int32, _P, _P, _P, _P, _P, _P, _P, C.c_int32, _P, _P, _P, _P, _P, _P, _P, C.c_int64,
-                                     _P, _P, _P, _P]),
-    "qagnn_adam_step": (C.c_int32, [C.c_int32, _P, _P, _P, _P, _P, _P, _P, C.c_int32, _P, _P, _P, _P, _P, _P, _P, C.c_int64,
-                                    _P, _P, _P, _P]),
-    "qagnn_sgd_step": (C.c_int32, [C.c_int32, _P, _P, _P, _P, _P, _P, _P, C.c_int32, _P, _P, _P, _P, _P, _P, _P, C.c_int64,
-                                   _P, _P, _P, _P]),
+    "qagnn_optim_step": (C.c_int32, [C.c_int32, C.c_int32, _P, _P, _P, _P, _P, _P, _P, C.c_int32, _P, _P, _P, _P, _P, _P, _P,
+                                     C.c_int64, _P, _P, _P, _P]),
     "qagnn_clip_grad_norm_slots": (C.c_int64, [C.c_int32, _P]),
     "qagnn_clip_grad_norm": (C.c_int32, [C.c_int32, _P, _P, C.c_double, _P, C.c_int64, _P, _P, _P, _P]),
     "qagnn_step_tail_block_bytes": (C.c_int64, [C.c_int32]),

@@ -13,7 +13,7 @@ using mt::kMaxTensors;
 using mt::kThreads;
 constexpr int kMaxGroups = 16;  // distinct param groups per launch
 
-// kAdam and kSgd are torch.optim.Adam's and SGD's default CUDA (foreach) updates (optim_torch.cu)
+// kAdam and kSgd are torch.optim.Adam's and SGD's default CUDA (foreach) updates
 enum class Rule { kRAdam, kAdamW, kAdam, kSgd };
 enum : int32_t { kKindNone = 0, kKindSgd = 1, kKindRect = 2 };
 // bit 2 is the rule's own: RAdam's degenerated_to_sgd, AdamW's correct_bias, SGD's nesterov; bit 4 is SGD's momentum != 0
@@ -88,9 +88,6 @@ struct TailArgs {
   int32_t last;            // the call's last launch: it updates the scale
 };
 static_assert(sizeof(TailArgs) <= 32764, "tail kernel parameters exceed the 32764 bytes sm_90 accepts");
-
-// Pass 2 of the captured tail for torch's Adam and SGD (optim_torch.cu): one launch of a's tensors
-int32_t launch_torch_tail_step(Rule rule, const TailArgs& a, cudaStream_t st);
 
 namespace {
 
@@ -323,13 +320,32 @@ int32_t group_flags(double wd, int32_t rule_flag, double b1) {
   return decay | (rule_flag ? (R == Rule::kRAdam ? kFlagDegenerated : kFlagCorrectBias) : 0);
 }
 
-// A group's hyperparameters as the rule's entry accepts them: betas in [0, 1) and a step table, or for SGD a finite
-// momentum >= 0 and a finite dampening
-template <Rule R>
-bool group_valid(double b1, double b2, const void* table) {
-  if constexpr (R == Rule::kSgd) return b1 >= 0.0 && b1 < INFINITY && b2 > -INFINITY && b2 < INFINITY;
-  return table && b1 >= 0.0 && b1 < 1.0 && b2 >= 0.0 && b2 < 1.0;
-}
+// One call's per-group hyperparameter columns as qagnn_optim_step and qagnn_step_tail_fill take them: the Python doubles, the
+// rule's per-group flag (group_flags) and the device step tables of table_len rows, which SGD does without
+struct GroupColumns {
+  const double *lr, *weight_decay, *beta1, *beta2, *eps;
+  const int32_t* rule_flag;
+  void* const* step_tables;
+  int64_t table_len;
+
+  // Group gi as the rule accepts it: every column given, and betas in [0, 1) with a step table of two rows or more, or for
+  // SGD a finite momentum >= 0 and a finite dampening
+  template <Rule R>
+  bool valid(int32_t gi) const {
+    if (!lr || !weight_decay || !beta1 || !beta2 || !eps || !rule_flag) return false;
+    const double b1 = beta1[gi], b2 = beta2[gi];
+    if constexpr (R == Rule::kSgd) return b1 >= 0.0 && b1 < INFINITY && b2 > -INFINITY && b2 < INFINITY;
+    return step_tables && table_len >= 2 && step_tables[gi] && b1 >= 0.0 && b1 < 1.0 && b2 >= 0.0 && b2 < 1.0;
+  }
+
+  // Fills the per-launch copy of group gi
+  template <Rule R>
+  void fill(StepGroup& gr, int32_t gi) const {
+    fill_group<R>(gr, lr[gi], weight_decay[gi], beta1[gi], beta2[gi], eps[gi],
+                  group_flags<R>(weight_decay[gi], rule_flag[gi], beta1[gi]),
+                  R == Rule::kSgd ? nullptr : (const double*)step_tables[gi]);
+  }
+};
 
 // Checks one step's tensor list: group indices in range, a step counter per tensor, data pointers for non-empty tensors.
 // SGD has no exp_avg_sqs, and exp_avgs[i] (its momentum buffer) may be null; where it must not be, its caller checks.
@@ -390,38 +406,16 @@ int32_t pack_launches(A& a, int32_t n_tensors, void* const* params, void* const*
   return launch(true);
 }
 
-// The host side of an eager step entry (optim.cu, optim_torch.cu): validation, per-launch packing (512 tensors, 16 groups,
-// an int32 chunk prefix) and the launches, launch(args) sending one.  rule_flag is the rule's per-group flag (group_flags).
-template <Rule R, class Launch>
-int32_t step_all(int32_t n_tensors, void* const* params, void* const* grads, void* const* exp_avgs, void* const* exp_avg_sqs,
-                 void* const* steps, const int64_t* numels, const int32_t* group_index, int32_t n_groups, const double* lr,
-                 const double* weight_decay, const double* beta1, const double* beta2, const double* eps,
-                 const int32_t* rule_flag, void* const* step_tables, int64_t table_len, const float* found_inf,
-                 const float* grad_scale, int32_t* counter, Launch launch) {
-  constexpr bool kSgd = R == Rule::kSgd;
-  if (n_tensors < 0 || n_groups < 0) return QAGNN_ERR_INVALID_ARGUMENT;
-  if (n_tensors == 0) return QAGNN_OK;
-  if (!tensors_valid<R>(n_tensors, params, grads, exp_avgs, exp_avg_sqs, steps, numels, group_index, n_groups) || !lr ||
-      !weight_decay || !beta1 || !beta2 || !eps || !rule_flag || (!kSgd && (!step_tables || table_len < 2)) || !counter)
-    return QAGNN_ERR_INVALID_ARGUMENT;
-  for (int32_t i = 0; i < n_tensors; ++i) {
-    const int32_t gi = group_index[i];
-    if (!group_valid<R>(beta1[gi], beta2[gi], kSgd ? nullptr : step_tables[gi])) return QAGNN_ERR_INVALID_ARGUMENT;
-    if (kSgd && numels[i] > 0 && beta1[gi] != 0.0 && !exp_avgs[i]) return QAGNN_ERR_INVALID_ARGUMENT;
+// Calls f(std::integral_constant<Rule, R>()) for the Rule of a QAGNN_RULE_* value; QAGNN_ERR_INVALID_ARGUMENT for any other
+template <class F>
+int32_t with_rule(int32_t rule, F f) {
+  switch (rule) {
+    case QAGNN_RULE_RADAM: return f(std::integral_constant<Rule, Rule::kRAdam>());
+    case QAGNN_RULE_ADAMW: return f(std::integral_constant<Rule, Rule::kAdamW>());
+    case QAGNN_RULE_ADAM: return f(std::integral_constant<Rule, Rule::kAdam>());
+    case QAGNN_RULE_SGD: return f(std::integral_constant<Rule, Rule::kSgd>());
+    default: return QAGNN_ERR_INVALID_ARGUMENT;
   }
-  static thread_local StepArgs a;  // 28 KB: kept off the stack
-  a.table_len = table_len;
-  a.found_inf = found_inf;
-  a.grad_scale = grad_scale;
-  a.counter = counter;
-  return pack_launches(
-      a, n_tensors, params, grads, exp_avgs, exp_avg_sqs, steps, numels, group_index,
-      [&](int32_t slot, int32_t gi) {
-        fill_group<R>(a.groups[slot], lr[gi], weight_decay[gi], beta1[gi], beta2[gi], eps[gi],
-                      group_flags<R>(weight_decay[gi], rule_flag[gi], beta1[gi]),
-                      kSgd ? nullptr : (const double*)step_tables[gi]);
-      },
-      [&](bool) { return launch(a); });
 }
 
 }  // namespace

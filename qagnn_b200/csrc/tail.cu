@@ -8,9 +8,8 @@
 // as torch._amp_foreach_non_finite_check_and_unscale_ tests it) sets found_inf to 1.  Without a clip the reference does not
 // call unscale_, and the pass is GradScaler._check_inf_per_device: inv_scale 1 and no norm.  It writes nothing per element.
 //
-// tail_{radam,adamw}_kernel (pass 2) are optim.cuh's step body with the groups read from the block; torch's Adam and SGD
-// take the same pass 2 in optim_torch.cu's tail_{adam,sgd} kernels.  Each element takes
-// c = (g * inv) * coef, the same two fp32 multiplies as unscale_ then clip_scale_kernel, each left out at a factor of 1 as
+// tail_{radam,adamw,adam,sgd}_kernel (pass 2) are optim.cuh's step body with the groups read from the block.  Each element
+// takes c = (g * inv) * coef, the same two fp32 multiplies as unscale_ then clip_scale_kernel, each left out at a factor of 1 as
 // they leave it; c goes back to .grad when either factor applies, found_inf or not.  Without a clip the step unscales as the
 // eager step does under GradScaler.step.  The last CTA of the call's last launch then applies torch._amp_update_scale_ to
 // the scaler's own tensors and clears found_inf.
@@ -46,19 +45,11 @@ __global__ void __launch_bounds__(kThreads) tail_norm_kernel(const __grid_consta
 
 __global__ void __launch_bounds__(kThreads) tail_radam_kernel(const __grid_constant__ TailArgs a) { step_body<Rule::kRAdam>(a); }
 __global__ void __launch_bounds__(kThreads) tail_adamw_kernel(const __grid_constant__ TailArgs a) { step_body<Rule::kAdamW>(a); }
+__global__ void __launch_bounds__(kThreads) tail_adam_kernel(const __grid_constant__ TailArgs a) { step_body<Rule::kAdam>(a); }
+__global__ void __launch_bounds__(kThreads) tail_sgd_kernel(const __grid_constant__ TailArgs a) { step_body<Rule::kSgd>(a); }
 
 int64_t block_bytes(int32_t n_groups) {
   return n_groups <= 0 ? -1 : (int64_t)sizeof(TailBlock) + (int64_t)n_groups * (int64_t)sizeof(StepGroup);
-}
-
-template <Rule R>
-void fill_groups(TailBlock& b, const double* lr, const double* wd, const double* b1, const double* b2, const double* eps,
-                    const int32_t* rule_flag, void* const* step_tables) {
-  constexpr bool kSgd = R == Rule::kSgd;
-  StepGroup* groups = const_cast<StepGroup*>(block_groups(&b));
-  for (int32_t gi = 0; gi < b.n_groups; ++gi)
-    fill_group<R>(groups[gi], lr[gi], wd[gi], b1[gi], b2[gi], eps[gi], group_flags<R>(wd[gi], rule_flag[gi], b1[gi]),
-                  kSgd ? nullptr : (const double*)step_tables[gi]);
 }
 
 template <Rule R>
@@ -68,8 +59,10 @@ int32_t launch_step(const TailArgs& a, cudaStream_t st) {
     tail_radam_kernel<<<blocks, kThreads, 0, st>>>(a);
   else if constexpr (R == Rule::kAdamW)
     tail_adamw_kernel<<<blocks, kThreads, 0, st>>>(a);
+  else if constexpr (R == Rule::kAdam)
+    tail_adam_kernel<<<blocks, kThreads, 0, st>>>(a);
   else
-    return launch_torch_tail_step(R, a, st);
+    tail_sgd_kernel<<<blocks, kThreads, 0, st>>>(a);
   QAGNN_CHECK_LAUNCH();
   return QAGNN_OK;
 }
@@ -140,30 +133,25 @@ extern "C" int32_t qagnn_step_tail_fill(int32_t rule, int32_t n_groups, const do
                                         const double* beta1, const double* beta2, const double* eps, const int32_t* rule_flag,
                                         void* const* step_tables, int64_t table_len, double max_norm, double growth_factor,
                                         double backoff_factor, int32_t growth_interval, void* block, int64_t n_bytes) {
-  const bool sgd = rule == QAGNN_RULE_SGD;  // SGD steps without a table
-  if (rule < QAGNN_RULE_RADAM || rule > QAGNN_RULE_SGD || n_groups <= 0 || !lr || !weight_decay || !beta1 || !beta2 ||
-      !eps || !rule_flag || (!sgd && (!step_tables || table_len < 2)) || !block)
-    return QAGNN_ERR_INVALID_ARGUMENT;
-  for (int32_t gi = 0; gi < n_groups; ++gi)
-    if (!(sgd ? group_valid<Rule::kSgd>(beta1[gi], beta2[gi], nullptr)
-              : group_valid<Rule::kRAdam>(beta1[gi], beta2[gi], step_tables[gi])))
-      return QAGNN_ERR_INVALID_ARGUMENT;
-  if (n_bytes < block_bytes(n_groups)) return QAGNN_ERR_WORKSPACE;
-  TailBlock& b = *(TailBlock*)block;
-  b.growth_factor = growth_factor;
-  b.backoff_factor = backoff_factor;
-  b.table_len = table_len;
-  b.max_norm = (float)max_norm;
-  b.growth_interval = growth_interval;
-  b.n_groups = n_groups;
-  b.pad = 0;
-  switch (rule) {
-    case QAGNN_RULE_RADAM: fill_groups<Rule::kRAdam>(b, lr, weight_decay, beta1, beta2, eps, rule_flag, step_tables); break;
-    case QAGNN_RULE_ADAMW: fill_groups<Rule::kAdamW>(b, lr, weight_decay, beta1, beta2, eps, rule_flag, step_tables); break;
-    case QAGNN_RULE_ADAM: fill_groups<Rule::kAdam>(b, lr, weight_decay, beta1, beta2, eps, rule_flag, step_tables); break;
-    default: fill_groups<Rule::kSgd>(b, lr, weight_decay, beta1, beta2, eps, rule_flag, step_tables);
-  }
-  return QAGNN_OK;
+  const GroupColumns c{lr, weight_decay, beta1, beta2, eps, rule_flag, step_tables, table_len};
+  return with_rule(rule, [&](auto r) {
+    constexpr Rule R = decltype(r)::value;
+    if (n_groups <= 0 || !block) return QAGNN_ERR_INVALID_ARGUMENT;
+    for (int32_t gi = 0; gi < n_groups; ++gi)
+      if (!c.valid<R>(gi)) return QAGNN_ERR_INVALID_ARGUMENT;
+    if (n_bytes < block_bytes(n_groups)) return QAGNN_ERR_WORKSPACE;
+    TailBlock& b = *(TailBlock*)block;
+    b.growth_factor = growth_factor;
+    b.backoff_factor = backoff_factor;
+    b.table_len = table_len;
+    b.max_norm = (float)max_norm;
+    b.growth_interval = growth_interval;
+    b.n_groups = n_groups;
+    b.pad = 0;
+    StepGroup* groups = const_cast<StepGroup*>(block_groups(&b));
+    for (int32_t gi = 0; gi < n_groups; ++gi) c.fill<R>(groups[gi], gi);
+    return QAGNN_OK;
+  });
 }
 
 extern "C" int32_t qagnn_step_tail(int32_t rule, int32_t n_tensors, void* const* params, void* const* grads,
@@ -172,15 +160,9 @@ extern "C" int32_t qagnn_step_tail(int32_t rule, int32_t n_tensors, void* const*
                                    const int64_t* norm_numels, int32_t clip, const void* block, double* slots, int64_t n_slots,
                                    int32_t* counter, float* total_norm, float* coef, float* found_inf, float* scale,
                                    int32_t* growth_tracker, void* stream) {
-#define QAGNN_TAIL(R)                                                                                                   \
-  tail_all<R>(n_tensors, params, grads, exp_avgs, exp_avg_sqs, steps, numels, group_index, n_groups, n_norm, norm_grads,   \
-              norm_numels, clip, block, slots, n_slots, counter, total_norm, coef, found_inf, scale, growth_tracker, stream)
-  switch (rule) {
-    case QAGNN_RULE_RADAM: return QAGNN_TAIL(Rule::kRAdam);
-    case QAGNN_RULE_ADAMW: return QAGNN_TAIL(Rule::kAdamW);
-    case QAGNN_RULE_ADAM: return QAGNN_TAIL(Rule::kAdam);
-    case QAGNN_RULE_SGD: return QAGNN_TAIL(Rule::kSgd);
-    default: return QAGNN_ERR_INVALID_ARGUMENT;
-  }
-#undef QAGNN_TAIL
+  return with_rule(rule, [&](auto r) {
+    return tail_all<decltype(r)::value>(n_tensors, params, grads, exp_avgs, exp_avg_sqs, steps, numels, group_index, n_groups,
+                                        n_norm, norm_grads, norm_numels, clip, block, slots, n_slots, counter, total_norm, coef,
+                                        found_inf, scale, growth_tracker, stream);
+  });
 }

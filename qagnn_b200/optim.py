@@ -1,10 +1,9 @@
-"""The reference's optimisers as one multi-tensor sm_90a launch per device (csrc/optim.cu).
+"""The reference's optimisers as one multi-tensor sm_90a launch per device (csrc/optim.cu, qagnn_optim_step).
 
-`RAdam` is the reference's `utils.optimization_utils.RAdam` (qagnn_radam_step) and `AdamW` is transformers' `AdamW` (3.4.0,
-the version the reference pins; qagnn_adamw_step).  `Adam` and `SGD` are torch.optim's, as torch 2.11 steps them by default
-on CUDA (qagnn_adam_step, qagnn_sgd_step; csrc/optim_torch.cu).  Each takes its original's arguments and param groups and reproduces its
-update bit for bit: the same fp32 operations in the same order, with the same rounding of every Python scalar.  They differ
-from the originals in how they run:
+`RAdam` is the reference's `utils.optimization_utils.RAdam` and `AdamW` is transformers' `AdamW` (3.4.0, the version the
+reference pins).  `Adam` and `SGD` are torch.optim's, as torch 2.11 steps them by default on CUDA.  Each takes its
+original's arguments and param groups and reproduces its update bit for bit: the same fp32 operations in the same order,
+with the same rounding of every Python scalar.  They differ from the originals in how they run:
 - one kernel launch per device per `step()` (one per 512 tensors), instead of about ten element-wise ops per tensor;
 - `state[p]['step']` is an int64 0-dim tensor on p's device, advanced by the kernel, so `step()` never reads the GPU;
 - they declare `_step_supports_amp_scaling`: `GradScaler.step` hands them `found_inf` and, when `unscale_` was not called,
@@ -21,6 +20,7 @@ the optimiser tail `scaler.unscale_; clip_grad_norm_; scaler.step; scaler.update
 that whole tail, scheduler step included, as one CUDA graph replay of two launches (csrc/tail.cu).
 """
 import ctypes as C
+import functools
 import math
 
 import torch
@@ -43,22 +43,10 @@ def step_size_row(beta1, beta2, t):
     return 0.0, 1.0 / (1 - beta1 ** t)
 
 
-def step_size_table(beta1, beta2, length):
-    """fp64 [length, 2]: row t is step_size_row(beta1, beta2, t); row 0 (never indexed) is (0, 0)."""
-    rows = [(0.0, 0.0)] + [step_size_row(beta1, beta2, t) for t in range(1, length)]
-    return torch.tensor(rows, dtype=torch.float64)
-
-
 def bias_correction_row(beta1, beta2, t):
     """(math.sqrt(bias_correction2), bias_correction1) of transformers' AdamW at step t >= 1, in Python doubles as it forms
     them; its step size is lr * row[0] / row[1]."""
     return math.sqrt(1.0 - beta2 ** t), 1.0 - beta1 ** t
-
-
-def bias_correction_table(beta1, beta2, length):
-    """fp64 [length, 2]: row t is bias_correction_row(beta1, beta2, t); row 0 (never indexed) is (0, 0)."""
-    rows = [(0.0, 0.0)] + [bias_correction_row(beta1, beta2, t) for t in range(1, length)]
-    return torch.tensor(rows, dtype=torch.float64)
 
 
 def adam_bias_correction_row(beta1, beta2, t):
@@ -68,10 +56,33 @@ def adam_bias_correction_row(beta1, beta2, t):
     return (1 - beta2 ** t) ** 0.5, 1 - beta1 ** t
 
 
-def adam_bias_correction_table(beta1, beta2, length):
-    """fp64 [length, 2]: row t is adam_bias_correction_row(beta1, beta2, t); row 0 (never indexed) is (0, 0)."""
-    rows = [(0.0, 0.0)] + [adam_bias_correction_row(beta1, beta2, t) for t in range(1, length)]
+def step_table(row, beta1, beta2, length):
+    """fp64 [length, 2]: row t is row(beta1, beta2, t), one of the *_row functions above; row 0 (never indexed) is (0, 0)."""
+    rows = [(0.0, 0.0)] + [row(beta1, beta2, t) for t in range(1, length)]
     return torch.tensor(rows, dtype=torch.float64)
+
+
+# each rule's table(beta1, beta2, length)
+step_size_table = functools.partial(step_table, step_size_row)
+bias_correction_table = functools.partial(step_table, bias_correction_row)
+adam_bias_correction_table = functools.partial(step_table, adam_bias_correction_row)
+
+
+def _arr(ct, vals):
+    return (ct * len(vals))(*vals)
+
+
+def _ptrs(ts):
+    """A void* array of the tensors' addresses, None a null pointer."""
+    return _arr(C.c_void_p, [None if t is None else t.data_ptr() for t in ts])
+
+
+def _tensor_arrays(items, states, moments):
+    """The per-tensor arrays of qagnn_optim_step and qagnn_step_tail for [(group index, p)], their states and
+    [(exp_avg, exp_avg_sq)]: params, grads, exp_avgs, exp_avg_sqs, steps, numels and group_index."""
+    return (_ptrs([p for _, p in items]), _ptrs([p.grad for _, p in items]), _ptrs([m for m, _ in moments]),
+            _ptrs([v for _, v in moments]), _ptrs([s["step"] for s in states]),
+            _arr(C.c_int64, [p.numel() for _, p in items]), _arr(C.c_int32, [gi for gi, _ in items]))
 
 
 def _refuse(name, options):
@@ -117,13 +128,12 @@ def _check_tensor(t, what, name):
 
 class _DeviceStepOptimizer(torch.optim.Optimizer):
     """What RAdam, AdamW, Adam and SGD share: the per-device work lists, the state, the step tables, the kernel's arrival
-    counter, the GradScaler hand-off and state_dict loading.  A subclass names its C entry (`_entry`) and tail rule
-    (`_rule`, QAGNN_RULE_*), its table builder (`_table_rows`, fp64 [length, 2] for (beta1, beta2); None for no table), its
-    state tensors (`_state_keys`: the entry's exp_avgs and exp_avg_sqs), its original's sparse-gradient message and host
-    caches in the groups, and supplies `_check_group` and `_rule_flags` (one int32 per group: the entry's per-group flag)."""
+    counter, the GradScaler hand-off and state_dict loading.  A subclass names its update rule (`_rule`, QAGNN_RULE_*), its
+    table builder (`_table_rows`, fp64 [length, 2] for (beta1, beta2); None for no table), its state tensors (`_state_keys`: the entry's
+    exp_avgs and exp_avg_sqs), its original's sparse-gradient message and host caches in the groups, and supplies
+    `_check_group` and `_rule_flags` (one int32 per group: the entry's per-group flag)."""
 
     _step_supports_amp_scaling = True
-    _entry = None
     _rule = None
     _table_rows = None
     _state_keys = ("exp_avg", "exp_avg_sq")
@@ -182,39 +192,52 @@ class _DeviceStepOptimizer(torch.optim.Optimizer):
             tables[gi] = self._table(device, hyper[gi][2], hyper[gi][3])
         return tables, min(t.shape[0] for t in tables if t is not None)
 
+    def _items(self, name, check_dense):
+        """[(group index, p)] of the parameters with a gradient, every group checked with `_check_group` and every gradient
+        against its parameter, in the messages of `name`.  check_dense(grad) raises the caller's error for a gradient that
+        is not dense."""
+        items = []
+        for gi, group in enumerate(self.param_groups):
+            self._check_group(group)
+            for p in group["params"]:
+                if p.grad is None:
+                    continue
+                check_dense(p.grad)
+                _check_tensor(p, "parameter", name)
+                _check_tensor(p.grad, "gradient", name)
+                if p.grad.shape != p.shape or p.grad.device != p.device:
+                    raise ValueError(f"qagnn_b200.optim.{name}: a gradient of shape {tuple(p.grad.shape)} on {p.grad.device} "
+                                     f"for a parameter of shape {tuple(p.shape)} on {p.device}")
+                items.append((gi, p))
+        return items
+
+    def _check_sparse(self, grad):
+        if grad.is_sparse:
+            raise RuntimeError(self._sparse_message)
+
+    def _group_columns(self):
+        """Each group's (lr, weight_decay, beta1, beta2, eps), and the entries' per-group host arrays: those five columns
+        and rule_flag."""
+        hyper = [self._hyper(g) for g in self.param_groups]
+        return hyper, [_arr(C.c_double, col) for col in zip(*hyper)] + [_arr(C.c_int32, self._rule_flags())]
+
     @torch.no_grad()
     def step(self, closure=None):
         loss = None
         if closure is not None:
             with torch.enable_grad():
                 loss = closure()
-        name = type(self).__name__
         work = {}  # device -> [(group index, p)]
-        for gi, group in enumerate(self.param_groups):
-            self._check_group(group)
-            for p in group["params"]:
-                if p.grad is None:
-                    continue
-                if p.grad.is_sparse:
-                    raise RuntimeError(self._sparse_message)
-                _check_tensor(p, "parameter", name)
-                _check_tensor(p.grad, "gradient", name)
-                if p.grad.shape != p.shape or p.grad.device != p.device:
-                    raise ValueError(f"qagnn_b200.optim.{name}: a gradient of shape {tuple(p.grad.shape)} on {p.grad.device} "
-                                     f"for a parameter of shape {tuple(p.shape)} on {p.device}")
-                work.setdefault(p.device, []).append((gi, p))
+        for gi, p in self._items(type(self).__name__, self._check_sparse):
+            work.setdefault(p.device, []).append((gi, p))
         if not work:
             return loss
         self._host_steps += 1
         found_inf = getattr(self, "found_inf", None)
         grad_scale = getattr(self, "grad_scale", None)
         lib = _lib.load()
-        entry = getattr(lib, self._entry)
         n_groups = len(self.param_groups)
-        hyper = [self._hyper(g) for g in self.param_groups]
-        arr = lambda ct, vals: (ct * len(vals))(*vals)  # noqa: E731
-        lr, wd, b1, b2, eps = (arr(C.c_double, col) for col in zip(*hyper))
-        flags = arr(C.c_int32, self._rule_flags())
+        hyper, columns = self._group_columns()
         for device, items in work.items():
             states = [self._state_for(p, self.param_groups[gi]) for gi, p in items]
             moments = [self._state_tensors(st) for st in states]
@@ -222,16 +245,11 @@ class _DeviceStepOptimizer(torch.optim.Optimizer):
             # GradScaler keeps found_inf and the scale on its own device: the copies to this one are enqueued, never read
             fi = None if found_inf is None else found_inf.to(device, torch.float32, non_blocking=True)
             gs = None if grad_scale is None else grad_scale.to(device, torch.float32, non_blocking=True)
-            n = len(items)
-            ptrs = lambda ts: arr(C.c_void_p, [None if t is None else t.data_ptr() for t in ts])  # noqa: E731
             with torch.cuda.device(device):
-                _lib.check(entry(
-                    n, ptrs([p for _, p in items]), ptrs([p.grad for _, p in items]), ptrs([m for m, _ in moments]),
-                    ptrs([v for _, v in moments]), ptrs([s["step"] for s in states]),
-                    arr(C.c_int64, [p.numel() for _, p in items]), arr(C.c_int32, [gi for gi, _ in items]), n_groups,
-                    lr, wd, b1, b2, eps, flags,
-                    arr(C.c_void_p, [0 if t is None else t.data_ptr() for t in tables]), length,
-                    _lib.ptr(fi), _lib.ptr(gs), _lib.ptr(self._counter(device)), _lib.stream_ptr(device)), self._entry)
+                _lib.check(lib.qagnn_optim_step(
+                    self._rule, len(items), *_tensor_arrays(items, states, moments), n_groups, *columns, _ptrs(tables),
+                    length, _lib.ptr(fi), _lib.ptr(gs), _lib.ptr(self._counter(device)), _lib.stream_ptr(device)),
+                    "qagnn_optim_step")
         return loss
 
     def _missing_step(self, st):
@@ -273,7 +291,6 @@ class RAdam(_DeviceStepOptimizer):
     tensors; a parameter whose `.grad` is None is skipped and its step does not advance.  `lr` (and every other
     hyperparameter) is read from each group at every `step()`, so LambdaLR schedules work as with the reference."""
 
-    _entry = "qagnn_radam_step"
     _rule = 0
     _table_rows = staticmethod(step_size_table)
     _sparse_message = "RAdam does not support sparse gradients"
@@ -299,7 +316,6 @@ class AdamW(_DeviceStepOptimizer):
     tensors; a parameter whose `.grad` is None is skipped and its step does not advance.  Every hyperparameter, `correct_bias`
     included, is read from each group at every `step()`."""
 
-    _entry = "qagnn_adamw_step"
     _rule = 1
     _table_rows = staticmethod(bias_correction_table)
     _sparse_message = "Adam does not support sparse gradients, please consider SparseAdam instead"
@@ -318,14 +334,13 @@ class AdamW(_DeviceStepOptimizer):
 class Adam(_DeviceStepOptimizer):
     """Adam(params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0, amsgrad=False, *, foreach=None, maximize=False,
     capturable=False, differentiable=False, fused=None, decoupled_weight_decay=False): torch.optim.Adam, the reference's
-    `--optim adam`, stepped on the GPU (qagnn_adam_step) bit for bit as torch 2.11 steps it by default on CUDA (its foreach
+    `--optim adam`, stepped on the GPU bit for bit as torch 2.11 steps it by default on CUDA (its foreach
     implementation).  The constructor, defaults, checks and param-group keys are torch's; amsgrad, maximize,
     decoupled_weight_decay and foreach / fused / capturable / differentiable set to True are refused (torch.optim.Adam has
     them).  The state keeps torch's keys, with `step` an int64 0-dim tensor on the parameter's device; `load_state_dict`
     takes torch's own state dict, whose fp32 CPU steps it converts.  Parameters and their gradients must be contiguous fp32
     CUDA tensors; a parameter whose `.grad` is None is skipped and its step does not advance."""
 
-    _entry = "qagnn_adam_step"
     _rule = 2
     _table_rows = staticmethod(adam_bias_correction_table)
     _sparse_message = "Adam does not support sparse gradients, please consider SparseAdam instead"
@@ -365,7 +380,7 @@ class Adam(_DeviceStepOptimizer):
 
 class SGD(_DeviceStepOptimizer):
     """SGD(params, lr=1e-3, momentum=0, dampening=0, weight_decay=0, nesterov=False, *, maximize=False, foreach=None,
-    differentiable=False, fused=None): torch.optim.SGD, the reference's `--optim sgd`, stepped on the GPU (qagnn_sgd_step)
+    differentiable=False, fused=None): torch.optim.SGD, the reference's `--optim sgd`, stepped on the GPU
     bit for bit as torch 2.11 steps it by default on CUDA (its foreach implementation).  The constructor, defaults, checks and
     param-group keys are torch's; maximize, fused and differentiable set to True are refused (torch.optim.SGD has them).  With
     momentum the state keeps torch's `momentum_buffer`, allocated as zeros, plus `step`, an int64 0-dim tensor on the
@@ -374,7 +389,6 @@ class SGD(_DeviceStepOptimizer):
     set).  Parameters and their gradients must be contiguous fp32 CUDA tensors; a parameter whose `.grad` is None is
     skipped."""
 
-    _entry = "qagnn_sgd_step"
     _rule = 3
     _state_keys = ("momentum_buffer",)
     _sparse_message = "qagnn_b200.optim.SGD does not support sparse gradients; use torch.optim.SGD for them"
@@ -399,7 +413,7 @@ class SGD(_DeviceStepOptimizer):
 
     @staticmethod
     def _hyper(group):
-        # qagnn_sgd_step's beta1 and beta2 are the momentum and the dampening
+        # SGD's beta1 and beta2 are the momentum and the dampening
         return float(group["lr"]), float(group["weight_decay"]), float(group["momentum"]), float(group["dampening"]), 0.0
 
     def _check_group(self, group):
@@ -527,23 +541,15 @@ class CapturedTail:
         self._graph = None
         self._bufs = None
 
+    @staticmethod
+    def _check_dense(grad):
+        if grad.layout != torch.strided:
+            raise TypeError(f"qagnn_b200.optim.CapturedTail: the gradient must be dense (got {grad.layout})")
+
     def _work(self):
         """[(group index, p)] of the parameters with a gradient, checked as the optimiser and the clip check them."""
-        opt, name = self.optimizer, "CapturedTail"
-        items = []
-        for gi, group in enumerate(opt.param_groups):
-            opt._check_group(group)
-            for p in group["params"]:
-                if p.grad is None:
-                    continue
-                if p.grad.layout != torch.strided:
-                    raise TypeError(f"qagnn_b200.optim.{name}: the gradient must be dense (got {p.grad.layout})")
-                _check_tensor(p, "parameter", name)
-                _check_tensor(p.grad, "gradient", name)
-                if p.grad.shape != p.shape or p.grad.device != p.device:
-                    raise ValueError(f"qagnn_b200.optim.{name}: a gradient of shape {tuple(p.grad.shape)} on {p.grad.device} "
-                                     f"for a parameter of shape {tuple(p.shape)} on {p.device}")
-                items.append((gi, p))
+        name = "CapturedTail"
+        items = self.optimizer._items(name, self._check_dense)
         if not items:
             raise RuntimeError(f"qagnn_b200.optim.{name}: no parameter has a gradient")
         devices = {p.device for _, p in items}
@@ -595,10 +601,8 @@ class CapturedTail:
             self.scheduler.step()
         opt._host_steps += 1
         lib = _lib.load()
-        hyper = [opt._hyper(g) for g in opt.param_groups]
+        hyper, columns = opt._group_columns()
         tables, table_len = opt._group_tables(device, hyper, range(len(hyper)))
-        arr = lambda ct, vals: (ct * len(vals))(*vals)  # noqa: E731
-        lr, wd, b1, b2, eps = (arr(C.c_double, col) for col in zip(*hyper))
         n_groups = len(hyper)
         n_bytes = lib.qagnn_step_tail_block_bytes(n_groups)
         if self._key != key:
@@ -608,8 +612,7 @@ class CapturedTail:
         staging = torch.empty(n_bytes, dtype=torch.uint8, pin_memory=True)
         sc = self.scaler
         _lib.check(lib.qagnn_step_tail_fill(
-            self._rule, n_groups, lr, wd, b1, b2, eps, arr(C.c_int32, opt._rule_flags()),
-            arr(C.c_void_p, [None if t is None else t.data_ptr() for t in tables]), table_len, self.max_grad_norm,
+            self._rule, n_groups, *columns, _ptrs(tables), table_len, self.max_grad_norm,
             float(sc._growth_factor) if sc else 2.0, float(sc._backoff_factor) if sc else 0.5,
             int(sc._growth_interval) if sc else 1, C.c_void_p(staging.data_ptr()), n_bytes), "qagnn_step_tail_fill")
         bufs["block"].copy_(staging, non_blocking=True)
@@ -637,13 +640,9 @@ class CapturedTail:
                     total_norm=torch.zeros((), dtype=torch.float32, device=device))
 
     def _launcher(self, lib, device, items, states, moments, norm_grads, clip, scale, tracker, n_groups):
-        arr = lambda ct, vals: (ct * len(vals))(*vals)  # noqa: E731
-        ptrs = lambda ts: arr(C.c_void_p, [None if t is None else t.data_ptr() for t in ts])  # noqa: E731
-        n, nn, b = len(items), len(norm_grads), self._bufs
-        args = (self._rule, n, ptrs([p for _, p in items]), ptrs([p.grad for _, p in items]),
-                ptrs([m for m, _ in moments]), ptrs([v for _, v in moments]), ptrs([s["step"] for s in states]),
-                arr(C.c_int64, [p.numel() for _, p in items]), arr(C.c_int32, [gi for gi, _ in items]), n_groups,
-                nn, ptrs(norm_grads), arr(C.c_int64, [g.numel() for g in norm_grads]), int(clip), _lib.ptr(b["block"]),
+        b = self._bufs
+        args = (self._rule, len(items), *_tensor_arrays(items, states, moments), n_groups, len(norm_grads), _ptrs(norm_grads),
+                _arr(C.c_int64, [g.numel() for g in norm_grads]), int(clip), _lib.ptr(b["block"]),
                 _lib.ptr(b["slots"]), b["slots"].numel(), _lib.ptr(b["counter"]), _lib.ptr(b["total_norm"]),
                 _lib.ptr(b["coef"]), _lib.ptr(b["found_inf"]), _lib.ptr(scale), _lib.ptr(tracker))
 

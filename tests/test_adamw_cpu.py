@@ -262,12 +262,13 @@ def _kernel(kernels, name):
     return found[0]
 
 
-def test_both_rules_compile_without_spills(compiled):
+def test_radam_and_adamw_compile_without_spills_among_four_kernels(compiled):
     report, _, _ = compiled
     props = re.findall(r"Function properties for (\S+)\n\s*(\d+) bytes stack frame, (\d+) bytes spill stores, "
                        r"(\d+) bytes spill loads\n.*?Used (\d+) registers", report)
-    got = {re.search(r"(radam|adamw)_kernel", n).group(0): tuple(int(x) for x in rest) for n, *rest in props}
-    assert set(got) == {"radam_kernel", "adamw_kernel"}, report
+    got = {re.search(r"(?:radam|adamw|adam|sgd)_kernel", n).group(0): tuple(int(x) for x in rest) for n, *rest in props}
+    assert set(got) == {"radam_kernel", "adamw_kernel", "adam_kernel", "sgd_kernel"}, report
+    got = {name: got[name] for name in ("radam_kernel", "adamw_kernel")}
     for name, (stack, stores, loads, regs) in got.items():
         assert stack == stores == loads == 0, (name, report)
     assert got["radam_kernel"][3] == 40

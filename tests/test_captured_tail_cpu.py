@@ -14,6 +14,7 @@ from qagnn_b200 import _lib, build, optim
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 ENTRIES = ("qagnn_step_tail_block_bytes", "qagnn_step_tail_fill", "qagnn_step_tail")
+TAIL_KERNELS = {"tail_norm_kernel", "tail_radam_kernel", "tail_adamw_kernel", "tail_adam_kernel", "tail_sgd_kernel"}
 
 
 def test_torch_sgd_and_adam_are_sent_to_the_eager_tail():
@@ -107,22 +108,22 @@ def compiled(tmp_path_factory):
             m = re.match(r"\s*/\*[0-9a-f]{4,}\*/\s+(?:@!?U?P\w+\s+)?([A-Z][A-Z0-9_.]*)", line)
             if m:
                 ops[m.group(1)] += 1
-        kernels[re.search(r"tail_(?:norm|radam|adamw)_kernel", body.split("\n", 1)[0]).group(0)] = ops
+        kernels[re.search(r"tail_(?:norm|radam|adamw|adam|sgd)_kernel", body.split("\n", 1)[0]).group(0)] = ops
     return r.stdout + r.stderr, kernels
 
 
-def test_no_tail_kernel_spills(compiled):
+def test_no_tail_kernel_of_any_rule_spills(compiled):
     report, _ = compiled
-    props = re.findall(r"Function properties for \S*(tail_(?:norm|radam|adamw)_kernel)\S*\n\s*(\d+) bytes stack frame, "
-                       r"(\d+) bytes spill stores, (\d+) bytes spill loads", report)
-    assert {name for name, *_ in props} == {"tail_norm_kernel", "tail_radam_kernel", "tail_adamw_kernel"}, report
+    props = re.findall(r"Function properties for \S*(tail_(?:norm|radam|adamw|adam|sgd)_kernel)\S*\n\s*(\d+) bytes stack "
+                       r"frame, (\d+) bytes spill stores, (\d+) bytes spill loads", report)
+    assert {name for name, *_ in props} == TAIL_KERNELS, report
     for name, stack, stores, loads in props:
         assert int(stack) == int(stores) == int(loads) == 0, (name, report)
 
 
-def test_vector_loads_and_no_floating_point_atomics(compiled):
+def test_every_tail_kernel_takes_vector_loads_and_no_floating_point_atomics(compiled):
     _, kernels = compiled
-    assert set(kernels) == {"tail_norm_kernel", "tail_radam_kernel", "tail_adamw_kernel"}
+    assert set(kernels) == TAIL_KERNELS
     for name, ops in kernels.items():
         atomics = [op for op in ops if op.split(".")[0] in ("RED", "REDG", "ATOM", "ATOMG", "ATOMS")]
         assert not [op for op in atomics if re.search(r"\.F(16|32|64)", op)], (name, atomics)

@@ -124,12 +124,13 @@ def test_captured_tail_takes_both():
         assert optim.CapturedTail(opt)._rule == opt._rule
 
 
-def test_entries_are_declared_and_bound_as_radams():
+def test_one_entry_is_declared_and_bound_for_every_rule():
     header = open(os.path.join(ROOT, "include", "qagnn_b200.h")).read()
-    for name in ("qagnn_adam_step", "qagnn_sgd_step"):
-        assert re.search(rf"\bint32_t {name}\s*\(", header), name
-        assert _lib.EXPORTS[name] == _lib.EXPORTS["qagnn_radam_step"], name
-    assert "QAGNN_RULE_ADAM = 2" in header and "QAGNN_RULE_SGD = 3" in header
+    assert re.search(r"\bint32_t qagnn_optim_step\s*\(int32_t rule,", header)
+    assert "qagnn_optim_step" in _lib.EXPORTS
+    for name in ("qagnn_radam_step", "qagnn_adamw_step", "qagnn_adam_step", "qagnn_sgd_step"):
+        assert name not in header and name not in _lib.EXPORTS, name
+    assert "QAGNN_RULE_RADAM = 0, QAGNN_RULE_ADAMW = 1, QAGNN_RULE_ADAM = 2, QAGNN_RULE_SGD = 3" in header
 
 
 def _tool(name):
@@ -141,26 +142,31 @@ def _tool(name):
 
 @pytest.fixture(scope="module")
 def kernels(tmp_path_factory):
-    """csrc/optim_torch.cu cross-compiled with the library's flags: {kernel: opcode counts}."""
+    """csrc/optim.cu and csrc/tail.cu cross-compiled with the library's flags: {kernel: opcode counts} of the Adam and SGD
+    kernels."""
     nvcc, cuobjdump = _tool("nvcc"), _tool("cuobjdump")
     if nvcc is None or cuobjdump is None:
         pytest.skip("no nvcc / cuobjdump")
-    obj = str(tmp_path_factory.mktemp("optim_torch") / "optim_torch.o")
-    subprocess.run([nvcc, "-c", os.path.join(build.CSRC, "optim_torch.cu"), "-o", obj] + build.NVCC_FLAGS,
-                   capture_output=True, text=True, check=True)
-    sass = subprocess.run([cuobjdump, "-sass", obj], capture_output=True, text=True, check=True).stdout
     out = {}
-    for body in re.split(r"\n\s*Function : ", sass)[1:]:
-        ops = collections.Counter()
-        for line in body.split("\n"):
-            m = re.match(r"\s*/\*[0-9a-f]{4,}\*/\s+(?:@!?U?P\w+\s+)?([A-Z][A-Z0-9_.]*)", line)
-            if m:
-                ops[m.group(1)] += 1
-        out[re.search(r"\d+((?:tail_)?(?:adam|sgd)_kernel)", body.split("\n", 1)[0]).group(1)] = ops
+    for src in ("optim.cu", "tail.cu"):
+        obj = str(tmp_path_factory.mktemp("optim") / (src + ".o"))
+        subprocess.run([nvcc, "-c", os.path.join(build.CSRC, src), "-o", obj] + build.NVCC_FLAGS,
+                       capture_output=True, text=True, check=True)
+        sass = subprocess.run([cuobjdump, "-sass", obj], capture_output=True, text=True, check=True).stdout
+        for body in re.split(r"\n\s*Function : ", sass)[1:]:
+            name = re.search(r"\d+((?:tail_)?(?:adam|sgd)_kernel)", body.split("\n", 1)[0])
+            if name is None:
+                continue
+            ops = collections.Counter()
+            for line in body.split("\n"):
+                m = re.match(r"\s*/\*[0-9a-f]{4,}\*/\s+(?:@!?U?P\w+\s+)?([A-Z][A-Z0-9_.]*)", line)
+                if m:
+                    ops[m.group(1)] += 1
+            out[name.group(1)] = ops
     return out
 
 
-def test_kernels_take_vector_loads_and_no_float_atomics(kernels):
+def test_adam_and_sgd_kernels_take_vector_loads_and_no_float_atomics(kernels):
     assert set(kernels) == {"adam_kernel", "sgd_kernel", "tail_adam_kernel", "tail_sgd_kernel"}
     for name, ops in kernels.items():
         atomics = [op for op in ops if op.split(".")[0] in ("RED", "REDG", "ATOM", "ATOMG", "ATOMS")]
