@@ -511,6 +511,37 @@ int32_t qagnn_keyed_dropout_forward_typed(int32_t dtype, int64_t A, int64_t G, i
 int32_t qagnn_keyed_dropout_backward_typed(int32_t dtype, int64_t n, double p, const uint32_t *mask, const void *dy, void *dx,
                                            void *stream);
 
+/* Status bits qagnn_schedule_batch ORs into a status word; graph prep's bits are below them. */
+enum {
+  QAGNN_SCHEDULE_BAD_ID = 1 << 20,     /* a question id of the batch outside [0, n_questions) */
+  QAGNN_SCHEDULE_PAST_EPOCH = 1 << 21  /* *counter outside [0, n_order / batch_size) */
+};
+
+/* The first launch of an optimiser batch replayed as one CUDA graph (qagnn_b200.pipeline.SplitTrainBatchGraph): batch c =
+ * *counter (device int64) of the device epoch order `order` (int64 [n_order]) into ids: ids[i] = order[c * batch_size + i]
+ * for the batch's (batch_size / micro_batch_size) * micro_batch_size first questions, so micro-batch j is ids[j mbs, (j+1) mbs).
+ * A counter outside [0, n_order / batch_size) sets QAGNN_SCHEDULE_PAST_EPOCH and an id outside [0, n_questions)
+ * QAGNN_SCHEDULE_BAD_ID in *status (device int32, ORed); either writes question 0 in place of what it refuses.  One launch,
+ * no host read. */
+int32_t qagnn_schedule_batch(const int64_t *order, int64_t n_order, const int64_t *counter, int64_t batch_size,
+                             int32_t micro_batch_size, int64_t n_questions, int64_t *ids, int32_t *status, void *stream);
+
+/* The last launch of such a batch: *total (device fp64) += (double)((losses[j] * (float)micro_batch_size) *
+ * (1.f / (float)batch_size)) for j = 0 ... n_micro - 1 in that order, each product one fp32 multiply rounded to nearest (torch's
+ * `loss * mbs / bs` on a CUDA fp32 loss), the sum Python's `total_loss += loss.item()`; then ++*counter (device int64).  One
+ * launch, no host read. */
+int32_t qagnn_batch_log(const float *losses, int32_t n_micro, int32_t micro_batch_size, int64_t batch_size, double *total,
+                        int64_t *counter, void *stream);
+
+/* Adds the CUDA graph `child_graph` (a cudaGraph_t, cloned) as a child-graph node of the graph `stream` is capturing, after the
+ * stream's current capture dependencies, and makes that node the stream's only dependency: the child runs where a replay of
+ * it on the stream would.  QAGNN_ERR_INVALID_ARGUMENT when the stream is not capturing. */
+int32_t qagnn_graph_add_child(void *stream, void *child_graph);
+
+/* Nodes of the cudaGraph_t `graph`: its own (a child graph counts one) or, with recursive nonzero, every non-graph node of it
+ * and its child graphs.  -1 on error. */
+int64_t qagnn_graph_node_count(void *graph, int32_t recursive);
+
 /* Launch counters since load (kernels this library enqueued); for bench.py's gpu_launches. */
 int64_t qagnn_launch_count(void);
 

@@ -116,6 +116,10 @@ EXPORTS = {
     "qagnn_keyed_dropout_forward_typed": (C.c_int32, [C.c_int32, C.c_int64, C.c_int64, C.c_int64, C.c_double, C.c_int64, _P, _P,
                                                       C.c_int32, C.c_int32, _P, _P, _P, _P]),
     "qagnn_keyed_dropout_backward_typed": (C.c_int32, [C.c_int32, C.c_int64, C.c_double, _P, _P, _P, _P]),
+    "qagnn_schedule_batch": (C.c_int32, [_P, C.c_int64, _P, C.c_int64, C.c_int32, C.c_int64, _P, _P, _P]),
+    "qagnn_batch_log": (C.c_int32, [_P, C.c_int32, C.c_int32, C.c_int64, _P, _P, _P]),
+    "qagnn_graph_add_child": (C.c_int32, [_P, _P]),
+    "qagnn_graph_node_count": (C.c_int64, [_P, C.c_int32]),
     "qagnn_launch_count": (C.c_int64, []),
     "qagnn_profile_enable": (C.c_int32, [C.c_int32]),
     "qagnn_profile_read": (C.c_int32, [C.POINTER(C.c_double), C.POINTER(C.c_int64)]),

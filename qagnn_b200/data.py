@@ -116,6 +116,12 @@ def _node_capacity(total, node_capacity):
     return int(node_capacity)
 
 
+def largest_edges(counts, m):
+    """Edges of the `m` largest sub-graphs of a split together, from its per-sub-graph edge counts."""
+    m = min(int(m), len(counts))
+    return int(np.sort(counts)[len(counts) - m:].sum()) if m > 0 else 0
+
+
 def split_node_capacity(adj_lengths, batch_size):
     """Node capacity of a ragged split read in a FIXED batch order (dev and test splits are not shuffled): the largest
     sum(adj_lengths) over its batches of `batch_size` questions.  adj_lengths is the split's [Q, num_choice] (or [Q]) tensor.  A
@@ -325,9 +331,7 @@ class FlatAdjCache:
     def max_batch_edges(self, batch_size):
         """Edges of the `batch_size * num_choice` largest sub-graphs together: an edge capacity that holds for every batch
         of `batch_size` questions, however the split is shuffled."""
-        counts = np.diff(self.graph_ptr)
-        m = min(int(batch_size) * self.num_choice, len(counts))
-        return int(np.sort(counts)[len(counts) - m:].sum()) if m > 0 else 0
+        return largest_edges(np.diff(self.graph_ptr), int(batch_size) * self.num_choice)
 
     def __getitem__(self, i):
         """What LM_QAGNN_DataLoader does with `adj_data` besides handing it to the batch generator
@@ -467,6 +471,11 @@ class DeviceSplit:
             if idx.numel():
                 q = int(idx[0, 0])
                 raise IndexError(f"DeviceSplit: question {q} has label {int(self.labels[q])}, outside [0, {nc})")
+
+    def max_batch_edges(self, batch_size):
+        """FlatAdjCache.max_batch_edges of the split's adjacency: an edge capacity that holds for every batch of `batch_size`
+        questions, however the split is shuffled."""
+        return largest_edges(self.counts, int(batch_size) * self.num_choice)
 
     def check(self, question_ids, edge_capacity, node_capacity=None):
         """The host checks of one batch, O(bs * num_choice), with FlatAdjCache.pack's exceptions: IndexError for a question id

@@ -539,7 +539,7 @@ class CapturedTail:
         self.captures = 0
         self._key = None
         self._graph = None
-        self._bufs = None
+        self._bufs = self._bufs_key = self._graph_bufs = None
 
     @staticmethod
     def _check_dense(grad):
@@ -580,6 +580,29 @@ class CapturedTail:
 
     @torch.no_grad()
     def __call__(self):
+        key, launcher = self.prepare()
+        if self._graph is not None and self._key == key and self._graph_bufs is self._bufs:
+            self._graph.replay()
+        else:
+            # this call's step runs directly, which also loads the kernels; the capture then records the same launches
+            self._graph = None
+            launch = launcher()
+            launch()
+            graph = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(graph):
+                launch()
+            self._graph, self._key, self._graph_bufs = graph, key, self._bufs
+            self.captures += 1
+        return self._bufs["total_norm"].clone() if self.max_grad_norm > 0 else None
+
+    @torch.no_grad()
+    def prepare(self):
+        """The host half of a call, which a graph holding the tail's launches runs before every replay: the checks, the
+        scheduler step, the optimiser's host step count and the upload of the per-call block, enqueued on the current stream.
+        Returns (key, launcher): `key` names what the launches bake in (the device, the clip, and the addresses and sizes of
+        the parameters, gradients, optimiser state and scaler tensors), and `launcher()` returns a function that enqueues the
+        tail's kernels on the current stream.  The device buffers they use, `self._bufs`, are replaced when the key changes;
+        a graph that holds the launches is valid while the key and that dict are the ones it was captured with."""
         opt = self.optimizer
         st = None if self.scaler is None else self.scaler._per_optimizer_states.get(id(opt))
         if st is not None and st["stage"] is OptState.UNSCALED:
@@ -605,8 +628,8 @@ class CapturedTail:
         tables, table_len = opt._group_tables(device, hyper, range(len(hyper)))
         n_groups = len(hyper)
         n_bytes = lib.qagnn_step_tail_block_bytes(n_groups)
-        if self._key != key:
-            self._bufs = self._buffers(device, n_bytes, norm_grads, lib)
+        if self._bufs_key != key:
+            self._bufs, self._bufs_key = self._buffers(device, n_bytes, norm_grads, lib), key
         bufs = self._bufs
         # a fresh pinned buffer per call from the caching host allocator, which keeps it until its copy has run
         staging = torch.empty(n_bytes, dtype=torch.uint8, pin_memory=True)
@@ -616,19 +639,7 @@ class CapturedTail:
             float(sc._growth_factor) if sc else 2.0, float(sc._backoff_factor) if sc else 0.5,
             int(sc._growth_interval) if sc else 1, C.c_void_p(staging.data_ptr()), n_bytes), "qagnn_step_tail_fill")
         bufs["block"].copy_(staging, non_blocking=True)
-        if self._key == key:
-            self._graph.replay()
-        else:
-            # this call's step runs directly, which also loads the kernels; the capture then records the same launches
-            self._graph = None
-            launch = self._launcher(lib, device, items, states, moments, norm_grads, clip, scale, tracker, n_groups)
-            launch()
-            graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(graph):
-                launch()
-            self._graph, self._key = graph, key
-            self.captures += 1
-        return bufs["total_norm"].clone() if clip else None
+        return key, lambda: self._launcher(lib, device, items, states, moments, norm_grads, clip, scale, tracker, n_groups)
 
     def _buffers(self, device, n_bytes, norm_grads, lib):
         n = len(norm_grads)

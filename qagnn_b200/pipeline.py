@@ -24,18 +24,26 @@ cross-entropy or margin-rank loss; its backward graph adds the parameter gradien
 
 `SplitTrainBatch` runs several such micro-steps of an optimiser batch at once on one GPU, each on a stream of its own, and sums
 their gradients in micro-batch order.
+
+`SplitTrainBatchGraph` replays a whole optimiser batch of a SplitTrainBatch, optimiser tail included, as one CUDA graph fed
+from an epoch order on the GPU.
 """
 import contextlib
+import ctypes as C
+import time
 
 import numpy as np
 import torch
 
+from . import _lib
 from . import distributed as _dist
 from .data import PackedAdj
 from .modeling_qagnn import _version_key, decoder_tail
 from .training import answer_loss, check_answer_loss, keyed_dropout
 
 _EVAL_AUTOCAST = (None, torch.bfloat16)
+# qagnn_schedule_batch's status bits (QAGNN_SCHEDULE_* in include/qagnn_b200.h), above graph prep's
+SCHEDULE_BAD_ID, SCHEDULE_PAST_EPOCH = 1 << 20, 1 << 21
 _TRAIN_AUTOCAST = (None, torch.float16, torch.bfloat16)
 
 
@@ -66,9 +74,11 @@ class StatusWord:
         self.host = None if device is None else torch.zeros(1, dtype=torch.int32).pin_memory()
         self.pending = None  # event after the last replay's copy
 
-    def record(self, word):
+    def record(self, word=None):
+        """ORs `word` (None: nothing) into the device word and copies that to pinned memory."""
         if self.accum is not None:
-            self.accum.bitwise_or_(word)
+            if word is not None:
+                self.accum.bitwise_or_(word)
             self.host.copy_(self.accum, non_blocking=True)
 
     def replayed(self):
@@ -84,6 +94,12 @@ class StatusWord:
         if bits != 0:
             self.accum.zero_()
             self.host.zero_()
+            if bits & SCHEDULE_PAST_EPOCH:
+                raise ValueError(f"qagnn_b200: a {what} replay's batch counter was past its epoch's last full batch (status "
+                                 f"bits {bits}); it trained on question 0 in place of a batch. Call set_epoch first")
+            if bits & SCHEDULE_BAD_ID:
+                raise IndexError(f"qagnn_b200: a {what} replay's batch held a question id outside the split (status bits "
+                                 f"{bits}); it trained on question 0 in its place")
             raise IndexError(f"qagnn_b200: a {what} replay saw edge_index / edge_type / node_type values out of range or "
                              f"crossing a sub-graph boundary (status bits {bits}); its results were computed from clamped indices")
 
@@ -253,13 +269,13 @@ class _TrainingGraphs:
     def _addresses(self):
         return tuple(t.data_ptr() for t in self._params + self._buffers)
 
-    def _capture_graphs(self, adj, node_type, forward, backward, owned=(), stream=None):
+    def _capture_graphs(self, adj, node_type, forward, backward, owned=(), stream=None, keep_graph=False):
         """Captures `forward()` -> (y, ...) and `backward(y, dy)` as two CUDA graphs in one pool, on the batch (adj,
         node_type) already in the static buffers.  capture_guard first validates that batch and runs forward + backward twice
         (dy = 1) on a side stream; the forward graph ends by recording graph prep's status word into self._status.  The
         warm-up really runs: the decoder's buffers, the .grad of its trainable parameters (self._params), the tensors `owned`
         and the CUDA RNG state are put back afterwards.  Both graphs are captured on `stream` (None: torch.cuda.graph's own
-        side stream).  Returns (forward's outputs, the static dy buffer, backward's result)."""
+        side stream); `keep_graph` keeps their cudaGraph_t (CUDAGraph.raw_cuda_graph) for a parent graph.  Returns (forward's outputs, the static dy buffer, backward's result)."""
         dec = self.decoder
         dev = node_type.device
         self._params = [p for p in dec.parameters() if p.requires_grad]
@@ -275,7 +291,7 @@ class _TrainingGraphs:
         try:
             with capture_guard(dec.gnn, adj, node_type, self.what, warmup) as status:
                 pool = torch.cuda.graph_pool_handle()
-                fwd, bwd = torch.cuda.CUDAGraph(), torch.cuda.CUDAGraph()
+                fwd, bwd = torch.cuda.CUDAGraph(keep_graph), torch.cuda.CUDAGraph(keep_graph)
                 with torch.cuda.graph(fwd, pool=pool, stream=stream):
                     out = forward()
                     status.record(dec.gnn._last_prep.status_word())
@@ -766,7 +782,7 @@ class SplitTrainStep(_TrainingGraphs, _SplitBatches):
         used = self._capture_split(lambda used, grads: torch._foreach_add_([bufs[i] for i in used], grads), owned=bufs)
         self._owned = [(self._params[i], bufs[i]) for i in used]
 
-    def _capture_split(self, sink, owned=(), forward=None, stream=None):
+    def _capture_split(self, sink, owned=(), forward=None, stream=None, keep_graph=False):
         """Captures the forward graph (`forward`, default self._forward) and the backward graph, which ends by handing the
         parameter gradients the loss reaches to `sink(used, grads)`, `used` their indices into self._params.  Returns `used`."""
         used = []
@@ -779,7 +795,8 @@ class SplitTrainStep(_TrainingGraphs, _SplitBatches):
 
         self._assemble()  # capture_guard validates this batch
         (self._loss, logits, pool_attn), self._d_loss, self._g_sv = self._capture_graphs(
-            self._adj, self._out["node_type_ids"], forward or self._forward, backward, owned=owned, stream=stream)
+            self._adj, self._out["node_type_ids"], forward or self._forward, backward, owned=owned, stream=stream,
+            keep_graph=keep_graph)
         self.logits, self.pool_attn = logits.detach(), pool_attn.detach()
         self._requires_grad = [p.requires_grad for p in self.decoder.parameters()]
         self.captures += 1
@@ -838,7 +855,8 @@ class _TrainBranch(SplitTrainStep):
     """One micro-step of a SplitTrainBatch: a SplitTrainStep's forward and backward graphs in a pool of their own, captured
     on the branch's stream with the branch's CUDA generator state, with the decoder's BatchNorm buffers pointing at the
     branch's copies (which the forward graph first loads from the live buffers), and a backward graph that writes the
-    parameter gradients into the branch's row of the batch's slot buffer.  Its ids are the branch's row of the batch's."""
+    parameter gradients into the branch's row of the batch's slot buffer.  Its ids are the branch's row of the batch's.  Both
+    graphs keep their cudaGraph_t, which SplitTrainBatchGraph adds to its batch graph as child graphs."""
 
     what = "SplitTrainBatch"
 
@@ -867,7 +885,7 @@ class _TrainBranch(SplitTrainStep):
         try:
             with tb._bn.pointing_at(tb._bn_rows[b], tb._nbt_rows[b]):
                 self._capture_split(lambda used, grads: torch._foreach_copy_(tb._row_views(b, used), grads),
-                                    forward=forward, stream=stream)
+                                    forward=forward, stream=stream, keep_graph=True)
         finally:
             gen.graphsafe_set_state(live_rng)
         self._keep = (self.decoder.gnn._last_prep,)  # graph prep's buffers, which both graphs baked in
@@ -1077,6 +1095,266 @@ class SplitTrainBatch(_TrainingGraphs):
         elif list(used) != self._used:
             raise RuntimeError("SplitTrainBatch: the branches' losses reach different decoder parameters")
         return self._grad_slots.rows[b]
+
+
+def _draws_dropout(decoder):
+    """True when `decoder` in .train() draws dropout masks (a dropout rate above 0 anywhere)."""
+    return (any(isinstance(m, torch.nn.Dropout) and m.p > 0 for m in decoder.modules())
+            or getattr(decoder.gnn, "dropout_rate", 0) > 0)
+
+
+class SplitTrainBatchGraph:
+    """A whole optimiser batch of a SplitTrainBatch as ONE CUDA graph replay: every full micro-batch of the batch, the ordered
+    gradient sums, the BatchNorm folds, and with a frozen encoder the optimiser tail, fed from an epoch order held on the GPU:
+
+        key = training.DropoutKey(seed, device)
+        tb = SplitTrainBatch(model.decoder.train(), split, mbs, branches=8, edge_capacity=K, max_edges=M,
+                             autocast_dtype=torch.float16, loss=args.loss, dropout_key=key)
+        tail = optim.CapturedTail(optimizer, scaler, scheduler, args.max_grad_norm, model.parameters())
+        gb = SplitTrainBatchGraph(tb, bs, scaler=scaler, tail=tail)      # tail=None with a trainable encoder
+        gb.set_epoch(order)                           # host int64: the epoch's shuffled training question ids, once
+        for b in range(gb.n_batches):
+            gb.sent_vecs.copy_(encoder_output_of(order[b * bs:(b + 1) * bs]))   # [bs * nc, S]
+            gb.step()
+        # the final partial batch, order[gb.n_batches * bs:], runs through tb and the eager partial micro-batch as before
+
+    One replay does what the eager composition does for batch `counter` of the order:
+
+        optimizer.zero_grad(set_to_none=True)
+        for chunk in tb.chunks(batch):
+            losses = tb(chunk, [sent_vecs of each micro-batch])
+            scaler.scale((losses * w).sum()).backward()     # w = mbs / bs in fp32 for every micro-batch
+        tail(); key.advance_()                              # the tail only when given
+
+    bit for bit in the parameters, `.grad`, the optimiser state, the scaler's scale and growth tracker, the BatchNorm running
+    statistics and num_batches_tracked, and each micro-batch's loss and logits (`losses` [n_micro] fp32, `logits`
+    [n_micro, mbs * nc, 1]).  It also adds each micro-batch's `loss * mbs / bs` into `total_loss` (fp64 [1]) in micro-batch
+    order, which is the reference's `total_loss += loss.item()` without the host reads; read and zero it once per log interval.
+
+    The graph is, in order: qagnn_schedule_batch, which writes the batch's question ids from the device order at the device
+    `counter`; per chunk, a copy of the chunk's ids into the branches' id rows, then on every branch's stream a copy of its
+    sent_vecs rows and of the loss seed (the scaler's device scale times w, or w) and the branch's forward and backward graphs as
+    child-graph nodes, then on the main stream the losses and logits, distributed.ordered_grad_sum_ of the branches' gradient
+    slots onto `.grad` (the first chunk starting from zero) and the BatchNorm fold; the tail's launches; qagnn_batch_log, which
+    adds the losses into `total_loss` and advances `counter`; key.advance_().  `step()` first makes each reached decoder
+    parameter's `.grad` the SplitTrainBatch's sum buffer (every other trainable decoder parameter's None) and runs the tail's
+    host half (CapturedTail.prepare: the scheduler step and the per-call block), then replays.  It reads nothing on the host.
+
+    With `tail=None` (a trainable encoder) the graph stops after the decoder's gradients and leaves each micro-batch's
+    dL/dsent_vecs, scaled like the loss seed, in `d_sent_vecs` [n_micro, mbs * nc, S]; the caller runs the encoder's backward
+    per micro-batch in micro-batch order and then the tail (INTEGRATION.md §1).
+
+    Checks: a question id of the order outside the split raises IndexError, and a counter past the epoch's last full batch
+    ValueError, at the next call, from a status word the schedule sets on the device (that replay trained on question 0 in
+    their place); the host refuses a call past the epoch's `n_batches` with ValueError before anything is enqueued.
+    Refusals at construction (ValueError): a batch size that is not a multiple of tb's micro-batch size, an edge capacity
+    below split.max_batch_edges(mbs), a decoder that draws dropout without tb's dropout key (a child graph does not advance
+    torch's generator), a tail whose scaler is not `scaler`.  At a call: RuntimeError without set_epoch and wherever
+    SplitTrainBatch raises it (.eval(), moved decoder parameters, another deterministic flag, another set of decoder parameters
+    requiring grad).  The first call, and a call whose tail moved (a frozen or unfrozen encoder parameter, another `.grad` or
+    optimiser state: CapturedTail's key) or whose epoch order grew, trains its batch directly and then captures the graph
+    again; `captures` counts the captures.  One GPU, padded batches."""
+
+    what = "SplitTrainBatchGraph"
+
+    def __init__(self, train_batch, batch_size, *, scaler=None, tail=None):
+        tb = train_batch
+        if not isinstance(tb, SplitTrainBatch):
+            raise ValueError(f"{self.what}: train_batch must be a SplitTrainBatch, got {type(tb).__name__}")
+        bs, mbs, split = int(batch_size), tb.batch_size, tb.split
+        if bs < mbs or bs % mbs:
+            raise ValueError(f"{self.what}: batch_size = {bs} is not a multiple of the micro-batch size {mbs}; the graph holds "
+                             f"full micro-batches only")
+        need = split.max_batch_edges(mbs)
+        if tb.edge_capacity < need:
+            raise ValueError(f"{self.what}: edge capacity {tb.edge_capacity} is below split.max_batch_edges({mbs}) = {need}, "
+                             f"which every micro-batch of any order must fit")
+        if tb.dropout_key is None and _draws_dropout(tb.decoder):
+            raise ValueError(f"{self.what}: the decoder draws dropout masks; give the SplitTrainBatch a training.DropoutKey "
+                             f"(a child graph replay does not advance torch's CUDA generator)")
+        if scaler is not None and not scaler.is_enabled():
+            scaler = None
+        if tail is not None and tail.scaler is not scaler:
+            raise ValueError(f"{self.what}: the tail's scaler is not `scaler`; the loss seed and the tail must use one scaler")
+        self.tb, self.tail, self.scaler = tb, tail, scaler
+        self.batch_size, self.micro_batch_size = bs, mbs
+        self.n_micro = bs // mbs
+        self.n_chunks = -(-self.n_micro // tb.branches)
+        dev = self.device = split.device
+        nc = split.num_choice
+        self.sent_vecs = torch.zeros(bs * nc, tb.decoder.svec2nvec.in_features, dtype=torch.float32, device=dev)
+        self.losses = torch.zeros(self.n_micro, dtype=torch.float32, device=dev)
+        self.logits = self.d_sent_vecs = None  # shaped by the branches' capture
+        self.total_loss = torch.zeros(1, dtype=torch.float64, device=dev)
+        self.counter = torch.zeros(1, dtype=torch.int64, device=dev)
+        self._ids = torch.zeros(self.n_chunks * tb.branches, mbs, dtype=torch.int64, device=dev)
+        self._seed = torch.full((), mbs / bs, dtype=torch.float32, device=dev)
+        self._w = self._seed.clone()
+        self._status = StatusWord(dev)
+        self._order = self._order_host = None
+        self.n_order = self.n_batches = self._done = 0
+        self._graph = self._key = None
+        self.captures = 0
+        self.instantiate_ms = None  # host time of the last capture's cudaGraphInstantiate
+        self.mode = "eager"
+
+    def set_epoch(self, order):
+        """Uploads one epoch's order (host int64 [n]: training question ids, shuffled as the caller likes) and resets
+        `counter`; `n_batches` = n // batch_size full batches follow, one per step()."""
+        q = np.asarray(order)
+        if q.ndim != 1 or not np.issubdtype(q.dtype, np.integer):
+            raise ValueError(f"{self.what}: the order must be a 1-d integer array, got {q.dtype} of shape {q.shape}")
+        q = np.ascontiguousarray(q, dtype=np.int64)
+        if self._order is None or self._order.numel() < q.size:
+            self._order = torch.zeros(max(q.size, 1), dtype=torch.int64, device=self.device)
+        if q.size:
+            # a pinned block from the caching host allocator: it is not reused before this copy has run
+            self._order[:q.size].copy_(torch.from_numpy(q).pin_memory(), non_blocking=True)
+        self.counter.zero_()
+        self._order_host, self.n_order = q, int(q.size)
+        self.n_batches, self._done = self.n_order // self.batch_size, 0
+
+    def step(self):
+        """Trains the next full batch of the epoch order with one graph replay (the first call, and one after the tail moved,
+        train it directly and capture)."""
+        tb = self.tb
+        if self._order is None:
+            raise RuntimeError(f"{self.what}: no epoch order; call set_epoch(order) first")
+        if not tb.decoder.training:
+            raise RuntimeError(f"{self.what} replays the training forward: call decoder.train() first")
+        captured = tb._slots is not None
+        if captured:
+            tb._check_fit()
+            tb._check_requires_grad()
+            for br in tb._branches:
+                br._status.check(self.what)
+        self._status.check(self.what)
+        if self._done >= self.n_batches:
+            raise ValueError(f"{self.what}: the epoch's {self.n_batches} full batches are done; call set_epoch for the next "
+                             f"epoch (a final partial batch runs through the SplitTrainBatch)")
+        if not captured:
+            self._capture_branches()
+        if self.logits is None:  # the first call after the branches were captured, here or by the SplitTrainBatch's own call
+            br = tb._branches[0]
+            self.logits = torch.zeros((self.n_micro,) + tuple(br.logits.shape), dtype=br.logits.dtype, device=self.device)
+            if self.tail is None:
+                self.d_sent_vecs = torch.zeros((self.n_micro,) + tuple(br._g_sv.shape), dtype=br._g_sv.dtype,
+                                               device=self.device)
+        gs = tb._grad_slots
+        for p in tb._params:  # as after zero_grad(set_to_none=True); the graph's first chunk writes the sums' buffer
+            p.grad = None
+        for p, g in zip(gs.tensors, gs.own):
+            p.grad = g
+        scale = None
+        if self.scaler is not None:
+            if self.scaler._scale is None:
+                self.scaler._lazy_init_scale_growth_tracker(self.device)
+            scale = self.scaler._scale
+        tail_key, tail_bufs, launch = None, None, None
+        if self.tail is not None:
+            tail_key, launcher = self.tail.prepare()
+            tail_bufs = self.tail._bufs
+        key = (tail_key, self._order.data_ptr(), self.n_order, None if scale is None else scale.data_ptr())
+        tb.calls += 1  # a backward through an earlier tb call's losses now raises: the replay overwrites their activations
+        if self._graph is not None and self._key[0] == key and self._key[1] is tail_bufs:
+            self._graph.replay()
+        else:
+            self._graph = None  # frees the previous capture's pool before the next one is made
+            launch = None if self.tail is None else launcher()
+            self._run(lambda g: g.replay(), launch, scale)  # this batch, directly; it also loads every kernel
+            self._capture(launch, scale)
+            self._key = (key, tail_bufs)
+        self._done += 1
+        self._status.replayed()
+        for br in tb._branches:
+            br._status.replayed()
+        # the replay changed the running statistics (and, with the tail, the parameters) behind autograd's back: the eval
+        # path's folded weights key on versions
+        torch.autograd.graph.increment_version(tb._bn.live + tb._bn.live_counts
+                                               + (tb._params if self.tail is not None else []))
+
+    def node_count(self, recursive=False):
+        """Nodes of the captured batch graph: its own (each branch graph one child-graph node) or, recursive, every node of it
+        and its child graphs."""
+        if self._graph is None:
+            raise RuntimeError(f"{self.what}: nothing is captured yet")
+        return int(_lib.load().qagnn_graph_node_count(C.c_void_p(self._graph.raw_cuda_graph()), int(recursive)))
+
+    def _capture_branches(self):
+        """The SplitTrainBatch's capture, on the first micro-batches of this call's batch (host ids, checked as a
+        SplitTrainBatch call checks them) and their rows of `sent_vecs`."""
+        tb, mbs = self.tb, self.micro_batch_size
+        rows = mbs * tb.split.num_choice
+        first = self._done * self.batch_size
+        n = min(tb.branches, self.n_micro)
+        chunk = [self._order_host[first + j * mbs:first + (j + 1) * mbs] for j in range(n)]
+        svs = [self.sent_vecs[j * rows:(j + 1) * rows] for j in range(n)]
+        ids = np.stack([tb._checked_ids(chunk[j % n], svs[j % n], tb._branches[j]) for j in range(tb.branches)])
+        tb._qids.copy_(torch.from_numpy(ids).pin_memory(), non_blocking=True)
+        tb._capture(svs)
+
+    def _run(self, child, launch, scale):
+        """Enqueues one batch on the current stream, with `child(graph)` running (or recording) a branch graph on the current
+        stream and `launch()` the tail's kernels (None: no tail)."""
+        tb, dev, lib = self.tb, self.device, _lib.load()
+        mbs, S, rows = self.micro_batch_size, tb.branches, self.micro_batch_size * tb.split.num_choice
+        cur = torch.cuda.current_stream(dev)
+        with torch.cuda.device(dev):
+            _lib.check(lib.qagnn_schedule_batch(_lib.ptr(self._order), self.n_order, _lib.ptr(self.counter), self.batch_size,
+                                                mbs, tb.split.n_questions, _lib.ptr(self._ids), _lib.ptr(self._status.accum),
+                                                _lib.stream_ptr(dev)), "qagnn_schedule_batch")
+        with torch.no_grad():
+            if scale is not None:
+                torch.mul(scale.view(()), self._w, out=self._seed)
+            gs = tb._grad_slots
+            for c in range(self.n_chunks):
+                a = c * S
+                n = min(S, self.n_micro - a)
+                branches = tb._branches[:n]
+                tb._qids[:n].copy_(self._ids[a:a + n])
+                for j, br in enumerate(branches):
+                    br.stream.wait_stream(cur)
+                    with torch.cuda.stream(br.stream):
+                        br._sv.copy_(self.sent_vecs[(a + j) * rows:(a + j + 1) * rows])
+                        br._d_loss.copy_(self._seed)
+                        child(br._fwd)
+                        child(br._bwd)
+                for br in branches:
+                    cur.wait_stream(br.stream)
+                torch.stack([br._loss for br in branches], out=self.losses[a:a + n])
+                torch.stack([br.logits for br in branches], out=self.logits[a:a + n])
+                if self.d_sent_vecs is not None:
+                    torch.stack([br._g_sv for br in branches], out=self.d_sent_vecs[a:a + n])
+                gs.sum_([None] * len(gs.tensors) if c == 0 else [p.grad for p in gs.tensors], n)
+                if tb._bn.bns:  # the branches' BatchNorm rows into the live buffers, in micro-batch order
+                    tb._bn.fold_(tb._bn.read(), (tb._bn_rows[:n], tb._nbt_rows[:n]))
+        if launch is not None:
+            launch()
+        with torch.cuda.device(dev):
+            _lib.check(lib.qagnn_batch_log(_lib.ptr(self.losses), self.n_micro, mbs, self.batch_size,
+                                           _lib.ptr(self.total_loss), _lib.ptr(self.counter), _lib.stream_ptr(dev)),
+                       "qagnn_batch_log")
+        if tb.dropout_key is not None:
+            tb.dropout_key.advance_()
+        self._status.record()
+
+    def _capture(self, launch, scale):
+        dev, lib = self.device, _lib.load()
+
+        def child(g):
+            _lib.check(lib.qagnn_graph_add_child(_lib.stream_ptr(dev), C.c_void_p(g.raw_cuda_graph())),
+                       "qagnn_graph_add_child")
+
+        graph = torch.cuda.CUDAGraph(keep_graph=True)
+        with torch.cuda.graph(graph):
+            self._run(child, launch, scale)
+        t0 = time.perf_counter()
+        graph.instantiate()
+        self.instantiate_ms = 1e3 * (time.perf_counter() - t0)
+        self._graph = graph
+        self.captures += 1
+        self.mode = ("one CUDA graph: schedule, " + f"{self.n_chunks} chunks of {self.tb.branches} branch graph pairs, sums "
+                     "and folds" + (", the optimiser tail" if self.tail is not None else "") + ", log")
 
 
 def packed_host_batch(adj, H, node_type, node_score, sent_vecs, adj_lengths):
